@@ -1,17 +1,18 @@
 #!/usr/bin/env python
 """bench.py - the hot path's benchmark (contract in the task prompt, section 4).
 
-    python bench.py --gpus 1 --steps K --warmup W            # B200 arm
+    python bench.py --gpus 1 --steps K --warmup W            # CUDA (H100) arm
     python bench.py --impl reference --steps K --warmup W    # reference CPU arm
     torchrun --nproc-per-node N ... bench.py --gpus N ...    # MCU-row sharded, weak scaling
 
 A "step" is one complete do_quantsmooth pass (all components, all iterations) over one
-synthetic image.  N=1 workload: BASELINE.json's metric configuration, 7680x4320 YCbCr
+synthetic image.  N=1 workload: BASELINE.md's metric configuration, 7680x4320 YCbCr
 4:2:0, q=3 (flags 0), niter=3.  N>1: the same image stacked N times vertically
 (7680 x 4320*N), sharded by MCU rows with one halo pixel row per component exchanged over
 NCCL between the IDCT and smoothing passes of every iteration (weak scaling).
 
-Prints ONE JSON line (rank 0).
+Prints ONE JSON line (rank 0).  --dump-outputs DIR also writes what the last timed step
+computed (see dump_outputs).
 """
 import argparse
 import json
@@ -37,7 +38,7 @@ def peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "data sheet (H100 SXM HBM3, 3.35 TB/s)"
 
 
 class ClockSampler:
@@ -92,6 +93,25 @@ class ClockSampler:
                     reasons.add(name)
         return {"sm_mhz": statistics.median(sm) if sm else None, "sm_max_mhz": max(mx) if mx else None,
                 "samples": len(sm), "scope": scope, "reasons": sorted(reasons)}
+
+
+DUMP_BLOCKS = 1 << 16                    # blocks per component in --dump-outputs (16 MB as float32)
+
+
+def dump_outputs(outdir, im, bufs):
+    """Writes the smoothed coefficients of the last timed step as comp<i>.npy (float32,
+    [blocks, 64]): every component's blocks in raster order, or, for a component with more than
+    DUMP_BLOCKS blocks, the same seeded sample of DUMP_BLOCKS of them (sorted) in every run.
+    Inputs are seeded too, so two builds can be compared output for output."""
+    import torch
+    os.makedirs(outdir, exist_ok=True)
+    for i, (c, t) in enumerate(zip(im.comps, bufs)):
+        flat = t.view(-1, 64)
+        n = flat.shape[0]
+        if n > DUMP_BLOCKS:
+            pick = np.sort(np.random.default_rng(1000 + i).choice(n, DUMP_BLOCKS, replace=False))
+            flat = flat.index_select(0, torch.from_numpy(pick).to(flat.device))
+        np.save(os.path.join(outdir, f"comp{i}.npy"), flat.float().cpu().numpy())
 
 
 def make_workload(world, rank):
@@ -211,6 +231,8 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's smoothed coefficients (float32 .npy) to DIR")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
     rank = int(os.environ.get("RANK", "0"))
@@ -224,7 +246,7 @@ def main():
     import jpegqs_b200 as qs
     from jpegqs_b200 import multigpu as mg
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device - the B200 arm has no CPU fallback")
+        raise SystemExit("bench.py: no CUDA device - the CUDA arm has no CPU fallback")
     torch.cuda.set_device(local_rank)
     dist = None
     if world > 1:
@@ -241,7 +263,11 @@ def main():
     nblocks_rank = im.num_blocks
     total_blocks = nblocks_rank
     K, Wm = args.steps, args.warmup
-    nbuf = K + Wm
+    # a distinct pristine input buffer per step while they fit in half of the free device memory;
+    # beyond that the buffers are reused and refreshed from a pristine copy before each step
+    set_bytes = sum(c.coef.nbytes for c in im.comps)
+    free_bytes = torch.cuda.mem_get_info(dev)[0]
+    nbuf = max(2, min(K + Wm, int(free_bytes // 2 // set_bytes) - 1))
     # a dedicated stream: the C ABI launches on it, the CUDA events below are recorded on it
     # and NCCL orders its halo exchange against it
     tstream = torch.cuda.Stream(device=dev)
@@ -252,13 +278,21 @@ def main():
     # ---- device-resident arm: a distinct pristine input buffer per step -----------------
     host_coefs = [torch.from_numpy(np.ascontiguousarray(c.coef)) for c in im.comps]
     dev_bufs = [[h.to(dev) for h in host_coefs] for _ in range(nbuf)]
+    pristine = [h.to(dev) for h in host_coefs] if nbuf < K + Wm else None
     torch.cuda.synchronize()
+
+    def bufs(i):
+        b = dev_bufs[i % nbuf]
+        if pristine is not None and i >= nbuf:
+            for t, p in zip(b, pristine):
+                t.copy_(p)
+        return b
 
     hblk_total, row0 = None, None
     link = None
     if world == 1:
         def step(i):
-            ret, _ = ctx.run_device(im, [t.data_ptr() for t in dev_bufs[i]], [], FLAGS, NITER, stream)
+            ret, _ = ctx.run_device(im, [t.data_ptr() for t in bufs(i)], [], FLAGS, NITER, stream)
             return ret
     else:
         # The C slab engine (include/jpegqs_cuda.h "one image sharded by MCU rows"): every rank
@@ -275,7 +309,7 @@ def main():
 
         def step(i):
             return ctx.run_slab(link, im, rank, world, row0, hblk_total, FLAGS, NITER,
-                                coef_ptrs=[t.data_ptr() for t in dev_bufs[i]], up_ptrs=[], stream=stream)[0]
+                                coef_ptrs=[t.data_ptr() for t in bufs(i)], up_ptrs=[], stream=stream)[0]
 
     def barrier():
         torch.cuda.synchronize()
@@ -314,6 +348,10 @@ def main():
         total_blocks = int(nb.item())
     ms_per_step = ms_total / K
     value = mpix_job / (ms_per_step / 1e3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, im, dev_bufs[(Wm + K - 1) % nbuf])
+    del dev_bufs, pristine
+    torch.cuda.empty_cache()
 
     # ---- e2e: the drop-in call itself --------------------------------------------------------
     # N=1: the library's exported do_quantsmooth(j_decompress_ptr, jvirt_barray_ptr*, jpegqs_control_t*)
@@ -326,23 +364,27 @@ def main():
     if not args.no_e2e:
         h2d = sum(c.coef.nbytes for c in im.comps)
         d2h = h2d
+        nhost = min(nbuf, 8)                         # host copies of the input: reloaded when reused
         if world == 1:
             import ctypes as C
             sys.path.insert(0, os.path.join(ROOT, "tests"))
             import oracle_lib as ol                   # only its fake libjpeg front end (no smoothing code)
             ol.ensure_built()
             fn = C.cast(qs.cuda.load().do_quantsmooth, C.c_void_p)
-            sessions = [ol.BoundarySession(im, scatter_rows=True) for _ in range(nbuf)]
+            sessions = [ol.BoundarySession(im, scatter_rows=True) for _ in range(nhost)]
+
+            def reload(i):
+                sessions[i % nhost].load()
 
             def e2e_step(i):
-                ret = sessions[i].run(fn, FLAGS | 64, NITER)          # 64 = JPEGQS_TRANSCODE
+                ret = sessions[i % nhost].run(fn, FLAGS | 64, NITER)          # 64 = JPEGQS_TRANSCODE
                 if ret != 0:
                     raise SystemExit(f"do_quantsmooth returned {ret}")
             api = ("do_quantsmooth(j_decompress_ptr, jvirt_barray_ptr*, jpegqs_control_t*) of libjpegqs_b200.so, "
                    "called through a fake libjpeg with scattered pageable block rows")
         else:
             pinned = []
-            for _ in range(nbuf):
+            for _ in range(nhost):
                 row = []
                 for c in im.comps:
                     p = qs.cuda.PinnedArray(c.coef.shape)
@@ -353,23 +395,32 @@ def main():
             from jpegqs_b200.image import CoefImage, Component
             hosts = [CoefImage(im.width, im.height, im.colorspace,
                                [Component(pinned[i][k].array, c.quant.copy(), c.h_samp, c.v_samp, c.quant_tbl_no)
-                                for k, c in enumerate(im.comps)]) for i in range(nbuf)]
+                                for k, c in enumerate(im.comps)]) for i in range(nhost)]
+
+            def reload(i):
+                for p, c in zip(pinned[i % nhost], im.comps):
+                    p.array[...] = c.coef
 
             def e2e_step(i):
-                ret = ctx.run_slab(link, hosts[i], rank, world, row0, hblk_total, FLAGS, NITER)[0]
+                ret = ctx.run_slab(link, hosts[i % nhost], rank, world, row0, hblk_total, FLAGS, NITER)[0]
                 if ret != 0:
                     raise SystemExit(f"run_slab returned {ret}")
             api = ("jpegqs_cuda_run_slab (C slab engine) on every rank with caller-pinned host slabs: "
                    "H2D, kernels + kernel-side halo exchange over CUDA IPC mailboxes, D2H")
 
         for i in range(Wm):
+            if i >= nhost:
+                reload(i)
             e2e_step(i)
         barrier()
-        t0 = time.perf_counter()
+        dt = 0.0
         for i in range(K):
+            if Wm + i >= nhost:
+                reload(Wm + i)                           # restoring the input is not part of the call
+            t0 = time.perf_counter()
             e2e_step(Wm + i)
-        barrier()
-        dt = time.perf_counter() - t0
+            barrier()
+            dt += time.perf_counter() - t0
         if dist is not None:
             t = torch.tensor([dt], dtype=torch.float64, device=dev)
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -393,14 +444,9 @@ def main():
         bytes_per_launch = ALGO_BYTES_PER_BLOCK_ITER * nblocks_rank
         avg_ms = smooth_ms / smooth_n
         achieved = bytes_per_launch / (avg_ms / 1e3) / 1e9
-        traffic = None
-        tp = os.path.join(ROOT, "profiles", "smooth_traffic.json")
-        if os.path.exists(tp):
-            with open(tp) as f:
-                traffic = json.load(f).get("dram_bytes_per_launch")
         roofline = {"bound": "hbm", "kernel": "qs_smooth_kernel" + ("" if world == 1 else " (rank 0's slab)"),
                     "achieved": round(achieved, 2),
-                    "peak": peak, "unit": "GB/s", "frac": round(achieved / peak, 5), "traffic": traffic,
+                    "peak": peak, "unit": "GB/s", "frac": round(achieved / peak, 5),
                     "peak_source": peak_src, "avg_launch_ms": round(avg_ms, 4),
                     "algorithmic_bytes_per_launch": bytes_per_launch,
                     "share_of_step": round(smooth_ms / (ms_total if ms_total else 1), 4),
@@ -423,15 +469,16 @@ def main():
             return total
         fp_inst = sum(min_fp_per_block(c.quant, bool(FLAGS & 1)) * c.wblk * c.hblk for c in im.comps) / 32.0
         fp_inst_plain = 8288 * 8 * nblocks_rank / 32.0                  # without the uniform-chunk sharing
-        sm_mhz = (clocks or {}).get("sm_mhz") or 1965.0
-        issue_peak = 148 * 4 * sm_mhz * 1e6                            # warp-instr/s at 1 per SMSP per clock
+        sm_mhz = (clocks or {}).get("sm_mhz") or 1980.0                # H100 SXM boost clock
+        n_sms = torch.cuda.get_device_properties(dev).multi_processor_count
+        issue_peak = n_sms * 4 * sm_mhz * 1e6                          # warp-instr/s at 1 per SMSP per clock
         roofline_fp32 = {"bound": "fp32-issue", "achieved": round(fp_inst / (avg_ms / 1e3) / 1e12, 4),
                          "peak": round(issue_peak / 1e12, 4), "unit": "T warp-instr/s",
                          "frac": round(fp_inst / (avg_ms / 1e3) / issue_peak, 4),
                          "frac_counting_8_per_term": round(fp_inst_plain / (avg_ms / 1e3) / issue_peak, 4),
                          "note": "minimum FP32-pipe instructions of the order-exact arithmetic for the chunk schedules in "
-                                 "use (uniform chunks: 3 + 5n per term) / (148 SM x 4 sub-partitions x measured SM clock); "
-                                 "frac_counting_8_per_term is round 1's figure (8 per term everywhere)"}
+                                 f"use (uniform chunks: 3 + 5n per term) / ({n_sms} SM x 4 sub-partitions x measured SM clock); "
+                                 "frac_counting_8_per_term counts 8 per term everywhere"}
     else:
         roofline_fp32 = None
 
@@ -450,8 +497,10 @@ def main():
             "config": {"workload": f"{WIDTH}x{HEIGHT * world} YCbCr 4:2:0 (8K x{world} stacked), q=3 (flags 0), "
                                    f"niter=3, quality-50 Annex-K tables, seed {SEED}",
                        "blocks": total_blocks,
-                       "cache": "a distinct pristine input buffer per step (100 MB each, "
-                                f"{nbuf} buffers > 126 MB L2)",
+                       "cache": f"pristine input buffers ({set_bytes / 1e6:.0f} MB each, {nbuf} of them, "
+                                f"{'one per step' if nbuf >= K + Wm else 'refreshed by a device copy inside each later step'}; "
+                                f"{torch.cuda.get_device_properties(dev).L2_cache_size / 2**20:.0f} MB L2)",
+                       "device": torch.cuda.get_device_name(dev),
                        "sharding": "none" if world == 1 else
                        f"MCU rows over {world} GPUs (one process each); halo rows + out-of-range masks exchanged by "
                        "CUDA kernels through peer mailboxes (CUDA IPC / NVLink), no host sync, no NCCL on the data path"},

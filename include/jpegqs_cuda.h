@@ -1,5 +1,5 @@
 /*
- * jpegqs_cuda.h - C ABI of the B200 (sm_100a) back end of libjpegqs.
+ * jpegqs_cuda.h - C ABI of the H100 (sm_90a) back end of libjpegqs.
  *
  * This is the boundary between the libjpeg-facing host code (csrc/do_quantsmooth.c, which
  * keeps the reference's own entry points of libjpegqs.h) and the CUDA implementation.  It
@@ -91,9 +91,10 @@ void jpegqs_cuda_kernel_stats(const jpegqs_cuda_ctx *ctx, float *idct_ms, int *i
  * key 7: blocks per slab wave for key 6; 0 = SM count x resident warps x 32 (tests force small values)
  * key 8: the two edge coefficients of an anti-diagonal ride along with up to two of its full
  *        coefficients in one "mixed" chunk instead of forming their own
- * keys 0, 2, 4 (lock-step level, warps per sub-partition, packed FP32x2 path) only exist in the
- * measurement build (make -C csrc experiments); the shipped library accepts their default values
- * and answers JPEGQS_ERR_UNSUPPORTED otherwise.  key 3: retired, ignored. */
+ * keys 0, 2 (lock-step level, warps per sub-partition) only exist in the measurement build
+ * (make -C csrc experiments); the shipped library accepts their default values and answers
+ * JPEGQS_ERR_UNSUPPORTED otherwise.  key 3: retired, ignored.  key 4: retired (a packed FP32x2
+ * path); every build accepts 0 only. */
 int jpegqs_cuda_set_tuning(jpegqs_cuda_ctx *ctx, int key, int value);
 
 /* pinned host memory for coefficient arrays: the copy engines read / write it directly.  Plain
@@ -156,7 +157,7 @@ int jpegqs_cuda_run_slab(jpegqs_cuda_ctx *ctx, jpegqs_cuda_link *link, jpegqs_cu
  * set): contexts + links for ndev devices (devices == NULL: ordinals 0..ndev-1; ndev <= 0: all),
  * one host thread per device inside run_host_multi.  An image is spread over as many devices as
  * it has waves of the smoothing kernel (JPEGQS_MIN_BLOCKS_PER_GPU luma blocks per device,
- * default 148*16*32), so a small image stays on device 0 with the slab-pipelined run_host. */
+ * default 132*16*32, one wave on an H100), so a small image stays on device 0 with the slab-pipelined run_host. */
 typedef struct jpegqs_cuda_multi jpegqs_cuda_multi;
 int jpegqs_cuda_multi_create(int ndev, const int *devices, jpegqs_cuda_multi **out);
 void jpegqs_cuda_multi_destroy(jpegqs_cuda_multi *m);

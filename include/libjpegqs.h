@@ -1,5 +1,5 @@
 /*
- * libjpegqs.h - public API of the B200-native quantsmooth library.
+ * libjpegqs.h - public API of the H100-native (sm_90a) quantsmooth library.
  *
  * Source compatible with the reference's API header (reference libjpegqs.h:14-55): the same
  * identifiers with the same values, the same jpegqs_control_t layout and the same three entry
@@ -11,7 +11,7 @@
  * Include <jpeglib.h> before this header.
  *
  * Behavioural differences (INTEGRATION.md):
- *   - the smoothing runs on a CUDA device (sm_100a).  There is no CPU fallback: without a
+ *   - the smoothing runs on a CUDA device (sm_90a).  There is no CPU fallback: without a
  *     usable device do_quantsmooth reports on stderr and returns a negative value, leaving
  *     the coefficients untouched;
  *   - jpegqs_control_t.threads is ignored (reference: OpenMP thread count,
@@ -64,8 +64,8 @@ enum jpegqs_limits { JPEGQS_ITER_MAX = 100 };   /* niter is clamped to [0, JPEGQ
 
 #define JPEGQS_VERSION "1.20230818-b200"
 /* the reference CLI prints this next to the version (quantsmooth.c:472); the algorithm is its
- * author's, the sm_100a back end is this repository's */
-#define JPEGQS_COPYRIGHT "algorithm (C) 2020-2026 Ilya Kurdyukov, B200 back end (C) 2026 jpeg-quantsmooth_b200"
+ * author's, the sm_90a back end is this repository's */
+#define JPEGQS_COPYRIGHT "algorithm (C) 2020-2026 Ilya Kurdyukov, CUDA back end (C) 2026 jpeg-quantsmooth_b200"
 
 typedef struct jpegqs_control {
 	int flags;                         /* JPEGQS_* bits                                          */

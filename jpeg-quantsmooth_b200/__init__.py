@@ -1,4 +1,4 @@
-"""jpegqs_b200 - B200-native (sm_100a) implementation of jpeg-quantsmooth's
+"""jpegqs_b200 - H100-native (sm_90a) implementation of jpeg-quantsmooth's
 coefficient-smoothing hot path.  See DESIGN.md.
 
 Host-side Python mirror of the reference's API surface for that path:

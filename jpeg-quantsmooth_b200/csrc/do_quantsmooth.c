@@ -213,8 +213,8 @@ int do_quantsmooth(j_decompress_ptr srcinfo, jvirt_barray_ptr *coef_arrays, jpeg
 	if (!ctx) { pthread_mutex_unlock(&g_lock); return JPEGQS_ERR_CUDA; }
 #ifdef WITH_LOG
 	if (flags & JPEGQS_INFO_CPU) {
-		if (multi) logfmt("SIMD type: CUDA sm_100a (%s x %d)\n", jpegqs_cuda_device_name(ctx), jpegqs_cuda_multi_devices(multi));
-		else logfmt("SIMD type: CUDA sm_100a (%s)\n", jpegqs_cuda_device_name(ctx));
+		if (multi) logfmt("SIMD type: CUDA sm_90a (%s x %d)\n", jpegqs_cuda_device_name(ctx), jpegqs_cuda_multi_devices(multi));
+		else logfmt("SIMD type: CUDA sm_90a (%s)\n", jpegqs_cuda_device_name(ctx));
 	}
 	LOG_COMP2                                          /* quantsmooth.h:2569-2572 */
 #endif

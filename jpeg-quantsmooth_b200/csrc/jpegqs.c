@@ -1,5 +1,5 @@
 /*
- * jpegqs.c - the `jpegqs` command line tool on top of the B200 back end.
+ * jpegqs.c - the `jpegqs` command line tool on top of the CUDA (sm_90a) back end.
  *
  * Same command line surface as the reference tool (reference quantsmooth.c:288-393):
  *   jpegqs [options] input.jpg output.jpg        ("-" = stdin / stdout)
@@ -58,7 +58,7 @@ static unsigned char *load_all(FILE *f, size_t *len) {
 
 static int usage(const char *prog) {
 	fprintf(stderr,
-		"jpegqs (B200 back end) version " JPEGQS_VERSION "\n"
+		"jpegqs (CUDA sm_90a back end) version " JPEGQS_VERSION "\n"
 		"Usage:\n  %s [options] input.jpg output.jpg\n\nOptions:\n"
 		"  -q, --quality n   Quality setting (0-6, default is 3)\n"
 		"  -n, --niter n     Number of iterations (default is 3)\n"
@@ -343,8 +343,8 @@ int main(int argc, char **argv) {
 	opts.threads = threads;
 	if (threads > 0) jq_set_threads(threads);
 
-	/* --batch: any number of "input output" pairs in one process, so that CUDA start-up (1-2 s in a
-	 * fresh process, profiles/README.md) is paid once; the exit status is the worst of the pairs */
+	/* --batch: any number of "input output" pairs in one process, so that CUDA start-up (context and
+	 * kernel image, seconds in a fresh process) is paid once; the exit status is the worst of the pairs */
 	{
 		qs_cfg g; qs_job *jobs; int n = (argc - i) / 2, k;
 		g.prog = argv[0]; g.opts = opts; g.copy = copy; g.optimize = optimize; g.verbose = verbose; g.ppm = ppm; g.cpu = cpu;

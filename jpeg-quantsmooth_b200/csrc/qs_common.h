@@ -1,5 +1,5 @@
 /*
- * qs_common.h - types shared by the host driver (qs_cuda.cu) and the sm_100a kernels
+ * qs_common.h - types shared by the host driver (qs_cuda.cu) and the sm_90a kernels
  * (qs_kernels.cu).  Nothing here is visible through the C ABI (include/jpegqs_cuda.h).
  */
 #ifndef QS_COMMON_H
@@ -109,20 +109,5 @@ typedef struct {
 #define QS_IDCT_DEQUANT 1     /* multiply by qraw, range-check (iteration 0) */
 #define QS_IDCT_CLAMP 2       /* write coefficients back clamped to +-1023 (2670-2689) */
 #define QS_IDCT_NOPLANE 4     /* do not render pixels (dequantize/clamp only) */
-
-#ifdef QS_EXPERIMENTS
-/* Pair schedule (packed FP32x2 path): every coefficient of an anti-diagonal belongs to one
- * pair slot (two coefficients that advance through the same terms in the two lanes of
- * FMUL2/FADD2; a coefficient without partner gets an all-zero dummy lane).  Each slot owns an
- * interleaved weight table float[TS][2]; sections a lane does not have (row-0 coefficients:
- * vertical, column-0 coefficients: horizontal) are simply zero there, which makes those terms
- * exact no-ops.  A chunk is 1 or 2 pair slots sharing the pixel work. */
-typedef struct {
-	uint8_t np, first, slot[2];
-	uint8_t idx[4];                 /* natural coefficient index per lane, 0xFF = dummy lane */
-} QsChunk2;
-#define QS_MAX_SLOTS 40
-
-#endif
 
 #endif

@@ -160,52 +160,6 @@ static int build_chunks(QsChunk *ch, int maxn, const uint16_t *q, int uniform, i
 	return n;
 }
 
-#ifdef QS_EXPERIMENTS
-/* pair schedule + interleaved pair tables of the packed FP32x2 path (qs_common.h QsChunk2):
- * per anti-diagonal the two edge coefficients form one pair, the others pair up in order, a
- * left-over coefficient gets a dummy lane.  out_tab: [nslots][size][2] floats. */
-static int build_pairs(QsChunk2 *ch, int *nslots_out, int maxpairs, uint8_t lanes[][2]) {
-	int n = 0, ns = 0;
-	for (int s = 14; s >= 1; s--) {
-		int list[8], nl = 0;
-		if (s <= 7) { list[nl++] = s; list[nl++] = s * 8; }       /* row-0 and column-0 coefficient */
-		for (int u = 1; u < 8; u++) { int v = s - u; if (v >= 1 && v <= 7) list[nl++] = v * 8 + u; }
-		int npairs = (nl + 1) / 2; bool first = true;
-		for (int p0 = 0; p0 < npairs; p0 += maxpairs) {
-			QsChunk2 c; memset(&c, 0xFF, sizeof(c));
-			c.np = (uint8_t)((npairs - p0) < maxpairs ? (npairs - p0) : maxpairs);
-			c.first = first; first = false;
-			for (int k = 0; k < c.np; k++) {
-				int a = list[2 * (p0 + k)], b = 2 * (p0 + k) + 1 < nl ? list[2 * (p0 + k) + 1] : 0xFF;
-				c.slot[k] = (uint8_t)ns; c.idx[2 * k] = (uint8_t)a; c.idx[2 * k + 1] = (uint8_t)b;
-				lanes[ns][0] = (uint8_t)a; lanes[ns][1] = (uint8_t)b; ns++;
-			}
-			ch[n++] = c;
-		}
-	}
-	*nslots_out = ns;
-	return n;
-}
-
-static void build_pair_tables(int flags, const uint8_t lanes[][2], int nslots, float prescale, float *out) {
-	const int size = (flags & QS_DIAGONALS) ? QS_TAB_DIAG : QS_TAB_PLAIN;
-	std::vector<float> t(64 * size);
-	build_tables(flags, t.data(), prescale);
-	for (int sl = 0; sl < nslots; sl++) for (int h = 0; h < 2; h++) {
-		int i = lanes[sl][h];
-		for (int p = 0; p < size; p++) {
-			float v = i < 64 ? t[i * size + p] : 0.0f;
-			/* the reference skips these sections (quantsmooth.h:1527, 1531); a zero weight makes
-			 * the term an exact no-op (adds +-0 to a2 and +0 to a3) */
-			if (i < 64 && (i & 7) == 0 && p < 64) v = 0.0f;
-			if (i < 64 && i <= 7 && p >= 96 && p < 160) v = 0.0f;
-			out[((size_t)sl * size + p) * 2 + h] = v;
-		}
-	}
-}
-
-#endif
-
 /* ------------------------------------------------------------------------------------------ */
 struct jpegqs_cuda_ctx {
 	int device, num_sms;
@@ -221,7 +175,6 @@ struct jpegqs_cuda_ctx {
 	std::vector<cudaEvent_t> sync_ev;      /* per group: coefficients uploaded / group finished */
 	std::vector<cudaEvent_t> slab_ev;      /* per slab of a pipelined group: uploaded / smoothed */
 	float *tab_plain, *tab_diag;
-	float *tab2_plain, *tab2_diag; int nslots2;   /* pair tables of the FP32x2 path */
 	QsQuantDev *quant_dev; int quant_cap;
 	QsJob *jobs_dev;                       /* two slots of QS_MAX_JOBS */
 	std::vector<QsJob> jobs_cache[2];
@@ -232,7 +185,7 @@ struct jpegqs_cuda_ctx {
 	float last_ms; int launches;
 	/* optional per-kernel timing (bench.py's roofline line): event pairs around launches */
 	int profiling;
-	int tune_sync, tune_maxn, tune_wpg, tune_gs, tune_x2, tune_uni, tune_slabs, tune_wave, tune_merge;              /* kernel variant knobs (jpegqs_cuda_set_tuning) */
+	int tune_sync, tune_maxn, tune_wpg, tune_gs, tune_uni, tune_slabs, tune_wave, tune_merge;              /* kernel variant knobs (jpegqs_cuda_set_tuning) */
 	std::vector<cudaEvent_t> ev_pool; size_t ev_used;
 	std::vector<int> ev_kind;              /* 0 = idct pass, 1 = smoothing pass, per pair */
 	float kernel_ms[2]; int kernel_launches[2];
@@ -273,7 +226,7 @@ extern "C" void jpegqs_cuda_destroy(jpegqs_cuda_ctx *ctx) {
 	if (ctx->stage) cudaFreeHost(ctx->stage);
 	for (cudaEvent_t e : ctx->sync_ev) cudaEventDestroy(e);
 	for (cudaEvent_t e : ctx->slab_ev) cudaEventDestroy(e);
-	cudaFree(ctx->tab_plain); cudaFree(ctx->tab_diag); cudaFree(ctx->tab2_plain); cudaFree(ctx->tab2_diag); cudaFree(ctx->quant_dev);
+	cudaFree(ctx->tab_plain); cudaFree(ctx->tab_diag); cudaFree(ctx->quant_dev);
 	cudaFree(ctx->jobs_dev); cudaFree(ctx->flags_dev); cudaFree(ctx->arena);
 	if (ctx->flags_host) cudaFreeHost(ctx->flags_host);
 	if (ctx->ev0) cudaEventDestroy(ctx->ev0);
@@ -293,16 +246,15 @@ extern "C" int jpegqs_cuda_create(int device, jpegqs_cuda_ctx **out) {
 	CK(cudaSetDevice(device));
 	cudaDeviceProp prop;
 	CK(cudaGetDeviceProperties(&prop, device));
-	if (prop.major < 10) {
-		snprintf(g_err, sizeof(g_err), "device %d (%s, sm_%d%d) is not a Blackwell sm_100 part; "
-				"this library carries sm_100a code only and has no fallback", device, prop.name, prop.major, prop.minor);
+	if (prop.major != 9 || prop.minor != 0) {
+		snprintf(g_err, sizeof(g_err), "device %d (%s, sm_%d%d) is not a Hopper sm_90 part; "
+				"this library carries sm_90a code only and has no fallback", device, prop.name, prop.major, prop.minor);
 		return JPEGQS_ERR_CUDA;
 	}
 	ctx = new jpegqs_cuda_ctx();
 	memset(ctx->err, 0, sizeof(ctx->err));
 	ctx->device = device; ctx->num_sms = prop.multiProcessorCount;
 	snprintf(ctx->devname, sizeof(ctx->devname), "%s", prop.name);
-	ctx->tab2_plain = ctx->tab2_diag = NULL; ctx->nslots2 = 0;
 	ctx->stream = NULL; ctx->up_stream = ctx->down_stream = NULL;
 	ctx->stage = NULL; ctx->stage_cap = 0; ctx->pool = NULL; ctx->up = ctx->down = NULL; ctx->io_ev_used = 0;
 	{
@@ -316,7 +268,7 @@ extern "C" int jpegqs_cuda_create(int device, jpegqs_cuda_ctx **out) {
 	ctx->jobs_dev = NULL; ctx->flags_dev = NULL; ctx->flags_host = NULL;
 	ctx->arena = NULL; ctx->arena_cap = ctx->arena_pos = 0; ctx->ev0 = ctx->ev1 = NULL;
 	ctx->last_ms = 0; ctx->launches = 0;
-	ctx->profiling = 0; ctx->ev_used = 0; ctx->tune_sync = 2; ctx->tune_maxn = 4; ctx->tune_wpg = 4; ctx->tune_gs = 1; ctx->tune_uni = 1; ctx->tune_merge = 1; ctx->tune_slabs = 1; ctx->tune_wave = 0; ctx->tune_x2 = 0;   /* packed FP32x2 measured slower: profiles/README.md */
+	ctx->profiling = 0; ctx->ev_used = 0; ctx->tune_sync = 2; ctx->tune_maxn = 4; ctx->tune_wpg = 4; ctx->tune_gs = 1; ctx->tune_uni = 1; ctx->tune_merge = 1; ctx->tune_slabs = 1; ctx->tune_wave = 0;
 	ctx->kernel_ms[0] = ctx->kernel_ms[1] = 0; ctx->kernel_launches[0] = ctx->kernel_launches[1] = 0;
 	int rc = [&]() -> int {
 		CK(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking));
@@ -336,21 +288,6 @@ extern "C" int jpegqs_cuda_create(int device, jpegqs_cuda_ctx **out) {
 			int n = build_chunks(ch, ctx->tune_maxn, NULL, 0, ctx->tune_merge);
 			CK(qs_set_chunks(ch, n));
 		}
-#ifdef QS_EXPERIMENTS
-		{
-			QsChunk2 ch2[QS_MAX_CHUNKS]; uint8_t lanes[QS_MAX_SLOTS][2]; int ns = 0;
-			int n2 = build_pairs(ch2, &ns, 2, lanes);
-			CK(qs_set_chunks2(ch2, n2, ns));
-			ctx->nslots2 = ns;
-			std::vector<float> t2((size_t)ns * QS_TAB_DIAG * 2);
-			build_pair_tables(0, lanes, ns, pre, t2.data());
-			CK(cudaMalloc(&ctx->tab2_plain, (size_t)ns * QS_TAB_PLAIN * 2 * sizeof(float)));
-			CK(cudaMemcpy(ctx->tab2_plain, t2.data(), (size_t)ns * QS_TAB_PLAIN * 2 * sizeof(float), cudaMemcpyHostToDevice));
-			build_pair_tables(QS_DIAGONALS, lanes, ns, pre, t2.data());
-			CK(cudaMalloc(&ctx->tab2_diag, (size_t)ns * QS_TAB_DIAG * 2 * sizeof(float)));
-			CK(cudaMemcpy(ctx->tab2_diag, t2.data(), (size_t)ns * QS_TAB_DIAG * 2 * sizeof(float), cudaMemcpyHostToDevice));
-		}
-#endif
 		CK(qs_smooth_configure());
 		CK(cudaMalloc(&ctx->jobs_dev, 2 * QS_MAX_JOBS * sizeof(QsJob)));
 		CK(cudaMalloc(&ctx->flags_dev, (QS_MAX_JOBS + 1) * sizeof(int)));
@@ -382,7 +319,7 @@ static void *arena_take(jpegqs_cuda_ctx *ctx, size_t bytes) {
 static size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
 
 /* pinned staging of the host entry points: grow-only, so a caller that smooths image after image
- * pays cudaHostAlloc once (round 1 allocated and freed 100-300 MB of pinned memory per call) */
+ * pays cudaHostAlloc once instead of allocating and freeing 100-300 MB of pinned memory per call */
 static int stage_reserve(jpegqs_cuda_ctx *ctx, size_t bytes) {
 	if (bytes <= ctx->stage_cap) return 0;
 	if (ctx->stage) { CK(cudaFreeHost(ctx->stage)); ctx->stage = NULL; ctx->stage_cap = 0; }
@@ -635,11 +572,11 @@ extern "C" int jpegqs_cuda_set_tuning(jpegqs_cuda_ctx *ctx, int key, int value) 
 #else
 	if (key == 0) return value == 2 ? 0 : JPEGQS_ERR_UNSUPPORTED;                              /* experiments build only */
 #endif
+	if (key == 4) return value == 0 ? 0 : JPEGQS_ERR_UNSUPPORTED;                              /* retired */
 #ifdef QS_EXPERIMENTS
-	if (key == 4) { ctx->tune_x2 = value ? 1 : 0; return 0; }
 	if (key == 2) { ctx->tune_wpg = value == 6 ? 6 : 4; return 0; }
 #else
-	if (key == 4 || key == 2) return value == (key == 4 ? 0 : 4) ? 0 : JPEGQS_ERR_UNSUPPORTED;   /* experiments build only */
+	if (key == 2) return value == 4 ? 0 : JPEGQS_ERR_UNSUPPORTED;                              /* experiments build only */
 #endif
 	if (key == 3) return 0;                            /* retired */
 	if (key == 1) {
@@ -870,7 +807,7 @@ static int run_images(jpegqs_cuda_ctx *ctx, int nimg, jpegqs_cuda_image *imgs, i
 			cudaEvent_t e; CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming)); ctx->slab_ev.push_back(e);
 		}
 		for (int g = 0; g < max_groups; g++) {
-			if (nimg == 1 && !progress && ctx->tune_slabs && !ctx->tune_x2 && !(flags & QS_LOW_QUALITY) &&
+			if (nimg == 1 && !progress && ctx->tune_slabs && !(flags & QS_LOW_QUALITY) &&
 					!S[0].skip && g < S[0].ngroups && niter >= 1) {
 				/* slab plan of this group: all its components alike and certain to iterate */
 				ImgState &s = S[0];
@@ -955,11 +892,6 @@ static int run_images(jpegqs_cuda_ctx *ctx, int nimg, jpegqs_cuda_image *imgs, i
 	auto launch_smooth = [&](const QsJob *jd, int nj, int tiles, int clampv) -> int {
 		if (prof_begin(ctx, 1, st)) return JPEGQS_ERR_CUDA;
 		if (flags & QS_LOW_QUALITY) CK(qs_launch_lowq(jd, nj, tiles, flags, clampv, NULL, st));
-#ifdef QS_EXPERIMENTS
-		else if (ctx->tune_x2) CK(qs_launch_smooth_x2(jd, nj, tiles,
-				(flags & QS_DIAGONALS) ? ctx->tab2_diag : ctx->tab2_plain, ctx->nslots2, tile_counter, flags, clampv,
-				ctx->num_sms, ctx->tune_sync, st));
-#endif
 		else CK(qs_launch_smooth(jd, nj, tiles, tabs, tile_counter, flags, clampv, ctx->num_sms, ctx->tune_sync, ctx->tune_wpg, NULL, st));
 		if (prof_end(ctx, st)) return JPEGQS_ERR_CUDA;
 		ctx->launches++;
@@ -1768,7 +1700,7 @@ extern "C" int jpegqs_cuda_multi_create(int ndev, const int *devices, jpegqs_cud
 	jpegqs_cuda_multi *m = new jpegqs_cuda_multi();
 	m->max_wblk = 0; m->err[0] = 0;
 	const char *e = getenv("JPEGQS_MIN_BLOCKS_PER_GPU");
-	m->min_blocks = e ? atol(e) : 148L * 16 * 32;        /* one wave of the persistent smoothing kernel */
+	m->min_blocks = e ? atol(e) : 132L * 16 * 32;        /* one wave of the persistent smoothing kernel (H100: 132 SMs) */
 	for (int i = 0; i < ndev; i++) {
 		jpegqs_cuda_ctx *c = NULL;
 		int rc = jpegqs_cuda_create(devices ? devices[i] : i, &c);
@@ -1938,10 +1870,6 @@ extern "C" int jpegqs_cuda_pass_smooth(jpegqs_cuda_ctx *ctx, int njobs, const jp
 	if (rc) return rc;
 	const float *tabs = (flags & QS_DIAGONALS) ? ctx->tab_diag : ctx->tab_plain;
 	if (flags & QS_LOW_QUALITY) CK(qs_launch_lowq(jd, njobs, tiles, flags, clamp_out, NULL, st));
-#ifdef QS_EXPERIMENTS
-	else if (ctx->tune_x2) CK(qs_launch_smooth_x2(jd, njobs, tiles, (flags & QS_DIAGONALS) ? ctx->tab2_diag : ctx->tab2_plain,
-			ctx->nslots2, ctx->flags_dev + QS_MAX_JOBS, flags, clamp_out, ctx->num_sms, ctx->tune_sync, st));
-#endif
 	else CK(qs_launch_smooth(jd, njobs, tiles, tabs, ctx->flags_dev + QS_MAX_JOBS, flags, clamp_out, ctx->num_sms, ctx->tune_sync, ctx->tune_wpg, NULL, st));
 	return 0;
 }

@@ -1,6 +1,6 @@
 /*
- * qs_kernels.cu - hand-written sm_100a kernels for the jpeg-quantsmooth coefficient
- * smoothing path.  Compile with -gencode arch=compute_100a,code=sm_100a -fmad=false.
+ * qs_kernels.cu - hand-written sm_90a (Hopper) kernels for the jpeg-quantsmooth coefficient
+ * smoothing path.  Compile with -gencode arch=compute_90a,code=sm_90a -fmad=false.
  *
  * Mapping (DESIGN.md section 3): ONE THREAD PER 8x8 BLOCK.  The reference's per-coefficient
  * sums a2/a3 (reference quantsmooth.h:1517-1545) must be accumulated sequentially in the
@@ -115,7 +115,7 @@ __device__ __forceinline__ void qs_islow_1d(const int *in, int *out) {
 	z3 = z5 - z3; z4 = z5 - z4;
 	t0 += z3 - z1; t1 += z4 - z2; t2 += z3 - z2; t3 += z4 - z1;
 	/* (forming the outputs as three-input sums e0 +- b +- t3 - fewer instructions, IADD3 on the
-	 * ALU pipe - measured slower: the refresh went from 60.8k to 65.1k cycles per warp tile) */
+	 * ALU pipe - was measured slower in the refresh IDCTs) */
 	out[0] = e0 + t3; out[7] = e0 - t3; out[1] = e1 + t2; out[6] = e1 - t2;
 	out[2] = e2 + t1; out[5] = e2 - t1; out[3] = e3 + t0; out[4] = e3 - t0;
 }
@@ -223,11 +223,10 @@ __device__ __forceinline__ float qs_regress(const uint8_t *__restrict__ A, const
 
 #ifndef QS_IDCT_COALESCED
 /* K1 as shipped: thread-private int4 loads at a 128-byte lane stride (the eight loads of a lane
- * walk one 128-byte line, which L1 keeps), register cap raised occupancy.  Measured per 8K
- * launch (average of the de-quantizing and the two plain passes of a step, profiles/README.md
- * round 2): 179 registers / 8 warps per SM (round 1) 83.8 us, 128 registers / 16 warps 67.1 us;
- * the shared-memory-transposed variant below (make variant DEFS=-DQS_IDCT_COALESCED) 151 / 97 /
- * 78 us at 8 / 16 / 24 warps: the transposition costs more than the uncoalesced requests. */
+ * walk one 128-byte line, which L1 keeps), register cap raised to allow 16 warps per SM.  The
+ * shared-memory-transposed variant below (make variant DEFS=-DQS_IDCT_COALESCED) was measured
+ * slower at 8, 16 and 24 warps per SM: the transposition costs more than the uncoalesced
+ * requests.  Neither has been timed on an H100 yet. */
 #ifndef QS_IDCT_MINB
 #define QS_IDCT_MINB 2
 #endif
@@ -551,10 +550,9 @@ __device__ __forceinline__ void qs_prep_slice(uint2 w, float *f, int c) {
  * PRMT->FADD chain sits in front of the FP work. */
 
 /* unroll factors of the row loops of the sections.  Measurement knobs: unrolling by 2 removes 2-4 %
- * of a loop's instructions (address arithmetic, the fp = fn copies) and is SLOWER - 2.507 ms per 8K
- * q3 launch rolled, 2.551 / 2.541 / 2.534 with the h / border / v loop unrolled by 2, 2.556 with
- * all three (profiles/README.md, GPU call M): the loop bodies (260-310 instructions at N = 4) stop
- * fitting the instruction cache the four lock-step warps share. */
+ * of a loop's instructions (address arithmetic, the fp = fn copies) but was measured slower for
+ * each loop and for all three: the loop bodies (260-310 instructions at N = 4) stop fitting the
+ * instruction cache the four lock-step warps share.  Not re-timed on an H100. */
 #ifndef QS_UNROLL_H
 #define QS_UNROLL_H 1
 #endif
@@ -688,15 +686,14 @@ __device__ __forceinline__ void qs_sec_diag(const uint2 *pw, const float *const 
 
 /* Lock-step execution: the 4 warps that share an SM sub-partition (warp id % 4) run the same
  * code region at the same time, separated by a named barrier, so that the sub-partition's
- * L0 instruction cache holds ONE unrolled loop body instead of four (the first ncu capture
- * showed stall_no_instruction = 4.3 per issue with free-running warps, profiles/). */
+ * L0 instruction cache holds ONE unrolled loop body instead of four (free-running warps stalled
+ * on instruction fetch). */
 /* SYNC encodes (level, warps per sub-partition, lock-step groups per sub-partition):
  * SYNC = level + 16 * WPS + 256 * GS; level 0 = free-running, 1 = barrier per section,
  * 2 = barrier per chunk only.  With GS > 1 a sub-partition hosts GS independent groups that
  * drift against each other, so the ALU-heavy refresh of one overlaps the FMA-heavy sums of
  * the other while the L0 instruction cache still only sees GS loop bodies. */
 #define QS_SYNC(level, wps, gs) ((level) + 16 * (wps) + 256 * (gs))
-#define QS_SYNC_X2 4096              /* packed FP32x2 pair path */
 #define QS_SYNC_LEVEL(s) ((s) & 15)
 #define QS_SYNC_WPS(s) (((s) >> 4) & 15)
 #define QS_SYNC_GS(s) (((s) >> 8) & 15)
@@ -850,9 +847,6 @@ __device__ __forceinline__ void qs_chunk_mixed(const QsChunk &ch, const float *t
 	QS_PH_MARK(ph, 9);
 }
 
-#ifdef QS_EXPERIMENTS
-#include "qs_experiments.cuh"
-#endif
 
 /* IDCT of the lane's block from shared coefficients into the shared pixel words */
 __device__ __forceinline__ void qs_refresh(const uint32_t *cw, uint2 *pw) {
@@ -899,8 +893,8 @@ __device__ __forceinline__ void qs_fdct_clamp(float *f, const QsQuantDev *__rest
 }
 
 /* the same for the LOW_QUALITY kernel: the transformed block is parked in shared memory
- * (fs[k * 32]) and the clamp loop is rolled - that kernel's top stall was instruction fetch
- * (profiles/README.md) - and, like qs_coef_update, it leaves the two sums of the rebalance step
+ * (fs[k * 32]) and the clamp loop is rolled - that kernel's top stall was instruction fetch -
+ * and, like qs_coef_update, it leaves the two sums of the rebalance step
  * (m0 = sum coef*a0, m1 = sum a0*a0 over the AC coefficients; the clamp keeps the new value in
  * the quantization interval of a0, so a0 is what the rebalance step would recompute) */
 __device__ __forceinline__ void qs_fdct_clamp_rolled(float *f, float *fs, const QsQuantDev *__restrict__ qd, uint16_t *cs,
@@ -985,13 +979,7 @@ __global__ void __launch_bounds__(QS_SYNC_WPS(SYNC) * 128, 1) qs_smooth_kernel(c
 	__shared__ int s_tile[16], s_next[16];
 	__shared__ int s_sig[32];
 	const int TS = DIAG ? QS_TAB_DIAG : QS_TAB_PLAIN;
-#ifdef QS_EXPERIMENTS
-	const bool X2 = (SYNC & QS_SYNC_X2) != 0;
-	const int tab_words = X2 ? c_nslots2 * 2 * TS : 64 * TS;
-#else
-	const bool X2 = false;
 	const int tab_words = 64 * TS;
-#endif
 	float *tabs = (float *)smem;
 	{
 		/* Stage the weight tables (40-80 KB) with one TMA bulk copy (cp.async.bulk, UBLKCP in
@@ -1157,20 +1145,7 @@ __global__ void __launch_bounds__(QS_SYNC_WPS(SYNC) * 128, 1) qs_smooth_kernel(c
 		}
 		QS_PH_MARK(ph, 1);
 
-#ifdef QS_EXPERIMENTS
-		if (X2) {
-			int nch2 = c_nchunks2;
-#pragma unroll 1
-			for (int ci = 0; ci < nch2; ci++) {
-				QsChunk2 ch = c_chunks2[ci];
-				qs_group_sync<SYNC>(gsync);
-				if (ch.first && !(ci == 0 && skip0)) { qs_refresh(cw, pw); qs_group_sync<SYNC>(gsync); }
-				if (ch.np == 2) qs_chunk_pairs<2, DIAG>(ch, tabs, pw, qd, cs, msum);
-				else qs_chunk_pairs<1, DIAG>(ch, tabs, pw, qd, cs, msum);
-			}
-		}
-#endif
-		int nch = X2 ? 0 : (mixed ? d_nchunks : __ldg(&qd->nchunks));
+		int nch = mixed ? d_nchunks : __ldg(&qd->nchunks);
 		/* 12-byte chunk headers (type, n, first, -, idx[8]); warp-uniform.  Each chunk fetches its
 		 * successor's header before its own divisions, so no chunk starts with a load latency. */
 		const uint32_t *cp = (const uint32_t *)(mixed ? d_chunks : qd->chunks);
@@ -1313,8 +1288,8 @@ __global__ void __launch_bounds__(128, QS_LOWQ_MINB) qs_lowq_kernel(const QsJob 
 		float r0[10], r1[10], r2[10];
 		qs_lowq_row(img - stride, r0); qs_lowq_row(img, r1);
 		/* rows in a rolled loop (one 8-pixel body instead of 64 pixels of straight-line code),
-		 * the filtered pixels parked in shared memory: 0.554 -> 0.493 ms per 8K launch together
-		 * with the rolled clamp loop (profiles/README.md, GPU call M) */
+		 * the filtered pixels parked in shared memory: together with the rolled clamp loop this
+		 * keeps the kernel's instruction footprint small */
 		float *f = sf + warp * 2048 + lane;
 #pragma unroll 1
 		for (int y = 0; y < 8; y++) {
@@ -1570,9 +1545,17 @@ __global__ void __launch_bounds__(512) qs_xchg_pull_kernel(const __grid_constant
 	}
 }
 
+/* grid-stride kernels are sized to the device: a few CTAs per SM */
+static int qs_num_sms(void) {
+	int dev = 0, n = 0;
+	if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
+		n = 132;
+	return n;
+}
+
 cudaError_t qs_launch_stop_fixup(const QsJob *jobs_dev, int njobs, const int *bad, cudaStream_t st) {
 	if (njobs <= 0) return cudaSuccess;
-	qs_stop_fixup_kernel<<<148 * 4, 256, 0, st>>>(jobs_dev, njobs, bad);
+	qs_stop_fixup_kernel<<<qs_num_sms() * 4, 256, 0, st>>>(jobs_dev, njobs, bad);
 	return cudaGetLastError();
 }
 cudaError_t qs_launch_xchg(const QsXchgPush *push, const QsXchgPull *pull, cudaStream_t st) {
@@ -1586,7 +1569,7 @@ cudaError_t qs_launch_xchg(const QsXchgPush *push, const QsXchgPull *pull, cudaS
 /* ------------------------------------------------------------------------------------------
  * Control-data movers.  Job lists and the "coefficient out of range" flags are a few hundred
  * bytes, but as cudaMemcpyAsync they queue on the copy engines BEHIND the bulk coefficient
- * transfers of the host entry points (measured: a 4-byte flag read waited 1.2 ms for a 66 MB
+ * transfers of the host entry points (a 4-byte flag read would wait for a whole bulk
  * download).  Kernel parameters and stores to mapped pinned memory do not touch the copy engines.
  * ------------------------------------------------------------------------------------------ */
 struct QsJobPack { QsJob j[QS_JOB_PACK]; };
@@ -1611,10 +1594,6 @@ cudaError_t qs_set_chunks(const QsChunk *chunks, int n) {
 typedef void (*qs_smooth_fn)(const QsJob *, int, int, const float *, int *, int, int, const int *);
 #define QS_V(d, lvl, wps, gs) qs_smooth_kernel<d, QS_SYNC(lvl, wps, gs)>
 #ifdef QS_EXPERIMENTS
-static qs_smooth_fn qs_smooth_variant_x2(int diag, int sync) {
-	if (diag) return sync == 1 ? qs_smooth_kernel<true, QS_SYNC(1, 4, 1) + QS_SYNC_X2> : qs_smooth_kernel<true, QS_SYNC(2, 4, 1) + QS_SYNC_X2>;
-	return sync == 1 ? qs_smooth_kernel<false, QS_SYNC(1, 4, 1) + QS_SYNC_X2> : qs_smooth_kernel<false, QS_SYNC(2, 4, 1) + QS_SYNC_X2>;
-}
 static qs_smooth_fn qs_smooth_variant(int diag, int sync, int wps) {
 	if (wps == 6) {
 		if (diag) return sync == 2 ? QS_V(true, 2, 6, 1) : QS_V(true, 1, 6, 1);
@@ -1625,8 +1604,7 @@ static qs_smooth_fn qs_smooth_variant(int diag, int sync, int wps) {
 }
 #else
 /* the shipped configuration: lock step with one barrier per chunk, 4 warps per sub-partition
- * (everything else was measured slower, profiles/README.md; the variants live behind
- * -DQS_EXPERIMENTS) */
+ * (the other variants were measured slower; they live behind -DQS_EXPERIMENTS) */
 static qs_smooth_fn qs_smooth_variant(int diag, int, int) {
 	return diag ? QS_V(true, 2, 4, 1) : QS_V(false, 2, 4, 1);
 }
@@ -1645,11 +1623,6 @@ cudaError_t qs_smooth_configure(void) {
 					cudaFuncAttributeMaxDynamicSharedMemorySize, (int)qs_smooth_smem_bytes(d, wps));
 			if (e != cudaSuccess) return e;
 		}
-	for (int d = 0; d < 2; d++) for (int sy = 1; sy <= 2; sy++) {
-		cudaError_t e = cudaFuncSetAttribute(qs_smooth_variant_x2(d, sy),
-				cudaFuncAttributeMaxDynamicSharedMemorySize, (int)qs_smooth_smem_bytes_x2(d, QS_MAX_SLOTS));
-		if (e != cudaSuccess) return e;
-	}
 #else
 	for (int d = 0; d < 2; d++) {
 		cudaError_t e = cudaFuncSetAttribute(qs_smooth_variant(d, 2, 4),
@@ -1660,33 +1633,6 @@ cudaError_t qs_smooth_configure(void) {
 	return cudaSuccess;
 }
 
-#ifdef QS_EXPERIMENTS
-size_t qs_smooth_smem_bytes_x2(int diag, int nslots) {
-	return (size_t)nslots * 2 * (diag ? QS_TAB_DIAG : QS_TAB_PLAIN) * 4 + (size_t)16 * QS_WARP_WORDS * 4;
-}
-cudaError_t qs_set_chunks2(const QsChunk2 *chunks, int n, int nslots) {
-	cudaError_t e = cudaMemcpyToSymbol(c_chunks2, chunks, sizeof(QsChunk2) * n);
-	if (e != cudaSuccess) return e;
-	e = cudaMemcpyToSymbol(c_nchunks2, &n, sizeof(int));
-	if (e != cudaSuccess) return e;
-	e = cudaMemcpyToSymbol(c_nslots2, &nslots, sizeof(int));
-	if (e != cudaSuccess) return e;
-	const unsigned long long one = 0x3f8000003f800000ull;
-	return cudaMemcpyToSymbol(c_one2, &one, sizeof(one));
-}
-cudaError_t qs_launch_smooth_x2(const QsJob *jobs_dev, int njobs, int total_tiles, const float *tables_dev,
-		int nslots, int *tile_counter, int flags, int clamp_out, int num_sms, int sync, cudaStream_t st) {
-	if (total_tiles <= 0) return cudaSuccess;
-	cudaError_t e = cudaMemsetAsync(tile_counter, 0, sizeof(int), st);
-	if (e != cudaSuccess) return e;
-	int diag = (flags & QS_DIAGONALS) ? 1 : 0;
-	int grid = (total_tiles + 15) / 16;
-	if (grid > num_sms) grid = num_sms;
-	qs_smooth_variant_x2(diag, sync == 1 ? 1 : 2)<<<grid, 512, qs_smooth_smem_bytes_x2(diag, nslots), st>>>(
-			jobs_dev, njobs, total_tiles, tables_dev, tile_counter, flags, clamp_out, NULL);
-	return cudaGetLastError();
-}
-#endif
 
 cudaError_t qs_launch_idct_pass(const QsJob *jobs_dev, int njobs, int total_tiles, int mode,
 		int *bad_flags, cudaStream_t st) {
@@ -1727,7 +1673,8 @@ cudaError_t qs_launch_scale_clamp(int16_t *coef, size_t n, const QsQuantDev *qd,
 		cudaStream_t st) {
 	if (!n) return cudaSuccess;
 	size_t blocks = (n + 255) / 256;
-	if (blocks > 148 * 16) blocks = 148 * 16;
+	size_t cap = (size_t)qs_num_sms() * 16;
+	if (blocks > cap) blocks = cap;
 	qs_scale_clamp_kernel<<<(unsigned)blocks, 256, 0, st>>>(coef, n, qd, dequant, clamp);
 	return cudaGetLastError();
 }

@@ -7,12 +7,6 @@
 size_t qs_smooth_smem_bytes(int diag, int wpg);
 cudaError_t qs_smooth_configure(void);
 cudaError_t qs_set_chunks(const QsChunk *chunks, int n);
-#ifdef QS_EXPERIMENTS
-cudaError_t qs_set_chunks2(const QsChunk2 *chunks, int n, int nslots);
-size_t qs_smooth_smem_bytes_x2(int diag, int nslots);
-cudaError_t qs_launch_smooth_x2(const QsJob *jobs_dev, int njobs, int total_tiles, const float *tables_dev,
-		int nslots, int *tile_counter, int flags, int clamp_out, int num_sms, int sync, cudaStream_t st);
-#endif
 cudaError_t qs_launch_idct_pass(const QsJob *jobs_dev, int njobs, int total_tiles, int mode,
 		int *bad_flags, cudaStream_t st);
 cudaError_t qs_launch_smooth(const QsJob *jobs_dev, int njobs, int total_tiles, const float *tables_dev,

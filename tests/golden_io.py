@@ -1,4 +1,7 @@
 """Load/save golden cases and build the adversarial inputs used by the edge-case tests."""
+import json
+import os
+
 import numpy as np
 
 from jpegqs_b200.image import CoefImage, Component, JCS_GRAYSCALE, JCS_YCbCr
@@ -68,3 +71,44 @@ def adversarial_image(kind):
         im.comps[0].quant[10] = 0              # damaged table: 0 -> 1 for the maths, 0 for dequant
         im.comps[0].quant[63] = 0
     return im
+
+
+# ---- stored answers of the reference (tests/golden/reference/make_reference_vectors.py) ------
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference")
+_stored = {}
+
+
+def put_result(d, key, ret, im):
+    """Stores one do_quantsmooth result (return value + every component) under `key`."""
+    d[f"{key}.ret"] = np.array(ret, dtype=np.int32)
+    for i, c in enumerate(im.comps):
+        d[f"{key}.coef{i}"] = c.coef
+        d[f"{key}.samp{i}"] = np.array([c.h_samp, c.v_samp, c.quant_tbl_no], dtype=np.int32)
+        if c.quant is not None:
+            d[f"{key}.quant{i}"] = c.quant
+
+
+def reference(name):
+    """tests/golden/reference/<name>.npz, loaded once."""
+    if name not in _stored:
+        _stored[name] = dict(np.load(os.path.join(GOLDEN, name + ".npz")))
+    return _stored[name]
+
+
+def reference_result(key, like):
+    """(ret, image) the reference returned for `key`; `like` (the input) gives the geometry."""
+    z = next(z for z in map(reference, ("ref_driver", "ref_sweep")) if f"{key}.ret" in z)
+    comps = []
+    for i, c in enumerate(like.comps):
+        s = z[f"{key}.samp{i}"]
+        q = z.get(f"{key}.quant{i}")
+        comps.append(Component(z[f"{key}.coef{i}"].copy(), None if q is None else q.copy(), int(s[0]), int(s[1]), int(s[2])))
+    return int(z[f"{key}.ret"]), CoefImage(like.width, like.height, like.colorspace, comps)
+
+
+def reference_files():
+    """tests/golden/reference/ref_files.json: SHA-256 of files the reference tools wrote."""
+    if "files" not in _stored:
+        with open(os.path.join(GOLDEN, "ref_files.json")) as f:
+            _stored["files"] = json.load(f)
+    return _stored["files"]

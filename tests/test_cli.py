@@ -2,8 +2,10 @@
 (csrc/jpegcoef.c).  CPU leg: the codec is a lossless transcoder (`-n 0` never reaches the
 CUDA back end) on baseline / progressive / sub-sampled / restart-marker / grayscale files
 written by Pillow's libjpeg-turbo, and markers are copied per `-c`.  GPU leg: the CUDA-backed
-tool must write byte-identical files to oracle/_ref/jpegqs_ref (the same front end linked
-against the UNMODIFIED reference do_quantsmooth, built by oracle/Makefile)."""
+tool must write byte-identical files to jpegqs_ref (the same front end linked against the
+UNMODIFIED reference do_quantsmooth, oracle/Makefile); the SHA-256 of what jpegqs_ref wrote is
+stored in tests/golden/reference/ref_files.json."""
+import hashlib
 import os
 import subprocess
 
@@ -14,7 +16,6 @@ PIL = pytest.importorskip("PIL.Image")
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EXE = os.path.join(ROOT, "jpeg-quantsmooth_b200", "csrc", "jpegqs")
-REF_EXE = os.path.join(ROOT, "oracle", "_ref", "jpegqs_ref")
 
 
 def _picture(w, h, gray, seed):
@@ -45,15 +46,26 @@ FILES = [
 ]
 
 
-@pytest.fixture(scope="module")
-def jpegs(tmp_path_factory):
-    d = tmp_path_factory.mktemp("jpegs")
+def write_jpegs(d):
     out = {}
     for k, (name, w, h, gray, kw) in enumerate(FILES):
-        p = str(d / (name + ".jpg"))
+        p = os.path.join(d, name + ".jpg")
         _picture(w, h, gray, k).save(p, comment=b"made by the test suite", **kw)
         out[name] = p
     return out
+
+
+def file_key(name, args):
+    return " ".join([name] + args)
+
+
+def sha256(path):
+    return hashlib.sha256(open(path, "rb").read()).hexdigest()
+
+
+@pytest.fixture(scope="module")
+def jpegs(tmp_path_factory):
+    return write_jpegs(str(tmp_path_factory.mktemp("jpegs")))
 
 
 def _pixels(path):
@@ -277,24 +289,25 @@ def test_no_cpu_fallback_in_the_tool(jpegs, tmp_path):
     assert not out.exists()
 
 
-@pytest.mark.gpu
-@pytest.mark.skipif(not os.path.exists(REF_EXE), reason="oracle/_ref/jpegqs_ref not built")
-@pytest.mark.parametrize("name,args", [
+REF_TOOL_CASES = [
     ("base420", ["-q", "3"]), ("base420", ["-q", "6", "-n", "2"]), ("prog420", ["-q", "4", "-n", "2", "-o"]),
     ("base444", ["-q", "5", "-n", "2"]), ("gray", ["-q", "3", "-n", "4"]), ("opt422", ["-q", "6"]),
     ("prog444", ["-q", "1", "-n", "2"]), ("rst", ["-q", "0"]), ("progrst", ["-q", "1", "-o"]),
     ("opt422", ["-q", "2", "-o"]),
     ("tinyprog", ["-q", "3"]), ("base420", ["-f", "16", "-n", "2"]),
-])
+]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name,args", REF_TOOL_CASES)
 def test_cuda_tool_writes_the_reference_tools_bytes(jpegs, tmp_path, name, args):
     # UPSAMPLE_UV cases use widths that are multiples of the MCU: for other widths the reference
     # reads uninitialised memory when it pads the up-sampled plane (DESIGN.md "reference quirks")
-    a, b = str(tmp_path / "cuda.jpg"), str(tmp_path / "ref.jpg")
+    from golden_io import reference_files
+    a = str(tmp_path / "cuda.jpg")
     r1 = subprocess.run([EXE, "-i", "0"] + args + [jpegs[name], a], capture_output=True, text=True)
-    r2 = subprocess.run([REF_EXE, "-i", "0"] + args + [jpegs[name], b], capture_output=True, text=True)
     assert r1.returncode == 0, r1.stderr
-    assert r2.returncode == 0, r2.stderr
-    assert open(a, "rb").read() == open(b, "rb").read()
+    assert sha256(a) == reference_files()["jpegqs_ref"][file_key(name, args)]
     PIL.open(a).load()                      # and it is a decodable JPEG
 
 

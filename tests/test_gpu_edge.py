@@ -8,7 +8,7 @@ import pytest
 
 import jpegqs_b200 as qs
 import oracle_lib as ol
-from golden_io import adversarial_image
+from golden_io import adversarial_image, reference_result
 from jpegqs_b200 import multigpu as mg
 
 pytestmark = pytest.mark.gpu
@@ -85,7 +85,10 @@ def test_progress_sequence_and_cancel(ctx):
     assert ol.images_equal(o1, o2)
 
 
-@pytest.mark.parametrize("flags,niter,ss", [(0, 3, "420"), (7, 2, "420"), (3, 2, "444"), (1, 1, "gray")])
+ENTRY_CASES = [(0, 3, "420"), (7, 2, "420"), (3, 2, "444"), (1, 1, "gray")]
+
+
+@pytest.mark.parametrize("flags,niter,ss", ENTRY_CASES)
 def test_libjpeg_facing_entry_point(flags, niter, ss):
     """do_quantsmooth(j_decompress_ptr, jvirt_barray_ptr*, jpegqs_control_t*) through the
     fake libjpeg front end, rows scattered in memory like libjpeg's virtual arrays."""
@@ -94,9 +97,8 @@ def test_libjpeg_facing_entry_point(flags, niter, ss):
     ret, out = ol.run_libjpeg_boundary(lib.do_quantsmooth, im, flags | 64, niter, scatter_rows=True)
     oret, oout = ol.run_oracle(im, flags, niter)
     assert ret == oret and ol.images_equal(out, oout)
-    if ol.have_ref("scalar"):
-        rret, rout = ol.run_reference(im, flags, niter, scatter_rows=True)
-        assert ret == rret and ol.images_equal(out, rout)
+    rret, rout = reference_result("entry_" + "_".join(str(v) for v in (flags, niter, ss)), im)
+    assert ret == rret and ol.images_equal(out, rout)
 
 
 def test_batch_entry_point(ctx):

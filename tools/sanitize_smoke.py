@@ -13,6 +13,5 @@ for (w, h, ss, flags, niter) in [(96, 64, "420", 0, 2), (90, 50, "420", 7, 1), (
     ret, out = ctx.do_quantsmooth(im, flags, niter)
     rgb = ctx.render_rgb(out)
     print(w, h, ss, flags, niter, "ret", ret, rgb.shape, flush=True)
-# (the packed FP32x2 path lives in the experiments build)
 ret, out = ctx.do_quantsmooth(qs.synth.make_image(96, 64, "420"), 1, 1)
 

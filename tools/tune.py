@@ -1,5 +1,5 @@
-"""Kernel-variant sweep on the 8K q3 workload (device-resident).  Usage on the GPU box:
-    python tools/tune.py [--flags 0] [--variants sync:maxn,...]
+"""Kernel-variant sweep on the 8K q3 workload (device-resident).  Usage on a GPU machine:
+    python tools/tune.py [--flags 0] [--variants sync:maxn[:wpg[:gs[:uni[:merge]]]],...]
 Prints per-variant average smoothing-pass launch time and checks that every variant
 produces byte-identical output."""
 import argparse
@@ -40,11 +40,8 @@ ref_hash = None
 for v in args.variants.split(","):
     f = [int(x) for x in v.split(":")]
     sync, maxn, wpg, gs = f[0], f[1], (f[2] if len(f) > 2 else 4), (f[3] if len(f) > 3 else 1)
-    x2 = f[4] if len(f) > 4 else 0
-    uni = f[5] if len(f) > 5 else 1
-    merge = f[6] if len(f) > 6 else None
-    if x2:
-        ctx.set_tuning(4, x2)
+    uni = f[4] if len(f) > 4 else 1
+    merge = f[5] if len(f) > 5 else None
     ctx.set_tuning(5, uni)
     if merge is not None:
         ctx.set_tuning(8, merge)
@@ -68,5 +65,5 @@ for v in args.variants.split(","):
     h = hashlib.sha1(b"".join(t.cpu().numpy().tobytes() for t in bufs)).hexdigest()
     if ref_hash is None:
         ref_hash = h
-    print(f"sync={sync} maxn={maxn} wpg={wpg} gs={gs} x2={x2} uni={uni} merge={merge}: smooth {sm / n:.3f} ms/launch, idct pass {1e3 * idm / max(idn, 1):.1f} us/launch, whole run {tot / args.steps:.3f} ms, "
+    print(f"sync={sync} maxn={maxn} wpg={wpg} gs={gs} uni={uni} merge={merge}: smooth {sm / n:.3f} ms/launch, idct pass {1e3 * idm / max(idn, 1):.1f} us/launch, whole run {tot / args.steps:.3f} ms, "
           f"{args.width * args.height / 1e6 / (tot / args.steps / 1e3):.0f} Mpix/s, same_output={h == ref_hash}, sha1={h[:12]}", flush=True)

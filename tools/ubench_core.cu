@@ -1,7 +1,7 @@
-// Micro-benchmark: what issue rate can the smoothing kernel's arithmetic reach on sm_100a?
+// Micro-benchmark: what issue rate can the smoothing kernel's arithmetic reach on sm_90a?
 // One CTA of 512 threads per SM (4 warps per sub-partition, like qs_smooth_kernel), bodies that
 // look like its inner loops.  Prints warp-instructions per clock per sub-partition.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -fmad=false -o ubench_core ubench_core.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -fmad=false -o ubench_core ubench_core.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 
@@ -57,14 +57,18 @@ template <int MODE> __global__ void __launch_bounds__(512, 1) k(float *out, int 
 }
 
 template <int MODE> static void run(const char *name, double inst_per_iter) {
-	float *out; long long *cyc, h[148];
-	cudaMalloc(&out, 148 * 512 * 4); cudaMalloc(&cyc, 148 * 8);
+	int dev = 0, nsm = 0;
+	cudaGetDevice(&dev);
+	cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);     /* one CTA per SM */
+	float *out; long long *cyc, *h = new long long[nsm];
+	cudaMalloc(&out, (size_t)nsm * 512 * 4); cudaMalloc(&cyc, (size_t)nsm * 8);
 	int iters = 20000;
-	k<MODE><<<148, 512>>>(out, 100, 1.0f, cyc);
-	k<MODE><<<148, 512>>>(out, iters, 1.0f, cyc);
-	cudaMemcpy(h, cyc, sizeof(h), cudaMemcpyDeviceToHost);
-	double c = 0; for (int i = 0; i < 148; i++) c += h[i];
-	c /= 148;
+	k<MODE><<<nsm, 512>>>(out, 100, 1.0f, cyc);
+	k<MODE><<<nsm, 512>>>(out, iters, 1.0f, cyc);
+	cudaMemcpy(h, cyc, (size_t)nsm * 8, cudaMemcpyDeviceToHost);
+	double c = 0; for (int i = 0; i < nsm; i++) c += h[i];
+	c /= nsm;
+	delete[] h;
 	// 16 warps per SM, 4 per sub-partition: warp-instructions per sub-partition = 4 * per-warp count
 	printf("%-44s %7.0f cycles  %.3f warp-instr/clk/sub-partition (counted FP%s instructions only)\n", name, c,
 			4.0 * inst_per_iter * iters / c, MODE >= 5 ? "+PRMT" : "");
