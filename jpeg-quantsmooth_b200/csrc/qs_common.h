@@ -75,7 +75,8 @@ typedef struct {
 	 * the same image, and the kernels decide by themselves what the reference's `stop` logic
 	 * (quantsmooth.h:2504, 2551-2566, 2602-2610) leaves to do: 0 = smooth, 1 = this component
 	 * overflowed (clamp only), 2 = an earlier one did (de-quantize only).  stop_aware = 0: the
-	 * host has already sorted that out (run_images). */
+	 * host has already sorted that out (run_images, and every job built by qs_cuda.cu make_job
+	 * unless run_job is given the run's flags). */
 	int32_t bad_first, stop_aware;
 } QsJob;
 

@@ -6,7 +6,9 @@
  * quantsmooth.h:2404-2878) as a schedule of kernel launches; the arithmetic itself lives in
  * qs_kernels.cu.  Independent components (and, in the batch entry point, independent
  * images) share launches; the luma -> chroma dependency of JOINT_YUV / UPSAMPLE_UV
- * (quantsmooth.h:2495, 2691-2815) splits a run into two phases.
+ * (quantsmooth.h:2495, 2691-2815) splits a run into two phases.  Two drivers schedule the same
+ * run steps (set-up, jobs, passes, post steps, results): run_images for whole images on one
+ * device, run_slab for one rank's slab of an image sharded over several.
  */
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -14,6 +16,7 @@
 #include <stdlib.h>
 #include <string.h>
 #include <algorithm>
+#include <functional>
 #include <memory>
 #include <unordered_map>
 #include <vector>
@@ -625,16 +628,16 @@ extern "C" void jpegqs_cuda_kernel_stats(const jpegqs_cuda_ctx *ctx, float *idct
 }
 
 /* ------------------------------------------------------------------------------------------
- * whole-image driver
+ * run steps shared by the whole-image driver (run_images) and the slab driver (run_slab)
  * ------------------------------------------------------------------------------------------ */
 struct CompWork {
 	int img, ci;
 	jpegqs_cuda_comp *c;
 	int16_t *coef_dev; uint8_t *plane;
 	int W, H, luma, qslot;
+	int qval;              /* OR of the raw quant values (quantsmooth.h:2498) */
 	int niter2, extra;
 	bool iterate;          /* takes part in the IDCT / smoothing iterations */
-	bool dequant_only;     /* stop was already set: quantsmooth.h:2551-2566 */
 	bool done_clamp;
 	bool downloaded;       /* the slab pipeline already sent the coefficients back */
 	/* host side (host entry points only): pinned memory the copy engines use, and the block-row
@@ -652,43 +655,47 @@ struct ImgState {
 	uint8_t *image2_buf, *mem_buf[2];
 	int16_t *coef_up_dev[2];
 	int ngroups;
+	/* where the block rows held sit in the image: all of it (rank 0 of 1, row0 0, hblk_total =
+	 * hblk), or one rank's slab (run_slab); top / bottom: they include the image's first / last row */
+	jpegqs_cuda_slab geom;
+	bool top, bottom;
 };
 
-/* Host entry points, one large image: a group's block rows are cut into slabs of about one
- * wave of the persistent smoothing kernel.  Iteration 0 then follows the upload slab by slab
- * (IDCT pass of slab k, smoothing of slab k-1 - which needs the first pixel row of slab k), and
- * the last iteration hands its slabs to the download as they finish, so that only the first
- * slab's upload and the last slab's download are not hidden behind kernels.  Results do not
- * depend on this: a pass reads only start-of-pass neighbour pixels (quantsmooth.h:1396-1401). */
-#define QS_MAX_SLABS 16
-struct SlabPlan { int K; int r[QS_MAX_SLABS + 1]; };
+/* the per-call state of a smoothing run */
+struct RunSetup {
+	int niter;                                          /* clamped, quantsmooth.h:2455-2456 */
+	std::vector<ImgState> S;
+	std::vector<std::vector<CompWork> > W;              /* [image][component] */
+	std::vector<std::unique_ptr<int16_t *[]> > rowstore;   /* block-row tables made up for flat pageable arrays */
+};
 
-static int run_images(jpegqs_cuda_ctx *ctx, int nimg, jpegqs_cuda_image *imgs, int flags, int niter,
-		int progprec, jpegqs_cuda_progress_fn progress, void *userdata, bool on_device, int *ret,
-		cudaStream_t st) {
-	if (!ctx || nimg < 0 || (nimg && !imgs)) return JPEGQS_ERR_ARG;
-	if (progress && nimg != 1) return JPEGQS_ERR_ARG;
+/* Everything a run needs before its first launch: the per-image decisions of quantsmooth.h:2447-2458,
+ * device memory (coefficients of host entry points, sample planes, down-sampled luma, up-sampled
+ * chroma), pinned staging and block-row tables of the host side, and the quant constants, uploaded
+ * on st.  Phases default to luma | chroma when the chroma needs the finished luma, or so that the
+ * chroma upload and the luma download of host buffers overlap with compute. */
+static int run_setup(jpegqs_cuda_ctx *ctx, int nimg, jpegqs_cuda_image *imgs, int flags, int niter, bool on_device,
+		cudaStream_t st, RunSetup &r) {
 	CK(cudaSetDevice(ctx->device));
 	ctx->launches = 0; ctx->last_ms = 0;
 	ctx->ev_kind.clear(); ctx->ev_used = 0;
 	if (niter < 0) niter = 0;
 	if (niter > 100) niter = 100;                       /* quantsmooth.h:2455-2456 */
+	r.niter = niter;
+	r.S.resize(nimg); r.W.resize(nimg);
 
-	std::vector<ImgState> S(nimg);
-	std::vector<CompWork> all;
-	size_t bytes = 0, stage_bytes = 0; int nquant = 0, max_groups = 0;
+	size_t bytes = 0, stage_bytes = 0; int nquant = 0;
 	if (ctx->up) ctx->up->drain();                      /* nothing of an earlier (failed) call may linger */
 	if (ctx->down) ctx->down->drain();
 	ctx->io_ev_used = 0;
 	for (int n = 0; n < nimg; n++) {
-		jpegqs_cuda_image *im = &imgs[n]; ImgState &s = S[n];
+		jpegqs_cuda_image *im = &imgs[n]; ImgState &s = r.S[n];
 		memset(&s, 0, sizeof(s)); s.im = im; im->upsampled = 0; s.stop_ci = 1 << 30;
 		if (im->ncomp < 1 || im->ncomp > JPEGQS_CUDA_MAX_COMP) return JPEGQS_ERR_ARG;
 		s.need_downsample = (flags & (QS_JOINT_YUV | QS_UPSAMPLE_UV)) && im->is_ycbcr && im->ncomp >= 3 &&
 				im->comp[1].h_samp == 1 && im->comp[1].v_samp == 1 &&
 				im->comp[2].h_samp == 1 && im->comp[2].v_samp == 1;          /* 2447-2453 */
 		s.skip = niter <= 0 && !((flags & QS_UPSAMPLE_UV) && s.need_downsample);   /* 2458 */
-		if (ret) ret[n] = 0;
 		if (s.skip) continue;
 		if (s.need_downsample && (im->comp[1].wblk != im->comp[2].wblk || im->comp[1].hblk != im->comp[2].hblk))
 			return JPEGQS_ERR_ARG;
@@ -718,35 +725,30 @@ static int run_images(jpegqs_cuda_ctx *ctx, int nimg, jpegqs_cuda_image *imgs, i
 				}
 			}
 		}
-		/* host buffers: luma and chroma are separate phases even when independent, so that the
-		 * chroma upload and the luma download overlap with compute (copy stream + events) */
-		s.ngroups = progress ? im->ncomp : ((s.need_downsample || (!on_device && im->ncomp > 1)) ? 2 : 1);
-		if (s.ngroups > max_groups) max_groups = s.ngroups;
+		s.ngroups = (s.need_downsample || (!on_device && im->ncomp > 1)) ? 2 : 1;
+		s.geom.rank = 0; s.geom.world = 1; s.top = s.bottom = true;
+		for (int ci = 0; ci < im->ncomp; ci++) s.geom.hblk_total[ci] = im->comp[ci].hblk;
 	}
 	if (arena_reserve(ctx, bytes + 4096)) return JPEGQS_ERR_CUDA;
 	if (quant_reserve(ctx, nquant)) return JPEGQS_ERR_CUDA;
 	if (stage_bytes && stage_reserve(ctx, stage_bytes)) return JPEGQS_ERR_CUDA;
 	size_t stage_pos = 0;
 	auto stage_take = [&](size_t b) { char *p = ctx->stage + stage_pos; stage_pos += align256(b); return (int16_t *)p; };
-	/* block-row tables made up for flat pageable arrays (one pointer per block row) */
-	std::vector<std::unique_ptr<int16_t *[]> > rowstore;
 	auto flat_rows = [&](int16_t *base, uint32_t wblk, uint32_t hblk) -> int16_t *const * {
-		rowstore.emplace_back(new int16_t *[hblk ? hblk : 1]);
-		int16_t **t = rowstore.back().get();
+		r.rowstore.emplace_back(new int16_t *[hblk ? hblk : 1]);
+		int16_t **t = r.rowstore.back().get();
 		for (uint32_t y = 0; y < hblk; y++) t[y] = base + (size_t)y * wblk * 64;
 		return t;
 	};
 
-	/* carve device memory, upload coefficients and quant constants */
+	/* carve device memory and pinned staging, upload quant constants */
 	std::vector<QsQuantDev> qhost; qhost.reserve(nquant);
-	std::vector<std::vector<CompWork> > W(nimg);
-	std::vector<std::vector<int> > qval(nimg);
 	for (int n = 0; n < nimg; n++) {
-		ImgState &s = S[n]; jpegqs_cuda_image *im = s.im;
+		ImgState &s = r.S[n]; jpegqs_cuda_image *im = s.im;
 		if (s.skip) continue;
-		W[n].resize(im->ncomp); qval[n].resize(im->ncomp);
+		r.W[n].resize(im->ncomp);
 		for (int ci = 0; ci < im->ncomp; ci++) {
-			jpegqs_cuda_comp *c = &im->comp[ci]; CompWork &w = W[n][ci];
+			jpegqs_cuda_comp *c = &im->comp[ci]; CompWork &w = r.W[n][ci];
 			memset(&w, 0, sizeof(w));
 			w.img = n; w.ci = ci; w.c = c; w.W = c->wblk; w.H = c->hblk;
 			w.luma = !ci || !im->is_ycbcr;                                /* 2639 */
@@ -760,7 +762,7 @@ static int run_images(jpegqs_cuda_ctx *ctx, int nimg, jpegqs_cuda_image *imgs, i
 			}
 			w.plane = (uint8_t *)arena_take(ctx, QS_PLANE_BYTES(c->wblk, c->hblk));
 			w.qslot = (int)qhost.size();
-			QsQuantDev q; quant_prepare(c->quant, &q, &qval[n][ci], ctx->tune_maxn, ctx->tune_uni, ctx->tune_merge); qhost.push_back(q);
+			QsQuantDev q; quant_prepare(c->quant, &q, &w.qval, ctx->tune_maxn, ctx->tune_uni, ctx->tune_merge); qhost.push_back(q);
 		}
 		bool sub = s.need_downsample && !(im->comp[0].h_samp == 1 && im->comp[0].v_samp == 1);
 		if (sub) {
@@ -770,7 +772,7 @@ static int run_images(jpegqs_cuda_ctx *ctx, int nimg, jpegqs_cuda_image *imgs, i
 				s.mem_buf[j] = (uint8_t *)arena_take(ctx, yb * 64);
 				s.coef_up_dev[j] = on_device ? im->comp[1 + j].coef_up : (int16_t *)arena_take(ctx, yb * 128);
 				if (!on_device) {
-					jpegqs_cuda_comp *c = &im->comp[1 + j]; CompWork &w = W[n][1 + j];
+					jpegqs_cuda_comp *c = &im->comp[1 + j]; CompWork &w = r.W[n][1 + j];
 					if (c->rows_up) { w.rows_up = c->rows_up; w.pin_up = stage_take(yb * 128); }
 					else if (is_pinned(c->coef_up)) { w.rows_up = NULL; w.pin_up = c->coef_up; }
 					else { w.rows_up = flat_rows(c->coef_up, im->comp[0].wblk, im->comp[0].hblk); w.pin_up = stage_take(yb * 128); }
@@ -782,12 +784,243 @@ static int run_images(jpegqs_cuda_ctx *ctx, int nimg, jpegqs_cuda_image *imgs, i
 	if (!qhost.empty())
 		CK(cudaMemcpyAsync(ctx->quant_dev, qhost.data(), qhost.size() * sizeof(QsQuantDev), cudaMemcpyHostToDevice, st));
 	ctx->jobs_cache[0].clear(); ctx->jobs_cache[1].clear();
+	return 0;
+}
 
-	auto group_range = [&](const ImgState &s, int g, int *c0, int *c1) {
-		if (progress) { *c0 = g; *c1 = g + 1; }
-		else if (s.ngroups == 2) { *c0 = g ? 1 : 0; *c1 = g ? s.im->ncomp : 1; }
-		else { *c0 = 0; *c1 = s.im->ncomp; }
-	};
+/* components [c0, c1) of phase g: the whole image, luma | chroma, or one component per phase */
+static void group_range(const ImgState &s, int g, int *c0, int *c1) {
+	if (s.ngroups == 1) { *c0 = 0; *c1 = s.im->ncomp; }
+	else if (s.ngroups == s.im->ncomp) { *c0 = g; *c1 = g + 1; }
+	else { *c0 = g ? 1 : 0; *c1 = g ? s.im->ncomp : 1; }
+}
+
+/* Host entry points, one large image: a group's block rows are cut into slabs of about one
+ * wave of the persistent smoothing kernel (run_images), or travel in bands of ~8 MB (run_slab). */
+#define QS_MAX_SLABS 16
+
+/* transfer events of the host entry points, per phase: uploaded / finished, and per slab or band */
+static int group_events(jpegqs_cuda_ctx *ctx, int ngroups) {
+	while ((int)ctx->sync_ev.size() < 2 * ngroups) {
+		cudaEvent_t e; CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming)); ctx->sync_ev.push_back(e);
+	}
+	while ((int)ctx->slab_ev.size() < 2 * ngroups * QS_MAX_SLABS) {
+		cudaEvent_t e; CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming)); ctx->slab_ev.push_back(e);
+	}
+	return 0;
+}
+
+/* block rows [r0, r1) of a component's coefficients / of its up-sampled chroma (luma sized) */
+static IoSeg seg_of(const CompWork &w, int r0, int r1) {
+	IoSeg sg; sg.dev = w.coef_dev; sg.pin = w.pin; sg.rows = w.rows; sg.wblk = w.W; sg.r0 = r0; sg.r1 = r1;
+	return sg;
+}
+static IoSeg seg_up_of(const ImgState &s, const CompWork &w, int r0, int r1) {
+	IoSeg sg; sg.dev = s.coef_up_dev[w.ci - 1]; sg.pin = w.pin_up; sg.rows = w.rows_up;
+	sg.wblk = s.im->comp[0].wblk; sg.r0 = r0; sg.r1 = r1;
+	return sg;
+}
+
+/* the job of block rows [r0, r1) of a component; plane2: the JOINT_YUV predictor or NULL */
+static QsJob make_job(jpegqs_cuda_ctx *ctx, const CompWork &w, const uint8_t *plane2, int r0, int r1,
+		int top_edge, int bottom_edge) {
+	QsJob j; memset(&j, 0, sizeof(j));
+	j.stride = QS_PLANE_STRIDE(w.W);
+	size_t poff = (size_t)r0 * 8 * j.stride;
+	j.coef = w.coef_dev + (size_t)r0 * w.W * 64; j.plane = w.plane + poff; j.plane2 = plane2 ? plane2 + poff : NULL;
+	j.quant = ctx->quant_dev + w.qslot;
+	j.wblk = w.W; j.hblk = r1 - r0; j.nblocks = w.W * (r1 - r0);
+	j.luma = w.luma; j.top_edge = top_edge; j.bottom_edge = bottom_edge;
+	return j;
+}
+
+/* The job of all rows a run holds of a component.  stop_flags == NULL: the host decides the
+ * reference's `stop` (run_images), and a launch's out-of-range flags are slots 0.. of its jobs.
+ * Otherwise stop_flags holds the run's flags, one per component, and the kernels decide `stop`
+ * from them (QsJob.stop_aware, run_slab). */
+static QsJob run_job(jpegqs_cuda_ctx *ctx, const ImgState &s, const CompWork &w, const uint8_t *plane2,
+		const int *stop_flags) {
+	QsJob j = make_job(ctx, w, plane2, 0, w.H, s.top, s.bottom);
+	if (stop_flags) { j.bad_slot = w.ci; j.bad_first = 0; j.stop_aware = 1; }
+	return j;
+}
+
+static const uint8_t *plane2_of(const ImgState &s, const CompWork &w, int flags) {
+	return (s.image2 && (flags & QS_JOINT_YUV) && w.ci > 0) ? s.image2 : NULL;
+}
+
+/* one launch of each pass kind, counted and (with profiling on) timed */
+static int launch_idct(jpegqs_cuda_ctx *ctx, const QsJob *jd, int nj, int tiles, int mode, cudaStream_t st) {
+	if (prof_begin(ctx, 0, st)) return JPEGQS_ERR_CUDA;
+	CK(qs_launch_idct_pass(jd, nj, tiles, mode, ctx->flags_dev, st));
+	if (prof_end(ctx, st)) return JPEGQS_ERR_CUDA;
+	ctx->launches++;
+	return 0;
+}
+static int launch_smooth(jpegqs_cuda_ctx *ctx, const QsJob *jd, int nj, int tiles, int flags, int clampv, int *bad,
+		cudaStream_t st) {
+	if (prof_begin(ctx, 1, st)) return JPEGQS_ERR_CUDA;
+	if (flags & QS_LOW_QUALITY) CK(qs_launch_lowq(jd, nj, tiles, flags, clampv, bad, st));
+	else CK(qs_launch_smooth(jd, nj, tiles, (flags & QS_DIAGONALS) ? ctx->tab_diag : ctx->tab_plain,
+			ctx->flags_dev + QS_MAX_JOBS, flags, clampv, ctx->num_sms, ctx->tune_sync, ctx->tune_wpg, bad, st));
+	if (prof_end(ctx, st)) return JPEGQS_ERR_CUDA;
+	ctx->launches++;
+	return 0;
+}
+
+/* per-component prelude, quantsmooth.h:2494-2566: passes of the component, `stop` raised by a
+ * quant value >= 0x800 (from then on components are de-quantized only), and whether it iterates:
+ * if so it joins works */
+static int comp_prelude(jpegqs_cuda_ctx *ctx, ImgState &s, CompWork &w, int niter, cudaStream_t st,
+		std::vector<CompWork *> &works) {
+	if (!w.c->has_qtbl) return 0;                                          /* 2494 */
+	w.extra = (s.image1 || (!w.ci && s.need_downsample)) ? 1 : 0;          /* 2495 */
+	w.niter2 = w.qval <= 1 ? 0 : niter;                                    /* 2501 */
+	if (w.qval >= 0x800 && !s.stop) { s.stop = 1; s.stop_ci = w.ci; }      /* 2504 */
+	if (w.niter2 + w.extra == 0) return 0;                                 /* 2542 */
+	if (s.stop) {                                                          /* 2551-2566 */
+		CK(qs_launch_scale_clamp(w.coef_dev, (size_t)w.W * w.H * 64, ctx->quant_dev + w.qslot, 1, 0, st));
+		ctx->launches++;
+		return 0;
+	}
+	if (!(w.W * w.H)) return 0;
+	w.iterate = true;
+	works.push_back(&w);
+	return 0;
+}
+
+/* IDCT pass of iteration iter, 2589-2620, over the components of works that still iterate: one
+ * launch per clamp mode.  The extra (render-only) pass also applies the final +-1023 clamp of
+ * 2670-2689 after rendering from unclamped values.  stop_flags: see run_job; without them a
+ * launch's flags are cleared before the range check of iteration 0.  launched(who) follows every
+ * launch with the components it covered. */
+static int idct_pass(jpegqs_cuda_ctx *ctx, const std::vector<ImgState> &S, const std::vector<CompWork *> &works,
+		int iter, int *stop_flags, cudaStream_t st, const std::function<int(const std::vector<CompWork *> &)> &launched) {
+	for (int clampv = 0; clampv < 2; clampv++) {
+		std::vector<QsJob> jobs; std::vector<CompWork *> who;
+		for (CompWork *w : works) {
+			if (!w->iterate || iter >= w->niter2 + w->extra) continue;
+			if (((iter == w->niter2) ? 1 : 0) != clampv) continue;
+			jobs.push_back(run_job(ctx, S[w->img], *w, NULL, stop_flags)); who.push_back(w);
+		}
+		if (jobs.empty()) continue;
+		const QsJob *jd; int tiles;
+		if (upload_jobs(ctx, 0, jobs, st, &jd, &tiles, stop_flags != NULL)) return JPEGQS_ERR_CUDA;
+		if (!stop_flags && iter == 0) CK(cudaMemsetAsync(ctx->flags_dev, 0, jobs.size() * sizeof(int), st));
+		int mode = (iter == 0 ? QS_IDCT_DEQUANT : 0) | (clampv ? QS_IDCT_CLAMP : 0);
+		if (launch_idct(ctx, jd, (int)jobs.size(), tiles, mode, st)) return JPEGQS_ERR_CUDA;
+		if (clampv) for (CompWork *w : who) w->done_clamp = true;
+		int rc = launched(who);
+		if (rc) return rc;
+	}
+	return 0;
+}
+
+/* smoothing pass of iteration iter, 2627-2640, over the components of works that still iterate;
+ * the last pass of a component without an extra pass clamps to +-1023.  stop_flags: see run_job */
+static int smooth_pass(jpegqs_cuda_ctx *ctx, const std::vector<ImgState> &S, const std::vector<CompWork *> &works,
+		int iter, int flags, int *stop_flags, cudaStream_t st) {
+	for (int clampv = 0; clampv < 2; clampv++) {
+		std::vector<QsJob> jobs; std::vector<CompWork *> who;
+		for (CompWork *w : works) {
+			if (!w->iterate || iter >= w->niter2) continue;
+			if (((iter == w->niter2 - 1 && !w->extra) ? 1 : 0) != clampv) continue;
+			const ImgState &s = S[w->img];
+			jobs.push_back(run_job(ctx, s, *w, plane2_of(s, *w, flags), stop_flags)); who.push_back(w);
+		}
+		if (jobs.empty()) continue;
+		const QsJob *jd; int tiles;
+		if (upload_jobs(ctx, 1, jobs, st, &jd, &tiles, stop_flags != NULL)) return JPEGQS_ERR_CUDA;
+		if (launch_smooth(ctx, jd, (int)jobs.size(), tiles, flags, clampv, stop_flags, st)) return JPEGQS_ERR_CUDA;
+		if (clampv) for (CompWork *w : who) w->done_clamp = true;
+	}
+	return 0;
+}
+
+struct XchgPlane { uint8_t *plane; int wblk, rows; };
+static int slab_exchange(jpegqs_cuda_ctx *ctx, jpegqs_cuda_link *l, const std::vector<XchgPlane> &planes,
+		int *bad_dev, int bad_n, cudaStream_t st);
+
+/* post steps of a component: chroma up-sampling (2691-2752) once the luma planes exist, the luma
+ * planes the chroma needs (2753-2815).  s.geom places the rows held in the image; in a sharded
+ * run the halo rows of the down-sampled luma then come from the neighbours over link. */
+static int post_step(jpegqs_cuda_ctx *ctx, ImgState &s, const CompWork &w, int flags, jpegqs_cuda_link *link,
+		cudaStream_t st) {
+	jpegqs_cuda_image *im = s.im;
+	if (w.ci > 0 && s.image1 && w.ci <= 2) {
+		int ws = im->comp[0].h_samp, hs = im->comp[0].v_samp;
+		int w1 = ((int)im->image_width + ws - 1) / ws, h1 = ((int)im->image_height + hs - 1) / hs;
+		int W0 = im->comp[0].wblk, H0 = im->comp[0].hblk;
+		uint8_t *mem = s.mem_buf[w.ci - 1];
+		CK(qs_launch_upsample(w.plane, s.image2, QS_PLANE_STRIDE(w.W), s.image1, QS_PLANE_STRIDE(W0),
+				mem, W0 * 8, w1, h1, ws, hs, W0 * 8, H0 * 8, (int)s.geom.row0[0] * 8, st));
+		CK(qs_launch_fdct_plane(mem, W0 * 8, s.coef_up_dev[w.ci - 1], W0, H0, st));
+		ctx->launches += 2;
+	} else if (w.ci == 0 && s.need_downsample) {
+		int ws = w.c->h_samp, hs = w.c->v_samp;
+		if (ws == 1 && hs == 1) s.image2 = w.plane;
+		else {
+			if (flags & QS_UPSAMPLE_UV) s.image1 = w.plane;
+			const jpegqs_cuda_comp *cc = &im->comp[1];
+			const uint32_t *row0 = s.geom.row0;
+			int h = (int)s.geom.hblk_total[0] * 8, h2 = (int)s.geom.hblk_total[1] * 8, h1_total = (h + hs - 1) / hs;
+			int first = s.top ? -1 : (int)row0[1] * 8;
+			int last = s.bottom ? h2 : (int)(row0[1] + cc->hblk) * 8 - 1;
+			int dstride = QS_PLANE_STRIDE(cc->wblk);
+			if (last >= first) {
+				CK(qs_launch_downsample(w.plane, QS_PLANE_STRIDE(w.W), w.W * 8, h,
+						s.image2_buf + (size_t)(first - (int)row0[1] * 8 + 1) * dstride, dstride, (int)cc->wblk * 8, h2,
+						ws, hs, (int)row0[0] * 8, first, last - first + 1, h1_total, st));
+				ctx->launches++;
+			}
+			s.image2 = s.image2_buf;
+			std::vector<XchgPlane> xp; xp.push_back({ s.image2_buf, (int)cc->wblk, (int)cc->hblk });
+			if (slab_exchange(ctx, link, xp, ctx->flags_dev, 0, st)) return JPEGQS_ERR_CUDA;
+		}
+	}
+	return 0;
+}
+
+/* results, quantsmooth.h:2834-2859: quant tables of the smoothed components set to 1, upsampled,
+ * the return values; device time and per-kernel timing of the run (ev1 recorded and complete) */
+static int run_results(jpegqs_cuda_ctx *ctx, RunSetup &r, int *ret) {
+	for (size_t n = 0; n < r.S.size(); n++) {
+		ImgState &s = r.S[n]; jpegqs_cuda_image *im = s.im;
+		if (ret) ret[n] = s.stop;
+		if (s.skip) continue;
+		for (int ci = 0; ci < im->ncomp; ci++)
+			if (im->comp[ci].has_qtbl) for (int k = 0; k < 64; k++) im->comp[ci].quant[k] = 1;
+		im->upsampled = (s.image1 && !s.stop) ? 1 : 0;
+	}
+	CK(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
+	return prof_collect(ctx);
+}
+
+/* ------------------------------------------------------------------------------------------
+ * whole-image driver
+ * ------------------------------------------------------------------------------------------ */
+
+/* Host entry points, one large image: iteration 0 follows the upload slab by slab (IDCT pass of
+ * slab k, smoothing of slab k-1 - which needs the first pixel row of slab k), and the last
+ * iteration hands its slabs to the download as they finish, so that only the first slab's upload
+ * and the last slab's download are not hidden behind kernels.  Results do not depend on this: a
+ * pass reads only start-of-pass neighbour pixels (quantsmooth.h:1396-1401). */
+struct SlabPlan { int K; int r[QS_MAX_SLABS + 1]; };
+
+static int run_images(jpegqs_cuda_ctx *ctx, int nimg, jpegqs_cuda_image *imgs, int flags, int niter,
+		int progprec, jpegqs_cuda_progress_fn progress, void *userdata, bool on_device, int *ret,
+		cudaStream_t st) {
+	if (!ctx || nimg < 0 || (nimg && !imgs)) return JPEGQS_ERR_ARG;
+	if (progress && nimg != 1) return JPEGQS_ERR_ARG;
+	RunSetup r;
+	int rc = run_setup(ctx, nimg, imgs, flags, niter, on_device, st, r);
+	if (rc) return rc;
+	niter = r.niter;
+	std::vector<ImgState> &S = r.S;
+	std::vector<std::vector<CompWork> > &W = r.W;
+	if (progress && !S[0].skip) S[0].ngroups = S[0].im->ncomp;      /* one phase per component */
+	int max_groups = 0;
+	for (const ImgState &s : S) max_groups = std::max(max_groups, s.ngroups);
+
 	std::vector<SlabPlan> plan(max_groups > 0 ? max_groups : 1);
 	for (SlabPlan &pl : plan) pl.K = 0;
 
@@ -795,17 +1028,8 @@ static int run_images(jpegqs_cuda_ctx *ctx, int nimg, jpegqs_cuda_image *imgs, i
 	HostIo io(ctx);
 	std::vector<int> unit_of_group(max_groups > 0 ? max_groups : 1, -1);
 	std::vector<std::vector<int> > unit_of_slab(max_groups > 0 ? max_groups : 1);
-	auto seg_of = [&](const CompWork &w, int r0, int r1) {
-		IoSeg sg; sg.dev = w.coef_dev; sg.pin = w.pin; sg.rows = w.rows; sg.wblk = w.W; sg.r0 = r0; sg.r1 = r1;
-		return sg;
-	};
 	if (!on_device) {
-		while ((int)ctx->sync_ev.size() < 2 * max_groups) {
-			cudaEvent_t e; CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming)); ctx->sync_ev.push_back(e);
-		}
-		while ((int)ctx->slab_ev.size() < 2 * max_groups * QS_MAX_SLABS) {
-			cudaEvent_t e; CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming)); ctx->slab_ev.push_back(e);
-		}
+		if (group_events(ctx, max_groups)) return JPEGQS_ERR_CUDA;
 		for (int g = 0; g < max_groups; g++) {
 			if (nimg == 1 && !progress && ctx->tune_slabs && !(flags & QS_LOW_QUALITY) &&
 					!S[0].skip && g < S[0].ngroups && niter >= 1) {
@@ -815,7 +1039,7 @@ static int run_images(jpegqs_cuda_ctx *ctx, int nimg, jpegqs_cuda_image *imgs, i
 				bool ok = c1 > c0;
 				for (int ci = c0; ci < c1 && ok; ci++) {
 					CompWork &w = W[0][ci];
-					ok = w.c->has_qtbl && qval[0][ci] > 1 && qval[0][ci] < 0x800 && w.W > 0 && w.H > 0 &&
+					ok = w.c->has_qtbl && w.qval > 1 && w.qval < 0x800 && w.W > 0 && w.H > 0 &&
 							w.W == W[0][c0].W && w.H == W[0][c0].H;
 				}
 				if (ok) {
@@ -858,8 +1082,7 @@ static int run_images(jpegqs_cuda_ctx *ctx, int nimg, jpegqs_cuda_image *imgs, i
 	auto up_wait = [&](int unit) -> int { return io.wait(unit, st); };
 	auto download = [&](std::vector<IoSeg> segs, cudaEvent_t after) -> int { return io.download(std::move(segs), after); };
 
-	const float *tabs = (flags & QS_DIAGONALS) ? ctx->tab_diag : ctx->tab_plain;
-	int *bad_dev = ctx->flags_dev, *tile_counter = ctx->flags_dev + QS_MAX_JOBS;
+	int *bad_dev = ctx->flags_dev;
 	CK(cudaEventRecord(ctx->ev0, st));
 
 	/* progress bookkeeping, quantsmooth.h:2474-2482 (single image only) */
@@ -872,36 +1095,10 @@ static int run_images(jpegqs_cuda_ctx *ctx, int nimg, jpegqs_cuda_image *imgs, i
 		prog_thr = progprec ? (int)((unsigned)(prog_max + progprec - 1) / (unsigned)progprec) : 0;
 	}
 
-	auto make_job = [&](const CompWork &w, const uint8_t *plane2) {
-		QsJob j; memset(&j, 0, sizeof(j));
-		j.coef = w.coef_dev; j.plane = w.plane; j.plane2 = plane2;
-		j.quant = ctx->quant_dev + w.qslot;
-		j.wblk = w.W; j.hblk = w.H; j.stride = QS_PLANE_STRIDE(w.W); j.nblocks = w.W * w.H;
-		j.luma = w.luma; j.top_edge = 1; j.bottom_edge = 1;
-		return j;
-	};
-	auto make_slab_job = [&](const CompWork &w, const uint8_t *plane2, int r0, int r1) {
-		QsJob j = make_job(w, plane2);
-		size_t poff = (size_t)r0 * 8 * j.stride;
-		j.coef += (size_t)r0 * w.W * 64; j.plane += poff;
-		if (plane2) j.plane2 += poff;
-		j.hblk = r1 - r0; j.nblocks = w.W * (r1 - r0);
-		j.top_edge = r0 == 0; j.bottom_edge = r1 == w.H;
-		return j;
-	};
-	auto launch_smooth = [&](const QsJob *jd, int nj, int tiles, int clampv) -> int {
-		if (prof_begin(ctx, 1, st)) return JPEGQS_ERR_CUDA;
-		if (flags & QS_LOW_QUALITY) CK(qs_launch_lowq(jd, nj, tiles, flags, clampv, NULL, st));
-		else CK(qs_launch_smooth(jd, nj, tiles, tabs, tile_counter, flags, clampv, ctx->num_sms, ctx->tune_sync, ctx->tune_wpg, NULL, st));
-		if (prof_end(ctx, st)) return JPEGQS_ERR_CUDA;
-		ctx->launches++;
-		return 0;
-	};
-
 	for (int g = 0; g < max_groups; g++) {
 		bool slab_in = !on_device && plan[g].K > 0 && !S[0].stop;
 		if (!on_device && !slab_in && up_wait(unit_of_group[g])) return JPEGQS_ERR_CUDA;
-		/* ---- which components belong to this phase; per-component prelude 2484-2566 ---- */
+		/* ---- which components belong to this phase ---- */
 		std::vector<CompWork *> works;
 		int prog_cur = 0, prog_inc = 0;
 		for (int n = 0; n < nimg; n++) {
@@ -911,28 +1108,12 @@ static int run_images(jpegqs_cuda_ctx *ctx, int nimg, jpegqs_cuda_image *imgs, i
 			for (int ci = c0; ci < c1; ci++) {
 				CompWork &w = W[n][ci];
 				if (progress) { prog_cur = prog_next; prog_inc = w.c->v_samp; prog_next += w.H * prog_inc * niter; }
-				if (!w.c->has_qtbl) continue;                              /* 2494 */
-				w.extra = (s.image1 || (!ci && s.need_downsample)) ? 1 : 0;      /* 2495 */
-				w.niter2 = qval[n][ci] <= 1 ? 0 : niter;                   /* 2501 */
-				if (qval[n][ci] >= 0x800 && !s.stop) { s.stop = 1; s.stop_ci = ci; }   /* 2504 */
-				if (w.niter2 + w.extra == 0) continue;                     /* 2542 */
-				if (s.stop) {                                              /* 2551-2566 */
-					CK(qs_launch_scale_clamp(w.coef_dev, (size_t)w.W * w.H * 64, ctx->quant_dev + w.qslot, 1, 0, st));
-					ctx->launches++;
-					continue;
-				}
-				if (!(w.W * w.H)) continue;
-				w.iterate = true;
-				works.push_back(&w);
+				if (comp_prelude(ctx, s, w, niter, st, works)) return JPEGQS_ERR_CUDA;
 			}
 		}
 
 		int max_pass = 0;
 		for (CompWork *w : works) if (w->niter2 + w->extra > max_pass) max_pass = w->niter2 + w->extra;
-		auto p2_of = [&](const CompWork *w) -> const uint8_t * {
-			ImgState &s = S[w->img];
-			return (s.image2 && (flags & QS_JOINT_YUV) && w->ci > 0) ? s.image2 : NULL;
-		};
 		if (slab_in) {
 			int c0, c1; group_range(S[0], g, &c0, &c1);
 			bool ok = (int)works.size() == c1 - c0;
@@ -954,18 +1135,16 @@ static int run_images(jpegqs_cuda_ctx *ctx, int nimg, jpegqs_cuda_image *imgs, i
 					if (k < pl.K) {
 						if (up_wait(unit_of_slab[g][k])) return JPEGQS_ERR_CUDA;
 						std::vector<QsJob> jobs;
-						for (CompWork *w : works) jobs.push_back(make_slab_job(*w, NULL, pl.r[k], pl.r[k + 1]));
+						for (CompWork *w : works) jobs.push_back(make_job(ctx, *w, NULL, pl.r[k], pl.r[k + 1], pl.r[k] == 0, pl.r[k + 1] == w->H));
 						if (upload_jobs(ctx, 0, jobs, st, &jd, &tiles)) return JPEGQS_ERR_CUDA;
-						if (prof_begin(ctx, 0, st)) return JPEGQS_ERR_CUDA;
-						CK(qs_launch_idct_pass(jd, (int)jobs.size(), tiles, QS_IDCT_DEQUANT, bad_dev, st));
-						if (prof_end(ctx, st)) return JPEGQS_ERR_CUDA;
-						ctx->launches++;
+						if (launch_idct(ctx, jd, (int)jobs.size(), tiles, QS_IDCT_DEQUANT, st)) return JPEGQS_ERR_CUDA;
 					}
 					if (k >= 1) {
 						std::vector<QsJob> jobs;
-						for (CompWork *w : works) jobs.push_back(make_slab_job(*w, p2_of(w), pl.r[k - 1], pl.r[k]));
+						for (CompWork *w : works)
+							jobs.push_back(make_job(ctx, *w, plane2_of(S[0], *w, flags), pl.r[k - 1], pl.r[k], pl.r[k - 1] == 0, pl.r[k] == w->H));
 						if (upload_jobs(ctx, 1, jobs, st, &jd, &tiles)) return JPEGQS_ERR_CUDA;
-						if (launch_smooth(jd, (int)jobs.size(), tiles, cl)) return JPEGQS_ERR_CUDA;
+						if (launch_smooth(ctx, jd, (int)jobs.size(), tiles, flags, cl, NULL, st)) return JPEGQS_ERR_CUDA;
 					}
 				}
 				CK(qs_copy_flags(bad_dev, ctx->flags_host, (int)works.size(), st));
@@ -985,54 +1164,38 @@ static int run_images(jpegqs_cuda_ctx *ctx, int nimg, jpegqs_cuda_image *imgs, i
 				}
 				slab_in = slab_out = false;
 			}
-			/* ---- IDCT pass, 2589-2620.  The extra (render-only) pass also applies the
-			 *      final +-1023 clamp of 2670-2689 after rendering from unclamped values. */
-			for (int clampv = 0; clampv < 2; clampv++) {
-				std::vector<QsJob> jobs; std::vector<CompWork *> who;
-				for (CompWork *w : works) {
-					if (!w->iterate || iter >= w->niter2 + w->extra) continue;
-					int cl = (iter == w->niter2) ? 1 : 0;
-					if (cl != clampv) continue;
-					jobs.push_back(make_job(*w, NULL)); who.push_back(w);
-				}
-				if (jobs.empty()) continue;
-				const QsJob *jd; int tiles;
-				if (upload_jobs(ctx, 0, jobs, st, &jd, &tiles)) return JPEGQS_ERR_CUDA;
-				int mode = (iter == 0 ? QS_IDCT_DEQUANT : 0) | (clampv ? QS_IDCT_CLAMP : 0);
-				if (iter == 0) CK(cudaMemsetAsync(bad_dev, 0, jobs.size() * sizeof(int), st));
-				if (prof_begin(ctx, 0, st)) return JPEGQS_ERR_CUDA;
-				CK(qs_launch_idct_pass(jd, (int)jobs.size(), tiles, mode, bad_dev, st));
-				if (prof_end(ctx, st)) return JPEGQS_ERR_CUDA;
-				ctx->launches++;
-				if (clampv) for (CompWork *w : who) w->done_clamp = true;
-				if (iter == 0) {                                           /* bad_coef, 2602-2610 */
-					CK(qs_copy_flags(bad_dev, ctx->flags_host, (int)jobs.size(), st));
-					CK(cudaStreamSynchronize(st));
-					for (size_t k = 0; k < who.size(); k++) {
-						CompWork *w = who[k]; ImgState &s = S[w->img];
-						if (s.stop && w->ci > s.stop_ci) {
-							/* an earlier component of this image already failed: the reference
-							 * would only have de-quantized this one - which the pass just did */
-							w->iterate = false; w->done_clamp = true;
-						} else if (ctx->flags_host[k]) {
-							/* components run in order in the reference: this one stops here (it
-							 * falls to the clamp below), earlier ones are unaffected */
-							s.stop = 1; s.stop_ci = w->ci; w->iterate = false;
-						}
+			/* ---- IDCT pass; in iteration 0 the host reads the out-of-range flags, bad_coef 2602-2610 ---- */
+			int rc = idct_pass(ctx, S, works, iter, NULL, st, [&](const std::vector<CompWork *> &who) -> int {
+				if (iter != 0) return 0;
+				CK(qs_copy_flags(bad_dev, ctx->flags_host, (int)who.size(), st));
+				CK(cudaStreamSynchronize(st));
+				for (size_t k = 0; k < who.size(); k++) {
+					CompWork *w = who[k]; ImgState &s = S[w->img];
+					if (s.stop && w->ci > s.stop_ci) {
+						/* an earlier component of this image already failed: the reference
+						 * would only have de-quantized this one - which the pass just did */
+						w->iterate = false; w->done_clamp = true;
+					} else if (ctx->flags_host[k]) {
+						/* components run in order in the reference: this one stops here (it
+						 * falls to the clamp below), earlier ones are unaffected */
+						s.stop = 1; s.stop_ci = w->ci; w->iterate = false;
 					}
 				}
-			}
-			/* ---- smoothing pass, 2627-2640 ---- */
+				return 0;
+			});
+			if (rc) return rc;
+			/* ---- smoothing pass ---- */
 			if (slab_out) for (CompWork *w : works) if (!w->iterate) slab_out = false;   /* a component stopped */
 			if (slab_out && iter == works[0]->niter2 - 1) {
 				/* last iteration: each finished slab goes straight to the download */
 				const SlabPlan &pl = plan[g];
 				for (int k = 0; k < pl.K; k++) {
 					std::vector<QsJob> jobs;
-					for (CompWork *w : works) jobs.push_back(make_slab_job(*w, p2_of(w), pl.r[k], pl.r[k + 1]));
+					for (CompWork *w : works)
+						jobs.push_back(make_job(ctx, *w, plane2_of(S[0], *w, flags), pl.r[k], pl.r[k + 1], pl.r[k] == 0, pl.r[k + 1] == w->H));
 					const QsJob *jd; int tiles;
 					if (upload_jobs(ctx, 1, jobs, st, &jd, &tiles)) return JPEGQS_ERR_CUDA;
-					if (launch_smooth(jd, (int)jobs.size(), tiles, 1)) return JPEGQS_ERR_CUDA;
+					if (launch_smooth(ctx, jd, (int)jobs.size(), tiles, flags, 1, NULL, st)) return JPEGQS_ERR_CUDA;
 					cudaEvent_t e = ctx->slab_ev[(2 * g + 1) * QS_MAX_SLABS + k];
 					CK(cudaEventRecord(e, st));
 					std::vector<IoSeg> segs;
@@ -1042,20 +1205,7 @@ static int run_images(jpegqs_cuda_ctx *ctx, int nimg, jpegqs_cuda_image *imgs, i
 				for (CompWork *w : works) { w->done_clamp = true; w->downloaded = true; }
 				continue;
 			}
-			for (int clampv = 0; clampv < 2; clampv++) {
-				std::vector<QsJob> jobs; std::vector<CompWork *> who;
-				for (CompWork *w : works) {
-					if (!w->iterate || iter >= w->niter2) continue;
-					int cl = (iter == w->niter2 - 1 && !w->extra) ? 1 : 0;
-					if (cl != clampv) continue;
-					jobs.push_back(make_job(*w, p2_of(w))); who.push_back(w);
-				}
-				if (jobs.empty()) continue;
-				const QsJob *jd; int tiles;
-				if (upload_jobs(ctx, 1, jobs, st, &jd, &tiles)) return JPEGQS_ERR_CUDA;
-				if (launch_smooth(jd, (int)jobs.size(), tiles, clampv)) return JPEGQS_ERR_CUDA;
-				if (clampv) for (CompWork *w : who) w->done_clamp = true;
-			}
+			if (smooth_pass(ctx, S, works, iter, flags, NULL, st)) return JPEGQS_ERR_CUDA;
 			if (progress && works.size() == 1 && works[0]->iterate && iter < works[0]->niter2) {   /* 2656-2664 */
 				CompWork *w = works[0]; ImgState &s = S[0];
 				int cur = prog_cur += w->H * prog_inc;
@@ -1074,73 +1224,33 @@ static int run_images(jpegqs_cuda_ctx *ctx, int nimg, jpegqs_cuda_image *imgs, i
 			CK(qs_launch_scale_clamp(w->coef_dev, (size_t)w->W * w->H * 64, ctx->quant_dev + w->qslot, 0, 1, st));
 			ctx->launches++; w->done_clamp = true;
 		}
-		/* ---- post steps: chroma up-sampling (2691-2752), luma planes (2753-2815) ---- */
+		/* ---- post steps of the images that did not stop ---- */
 		for (CompWork *w : works) {
-			ImgState &s = S[w->img]; jpegqs_cuda_image *im = s.im;
+			ImgState &s = S[w->img];
 			if (s.stop) continue;
-			if (w->ci > 0 && s.image1 && w->ci <= 2) {
-				int ws = im->comp[0].h_samp, hs = im->comp[0].v_samp;
-				int w1 = (im->image_width + ws - 1) / ws, h1 = (im->image_height + hs - 1) / hs;
-				int W0 = im->comp[0].wblk, H0 = im->comp[0].hblk;
-				uint8_t *mem = s.mem_buf[w->ci - 1];
-				CK(qs_launch_upsample(w->plane, s.image2, QS_PLANE_STRIDE(w->W), s.image1, QS_PLANE_STRIDE(W0),
-						mem, W0 * 8, w1, h1, ws, hs, W0 * 8, H0 * 8, 0, st));
-				CK(qs_launch_fdct_plane(mem, W0 * 8, s.coef_up_dev[w->ci - 1], W0, H0, st));
-				ctx->launches += 2;
-			} else if (w->ci == 0 && s.need_downsample) {
-				int ws = w->c->h_samp, hs = w->c->v_samp;
-				if (ws == 1 && hs == 1) s.image2 = w->plane;
-				else {
-					if (flags & QS_UPSAMPLE_UV) s.image1 = w->plane;
-					int w2 = im->comp[1].wblk * 8, h2 = im->comp[1].hblk * 8;
-					int h1 = (w->H * 8 + hs - 1) / hs;
-					CK(qs_launch_downsample(w->plane, QS_PLANE_STRIDE(w->W), w->W * 8, w->H * 8,
-							s.image2_buf, QS_PLANE_STRIDE(im->comp[1].wblk), w2, h2, ws, hs, 0, -1, h2 + 2, h1, st));
-					ctx->launches++;
-					s.image2 = s.image2_buf;
-				}
-			}
+			if (post_step(ctx, s, *w, flags, NULL, st)) return JPEGQS_ERR_CUDA;
 		}
 		/* ---- downloads of this phase, on the copy stream, behind the phase's last kernel ---- */
 		if (!on_device) {
 			CK(cudaEventRecord(ctx->sync_ev[2 * g + 1], st));
 			std::vector<IoSeg> segs;
 			for (int n = 0; n < nimg; n++) {
-				ImgState &s = S[n]; jpegqs_cuda_image *im = s.im;
+				ImgState &s = S[n];
 				if (s.skip || g >= s.ngroups) continue;
 				int c0, c1; group_range(s, g, &c0, &c1);
 				for (int ci = c0; ci < c1; ci++) {
 					CompWork &w = W[n][ci];
 					if (w.W && w.H && !w.downloaded) segs.push_back(seg_of(w, 0, w.H));
-					if (s.image1 && !s.stop && ci >= 1 && ci <= 2) {
-						IoSeg sg; sg.dev = s.coef_up_dev[ci - 1]; sg.pin = w.pin_up; sg.rows = w.rows_up;
-						sg.wblk = im->comp[0].wblk; sg.r0 = 0; sg.r1 = im->comp[0].hblk;
-						segs.push_back(sg);
-					}
+					if (s.image1 && !s.stop && ci >= 1 && ci <= 2) segs.push_back(seg_up_of(s, w, 0, s.im->comp[0].hblk));
 				}
 			}
 			if (download(std::move(segs), ctx->sync_ev[2 * g + 1])) return JPEGQS_ERR_CUDA;
 		}
 	}
 	CK(cudaEventRecord(ctx->ev1, st));
-
-	/* ---- results ---- */
-	for (int n = 0; n < nimg; n++) {
-		ImgState &s = S[n]; jpegqs_cuda_image *im = s.im;
-		if (s.skip) continue;
-		bool ups = s.image1 && !s.stop;                                 /* 2834-2849 */
-		for (int ci = 0; ci < im->ncomp; ci++) {
-			CompWork &w = W[n][ci];
-			if (w.c->has_qtbl) for (int k = 0; k < 64; k++) w.c->quant[k] = 1;      /* 2851-2859 */
-		}
-		im->upsampled = ups ? 1 : 0;
-		if (ret) ret[n] = s.stop;
-	}
 	CK(cudaStreamSynchronize(st));
 	if (!on_device && io.finish()) return JPEGQS_ERR_CUDA;  /* the last scatter has finished */
-	CK(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
-	if (prof_collect(ctx)) return JPEGQS_ERR_CUDA;
-	return 0;
+	return run_results(ctx, r, ret);
 }
 
 extern "C" int jpegqs_cuda_run_host(jpegqs_cuda_ctx *ctx, jpegqs_cuda_image *img, int flags, int niter,
@@ -1300,8 +1410,6 @@ static char *box_rows(const jpegqs_cuda_link *l, char *box, int parity, int side
 	return box + QS_BOX_ROWS + (((size_t)parity * 2 + side) * QS_XCHG_SLOTS + slot) * l->row_bytes;
 }
 
-struct XchgPlane { uint8_t *plane; int wblk, rows; };
-
 /* one exchange on stream st: first / last pixel row of every plane to the neighbours, theirs into
  * the halo rows; with bad_n > 0 also the OR of bad_dev[0..bad_n) over all ranks */
 static int slab_exchange(jpegqs_cuda_ctx *ctx, jpegqs_cuda_link *l, const std::vector<XchgPlane> &planes,
@@ -1355,128 +1463,41 @@ static int slab_exchange(jpegqs_cuda_ctx *ctx, jpegqs_cuda_link *l, const std::v
 }
 
 /* do_quantsmooth on ONE SLAB of an image: img describes the slab (comp[].hblk = block rows held
- * by this rank, coef / rows = those rows), geom where it sits.  The slab-local restatement of
- * run_images (itself the reference driver, quantsmooth.h:2404-2878); the schedule is
- * unconditional - what the reference decides with `stop` is decided on the device from the
- * run's out-of-range flags (QsJob.stop_aware), which the ranks OR-combine in the first exchange
- * of a phase - so every rank issues the same exchanges whatever its data look like. */
+ * by this rank, coef / rows = those rows), geom where it sits.  It shares run_images's set-up,
+ * passes and post steps; its schedule is unconditional - what the reference decides with `stop` is
+ * decided on the device from the run's out-of-range flags (QsJob.stop_aware), which the ranks
+ * OR-combine in the first exchange of a phase - so every rank issues the same exchanges whatever
+ * its data look like. */
 static int run_slab(jpegqs_cuda_ctx *ctx, jpegqs_cuda_link *link, jpegqs_cuda_image *im, const jpegqs_cuda_slab *geom,
 		int flags, int niter, bool on_device, int *ret, cudaStream_t st) {
 	if (!ctx || !im || !geom) return JPEGQS_ERR_ARG;
 	const int rank = link ? link->rank : 0, world = link ? link->world : 1;
 	if (link && (link->ctx != ctx || !link->connected)) return JPEGQS_ERR_ARG;
 	if (geom->rank != rank || geom->world != world) return JPEGQS_ERR_ARG;
-	CK(cudaSetDevice(ctx->device));
-	ctx->launches = 0; ctx->last_ms = 0; ctx->ev_kind.clear(); ctx->ev_used = 0;
-	if (niter < 0) niter = 0;
-	if (niter > 100) niter = 100;
+	RunSetup r;
+	int rc = run_setup(ctx, 1, im, flags, niter, on_device, st, r);
+	if (rc) return rc;
+	niter = r.niter;
+	ImgState &s = r.S[0];
+	std::vector<CompWork> &W = r.W[0];
+	if (s.skip) return 0;                                                  /* 2458 */
 	const int nc = im->ncomp;
-	if (nc < 1 || nc > JPEGQS_CUDA_MAX_COMP) return JPEGQS_ERR_ARG;
-	const bool top = rank == 0, bottom = rank == world - 1;
-	im->upsampled = 0;
-	if (ret) *ret = 0;
-	bool need_ds = (flags & (QS_JOINT_YUV | QS_UPSAMPLE_UV)) && im->is_ycbcr && nc >= 3 &&
-			im->comp[1].h_samp == 1 && im->comp[1].v_samp == 1 && im->comp[2].h_samp == 1 && im->comp[2].v_samp == 1;
-	if (niter <= 0 && !((flags & QS_UPSAMPLE_UV) && need_ds)) return 0;                   /* 2458 */
-	if (need_ds && (im->comp[1].wblk != im->comp[2].wblk || im->comp[1].hblk != im->comp[2].hblk)) return JPEGQS_ERR_ARG;
-	const bool sub = need_ds && !(im->comp[0].h_samp == 1 && im->comp[0].v_samp == 1);
-	const bool ups = sub && (flags & QS_UPSAMPLE_UV);
-	if (ctx->up) ctx->up->drain();
-	if (ctx->down) ctx->down->drain();
-	ctx->io_ev_used = 0;
-
-	/* ---- memory ---- */
-	size_t bytes = 0, stage_bytes = 0;
-	for (int ci = 0; ci < nc; ci++) {
-		jpegqs_cuda_comp *c = &im->comp[ci];
-		if (!(c->coef || (!on_device && c->rows)) && c->wblk && c->hblk) return JPEGQS_ERR_ARG;
-		if (world > 1 && (!c->hblk || !c->wblk)) {
+	for (int ci = 0; ci < nc; ci++)
+		if (world > 1 && (!im->comp[ci].hblk || !im->comp[ci].wblk)) {
 			snprintf(ctx->err, sizeof(ctx->err), "sharded run: rank %d holds no block row of component %d", rank, ci);
 			return JPEGQS_ERR_ARG;
 		}
-		size_t cb = (size_t)c->wblk * c->hblk * 128;
-		if (!on_device) { bytes += align256(cb); if (c->rows || !is_pinned(c->coef)) stage_bytes += align256(cb); }
-		bytes += align256(QS_PLANE_BYTES(c->wblk, c->hblk));
-	}
-	const size_t yb = (size_t)im->comp[0].wblk * im->comp[0].hblk;
-	if (sub) {
-		bytes += align256(QS_PLANE_BYTES(im->comp[1].wblk, im->comp[1].hblk));
-		if (ups) for (int j = 0; j < 2; j++) {
-			jpegqs_cuda_comp *c = &im->comp[1 + j];
-			if (!c->coef_up && !(!on_device && c->rows_up)) return JPEGQS_ERR_ARG;
-			bytes += align256(yb * 64);
-			if (!on_device) { bytes += align256(yb * 128); if (c->rows_up || !is_pinned(c->coef_up)) stage_bytes += align256(yb * 128); }
-		}
-	}
-	if (arena_reserve(ctx, bytes + 4096)) return JPEGQS_ERR_CUDA;
-	if (quant_reserve(ctx, nc)) return JPEGQS_ERR_CUDA;
-	if (stage_bytes && stage_reserve(ctx, stage_bytes)) return JPEGQS_ERR_CUDA;
-	size_t stage_pos = 0;
-	auto stage_take = [&](size_t b) { char *p = ctx->stage + stage_pos; stage_pos += align256(b); return (int16_t *)p; };
-	std::vector<std::unique_ptr<int16_t *[]> > rowstore;
-	auto flat_rows = [&](int16_t *base, uint32_t wblk, uint32_t hblk) -> int16_t *const * {
-		rowstore.emplace_back(new int16_t *[hblk ? hblk : 1]);
-		int16_t **t = rowstore.back().get();
-		for (uint32_t y = 0; y < hblk; y++) t[y] = base + (size_t)y * wblk * 64;
-		return t;
-	};
-	std::vector<CompWork> W(nc); std::vector<QsQuantDev> qhost(nc); std::vector<int> qval(nc);
-	for (int ci = 0; ci < nc; ci++) {
-		jpegqs_cuda_comp *c = &im->comp[ci]; CompWork &w = W[ci];
-		memset(&w, 0, sizeof(w));
-		w.ci = ci; w.c = c; w.W = c->wblk; w.H = c->hblk; w.luma = !ci || !im->is_ycbcr; w.qslot = ci;
-		size_t cb = (size_t)c->wblk * c->hblk * 128;
-		if (on_device) w.coef_dev = c->coef;
-		else {
-			w.coef_dev = (int16_t *)arena_take(ctx, cb);
-			if (c->rows) { w.rows = c->rows; w.pin = stage_take(cb); }
-			else if (is_pinned(c->coef)) { w.rows = NULL; w.pin = c->coef; }
-			else { w.rows = flat_rows(c->coef, c->wblk, c->hblk); w.pin = stage_take(cb); }
-		}
-		w.plane = (uint8_t *)arena_take(ctx, QS_PLANE_BYTES(c->wblk, c->hblk));
-		quant_prepare(c->quant, &qhost[ci], &qval[ci], ctx->tune_maxn, ctx->tune_uni, ctx->tune_merge);
-	}
-	uint8_t *image2_buf = NULL, *mem_buf[2] = { NULL, NULL }; int16_t *coef_up_dev[2] = { NULL, NULL };
-	if (sub) {
-		image2_buf = (uint8_t *)arena_take(ctx, QS_PLANE_BYTES(im->comp[1].wblk, im->comp[1].hblk));
-		if (ups) for (int j = 0; j < 2; j++) {
-			jpegqs_cuda_comp *c = &im->comp[1 + j]; CompWork &w = W[1 + j];
-			mem_buf[j] = (uint8_t *)arena_take(ctx, yb * 64);
-			coef_up_dev[j] = on_device ? c->coef_up : (int16_t *)arena_take(ctx, yb * 128);
-			if (!on_device) {
-				if (c->rows_up) { w.rows_up = c->rows_up; w.pin_up = stage_take(yb * 128); }
-				else if (is_pinned(c->coef_up)) { w.rows_up = NULL; w.pin_up = c->coef_up; }
-				else { w.rows_up = flat_rows(c->coef_up, im->comp[0].wblk, im->comp[0].hblk); w.pin_up = stage_take(yb * 128); }
-			}
-		}
-	}
-	assign_sched_slots(qhost.data(), nc);
-	CK(cudaMemcpyAsync(ctx->quant_dev, qhost.data(), (size_t)nc * sizeof(QsQuantDev), cudaMemcpyHostToDevice, st));
-	ctx->jobs_cache[0].clear(); ctx->jobs_cache[1].clear();
+	s.geom = *geom; s.top = rank == 0; s.bottom = rank == world - 1;
 
-	/* ---- phases (luma | chroma when the chroma needs the finished luma, or to overlap the
-	 *      transfers of host buffers), uploads ---- */
-	const int ngroups = (need_ds || (!on_device && nc > 1)) ? 2 : 1;
-	auto group_range = [&](int g, int *c0, int *c1) {
-		if (ngroups == 2) { *c0 = g ? 1 : 0; *c1 = g ? nc : 1; } else { *c0 = 0; *c1 = nc; }
-	};
+	/* ---- uploads ---- */
 	HostIo io(ctx);
 	int unit_of_group[2] = { -1, -1 }, nbands[2] = { 1, 1 };
-	auto seg_of = [&](const CompWork &w, int r0, int r1) {
-		IoSeg sg; sg.dev = w.coef_dev; sg.pin = w.pin; sg.rows = w.rows; sg.wblk = w.W; sg.r0 = r0; sg.r1 = r1;
-		return sg;
-	};
 	if (!on_device) {
-		while ((int)ctx->sync_ev.size() < 2 * ngroups) {
-			cudaEvent_t e; CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming)); ctx->sync_ev.push_back(e);
-		}
+		if (group_events(ctx, s.ngroups)) return JPEGQS_ERR_CUDA;
 		/* a phase travels in bands of ~8 MB: the H2D copy of band k runs while band k+1 is being
 		 * gathered (and, on the way back, band k is scattered while band k+1 is still in flight) */
-		while ((int)ctx->slab_ev.size() < 2 * ngroups * QS_MAX_SLABS) {
-			cudaEvent_t e; CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming)); ctx->slab_ev.push_back(e);
-		}
-		for (int g = 0; g < ngroups; g++) {
-			int c0, c1; group_range(g, &c0, &c1);
+		for (int g = 0; g < s.ngroups; g++) {
+			int c0, c1; group_range(s, g, &c0, &c1);
 			size_t gb = 0;
 			for (int ci = c0; ci < c1; ci++) gb += (size_t)W[ci].W * W[ci].H * 128;
 			nbands[g] = (int)std::min<size_t>(QS_MAX_SLABS, std::max<size_t>(1, gb >> 23));
@@ -1492,89 +1513,29 @@ static int run_slab(jpegqs_cuda_ctx *ctx, jpegqs_cuda_link *link, jpegqs_cuda_im
 		if (io.start()) return JPEGQS_ERR_CUDA;
 	}
 
-	const float *tabs = (flags & QS_DIAGONALS) ? ctx->tab_diag : ctx->tab_plain;
-	int *bad_dev = ctx->flags_dev, *tile_counter = ctx->flags_dev + QS_MAX_JOBS;
+	int *bad_dev = ctx->flags_dev;
 	CK(cudaMemsetAsync(bad_dev, 0, 16 * sizeof(int), st));
 	CK(cudaEventRecord(ctx->ev0, st));
-	auto make_job = [&](const CompWork &w, const uint8_t *plane2) {
-		QsJob j; memset(&j, 0, sizeof(j));
-		j.coef = w.coef_dev; j.plane = w.plane; j.plane2 = plane2;
-		j.quant = ctx->quant_dev + w.qslot;
-		j.wblk = w.W; j.hblk = w.H; j.stride = QS_PLANE_STRIDE(w.W); j.nblocks = w.W * w.H;
-		j.luma = w.luma; j.top_edge = top; j.bottom_edge = bottom;
-		j.bad_slot = w.ci; j.bad_first = 0; j.stop_aware = 1;
-		return j;
-	};
-	int static_stop_ci = 1 << 30;                          /* quantsmooth.h:2504: a quant value >= 0x800 */
-	uint8_t *image1 = NULL, *image2 = NULL;
-
-	for (int g = 0; g < ngroups; g++) {
+	for (int g = 0; g < s.ngroups; g++) {
 		if (!on_device && io.wait(unit_of_group[g], st)) return JPEGQS_ERR_CUDA;
-		int c0, c1; group_range(g, &c0, &c1);
+		int c0, c1; group_range(s, g, &c0, &c1);
 		std::vector<CompWork *> works;
-		for (int ci = c0; ci < c1; ci++) {
-			CompWork &w = W[ci];
-			if (!w.c->has_qtbl) continue;                                  /* 2494 */
-			w.extra = (image1 || (!ci && need_ds)) ? 1 : 0;                /* 2495 */
-			w.niter2 = qval[ci] <= 1 ? 0 : niter;                          /* 2501 */
-			if (qval[ci] >= 0x800 && ci < static_stop_ci) static_stop_ci = ci;
-			if (w.niter2 + w.extra == 0) continue;                         /* 2542 */
-			if (ci >= static_stop_ci) {                                    /* 2551-2566 */
-				CK(qs_launch_scale_clamp(w.coef_dev, (size_t)w.W * w.H * 64, ctx->quant_dev + w.qslot, 1, 0, st));
-				ctx->launches++;
-				continue;
-			}
-			if (!(w.W * w.H)) continue;
-			w.iterate = true;
-			works.push_back(&w);
-		}
+		for (int ci = c0; ci < c1; ci++) if (comp_prelude(ctx, s, W[ci], niter, st, works)) return JPEGQS_ERR_CUDA;
 		int max_pass = 0;
 		for (CompWork *w : works) max_pass = std::max(max_pass, w->niter2 + w->extra);
-		auto p2_of = [&](const CompWork *w) -> const uint8_t * {
-			return (image2 && (flags & QS_JOINT_YUV) && w->ci > 0) ? image2 : NULL;
-		};
 		for (int iter = 0; iter < max_pass; iter++) {
 			std::vector<XchgPlane> xp;
-			for (int clampv = 0; clampv < 2; clampv++) {                   /* IDCT pass, 2589-2620 (+ final clamp) */
-				std::vector<QsJob> jobs;
-				for (CompWork *w : works) {
-					if (iter >= w->niter2 + w->extra) continue;
-					if (((iter == w->niter2) ? 1 : 0) != clampv) continue;
-					jobs.push_back(make_job(*w, NULL));
-					xp.push_back({ w->plane, w->W, w->H });
-				}
-				if (jobs.empty()) continue;
-				const QsJob *jd; int tiles;
-				if (upload_jobs(ctx, 0, jobs, st, &jd, &tiles, true)) return JPEGQS_ERR_CUDA;
-				int mode = (iter == 0 ? QS_IDCT_DEQUANT : 0) | (clampv ? QS_IDCT_CLAMP : 0);
-				if (prof_begin(ctx, 0, st)) return JPEGQS_ERR_CUDA;
-				CK(qs_launch_idct_pass(jd, (int)jobs.size(), tiles, mode, bad_dev, st));
-				if (prof_end(ctx, st)) return JPEGQS_ERR_CUDA;
-				ctx->launches++;
-			}
+			if (idct_pass(ctx, r.S, works, iter, bad_dev, st, [&](const std::vector<CompWork *> &who) -> int {
+					for (CompWork *w : who) xp.push_back({ w->plane, w->W, w->H });
+					return 0;
+				})) return JPEGQS_ERR_CUDA;
 			/* halo rows from the neighbours; the first exchange of a phase also ORs the flags */
 			if ((!xp.empty() || iter == 0) && slab_exchange(ctx, link, xp, bad_dev, iter == 0 ? nc : 0, st)) return JPEGQS_ERR_CUDA;
-			for (int clampv = 0; clampv < 2; clampv++) {                   /* smoothing pass, 2627-2640 */
-				std::vector<QsJob> jobs;
-				for (CompWork *w : works) {
-					if (iter >= w->niter2) continue;
-					if (((iter == w->niter2 - 1 && !w->extra) ? 1 : 0) != clampv) continue;
-					jobs.push_back(make_job(*w, p2_of(w)));
-				}
-				if (jobs.empty()) continue;
-				const QsJob *jd; int tiles;
-				if (upload_jobs(ctx, 1, jobs, st, &jd, &tiles, true)) return JPEGQS_ERR_CUDA;
-				if (prof_begin(ctx, 1, st)) return JPEGQS_ERR_CUDA;
-				if (flags & QS_LOW_QUALITY) CK(qs_launch_lowq(jd, (int)jobs.size(), tiles, flags, clampv, bad_dev, st));
-				else CK(qs_launch_smooth(jd, (int)jobs.size(), tiles, tabs, tile_counter, flags, clampv, ctx->num_sms,
-						ctx->tune_sync, ctx->tune_wpg, bad_dev, st));
-				if (prof_end(ctx, st)) return JPEGQS_ERR_CUDA;
-				ctx->launches++;
-			}
+			if (smooth_pass(ctx, r.S, works, iter, flags, bad_dev, st)) return JPEGQS_ERR_CUDA;
 		}
 		{	/* the component that overflowed is clamped only (2602-2610, 2670-2689); on the device */
 			std::vector<QsJob> jobs;
-			for (CompWork *w : works) jobs.push_back(make_job(*w, NULL));
+			for (CompWork *w : works) jobs.push_back(run_job(ctx, s, *w, NULL, bad_dev));
 			if (!jobs.empty()) {
 				const QsJob *jd; int tiles;
 				if (upload_jobs(ctx, 0, jobs, st, &jd, &tiles, true)) return JPEGQS_ERR_CUDA;
@@ -1582,39 +1543,8 @@ static int run_slab(jpegqs_cuda_ctx *ctx, jpegqs_cuda_link *link, jpegqs_cuda_im
 				ctx->launches++;
 			}
 		}
-		/* post steps: chroma up-sampling (2691-2752), luma planes (2753-2815); results are dropped
-		 * at the end if the run stopped */
-		for (CompWork *w : works) {
-			if (w->ci > 0 && image1 && w->ci <= 2) {
-				int ws = im->comp[0].h_samp, hs = im->comp[0].v_samp;
-				int w1 = ((int)im->image_width + ws - 1) / ws, h1 = ((int)im->image_height + hs - 1) / hs;
-				int W0 = im->comp[0].wblk, H0 = im->comp[0].hblk;
-				CK(qs_launch_upsample(w->plane, image2, QS_PLANE_STRIDE(w->W), image1, QS_PLANE_STRIDE(W0),
-						mem_buf[w->ci - 1], W0 * 8, w1, h1, ws, hs, W0 * 8, H0 * 8, (int)geom->row0[0] * 8, st));
-				CK(qs_launch_fdct_plane(mem_buf[w->ci - 1], W0 * 8, coef_up_dev[w->ci - 1], W0, H0, st));
-				ctx->launches += 2;
-			} else if (w->ci == 0 && need_ds) {
-				int ws = w->c->h_samp, hs = w->c->v_samp;
-				if (ws == 1 && hs == 1) image2 = w->plane;
-				else {
-					if (flags & QS_UPSAMPLE_UV) image1 = w->plane;
-					const jpegqs_cuda_comp *cc = &im->comp[1];
-					int h = (int)geom->hblk_total[0] * 8, h2 = (int)geom->hblk_total[1] * 8, h1_total = (h + hs - 1) / hs;
-					int first = top ? -1 : (int)geom->row0[1] * 8;
-					int last = bottom ? h2 : (int)(geom->row0[1] + cc->hblk) * 8 - 1;
-					int dstride = QS_PLANE_STRIDE(cc->wblk);
-					if (last >= first) {
-						CK(qs_launch_downsample(w->plane, QS_PLANE_STRIDE(w->W), w->W * 8, h,
-								image2_buf + (size_t)(first - (int)geom->row0[1] * 8 + 1) * dstride, dstride, (int)cc->wblk * 8, h2,
-								ws, hs, (int)geom->row0[0] * 8, first, last - first + 1, h1_total, st));
-						ctx->launches++;
-					}
-					image2 = image2_buf;
-					std::vector<XchgPlane> xp; xp.push_back({ image2_buf, (int)cc->wblk, (int)cc->hblk });
-					if (slab_exchange(ctx, link, xp, bad_dev, 0, st)) return JPEGQS_ERR_CUDA;
-				}
-			}
-		}
+		/* post steps; their results are dropped at the end if the run stopped */
+		for (CompWork *w : works) if (post_step(ctx, s, *w, flags, link, st)) return JPEGQS_ERR_CUDA;
 		if (!on_device) {                                                  /* downloads of this phase, band by band */
 			CK(cudaEventRecord(ctx->sync_ev[2 * g + 1], st));
 			for (int k = 0; k < nbands[g]; k++) {
@@ -1623,10 +1553,9 @@ static int run_slab(jpegqs_cuda_ctx *ctx, jpegqs_cuda_link *link, jpegqs_cuda_im
 					CompWork &w = W[ci];
 					int r0 = (int)((long)k * w.H / nbands[g]), r1 = (int)((long)(k + 1) * w.H / nbands[g]);
 					if (w.W && r1 > r0) segs.push_back(seg_of(w, r0, r1));
-					if (image1 && ci >= 1 && ci <= 2) {
+					if (s.image1 && ci >= 1 && ci <= 2) {
 						int H0 = (int)im->comp[0].hblk;
-						IoSeg sg; sg.dev = coef_up_dev[ci - 1]; sg.pin = w.pin_up; sg.rows = w.rows_up;
-						sg.wblk = im->comp[0].wblk; sg.r0 = (int)((long)k * H0 / nbands[g]); sg.r1 = (int)((long)(k + 1) * H0 / nbands[g]);
+						IoSeg sg = seg_up_of(s, w, (int)((long)k * H0 / nbands[g]), (int)((long)(k + 1) * H0 / nbands[g]));
 						if (sg.r1 > sg.r0) segs.push_back(sg);
 					}
 				}
@@ -1641,20 +1570,15 @@ static int run_slab(jpegqs_cuda_ctx *ctx, jpegqs_cuda_link *link, jpegqs_cuda_im
 	if (link && *link->timeout_host) {
 		int *t = link->timeout_host;
 		snprintf(ctx->err, sizeof(ctx->err), "sharded run: rank %d of %d waited 10 s for %s %d: sequence %d expected, %d found "
-				"(its own count: %u)", rank, world, t[1] > 32 ? "the mask message of peer" : "the halo rows of neighbour", 
+				"(its own count: %u)", rank, world, t[1] > 32 ? "the mask message of peer" : "the halo rows of neighbour",
 				t[1] > 32 ? t[1] - 33 : t[1] - 1, t[2], t[3], link->seq);
 		memset(t, 0, 4 * sizeof(int));
 		return JPEGQS_ERR_TIMEOUT;
 	}
-	int stop = static_stop_ci < (1 << 30) ? 1 : 0;
-	for (int ci = 0; ci < nc; ci++) if (W[ci].iterate && ctx->flags_host[ci]) stop = 1;
-	/* NOTE on upsampled chroma when the run stopped: coef_up holds data nobody will look at */
-	for (int ci = 0; ci < nc; ci++) if (im->comp[ci].has_qtbl) for (int k = 0; k < 64; k++) im->comp[ci].quant[k] = 1;
-	im->upsampled = (image1 && !stop) ? 1 : 0;
-	if (ret) *ret = stop;
-	CK(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
-	if (prof_collect(ctx)) return JPEGQS_ERR_CUDA;
-	return 0;
+	/* `stop`: raised by a quant value (s.stop) or by an out-of-range coefficient on some rank.
+	 * NOTE on upsampled chroma when the run stopped: coef_up holds data nobody will look at */
+	for (int ci = 0; ci < nc; ci++) if (W[ci].iterate && ctx->flags_host[ci]) s.stop = 1;
+	return run_results(ctx, r, ret);
 }
 
 extern "C" int jpegqs_cuda_run_slab(jpegqs_cuda_ctx *ctx, jpegqs_cuda_link *link, jpegqs_cuda_image *slab,
@@ -1827,12 +1751,9 @@ static int stage_jobs(jpegqs_cuda_ctx *ctx, int njobs, const jpegqs_cuda_job *jo
 	std::vector<QsQuantDev> q(njobs); std::vector<QsJob> v(njobs);
 	for (int i = 0; i < njobs; i++) {
 		int val; quant_prepare(jobs[i].quant, &q[i], &val, ctx->tune_maxn, ctx->tune_uni, ctx->tune_merge);
-		QsJob &j = v[i]; memset(&j, 0, sizeof(j));
-		j.coef = jobs[i].coef; j.plane = jobs[i].plane; j.plane2 = jobs[i].plane2;
-		j.quant = ctx->quant_dev + i;
-		j.wblk = jobs[i].wblk; j.hblk = jobs[i].hblk; j.stride = QS_PLANE_STRIDE(j.wblk);
-		j.nblocks = j.wblk * j.hblk; j.luma = jobs[i].luma;
-		j.top_edge = jobs[i].top_edge; j.bottom_edge = jobs[i].bottom_edge;
+		CompWork w; memset(&w, 0, sizeof(w));
+		w.coef_dev = jobs[i].coef; w.plane = jobs[i].plane; w.W = jobs[i].wblk; w.H = jobs[i].hblk; w.luma = jobs[i].luma; w.qslot = i;
+		v[i] = make_job(ctx, w, jobs[i].plane2, 0, w.H, jobs[i].top_edge, jobs[i].bottom_edge);
 	}
 	assign_sched_slots(q.data(), njobs);
 	if (njobs) CK(cudaMemcpyAsync(ctx->quant_dev, q.data(), njobs * sizeof(QsQuantDev), cudaMemcpyHostToDevice, st));
@@ -1946,10 +1867,9 @@ extern "C" int jpegqs_cuda_render_rgb(jpegqs_cuda_ctx *ctx, const jpegqs_cuda_im
 		}
 		uint8_t *pl = (uint8_t *)arena_take(ctx, QS_PLANE_BYTES(cc->wblk, cc->hblk));
 		quant_prepare(cc->quant, &q[c], &val);
-		QsJob j; memset(&j, 0, sizeof(j));
-		j.coef = cd; j.plane = pl; j.quant = ctx->quant_dev + c;
-		j.wblk = cc->wblk; j.hblk = cc->hblk; j.stride = QS_PLANE_STRIDE(cc->wblk); j.nblocks = cc->wblk * cc->hblk;
-		j.top_edge = j.bottom_edge = 1;
+		CompWork w; memset(&w, 0, sizeof(w));
+		w.coef_dev = cd; w.plane = pl; w.W = cc->wblk; w.H = cc->hblk; w.qslot = c;
+		QsJob j = make_job(ctx, w, NULL, 0, w.H, 1, 1);
 		/* tables that are not all ones: the coefficients are still quantized (plain decode).
 		 * NOTE: on_device coefficients are de-quantized in place in that case. */
 		jobs[cc->has_qtbl && val > 1 ? 1 : 0].push_back(j);
