@@ -12,6 +12,13 @@ reference built into oracle/_ref by oracle/Makefile:
   ref_files.json      SHA-256 of the files the reference tools write for the JPEG files the
                       CLI tests generate (tests/test_cli.py, tests/test_real_libjpeg.py) and of
                       the lossless transcodes of tools/codec_difftest.py
+  ref_saturated.npz   the reference's results on small saturated-content images
+  ref_saturated.json  golden_io.result_digest of its results on wave-scale saturated-content
+                      images (tests/hard_content.py; tests/test_oracle_vs_reference.py)
+
+An archive is only rewritten when its arrays change (numpy stamps each member with the time it
+was written), so regenerating leaves unchanged files byte-identical.  Name parts to regenerate
+only those: kernels, driver, files, saturated.
 
 Inputs are not stored: every test regenerates them from its seed (numpy RandomState, Pillow).
 """
@@ -32,6 +39,15 @@ import jpegqs_b200 as qs          # noqa: E402
 import oracle_lib as ol           # noqa: E402
 import golden_io as gio           # noqa: E402
 REFDIR = os.path.join(ROOT, "oracle", "_ref")
+
+
+def _save_npz(path, d):
+    if os.path.exists(path):
+        with np.load(path) as z:
+            if sorted(z.files) == sorted(d) and all(np.array_equal(z[k], np.asarray(d[k])) and
+                                                    z[k].dtype == np.asarray(d[k]).dtype for k in d):
+                return
+    np.savez_compressed(path, **d)
 
 
 def kernels():
@@ -62,7 +78,7 @@ def kernels():
         a = np.zeros((64, size), dtype=np.float32)
         assert ref.qsref_tables(flags, a.ctypes.data) == size
         d[f"tables{flags}"] = a
-    np.savez_compressed(os.path.join(HERE, "ref_kernels.npz"), **d)
+    _save_npz(os.path.join(HERE, "ref_kernels.npz"), d)
 
 
 def driver():
@@ -91,8 +107,21 @@ def driver():
     for case in te.ENTRY_CASES:
         flags, niter, ss = case
         gio.put_result(e, tv.case_key("entry", case), *ol.run_reference(qs.synth.make_image(120, 72, ss), flags, niter, scatter_rows=True))
-    np.savez_compressed(os.path.join(HERE, "ref_driver.npz"), **d)
-    np.savez_compressed(os.path.join(HERE, "ref_sweep.npz"), **e)
+    _save_npz(os.path.join(HERE, "ref_driver.npz"), d)
+    _save_npz(os.path.join(HERE, "ref_sweep.npz"), e)
+
+
+def saturated():
+    import test_oracle_vs_reference as tv
+    d = {}
+    for case in tv.SATURATED_SMALL:
+        gio.put_result(d, tv.case_key("sat", case), *ol.run_reference(*tv.saturated_case(case)))
+    _save_npz(os.path.join(HERE, "ref_saturated.npz"), d)
+    digests = {tv.case_key("satw", case): gio.result_digest(*ol.run_reference(*tv.saturated_case(case)))
+               for case in tv.SATURATED_WAVE}
+    with open(os.path.join(HERE, "ref_saturated.json"), "w") as f:
+        json.dump(digests, f, indent=1, sort_keys=True)
+        f.write("\n")
 
 
 def _sha(path):
@@ -125,6 +154,6 @@ def files():
 if __name__ == "__main__":
     ol.ensure_built()
     assert ol.have_ref("scalar"), "needs oracle/_ref (make -C oracle ref with the reference sources)"
-    kernels()
-    driver()
-    files()
+    parts = sys.argv[1:] or ["kernels", "driver", "files", "saturated"]
+    for part in parts:
+        {"kernels": kernels, "driver": driver, "files": files, "saturated": saturated}[part]()

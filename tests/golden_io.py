@@ -1,4 +1,5 @@
 """Load/save golden cases and build the adversarial inputs used by the edge-case tests."""
+import hashlib
 import json
 import os
 
@@ -97,13 +98,33 @@ def reference(name):
 
 def reference_result(key, like):
     """(ret, image) the reference returned for `key`; `like` (the input) gives the geometry."""
-    z = next(z for z in map(reference, ("ref_driver", "ref_sweep")) if f"{key}.ret" in z)
+    z = next(z for z in map(reference, ("ref_driver", "ref_sweep", "ref_saturated")) if f"{key}.ret" in z)
     comps = []
     for i, c in enumerate(like.comps):
         s = z[f"{key}.samp{i}"]
         q = z.get(f"{key}.quant{i}")
         comps.append(Component(z[f"{key}.coef{i}"].copy(), None if q is None else q.copy(), int(s[0]), int(s[1]), int(s[2])))
     return int(z[f"{key}.ret"]), CoefImage(like.width, like.height, like.colorspace, comps)
+
+
+def result_digest(ret, im):
+    """SHA-256 of one do_quantsmooth result: return value, then per component the coefficients,
+    the sampling factors and the quant table."""
+    h = hashlib.sha256(np.array(ret, dtype=np.int32).tobytes())
+    for c in im.comps:
+        h.update(np.ascontiguousarray(c.coef, dtype=np.int16).tobytes())
+        h.update(np.array([c.h_samp, c.v_samp], dtype=np.int32).tobytes())
+        if c.quant is not None:
+            h.update(np.asarray(c.quant, dtype=np.uint16).tobytes())
+    return h.hexdigest()
+
+
+def reference_digests():
+    """tests/golden/reference/ref_saturated.json: result_digest of the reference's results."""
+    if "digests" not in _stored:
+        with open(os.path.join(GOLDEN, "ref_saturated.json")) as f:
+            _stored["digests"] = json.load(f)
+    return _stored["digests"]
 
 
 def reference_files():

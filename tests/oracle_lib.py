@@ -218,8 +218,9 @@ class QsoImage(C.Structure):
                 ("image_height", C.c_uint32), ("comp", QsoComp * 4), ("upsampled", C.c_int)]
 
 
-def run_oracle(image, flags, niter, progprec=0, progress=None, threads=0):
-    """The C restatement on flat arrays.  Returns (ret, result_image)."""
+def run_oracle(image, flags, niter, progprec=0, progress=None, threads=0, with_upsampled=False):
+    """The C restatement on flat arrays.  Returns (ret, result_image), and with_upsampled=True
+    also whether the chroma came back up-sampled: (ret, result_image, upsampled)."""
     from jpegqs_b200.image import JCS_YCbCr
     lib = oraclelib()
     lib.qso_set_threads(threads)
@@ -254,6 +255,8 @@ def run_oracle(image, flags, niter, progprec=0, progress=None, threads=0):
             c.h_samp = c.v_samp = 1
         if c.quant is not None:
             c.quant = np.array(list(qi.comp[i].quant), dtype=np.uint16)
+    if with_upsampled:
+        return ret, out, bool(qi.upsampled)
     return ret, out
 
 

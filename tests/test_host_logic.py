@@ -122,3 +122,83 @@ def test_chunk_schedule_covers_every_coefficient_once():
     assert len(cuda.chunk_schedule(None, 4, False, False)) == 25
     merged = cuda.chunk_schedule(None, 4, False, True)
     assert sum(typ == 3 for typ, _, _ in merged) == 6 and sum(typ == 1 for typ, _, _ in merged) == 1   # s = 2..7 merged, s = 1 has no full coefficient
+
+
+# ---- launch geometry of the smoothing kernel (tests/wave_geometry.py) ------------------------
+def test_wave_geometry_known_figures():
+    import wave_geometry as wg
+    # 7680x4320 4:2:0 q3 on the device entry point: luma + both chroma in one launch per iteration
+    im = wg.geometry(7680, 4320, "420")
+    launches = wg.smooth_launches(im, 0, 2, "device", 132)
+    assert [l.tiles for l in launches] == [24300, 24300]       # 16200 + 2 * 4050 warp tiles
+    assert (launches[0].grid, launches[0].a_tiles, launches[0].left) == (132, 5808, 1068)
+    assert wg.regimes(launches) == {"dynamic+tail"}
+    # 1920x1080 4:2:0 is below one wave (16 * 132 warp tiles): the tail only, whatever the route
+    for route in ("device", "host", "slab_device", "slab_host"):
+        ls = wg.smooth_launches(wg.geometry(1920, 1080, "420"), 0, 3, route, 132)
+        assert ls and wg.regimes(ls) == {"tail"}
+    assert [l.tiles for l in wg.smooth_launches(wg.geometry(1920, 1080, "420"), 0, 1, "device", 132)] == [1523]
+    # 512x512 gray: 128 warp tiles on 8 CTAs, four whole rounds of 32 group tiles, no tail
+    ls = wg.smooth_launches(wg.geometry(512, 512, "gray"), 0, 3, "device", 132)
+    assert [(l.grid, l.a_tiles, l.left, l.regime) for l in ls] == [(8, 32, 0, "rounds")] * 3
+
+
+def test_wave_geometry_launch_forming():
+    import wave_geometry as wg
+    im = wg.geometry(7680, 4320, "420")
+    # JOINT_YUV: luma phase, then chroma phase; the luma's last pass is the extra IDCT pass
+    ls = wg.smooth_launches(im, 3, 2, "device", 132)
+    assert [[(j.ci, j.tiles) for j in l.jobs] for l in ls] == [[(0, 16200)]] * 2 + [[(1, 4050), (2, 4050)]] * 2
+    assert [l.jobs[-1].sig[1] for l in ls] == [True, True, False, False]     # chroma has the predictor
+    # the host entry point cuts the luma phase into one-wave slabs for iteration 0 only (the
+    # luma is not the last phase), and the chroma phase's last iteration
+    ls = wg.smooth_launches(im, 0, 2, "host", 132)
+    assert [l.tiles for l in ls] == [2010, 2040] * 4 + [16200, 8100] + [2010, 2040] * 2
+    assert all(l.tiles <= 16 * 132 for l in ls if l.tiles != 16200 and l.tiles != 8100)
+    assert [l.tiles for l in wg.smooth_launches(im, 0, 2, "host", 132, slabs=False)] == [16200, 16200, 8100, 8100]
+    # gray: one phase, iteration 0 and the last iteration slabbed, the middle one whole
+    ls = wg.smooth_launches(wg.geometry(4096, 4096, "gray"), 0, 3, "host", 132)
+    assert len(ls) == 2 * 4 + 1 and ls[4].tiles == 512 * 512 // 32
+    # LOW_QUALITY has no persistent schedule; a quant value >= 0x800 stops the components from there
+    assert wg.smooth_launches(im, 8, 2, "device", 132) == []
+    big = wg.geometry(7680, 4320, "420")
+    big.comps[1].quant = big.comps[1].quant.copy()
+    big.comps[1].quant[63] = 0x800
+    assert [[j.ci for j in l.jobs] for l in wg.smooth_launches(big, 0, 1, "device", 132)] == [[0]]
+
+
+def test_wave_geometry_mixed_group_tiles():
+    import wave_geometry as wg
+    from hard_content import TABLES
+    J = wg.Job
+    # a job boundary inside a dynamic group tile mixes it only if the signatures differ
+    jobs = [J(0, 0, 32 * 4 * 300 + 64, ("a", True)), J(0, 1, 32 * 4 * 300, ("b", True))]
+    l = wg.Launch(jobs, 132)
+    assert l.a_tiles > 300 and l.mixed == [300]
+    jobs[1].sig = ("a", True)
+    assert wg.Launch(jobs, 132).mixed == []
+    jobs[1].sig = ("a", False)                               # the JOINT_YUV predictor changes the signature
+    assert wg.Launch(jobs, 132).mixed == [300]
+    # equal tables share a schedule; the Annex-K luma and chroma tables' schedules differ
+    assert wg.sched_key(TABLES["k50"][0]) != wg.sched_key(TABLES["k50"][1])
+    assert wg.sched_key(TABLES["flat"][0]) == wg.sched_key(TABLES["flat"][1])
+
+
+def test_hard_content_is_saturated_and_deterministic():
+    import hard_content as hc
+    for ss in hc.SAMPLINGS:
+        a = hc.make_image(136, 88, ss, hc.TABLES["k50"], "saturated", seed=4, chunk_rows=64)
+        b = hc.make_image(136, 88, ss, hc.TABLES["k50"], "saturated", seed=4, chunk_rows=3)
+        assert _digest(a) == _digest(b)
+        s = hc.make_image(136, 88, ss, hc.TABLES["k50"], "synth", seed=4)
+        assert _digest(s) == _digest(qs.synth.make_image(136, 88, ss, quality=50, seed=4))
+    px = hc.saturated_pixels(0, 0, 96, 200, 1, 1, 4, 96, 200)
+    assert px.min() == 0 and px.max() == 255 and np.mean((px == 0) | (px == 255)) > 0.4
+    # a letterbox block: DC -1024 at q = 1, which the final clamp must bring to -1023
+    im = hc.make_image(64, 64, "gray", hc.flat(1), "saturated")
+    assert im.comps[0].coef[0, 0, 0] == -1024
+    for stop in (False, True):
+        e = hc.with_dequant_edge(hc.make_image(96, 64, "420", hc.TABLES["k90"], "saturated"), stop)
+        d = e.comps[1].coef.astype(np.int32) * e.comps[1].quant.astype(np.int32)
+        assert d.max() == (2048 if stop else 2047) and d.min() == -2048
+        assert e.comps[1].quant_tbl_no == 2
