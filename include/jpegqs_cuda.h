@@ -120,6 +120,54 @@ int jpegqs_cuda_run_device(jpegqs_cuda_ctx *ctx, jpegqs_cuda_image *img, int fla
 int jpegqs_cuda_run_batch(jpegqs_cuda_ctx *ctx, int nimages, jpegqs_cuda_image *imgs, int flags,
 		int niter, int on_device, int *ret, void *stream);
 
+/* ---- stream-ordered, graph-capturable run over device buffers ---------------------------
+ * What jpegqs_cuda_run_batch(on_device = 1) computes, for a caller that keeps its data on the GPU
+ * and its host thread free:
+ *   - comp[].coef / coef_up are DEVICE pointers on the context's device; rows / rows_up must be
+ *     NULL.  No progress callback.
+ *   - Nothing is read back and nothing waits: the call returns once all its work is enqueued on
+ *     stream (NULL: the context's stream).  status_dev[i] (device memory) receives image i's
+ *     {stop, upsampled} on the stream - the values run_device returns and puts in img->upsampled;
+ *     img->upsampled is left at 0 here.  quant[] is set to 1 on return, as by the other entry
+ *     points (it does not depend on the data).
+ *   - Argument errors change nothing: every check runs before the first enqueue and a failed one
+ *     returns JPEGQS_ERR_ARG with nothing enqueued.  Checked: workspace too small or not 256-byte
+ *     aligned, status_dev NULL, malformed geometry (ncomp outside 1..10, a sampling factor outside
+ *     1..4, a non-empty component without coef, unequal chroma components where JOINT_YUV /
+ *     UPSAMPLE_UV down-sample the luma - whatever niter is), and coef_up missing where UPSAMPLE_UV
+ *     can trigger.  A CUDA error while enqueueing returns JPEGQS_ERR_CUDA.
+ *   - All per-call device state lives in the workspace: sample planes, the down-sampled luma, the
+ *     up-sampled chroma planes, quant constants, job lists, out-of-range flags and the tile
+ *     counter.  The call writes all of it earlier in its own stream work than anything reads it, so
+ *       . the next call on the same stream may reuse the workspace without clearing it;
+ *       . two calls on different streams of one context, with separate workspaces, may be in
+ *         flight together;
+ *       . a CUDA graph captured around the call replays correctly: a replay re-runs the call on
+ *         the current contents of the same coefficient, coef_up, workspace and status buffers,
+ *         with the geometry, quant tables, flags and niter fixed at capture.
+ *   - Host memory is released at return: job lists and quant constants travel as kernel
+ *     parameters, and the call reads nothing of imgs afterwards.
+ *   - No cudaMalloc, no synchronisation, no event query or record: the call is legal under
+ *     cudaStreamCaptureModeGlobal (what torch.cuda.graph uses).  So jpegqs_cuda_last_device_ms
+ *     keeps its value and profiling is ignored; jpegqs_cuda_last_launches counts the launches.
+ *   - Batches of more than 1024 components run as sub-batches one after another on the stream.
+ *   - As everywhere: one calling thread per context at a time.
+ * Returns 0 or a negative error. */
+typedef struct { int32_t stop, upsampled; } jpegqs_cuda_status;
+
+/* Device bytes of workspace jpegqs_cuda_run_async needs for these images and flags (host-only, no
+ * device needed; checks the geometry as jpegqs_cuda_run_async does, not the pointers).  With
+ * A(x) = x rounded up to a multiple of 256 and C = the number of components of all images:
+ *   168192 + A(1544 * C)                             flags + tile counter, job lists, quant constants
+ *   + for every component:  A(jpegqs_cuda_plane_bytes(wblk, hblk))       its sample plane
+ *   + for every image whose chroma JOINT_YUV / UPSAMPLE_UV feed from a down-sampled luma (YCbCr,
+ *     >= 3 components, components 1 and 2 sampled 1x1, component 0 not):
+ *       A(jpegqs_cuda_plane_bytes(comp[1].wblk, comp[1].hblk))          the down-sampled luma
+ *       + with UPSAMPLE_UV: 2 * A(comp[0].wblk * comp[0].hblk * 64)     the up-sampled chroma   */
+int jpegqs_cuda_async_workspace_bytes(int nimages, const jpegqs_cuda_image *imgs, int flags, size_t *bytes);
+int jpegqs_cuda_run_async(jpegqs_cuda_ctx *ctx, int nimages, jpegqs_cuda_image *imgs, int flags, int niter,
+		void *workspace, size_t workspace_bytes, jpegqs_cuda_status *status_dev, void *stream);
+
 /* ---- one image sharded by MCU rows over several GPUs (SURVEY.md 8e) ----------------------
  * Every rank - a device of this process, or another process on the same box - smooths one slab
  * of contiguous MCU rows and exchanges ONE pixel row per plane with each neighbour after every

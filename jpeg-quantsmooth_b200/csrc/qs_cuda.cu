@@ -184,6 +184,9 @@ struct jpegqs_cuda_ctx {
 	int *flags_dev;                        /* [QS_MAX_JOBS] bad flags + [1] tile counter */
 	int *flags_host;                       /* pinned */
 	char *arena; size_t arena_cap, arena_pos;
+	/* inside jpegqs_cuda_run_async: arena, quant_dev, jobs_dev (+ jobs_cache) and flags_dev point
+	 * into the caller's workspace (WorkspaceScope) */
+	bool workspace;
 	cudaEvent_t ev0, ev1;
 	float last_ms; int launches;
 	/* optional per-kernel timing (bench.py's roofline line): event pairs around launches */
@@ -269,7 +272,7 @@ extern "C" int jpegqs_cuda_create(int device, jpegqs_cuda_ctx **out) {
 	}
 	ctx->tab_plain = ctx->tab_diag = NULL; ctx->quant_dev = NULL; ctx->quant_cap = 0;
 	ctx->jobs_dev = NULL; ctx->flags_dev = NULL; ctx->flags_host = NULL;
-	ctx->arena = NULL; ctx->arena_cap = ctx->arena_pos = 0; ctx->ev0 = ctx->ev1 = NULL;
+	ctx->arena = NULL; ctx->arena_cap = ctx->arena_pos = 0; ctx->workspace = false; ctx->ev0 = ctx->ev1 = NULL;
 	ctx->last_ms = 0; ctx->launches = 0;
 	ctx->profiling = 0; ctx->ev_used = 0; ctx->tune_sync = 2; ctx->tune_maxn = 4; ctx->tune_wpg = 4; ctx->tune_gs = 1; ctx->tune_uni = 1; ctx->tune_merge = 1; ctx->tune_slabs = 1; ctx->tune_wave = 0;
 	ctx->kernel_ms[0] = ctx->kernel_ms[1] = 0; ctx->kernel_launches[0] = ctx->kernel_launches[1] = 0;
@@ -659,6 +662,7 @@ struct ImgState {
 	 * hblk), or one rank's slab (run_slab); top / bottom: they include the image's first / last row */
 	jpegqs_cuda_slab geom;
 	bool top, bottom;
+	int flag0;             /* device-decided `stop`: slot of component 0 in the run's flags */
 };
 
 /* the per-call state of a smoothing run */
@@ -729,8 +733,16 @@ static int run_setup(jpegqs_cuda_ctx *ctx, int nimg, jpegqs_cuda_image *imgs, in
 		s.geom.rank = 0; s.geom.world = 1; s.top = s.bottom = true;
 		for (int ci = 0; ci < im->ncomp; ci++) s.geom.hblk_total[ci] = im->comp[ci].hblk;
 	}
-	if (arena_reserve(ctx, bytes + 4096)) return JPEGQS_ERR_CUDA;
-	if (quant_reserve(ctx, nquant)) return JPEGQS_ERR_CUDA;
+	if (ctx->workspace) {
+		/* the caller's workspace: jpegqs_cuda_run_async has sized it for the whole call */
+		if (ctx->arena_pos + bytes > ctx->arena_cap || nquant > ctx->quant_cap) {
+			snprintf(ctx->err, sizeof(ctx->err), "workspace too small");
+			return JPEGQS_ERR_ARG;
+		}
+	} else {
+		if (arena_reserve(ctx, bytes + 4096)) return JPEGQS_ERR_CUDA;
+		if (quant_reserve(ctx, nquant)) return JPEGQS_ERR_CUDA;
+	}
 	if (stage_bytes && stage_reserve(ctx, stage_bytes)) return JPEGQS_ERR_CUDA;
 	size_t stage_pos = 0;
 	auto stage_take = [&](size_t b) { char *p = ctx->stage + stage_pos; stage_pos += align256(b); return (int16_t *)p; };
@@ -781,7 +793,9 @@ static int run_setup(jpegqs_cuda_ctx *ctx, int nimg, jpegqs_cuda_image *imgs, in
 		}
 	}
 	assign_sched_slots(qhost.data(), (int)qhost.size());
-	if (!qhost.empty())
+	/* a workspace run leaves nothing on the host to be read after it returns: kernel parameters */
+	if (!qhost.empty() && ctx->workspace) CK(qs_store_quant(ctx->quant_dev, qhost.data(), (int)qhost.size(), st));
+	else if (!qhost.empty())
 		CK(cudaMemcpyAsync(ctx->quant_dev, qhost.data(), qhost.size() * sizeof(QsQuantDev), cudaMemcpyHostToDevice, st));
 	ctx->jobs_cache[0].clear(); ctx->jobs_cache[1].clear();
 	return 0;
@@ -835,12 +849,12 @@ static QsJob make_job(jpegqs_cuda_ctx *ctx, const CompWork &w, const uint8_t *pl
 
 /* The job of all rows a run holds of a component.  stop_flags == NULL: the host decides the
  * reference's `stop` (run_images), and a launch's out-of-range flags are slots 0.. of its jobs.
- * Otherwise stop_flags holds the run's flags, one per component, and the kernels decide `stop`
- * from them (QsJob.stop_aware, run_slab). */
+ * Otherwise stop_flags holds the run's flags, one per component from the image's s.flag0 on, and
+ * the kernels decide `stop` from them (QsJob.stop_aware, run_slab and run_async_images). */
 static QsJob run_job(jpegqs_cuda_ctx *ctx, const ImgState &s, const CompWork &w, const uint8_t *plane2,
 		const int *stop_flags) {
 	QsJob j = make_job(ctx, w, plane2, 0, w.H, s.top, s.bottom);
-	if (stop_flags) { j.bad_slot = w.ci; j.bad_first = 0; j.stop_aware = 1; }
+	if (stop_flags) { j.bad_slot = s.flag0 + w.ci; j.bad_first = s.flag0; j.stop_aware = 1; }
 	return j;
 }
 
@@ -981,8 +995,8 @@ static int post_step(jpegqs_cuda_ctx *ctx, ImgState &s, const CompWork &w, int f
 }
 
 /* results, quantsmooth.h:2834-2859: quant tables of the smoothed components set to 1, upsampled,
- * the return values; device time and per-kernel timing of the run (ev1 recorded and complete) */
-static int run_results(jpegqs_cuda_ctx *ctx, RunSetup &r, int *ret) {
+ * the return values */
+static void host_results(RunSetup &r, int *ret) {
 	for (size_t n = 0; n < r.S.size(); n++) {
 		ImgState &s = r.S[n]; jpegqs_cuda_image *im = s.im;
 		if (ret) ret[n] = s.stop;
@@ -991,8 +1005,44 @@ static int run_results(jpegqs_cuda_ctx *ctx, RunSetup &r, int *ret) {
 			if (im->comp[ci].has_qtbl) for (int k = 0; k < 64; k++) im->comp[ci].quant[k] = 1;
 		im->upsampled = (s.image1 && !s.stop) ? 1 : 0;
 	}
+}
+/* the same plus device time and per-kernel timing of the run (ev1 recorded and complete) */
+static int run_results(jpegqs_cuda_ctx *ctx, RunSetup &r, int *ret) {
+	host_results(r, ret);
 	CK(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
 	return prof_collect(ctx);
+}
+
+/* One phase whose `stop` is decided on the device from the run's flags at bad_dev (run_job with
+ * stop_flags): the iterations over works - IDCT pass, the halo rows from the neighbours over link
+ * (none at world 1), smoothing pass -, the clamp of the components that overflowed, and the post
+ * steps, whose results are dropped at the end if their image stopped.  The first exchange also
+ * OR-combines bad_n flags over the ranks. */
+static int device_phase(jpegqs_cuda_ctx *ctx, RunSetup &r, const std::vector<CompWork *> &works, int flags,
+		jpegqs_cuda_link *link, int *bad_dev, int bad_n, cudaStream_t st) {
+	int max_pass = 0;
+	for (CompWork *w : works) max_pass = std::max(max_pass, w->niter2 + w->extra);
+	for (int iter = 0; iter < max_pass; iter++) {
+		std::vector<XchgPlane> xp;
+		if (idct_pass(ctx, r.S, works, iter, bad_dev, st, [&](const std::vector<CompWork *> &who) -> int {
+				for (CompWork *w : who) xp.push_back({ w->plane, w->W, w->H });
+				return 0;
+			})) return JPEGQS_ERR_CUDA;
+		if ((!xp.empty() || iter == 0) && slab_exchange(ctx, link, xp, bad_dev, iter == 0 ? bad_n : 0, st)) return JPEGQS_ERR_CUDA;
+		if (smooth_pass(ctx, r.S, works, iter, flags, bad_dev, st)) return JPEGQS_ERR_CUDA;
+	}
+	{	/* the component that overflowed is clamped only (2602-2610, 2670-2689); on the device */
+		std::vector<QsJob> jobs;
+		for (CompWork *w : works) jobs.push_back(run_job(ctx, r.S[w->img], *w, NULL, bad_dev));
+		if (!jobs.empty()) {
+			const QsJob *jd; int tiles;
+			if (upload_jobs(ctx, 0, jobs, st, &jd, &tiles, true)) return JPEGQS_ERR_CUDA;
+			CK(qs_launch_stop_fixup(jd, (int)jobs.size(), bad_dev, st));
+			ctx->launches++;
+		}
+	}
+	for (CompWork *w : works) if (post_step(ctx, r.S[w->img], *w, flags, link, st)) return JPEGQS_ERR_CUDA;
+	return 0;
 }
 
 /* ------------------------------------------------------------------------------------------
@@ -1521,30 +1571,8 @@ static int run_slab(jpegqs_cuda_ctx *ctx, jpegqs_cuda_link *link, jpegqs_cuda_im
 		int c0, c1; group_range(s, g, &c0, &c1);
 		std::vector<CompWork *> works;
 		for (int ci = c0; ci < c1; ci++) if (comp_prelude(ctx, s, W[ci], niter, st, works)) return JPEGQS_ERR_CUDA;
-		int max_pass = 0;
-		for (CompWork *w : works) max_pass = std::max(max_pass, w->niter2 + w->extra);
-		for (int iter = 0; iter < max_pass; iter++) {
-			std::vector<XchgPlane> xp;
-			if (idct_pass(ctx, r.S, works, iter, bad_dev, st, [&](const std::vector<CompWork *> &who) -> int {
-					for (CompWork *w : who) xp.push_back({ w->plane, w->W, w->H });
-					return 0;
-				})) return JPEGQS_ERR_CUDA;
-			/* halo rows from the neighbours; the first exchange of a phase also ORs the flags */
-			if ((!xp.empty() || iter == 0) && slab_exchange(ctx, link, xp, bad_dev, iter == 0 ? nc : 0, st)) return JPEGQS_ERR_CUDA;
-			if (smooth_pass(ctx, r.S, works, iter, flags, bad_dev, st)) return JPEGQS_ERR_CUDA;
-		}
-		{	/* the component that overflowed is clamped only (2602-2610, 2670-2689); on the device */
-			std::vector<QsJob> jobs;
-			for (CompWork *w : works) jobs.push_back(run_job(ctx, s, *w, NULL, bad_dev));
-			if (!jobs.empty()) {
-				const QsJob *jd; int tiles;
-				if (upload_jobs(ctx, 0, jobs, st, &jd, &tiles, true)) return JPEGQS_ERR_CUDA;
-				CK(qs_launch_stop_fixup(jd, (int)jobs.size(), bad_dev, st));
-				ctx->launches++;
-			}
-		}
-		/* post steps; their results are dropped at the end if the run stopped */
-		for (CompWork *w : works) if (post_step(ctx, s, *w, flags, link, st)) return JPEGQS_ERR_CUDA;
+		/* iterations with the neighbour exchanges, clamp fixup, post steps */
+		if (device_phase(ctx, r, works, flags, link, bad_dev, nc, st)) return JPEGQS_ERR_CUDA;
 		if (!on_device) {                                                  /* downloads of this phase, band by band */
 			CK(cudaEventRecord(ctx->sync_ev[2 * g + 1], st));
 			for (int k = 0; k < nbands[g]; k++) {
@@ -1587,6 +1615,156 @@ extern "C" int jpegqs_cuda_run_slab(jpegqs_cuda_ctx *ctx, jpegqs_cuda_link *link
 	if (!ctx) return JPEGQS_ERR_ARG;
 	int rc = run_slab(ctx, link, slab, geom, flags, niter, on_device != 0, &ret, stream ? (cudaStream_t)stream : ctx->stream);
 	return rc < 0 ? rc : ret;
+}
+
+/* ------------------------------------------------------------------------------------------
+ * Stream-ordered driver (jpegqs_cuda_run_async): whole images on device buffers, the phases of
+ * run_images and the device-decided `stop` of run_slab, so nothing is read back and nothing waits.
+ * All per-call device state lives in the caller's workspace, laid out as
+ *   [flags: QS_MAX_JOBS out-of-range flags + the tile counter] [two job-list slots]
+ *   [quant constants, one record per component of the call] [sample planes, as run_setup carves them]
+ * ------------------------------------------------------------------------------------------ */
+#define QS_WS_FLAGS_BYTES (((QS_MAX_JOBS + 1) * sizeof(int) + 255) & ~(size_t)255)
+#define QS_WS_JOBS_BYTES (2 * QS_MAX_JOBS * sizeof(QsJob))
+/* record sizes the formula in include/jpegqs_cuda.h states */
+static_assert(sizeof(QsJob) == 80 && QS_WS_FLAGS_BYTES + QS_WS_JOBS_BYTES == 168192, "jpegqs_cuda.h: fixed workspace part");
+static_assert(sizeof(QsQuantDev) == 1544, "jpegqs_cuda.h: quant record bytes");
+static_assert(sizeof(jpegqs_cuda_status) == sizeof(int2), "status record");
+
+/* The images of a run_async call, checked as run_setup checks them whatever niter will be (plus
+ * the sampling factors), and the workspace they need.  ptrs: also the pointers the run uses. */
+static int async_plan(int nimg, const jpegqs_cuda_image *imgs, int flags, bool ptrs, size_t *bytes, int *ncomp_total) {
+	if (nimg < 0 || (nimg && !imgs)) return JPEGQS_ERR_ARG;
+	size_t b = 0; int nq = 0;
+	for (int n = 0; n < nimg; n++) {
+		const jpegqs_cuda_image *im = &imgs[n];
+		if (im->ncomp < 1 || im->ncomp > JPEGQS_CUDA_MAX_COMP) return JPEGQS_ERR_ARG;
+		for (int ci = 0; ci < im->ncomp; ci++) {
+			const jpegqs_cuda_comp *c = &im->comp[ci];
+			if (c->h_samp < 1 || c->h_samp > 4 || c->v_samp < 1 || c->v_samp > 4) return JPEGQS_ERR_ARG;
+			if (ptrs && (c->rows || c->rows_up || (!c->coef && c->wblk && c->hblk))) return JPEGQS_ERR_ARG;
+			b += align256(QS_PLANE_BYTES(c->wblk, c->hblk));
+			nq++;
+		}
+		bool need_downsample = (flags & (QS_JOINT_YUV | QS_UPSAMPLE_UV)) && im->is_ycbcr && im->ncomp >= 3 &&
+				im->comp[1].h_samp == 1 && im->comp[1].v_samp == 1 && im->comp[2].h_samp == 1 && im->comp[2].v_samp == 1;
+		if (!need_downsample) continue;
+		if (im->comp[1].wblk != im->comp[2].wblk || im->comp[1].hblk != im->comp[2].hblk) return JPEGQS_ERR_ARG;
+		if (im->comp[0].h_samp == 1 && im->comp[0].v_samp == 1) continue;
+		b += align256(QS_PLANE_BYTES(im->comp[1].wblk, im->comp[1].hblk));          /* down-sampled luma */
+		if (flags & QS_UPSAMPLE_UV) for (int j = 1; j <= 2; j++) {
+			if (ptrs && !im->comp[j].coef_up) return JPEGQS_ERR_ARG;
+			b += align256((size_t)im->comp[0].wblk * im->comp[0].hblk * 64);       /* up-sampled pixel plane */
+		}
+	}
+	*bytes = QS_WS_FLAGS_BYTES + QS_WS_JOBS_BYTES + align256((size_t)nq * sizeof(QsQuantDev)) + b;
+	if (ncomp_total) *ncomp_total = nq;
+	return 0;
+}
+
+/* Points the context's per-call device state into the workspace for one run_async call, and gives
+ * the context its own memory back on every way out.  The run steps then use it unchanged; profiling
+ * events and last_device_ms are left alone (neither may be touched inside a graph capture). */
+struct WorkspaceScope {
+	jpegqs_cuda_ctx *ctx;
+	char *arena; size_t arena_cap, arena_pos;
+	QsQuantDev *quant_dev; int quant_cap;
+	QsJob *jobs_dev; int *flags_dev;
+	std::vector<QsJob> jobs_cache[2];
+	int profiling; float last_ms;
+	WorkspaceScope(jpegqs_cuda_ctx *c, char *ws, size_t bytes, int nquant) : ctx(c) {
+		arena = c->arena; arena_cap = c->arena_cap; arena_pos = c->arena_pos;
+		quant_dev = c->quant_dev; quant_cap = c->quant_cap; jobs_dev = c->jobs_dev; flags_dev = c->flags_dev;
+		profiling = c->profiling; last_ms = c->last_ms;
+		size_t qb = align256((size_t)nquant * sizeof(QsQuantDev));
+		c->flags_dev = (int *)ws;
+		c->jobs_dev = (QsJob *)(ws + QS_WS_FLAGS_BYTES);
+		c->quant_dev = (QsQuantDev *)(ws + QS_WS_FLAGS_BYTES + QS_WS_JOBS_BYTES); c->quant_cap = nquant;
+		c->arena = ws + QS_WS_FLAGS_BYTES + QS_WS_JOBS_BYTES + qb;
+		c->arena_cap = bytes - (QS_WS_FLAGS_BYTES + QS_WS_JOBS_BYTES + qb); c->arena_pos = 0;
+		for (int k = 0; k < 2; k++) jobs_cache[k].swap(c->jobs_cache[k]);   /* the workspace slots hold nothing yet */
+		c->profiling = 0; c->workspace = true;
+	}
+	~WorkspaceScope() {
+		ctx->arena = arena; ctx->arena_cap = arena_cap; ctx->arena_pos = arena_pos;
+		ctx->quant_dev = quant_dev; ctx->quant_cap = quant_cap; ctx->jobs_dev = jobs_dev; ctx->flags_dev = flags_dev;
+		for (int k = 0; k < 2; k++) jobs_cache[k].swap(ctx->jobs_cache[k]);
+		ctx->profiling = profiling; ctx->last_ms = last_ms; ctx->workspace = false;
+	}
+};
+
+/* one sub-batch (at most QS_MAX_JOBS components): phases over all images as in run_images, each
+ * image's flags from s.flag0 on, and at the end the status kernel instead of a read-back */
+static int run_async_images(jpegqs_cuda_ctx *ctx, int nimg, jpegqs_cuda_image *imgs, int flags, int niter,
+		jpegqs_cuda_status *status, cudaStream_t st) {
+	RunSetup r;
+	int rc = run_setup(ctx, nimg, imgs, flags, niter, true, st, r);
+	if (rc) return rc;
+	std::vector<ImgState> &S = r.S;
+	int nflags = 0, max_groups = 0;
+	for (ImgState &s : S) {
+		if (s.skip) continue;
+		s.flag0 = nflags; nflags += s.im->ncomp;
+		max_groups = std::max(max_groups, s.ngroups);
+	}
+	int *bad_dev = ctx->flags_dev;
+	if (nflags) CK(cudaMemsetAsync(bad_dev, 0, nflags * sizeof(int), st));
+	for (int g = 0; g < max_groups; g++) {
+		std::vector<CompWork *> works;
+		for (int n = 0; n < nimg; n++) {
+			ImgState &s = S[n];
+			if (s.skip || g >= s.ngroups) continue;
+			int c0, c1; group_range(s, g, &c0, &c1);
+			for (int ci = c0; ci < c1; ci++) if (comp_prelude(ctx, s, r.W[n][ci], r.niter, st, works)) return JPEGQS_ERR_CUDA;
+		}
+		if (device_phase(ctx, r, works, flags, NULL, bad_dev, 0, st)) return JPEGQS_ERR_CUDA;
+	}
+	/* every image's status, skipped ones included, so that a replayed graph rewrites all of them */
+	QsStatusPack p;
+	memset(&p, 0, sizeof(p));
+	for (int n = 0; n < nimg; n++) {
+		const ImgState &s = S[n]; QsStatusImg &m = p.img[n];
+		if (s.skip) continue;
+		m.flag0 = s.flag0; m.host_stop = s.stop ? 1 : 0; m.kept = s.image1 ? 1 : 0;
+		for (int ci = 0; ci < s.im->ncomp; ci++) if (r.W[n][ci].iterate) m.iter_mask |= (uint16_t)(1u << ci);
+	}
+	CK(qs_launch_async_status(&p, nimg, bad_dev, (int2 *)status, st));
+	ctx->launches++;
+	host_results(r, NULL);
+	for (int n = 0; n < nimg; n++) imgs[n].upsampled = 0;       /* the answer is status[n].upsampled */
+	return 0;
+}
+
+extern "C" int jpegqs_cuda_async_workspace_bytes(int nimages, const jpegqs_cuda_image *imgs, int flags, size_t *bytes) {
+	if (!bytes) return JPEGQS_ERR_ARG;
+	return async_plan(nimages, imgs, flags, false, bytes, NULL);
+}
+
+extern "C" int jpegqs_cuda_run_async(jpegqs_cuda_ctx *ctx, int nimages, jpegqs_cuda_image *imgs, int flags, int niter,
+		void *workspace, size_t workspace_bytes, jpegqs_cuda_status *status_dev, void *stream) {
+	if (!ctx) return JPEGQS_ERR_ARG;
+	size_t need = 0; int nquant = 0;
+	if (async_plan(nimages, imgs, flags, true, &need, &nquant)) {
+		snprintf(ctx->err, sizeof(ctx->err), "run_async: malformed image, host block-row tables, or a missing device pointer");
+		return JPEGQS_ERR_ARG;
+	}
+	if (!status_dev || !workspace || ((uintptr_t)workspace & 255) || workspace_bytes < need) {
+		snprintf(ctx->err, sizeof(ctx->err), "run_async: %s", !status_dev ? "status is NULL" : !workspace ? "workspace is NULL" :
+				((uintptr_t)workspace & 255) ? "workspace not 256-byte aligned" : "workspace too small");
+		return JPEGQS_ERR_ARG;
+	}
+	cudaStream_t st = stream ? (cudaStream_t)stream : ctx->stream;
+	WorkspaceScope scope(ctx, (char *)workspace, need, nquant);
+	/* a launch carries at most QS_MAX_JOBS components: larger batches run as several sub-batches,
+	 * one after another on st, each with its own sample planes */
+	for (int i = 0; i < nimages; ) {
+		int n = 0, jobs = 0;
+		while (i + n < nimages && jobs + imgs[i + n].ncomp <= QS_MAX_JOBS) jobs += imgs[i + n++].ncomp;
+		int rc = run_async_images(ctx, n, imgs + i, flags, niter, status_dev + i, st);
+		if (rc) return rc;
+		i += n;
+	}
+	return 0;
 }
 
 /* ---- the devices of one process behind one call ------------------------------------------- */

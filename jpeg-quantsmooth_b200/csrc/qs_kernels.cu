@@ -1581,6 +1581,28 @@ __global__ void qs_copy_flags_kernel(const int *__restrict__ src, volatile int *
 	for (int i = threadIdx.x; i < n; i += blockDim.x) dst[i] = src[i];
 	__threadfence_system();
 }
+/* quant constants of the stream-ordered entry point: ~1.5 KB per record, as many per launch as
+ * the 32 KB parameter space of sm_90 holds */
+struct QsQuantPack { QsQuantDev q[QS_QUANT_PACK]; };
+static_assert(sizeof(QsQuantPack) + sizeof(void *) + sizeof(int) <= 32764, "QS_QUANT_PACK exceeds the kernel parameter space");
+static_assert(sizeof(QsQuantDev) % 4 == 0, "QsQuantDev is copied as 32-bit words");
+__global__ void __launch_bounds__(256) qs_store_quant_kernel(const __grid_constant__ QsQuantPack pack,
+		QsQuantDev *__restrict__ dst, int n) {
+	const uint32_t *s = (const uint32_t *)pack.q;
+	uint32_t *d = (uint32_t *)dst;
+	for (int i = threadIdx.x; i < n * (int)(sizeof(QsQuantDev) / 4); i += blockDim.x) d[i] = s[i];
+}
+/* end of a stream-ordered run: per image, stop = the host's stop | the out-of-range flags of its
+ * iterating components, upsampled = the full-resolution luma plane was kept and nothing stopped */
+__global__ void qs_async_status_kernel(const __grid_constant__ QsStatusPack p, int n, const int *__restrict__ flags,
+		int2 *__restrict__ status) {
+	int i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	const QsStatusImg &m = p.img[i];
+	int stop = m.host_stop;
+	for (int ci = 0; ci < 16; ci++) if ((m.iter_mask >> ci) & 1) stop |= flags[m.flag0 + ci] ? 1 : 0;
+	status[i] = make_int2(stop, m.kept && !stop ? 1 : 0);
+}
 
 /* ------------------------------------------------------------------------------------------
  * launch wrappers
@@ -1796,5 +1818,24 @@ cudaError_t qs_store_jobs(QsJob *dst, const QsJob *jobs_host, int n, cudaStream_
 
 cudaError_t qs_copy_flags(const int *src_dev, int *dst_mapped, int n, cudaStream_t st) {
 	qs_copy_flags_kernel<<<1, 128, 0, st>>>(src_dev, dst_mapped, n);
+	return cudaGetLastError();
+}
+
+cudaError_t qs_store_quant(QsQuantDev *dst, const QsQuantDev *q_host, int n, cudaStream_t st) {
+	for (int off = 0; off < n; off += QS_QUANT_PACK) {
+		QsQuantPack pack;
+		int cnt = n - off < QS_QUANT_PACK ? n - off : QS_QUANT_PACK;
+		memcpy(pack.q, q_host + off, (size_t)cnt * sizeof(QsQuantDev));
+		if (cnt < QS_QUANT_PACK) memset(pack.q + cnt, 0, (size_t)(QS_QUANT_PACK - cnt) * sizeof(QsQuantDev));
+		qs_store_quant_kernel<<<1, 256, 0, st>>>(pack, dst + off, cnt);
+		cudaError_t e = cudaGetLastError();
+		if (e != cudaSuccess) return e;
+	}
+	return cudaSuccess;
+}
+
+cudaError_t qs_launch_async_status(const QsStatusPack *p, int n, const int *flags, int2 *status, cudaStream_t st) {
+	if (n <= 0) return cudaSuccess;
+	qs_async_status_kernel<<<(n + 127) / 128, 128, 0, st>>>(*p, n, flags, status);
 	return cudaGetLastError();
 }

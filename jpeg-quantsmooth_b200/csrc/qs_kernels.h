@@ -30,5 +30,16 @@ extern "C" int qs_host_orig_coef(int c, int q);
 #define QS_JOB_PACK 48
 cudaError_t qs_store_jobs(QsJob *dst, const QsJob *jobs_host, int n, cudaStream_t st);
 cudaError_t qs_copy_flags(const int *src_dev, int *dst_mapped, int n, cudaStream_t st);
+#define QS_QUANT_PACK 21
+cudaError_t qs_store_quant(QsQuantDev *dst, const QsQuantDev *q_host, int n, cudaStream_t st);
+/* per image of a stream-ordered run (qs_cuda.cu run_async): what its status is made of */
+typedef struct {
+	int32_t flag0;          /* slot of component 0 in the run's out-of-range flags */
+	uint16_t iter_mask;     /* bit ci: component ci took part in the iterations */
+	uint8_t host_stop;      /* a quant value >= 0x800 stopped it (quantsmooth.h:2504) */
+	uint8_t kept;           /* the full-resolution luma plane was kept for UPSAMPLE_UV */
+} QsStatusImg;
+typedef struct { QsStatusImg img[QS_MAX_JOBS]; } QsStatusPack;
+cudaError_t qs_launch_async_status(const QsStatusPack *p, int n, const int *flags, int2 *status, cudaStream_t st);
 
 #endif

@@ -122,6 +122,9 @@ def load():
     lib.jpegqs_cuda_multi_last_error.restype = C.c_char_p
     lib.jpegqs_cuda_multi_plan.argtypes = [C.c_void_p, C.POINTER(_Image)]
     lib.jpegqs_cuda_run_host_multi.argtypes = [C.c_void_p, C.POINTER(_Image), C.c_int, C.c_int]
+    lib.jpegqs_cuda_async_workspace_bytes.argtypes = [C.c_int, C.POINTER(_Image), C.c_int, C.POINTER(C.c_size_t)]
+    lib.jpegqs_cuda_run_async.argtypes = [C.c_void_p, C.c_int, C.POINTER(_Image), C.c_int, C.c_int, C.c_void_p,
+                                          C.c_size_t, C.c_void_p, C.c_void_p]
     lib.jpegqs_cuda_tables.argtypes = [C.c_int, C.c_void_p]
     lib.jpegqs_cuda_orig_coef.argtypes = [C.c_int, C.c_int]
     _lib = lib
@@ -197,6 +200,45 @@ def _fill_image(ci: _Image, image: CoefImage, coef_ptrs: Sequence[int], up_ptrs:
         cc.coef_up = up_ptrs[i] if i < len(up_ptrs) and up_ptrs[i] else None
 
 
+def _image_array(images: Sequence[CoefImage], coef_ptrs=None, up_ptrs=None):
+    arr = (_Image * max(len(images), 1))()
+    for n, im in enumerate(images):
+        _fill_image(arr[n], im, coef_ptrs[n] if coef_ptrs else [None] * len(im.comps),
+                    up_ptrs[n] if up_ptrs else [])
+    return arr
+
+
+def upsample_can_trigger(image: CoefImage, flags: int) -> bool:
+    """UPSAMPLE_UV replaces this image's chroma with luma-sized arrays unless the run stops
+    (reference quantsmooth.h:2447-2453, 2691-2752)."""
+    cs = image.comps
+    return bool(flags & 4) and image.colorspace == JCS_YCbCr and len(cs) >= 3 and \
+        all((c.h_samp, c.v_samp) == (1, 1) for c in cs[1:3]) and (cs[0].h_samp, cs[0].v_samp) != (1, 1)
+
+
+def async_workspace_bytes(images: Sequence[CoefImage], flags: int) -> int:
+    """Device bytes of workspace QsContext.run_async needs for these images (host-only)."""
+    lib = load()
+    out = C.c_size_t(0)
+    arr = _image_array(images)
+    rc = lib.jpegqs_cuda_async_workspace_bytes(len(images), arr, flags & 0x7f, C.byref(out))
+    if rc < 0:
+        raise QsError(f"jpegqs_cuda_async_workspace_bytes: malformed image ({rc})")
+    return int(out.value)
+
+
+def _check_tensor(t, shape, what: str):
+    import torch
+    if not isinstance(t, torch.Tensor):
+        raise TypeError(f"{what}: expected a torch.Tensor, got {type(t).__name__}")
+    if t.dtype != torch.int16:
+        raise TypeError(f"{what}: dtype {t.dtype}, expected torch.int16")
+    if tuple(t.shape) != tuple(shape):
+        raise ValueError(f"{what}: shape {tuple(t.shape)}, expected {tuple(shape)}")
+    if not t.is_contiguous():
+        raise ValueError(f"{what}: not contiguous")
+
+
 class QsContext:
     """One device context (stream, tables, scratch arena).  Mirrors the process-wide state
     the reference keeps implicitly (its tables are rebuilt per call, quantsmooth.h:2460-2464)."""
@@ -209,6 +251,7 @@ class QsContext:
             raise QsError(f"jpegqs_cuda_create failed ({rc}): "
                           f"{self.lib.jpegqs_cuda_last_error(None).decode()}")
         self.h = h
+        self.device = device
 
     def close(self):
         if getattr(self, "h", None):
@@ -361,6 +404,72 @@ class QsContext:
         self._check(self.lib.jpegqs_cuda_run_batch(self.h, len(images), arr, flags & 0x7f, niter, 1, rets,
                                                    C.c_void_p(stream or None)))
         return list(rets), [bool(a.upsampled) for a in arr]
+
+    # ---- stream-ordered on torch tensors (include/jpegqs_cuda.h jpegqs_cuda_run_async) ----
+    def run_async(self, images: Sequence[CoefImage], coefs, flags: int, niter: int, up=None, stream=None):
+        """Smooth device-resident coefficients in place without blocking the calling thread.
+
+        images: CoefImages carrying geometry and quant tables (their arrays are not read).
+        coefs[i][c]: CUDA int16 contiguous tensors [hblk, wblk, 64] on this context's device.
+        up[i]: the two luma-sized int16 tensors for image i's up-sampled chroma, or None; they are
+        allocated when UPSAMPLE_UV can trigger and not given.  stream: a torch.cuda.Stream
+        (default: the current one).  Everything, including the workspace, is enqueued on that
+        stream; the call returns before the GPU has done anything.  The images' quant tables
+        are set to ones on return, as do_quantsmooth does.
+
+        Returns (status, up): status is an int32 device tensor [n, 2] of (stop, upsampled) per
+        image, up the per-image pairs of up-sampled chroma tensors (None where UPSAMPLE_UV cannot
+        trigger); they hold the result only where status[i, 1] is 1.  Capturable with
+        torch.cuda.graph: a replay re-runs on the current contents of the same tensors."""
+        import torch
+        n = len(images)
+        if len(coefs) != n or (up is not None and len(up) != n):
+            raise ValueError("images, coefs and up must have one entry per image")
+        ups, tensors = [], []
+        for i, im in enumerate(images):
+            if len(coefs[i]) != len(im.comps):
+                raise ValueError(f"image {i}: {len(coefs[i])} coefficient tensors for {len(im.comps)} components")
+            for c, (comp, t) in enumerate(zip(im.comps, coefs[i])):
+                _check_tensor(t, (comp.hblk, comp.wblk, 64), f"coefs[{i}][{c}]")
+                tensors.append((f"coefs[{i}][{c}]", t))
+            given = up[i] if up is not None else None
+            if given is not None:
+                if len(given) != 2:
+                    raise ValueError(f"up[{i}]: expected two tensors")
+                y = im.comps[0]
+                for j, t in enumerate(given):
+                    _check_tensor(t, (y.hblk, y.wblk, 64), f"up[{i}][{j}]")
+                    tensors.append((f"up[{i}][{j}]", t))
+            ups.append(given)
+        device = self.device if self.device >= 0 else torch.cuda.current_device()
+        for what, t in tensors:
+            if not t.is_cuda or t.device.index != device:
+                raise ValueError(f"{what}: on {t.device}, expected cuda:{device}")
+        stream = stream if stream is not None else torch.cuda.current_stream(device)
+        with torch.cuda.device(device), torch.cuda.stream(stream):
+            for i, im in enumerate(images):
+                if ups[i] is None and upsample_can_trigger(im, flags):
+                    y = im.comps[0]
+                    ups[i] = tuple(torch.empty((y.hblk, y.wblk, 64), dtype=torch.int16, device=device)
+                                   for _ in range(2))
+            coef_ptrs = [[t.data_ptr() for t in coefs[i]] for i in range(n)]
+            up_ptrs = [[None, ups[i][0].data_ptr(), ups[i][1].data_ptr()] if ups[i] is not None else []
+                       for i in range(n)]
+            arr = _image_array(images, coef_ptrs, up_ptrs)
+            size = C.c_size_t(0)
+            self._check(self.lib.jpegqs_cuda_async_workspace_bytes(n, arr, flags & 0x7f, C.byref(size)))
+            # allocated on `stream`: the caching allocator hands the memory out again only to work
+            # queued after this call's kernels on that stream, so it may be released at return
+            ws = torch.empty(max(size.value, 1), dtype=torch.uint8, device=device)
+            status = torch.empty((n, 2), dtype=torch.int32, device=device)
+            self._check(self.lib.jpegqs_cuda_run_async(self.h, n, arr, flags & 0x7f, niter, ws.data_ptr(),
+                                                       size.value, status.data_ptr() if n else None,
+                                                       C.c_void_p(stream.cuda_stream)))
+        for i, im in enumerate(images):
+            for c, comp in enumerate(im.comps):
+                if comp.quant is not None:
+                    comp.quant = np.array(list(arr[i].comp[c].quant), dtype=np.uint16)
+        return status, [tuple(u) if u is not None else None for u in ups]
 
     # ---- one slab of a sharded image (include/jpegqs_cuda.h "one image sharded by MCU rows") ----
     def run_slab(self, link, slab: CoefImage, rank: int, world: int, row0: Sequence[int],
@@ -551,3 +660,14 @@ def do_quantsmooth(image: CoefImage, flags: int, niter: int, progprec: int = 0, 
     """Python mirror of `int do_quantsmooth(srcinfo, coef_arrays, opts)` (reference
     libjpegqs.h:47-48): returns (stop, smoothed image)."""
     return default_context(device).do_quantsmooth(image, flags, niter, progprec, progress)
+
+
+def run_async(images: Sequence[CoefImage], coefs, flags: int, niter: int, up=None, stream=None):
+    """QsContext.run_async on the default context of the tensors' device: smooths CUDA tensors
+    in place, enqueued on `stream` (default: the current one) without waiting.  Returns
+    (status [n, 2] int32 device tensor of (stop, upsampled), up-sampled chroma pairs)."""
+    import torch
+    first = next((t for ts in coefs for t in ts), None)
+    if not isinstance(first, torch.Tensor) or not first.is_cuda:
+        raise ValueError("run_async: the coefficient tensors must be CUDA tensors")
+    return default_context(first.device.index).run_async(images, coefs, flags, niter, up, stream)
