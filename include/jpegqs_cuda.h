@@ -168,6 +168,49 @@ int jpegqs_cuda_async_workspace_bytes(int nimages, const jpegqs_cuda_image *imgs
 int jpegqs_cuda_run_async(jpegqs_cuda_ctx *ctx, int nimages, jpegqs_cuda_image *imgs, int flags, int niter,
 		void *workspace, size_t workspace_bytes, jpegqs_cuda_status *status_dev, void *stream);
 
+/* ---- stream-ordered, graph-capturable render of device-resident images to 8-bit RGB -------
+ * What libjpeg's jpeg_read_scanlines gives for these coefficients with out_color_space JCS_RGB,
+ * JDCT_ISLOW and fancy up-sampling (the pixels jpegqs_cuda_render_rgb computes), for a caller
+ * whose coefficients are on the GPU - typically right after jpegqs_cuda_run_async, in the same
+ * stream or CUDA graph.  One fused kernel per batch: IDCT, up-sampling and colour conversion
+ * without any sample plane in device memory and without a workspace.
+ *   - Inputs.  comp[].coef / coef_up are DEVICE pointers on the context's device, 16-byte aligned
+ *     (blocks are read as 16-byte vectors); rows / rows_up must be NULL.  1 or 3 components: 3 are converted YCbCr -> RGB when is_ycbcr is set and
+ *     copied otherwise, 1 is replicated to R = G = B (JCS_GRAYSCALE -> JCS_RGB).  Any other count,
+ *     or sampling factors whose ratios are not integral (libjpeg cannot decode those either),
+ *     returns JPEGQS_ERR_UNSUPPORTED with nothing enqueued.
+ *   - Coefficients are only read.  A component with has_qtbl and a quant table that is not all
+ *     ones (render_rgb's rule: still quantized) is de-quantized in registers, in int32 as libjpeg
+ *     does, so a never-smoothed coefficient set decodes too; nothing is written back.  Component
+ *     c's table applies to whichever array is read for it (after run_async all tables are ones).
+ *   - Chroma source.  Components 1 and 2 come from coef_up, at component 0's geometry with 1x1
+ *     sampling, when the image is up-sampled, and from coef otherwise:
+ *       . status_dev != NULL: up-sampled means status_dev[i].upsampled != 0, read on the device,
+ *         for images whose two coef_up pointers are non-NULL; other images always read coef.  So
+ *         one graph may hold run_async followed by this call, and a replay in which an image
+ *         stops (and so is not up-sampled) renders it from coef.
+ *       . status_dev == NULL: imgs[i].upsampled decides (callers of run_device and run_batch).
+ *   - Output.  out_dev[i]: image_width * image_height * 3 bytes of device memory at any byte
+ *     alignment (a slice of a batched [N, H, W, 3] tensor works), in layout JPEGQS_RENDER_HWC or
+ *     JPEGQS_RENDER_CHW.
+ *   - Argument errors change nothing: every check runs before the first enqueue and a failed one
+ *     returns JPEGQS_ERR_ARG with nothing enqueued.  Checked: out_dev or an entry of it NULL, a
+ *     coef pointer NULL (or a coef_up one for a host-flagged up-sampled image), a coef or coef_up
+ *     pointer not 16-byte aligned, rows / rows_up set, a sampling factor outside 1..4, a component whose blocks do not cover its samples
+ *     (wblk * 8 < cw or hblk * 8 < ch, with cw = ceil(image_width * h_samp / max_h_samp) and ch
+ *     likewise, libjpeg's downsampled_width / height), and an unknown layout.
+ *   - The stream rules of run_async: no cudaMalloc, synchronisation, event record or query, and no
+ *     context memory (per-image descriptors and quant tables travel as kernel parameters), so the
+ *     call is legal under cudaStreamCaptureModeGlobal and may be in flight with run_async or
+ *     render_async calls on other streams of the same context.  Host structs may be freed at
+ *     return.  jpegqs_cuda_last_launches counts its launches; batches larger than one launch's
+ *     parameter space (60 images) run as several launches, one after another on the stream.
+ * Returns 0 or a negative error. */
+#define JPEGQS_RENDER_HWC 0   /* R,G,B interleaved per pixel: libjpeg's JCS_RGB scanlines      */
+#define JPEGQS_RENDER_CHW 1   /* three planes R, G, B of image_width * image_height bytes each */
+int jpegqs_cuda_render_async(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image *imgs,
+		const jpegqs_cuda_status *status_dev, int layout, uint8_t *const *out_dev, void *stream);
+
 /* ---- one image sharded by MCU rows over several GPUs (SURVEY.md 8e) ----------------------
  * Every rank - a device of this process, or another process on the same box - smooths one slab
  * of contiguous MCU rows and exchanges ONE pixel row per plane with each neighbour after every
@@ -267,7 +310,8 @@ int jpegqs_cuda_pass_upsample(jpegqs_cuda_ctx *ctx, const uint8_t *cplane, const
  * YCbCr -> RGB with libjpeg's fixed-point constants.  1 or 3 components.  Components whose
  * quant table is not all ones are de-quantized first, so the call also decodes an untouched
  * coefficient set.  rgb: image_width * image_height * 3 bytes (host, or device if on_device;
- * device coefficient arrays that still carry quant tables are de-quantized in place). */
+ * device coefficient arrays that still carry quant tables are de-quantized in place).  Unlike
+ * jpegqs_cuda_render_async it does not check that the blocks cover the image. */
 int jpegqs_cuda_render_rgb(jpegqs_cuda_ctx *ctx, const jpegqs_cuda_image *img, int on_device,
 		uint8_t *rgb, void *stream);
 

@@ -39,7 +39,7 @@ def quality_to_flags(quality: int) -> int:
 def __getattr__(name):
     # the CUDA binding is imported lazily so that the host-only helpers
     # (synth, image) work on a machine without the built extension
-    if name in ("cuda", "do_quantsmooth", "run_async", "async_workspace_bytes", "QsContext", "lib_path"):
+    if name in ("cuda", "do_quantsmooth", "run_async", "render_async", "async_workspace_bytes", "QsContext", "lib_path"):
         import importlib
         _cuda = importlib.import_module(__name__ + ".cuda")
         if name == "cuda":

@@ -2072,3 +2072,76 @@ extern "C" int jpegqs_cuda_render_rgb(jpegqs_cuda_ctx *ctx, const jpegqs_cuda_im
 	CK(cudaStreamSynchronize(st));
 	return 0;
 }
+
+/* ---- stream-ordered render of device-resident images (see the header) ----------------------- */
+extern "C" int jpegqs_cuda_render_async(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image *imgs,
+		const jpegqs_cuda_status *status_dev, int layout, uint8_t *const *out_dev, void *stream) {
+	if (!ctx) return JPEGQS_ERR_ARG;
+	const char *bad = nimages < 0 || (nimages && (!imgs || !out_dev)) ? "images or outputs missing"
+			: layout != JPEGQS_RENDER_HWC && layout != JPEGQS_RENDER_CHW ? "unknown layout" : NULL;
+	std::vector<QsRenderImg> d(bad ? 0 : nimages);
+	int unsupported = 0;
+	for (int i = 0; i < nimages && !bad && !unsupported; i++) {
+		const jpegqs_cuda_image *im = &imgs[i];
+		QsRenderImg &r = d[i];
+		memset(&r, 0, sizeof(r));
+		if (im->ncomp != 1 && im->ncomp != 3) { unsupported = 1; break; }
+		int maxh = 1, maxv = 1;
+		for (int c = 0; c < im->ncomp && !bad; c++) {
+			const jpegqs_cuda_comp *cc = &im->comp[c];
+			if (cc->h_samp < 1 || cc->h_samp > 4 || cc->v_samp < 1 || cc->v_samp > 4) bad = "sampling factor outside 1..4";
+			else if (!cc->coef || cc->rows || cc->rows_up) bad = "coef NULL, or host block-row tables";
+			else if (((uintptr_t)cc->coef | (c ? (uintptr_t)cc->coef_up : 0)) & 15) bad = "coef or coef_up not 16-byte aligned";
+			else { maxh = std::max(maxh, cc->h_samp); maxv = std::max(maxv, cc->v_samp); }
+		}
+		if (!out_dev[i]) bad = "output NULL";
+		for (int c = 0; c < im->ncomp && !bad && !unsupported; c++) {
+			const jpegqs_cuda_comp *cc = &im->comp[c];
+			if (maxh % cc->h_samp || maxv % cc->v_samp) { unsupported = 1; break; }   /* libjpeg cannot either */
+			r.cw[c] = (int)(((uint64_t)im->image_width * cc->h_samp + maxh - 1) / maxh);
+			r.ch[c] = (int)(((uint64_t)im->image_height * cc->v_samp + maxv - 1) / maxv);
+			/* the blocks must hold every real sample: the kernel reads up to column cw - 1, row ch - 1 */
+			if ((uint64_t)cc->wblk * 8 < (uint64_t)r.cw[c] || (uint64_t)cc->hblk * 8 < (uint64_t)r.ch[c]) bad = "blocks do not cover the image";
+			r.coef[c] = cc->coef; r.wblk[c] = (int32_t)cc->wblk;
+			r.hs[c] = (uint8_t)(maxh / cc->h_samp); r.vs[c] = (uint8_t)(maxv / cc->v_samp);
+			int val = 0;
+			for (int k = 0; k < 64; k++) val |= cc->quant[k];
+			bool deq = cc->has_qtbl && val > 1;             /* render_rgb's rule: still quantized */
+			for (int k = 0; k < 64; k++) r.q[c][k] = deq ? cc->quant[k] : 1;
+		}
+		if (bad || unsupported) break;
+		if (im->ncomp == 3) {
+			r.coef_up[0] = im->comp[1].coef_up; r.coef_up[1] = im->comp[2].coef_up;
+			if (status_dev) r.up_mode = r.coef_up[0] && r.coef_up[1] ? 2 : 0;
+			else if (im->upsampled) {
+				if (!r.coef_up[0] || !r.coef_up[1]) bad = "upsampled without coef_up";
+				r.up_mode = 1;
+			}
+		}
+		r.out = out_dev[i]; r.width = (int32_t)im->image_width; r.height = (int32_t)im->image_height;
+		r.ncomp = (uint8_t)im->ncomp; r.ycc = im->is_ycbcr ? 1 : 0;
+	}
+	if (unsupported) {
+		snprintf(ctx->err, sizeof(ctx->err), "render_async: 1 or 3 components with integral sampling ratios only");
+		return JPEGQS_ERR_UNSUPPORTED;
+	}
+	if (bad) {
+		snprintf(ctx->err, sizeof(ctx->err), "render_async: %s", bad);
+		return JPEGQS_ERR_ARG;
+	}
+	CK(cudaSetDevice(ctx->device));
+	cudaStream_t st = stream ? (cudaStream_t)stream : ctx->stream;
+	ctx->launches = 0;
+	/* the descriptors travel as kernel parameters: QS_RENDER_PACK images per launch */
+	for (int i0 = 0; i0 < nimages; i0 += QS_RENDER_PACK) {
+		int n = std::min(QS_RENDER_PACK, nimages - i0), tiles = 0;
+		for (int i = 0; i < n; i++) {
+			QsRenderImg &r = d[i0 + i];
+			r.tile_begin = tiles;
+			tiles += ((r.width + QS_RENDER_TW - 1) / QS_RENDER_TW) * ((r.height + QS_RENDER_TH - 1) / QS_RENDER_TH);
+		}
+		CK(qs_launch_render_async(d.data() + i0, n, tiles, status_dev ? (const int2 *)(status_dev + i0) : NULL, layout, st));
+		if (tiles) ctx->launches++;
+	}
+	return 0;
+}

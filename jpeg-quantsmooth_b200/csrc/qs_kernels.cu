@@ -1743,51 +1743,218 @@ typedef struct {
 	int ncomp, width, height, ycc;
 } QsRenderArgs;
 
-__device__ __forceinline__ int qs_plane_px(const uint8_t *p, int stride, int x, int y) {
-	return p[(size_t)(y + 1) * stride + QS_PLANE_PAD + x];
-}
+/* sample (x, y) of a padded sample plane */
+struct QsPlanePx {
+	const uint8_t *p; int stride;
+	__device__ __forceinline__ int operator()(int x, int y) const { return p[(size_t)(y + 1) * stride + QS_PLANE_PAD + x]; }
+};
 
-/* one up-sampled sample of component c at output pixel (ox, oy) */
-__device__ __forceinline__ int qs_upsampled(const QsRenderArgs &a, int c, int ox, int oy) {
-	const uint8_t *p = a.plane[c]; int st = a.stride[c], hs = a.hs[c], vs = a.vs[c], cw = a.cw[c], ch = a.ch[c];
-	if (hs == 1 && vs == 1) return qs_plane_px(p, st, ox, oy);
+/* One up-sampled sample at output pixel (ox, oy) of a component whose expansion factors are
+ * hs x vs and whose real (not block padded) size is cw x ch; px(x, y) reads its sample (x, y).
+ * Edges replicate the last real sample, column cw - 1 / row ch - 1, as libjpeg does. */
+template <class Px>
+__device__ __forceinline__ int qs_upsample_at(const Px &px, int hs, int vs, int cw, int ch, int ox, int oy) {
+	if (hs == 1 && vs == 1) return px(ox, oy);
 	if (hs == 2 && vs == 1 && cw > 2) {                 /* h2v1_fancy_upsample */
-		int x = ox >> 1, v = qs_plane_px(p, st, x, oy);
-		if (ox & 1) return x == cw - 1 ? v : (v * 3 + qs_plane_px(p, st, x + 1, oy) + 2) >> 2;
-		return x == 0 ? v : (v * 3 + qs_plane_px(p, st, x - 1, oy) + 1) >> 2;
+		int x = ox >> 1, v = px(x, oy);
+		if (ox & 1) return x == cw - 1 ? v : (v * 3 + px(x + 1, oy) + 2) >> 2;
+		return x == 0 ? v : (v * 3 + px(x - 1, oy) + 1) >> 2;
 	}
 	if (hs == 2 && vs == 2 && cw > 2) {                 /* h2v2_fancy_upsample */
 		int x = ox >> 1, y = oy >> 1;
 		int y1 = (oy & 1) ? min(y + 1, ch - 1) : max(y - 1, 0);   /* nearer neighbour row, edge replicated */
-		int cur = qs_plane_px(p, st, x, y) * 3 + qs_plane_px(p, st, x, y1);
+		int cur = px(x, y) * 3 + px(x, y1);
 		if (ox & 1) {
 			if (x == cw - 1) return (cur * 4 + 7) >> 4;
-			return (cur * 3 + qs_plane_px(p, st, x + 1, y) * 3 + qs_plane_px(p, st, x + 1, y1) + 7) >> 4;
+			return (cur * 3 + px(x + 1, y) * 3 + px(x + 1, y1) + 7) >> 4;
 		}
 		if (x == 0) return (cur * 4 + 8) >> 4;
-		return (cur * 3 + qs_plane_px(p, st, x - 1, y) * 3 + qs_plane_px(p, st, x - 1, y1) + 8) >> 4;
+		return (cur * 3 + px(x - 1, y) * 3 + px(x - 1, y1) + 8) >> 4;
 	}
 	if (hs == 1 && vs == 2) {                           /* h1v2_fancy_upsample (libjpeg-turbo >= 2.0) */
 		int y = oy >> 1, y1 = (oy & 1) ? min(y + 1, ch - 1) : max(y - 1, 0);
-		return (qs_plane_px(p, st, ox, y) * 3 + qs_plane_px(p, st, ox, y1) + ((oy & 1) ? 2 : 1)) >> 2;
+		return (px(ox, y) * 3 + px(ox, y1) + ((oy & 1) ? 2 : 1)) >> 2;
 	}
-	return qs_plane_px(p, st, min(ox / hs, cw - 1), min(oy / vs, ch - 1));   /* box replication (int_upsample) */
+	return px(min(ox / hs, cw - 1), min(oy / vs, ch - 1));   /* box replication (int_upsample) */
+}
+
+/* one output pixel, r | g << 8 | b << 16: YCbCr -> RGB with the fixed-point tables of jdcolor.c
+ * (build_ycc_rgb_table / ycc_rgb_convert, SCALEBITS 16) when ycc, the three samples as they are
+ * otherwise (a grey image passes its sample three times) */
+__device__ __forceinline__ uint32_t qs_rgb_pixel(int y, int c1, int c2, bool ycc) {
+	int r = y, g = c1, b = c2;
+	if (ycc) {
+		int cb = c1 - 128, cr = c2 - 128;
+		r = min(max(y + ((91881 * cr + 32768) >> 16), 0), 255);
+		g = min(max(y + ((-22554 * cb + 32768 - 46802 * cr) >> 16), 0), 255);
+		b = min(max(y + ((116130 * cb + 32768) >> 16), 0), 255);
+	}
+	return (uint32_t)r | ((uint32_t)g << 8) | ((uint32_t)b << 16);
 }
 
 __global__ void qs_render_rgb_kernel(QsRenderArgs a, uint8_t *__restrict__ rgb) {
 	int ox = blockIdx.x * blockDim.x + threadIdx.x, oy = blockIdx.y * blockDim.y + threadIdx.y;
 	if (ox >= a.width || oy >= a.height) return;
 	uint8_t *o = rgb + ((size_t)oy * a.width + ox) * 3;
-	int y = qs_upsampled(a, 0, ox, oy);
-	if (a.ncomp < 3) { o[0] = o[1] = o[2] = (uint8_t)y; return; }
-	int c1 = qs_upsampled(a, 1, ox, oy), c2 = qs_upsampled(a, 2, ox, oy);
-	if (!a.ycc) { o[0] = (uint8_t)y; o[1] = (uint8_t)c1; o[2] = (uint8_t)c2; return; }
-	/* jdcolor.c build_ycc_rgb_table / ycc_rgb_convert, SCALEBITS 16 */
-	int cb = c1 - 128, cr = c2 - 128;
-	int r = y + ((91881 * cr + 32768) >> 16);
-	int g = y + ((-22554 * cb + 32768 - 46802 * cr) >> 16);
-	int b = y + ((116130 * cb + 32768) >> 16);
-	o[0] = (uint8_t)min(max(r, 0), 255); o[1] = (uint8_t)min(max(g, 0), 255); o[2] = (uint8_t)min(max(b, 0), 255);
+	int y = qs_upsample_at(QsPlanePx{a.plane[0], a.stride[0]}, a.hs[0], a.vs[0], a.cw[0], a.ch[0], ox, oy), c1 = y, c2 = y;
+	if (a.ncomp >= 3) {
+		c1 = qs_upsample_at(QsPlanePx{a.plane[1], a.stride[1]}, a.hs[1], a.vs[1], a.cw[1], a.ch[1], ox, oy);
+		c2 = qs_upsample_at(QsPlanePx{a.plane[2], a.stride[2]}, a.hs[2], a.vs[2], a.cw[2], a.ch[2], ox, oy);
+	}
+	uint32_t px = qs_rgb_pixel(y, c1, c2, a.ncomp >= 3 && a.ycc);
+	o[0] = (uint8_t)px; o[1] = (uint8_t)(px >> 8); o[2] = (uint8_t)(px >> 16);
+}
+
+/* ------------------------------------------------------------------------------------------
+ * Stream-ordered render (qs_cuda.cu jpegqs_cuda_render_async): coefficients -> islow IDCT ->
+ * libjpeg's up-sampling -> colour conversion -> pixels in one launch per batch; no sample plane
+ * goes through global memory.  A CTA renders one QS_RENDER_TW x QS_RENDER_TH tile of output
+ * pixels.  It IDCTs into shared memory every block of every component under the tile, plus the
+ * blocks holding the one-sample ring the fancy up-sampler reads, then computes the tile's pixels
+ * from there.  Per component the window is at most 16 x 8 blocks: 16 x 8 at full resolution, 10 x 6
+ * with 2:1 sub-sampling and its ring, fewer for 3:1 and 4:1 (which replicate and need no ring).
+ * Coefficients are only read; de-quantization happens in registers, in int32 (jidctint.c).
+ * ------------------------------------------------------------------------------------------ */
+#define QS_RT_THREADS 256
+#define QS_RS_W 128
+#define QS_RS_H 64
+static_assert(QS_RENDER_TW == 128 && QS_RENDER_TH == 64, "the shared sample window is sized for 128 x 64 tiles");
+
+struct QsRenderPack { QsRenderImg img[QS_RENDER_PACK]; };
+static_assert(sizeof(QsRenderPack) + 2 * sizeof(void *) + 2 * sizeof(int) <= 32764,
+		"QS_RENDER_PACK exceeds the kernel parameter space");
+
+/* sample (x, y) of a component's shared window whose first sample is (x0, y0) */
+struct QsSmemPx {
+	const uint8_t *s; int x0, y0;
+	__device__ __forceinline__ int operator()(int x, int y) const { return s[(y - y0) * QS_RS_W + (x - x0)]; }
+};
+
+struct QsRenderComp { const int16_t *coef; int wblk, bx0, by0, nbx, nby, cw, ch, hs, vs; };
+
+__global__ void __launch_bounds__(QS_RT_THREADS, 2) qs_render_async_kernel(const __grid_constant__ QsRenderPack p,
+		int n, const int2 *__restrict__ status, int layout) {
+	__shared__ __align__(16) uint8_t pix[3][QS_RS_H * QS_RS_W];
+	__shared__ int qmul[3][64];
+	__shared__ QsRenderComp g[3];
+	const int tile = blockIdx.x;
+	int lo = 0, hi = n - 1;
+	while (lo < hi) {                                    /* last image with tile_begin <= tile */
+		int mid = (lo + hi + 1) >> 1;
+		if (p.img[mid].tile_begin <= tile) lo = mid; else hi = mid - 1;
+	}
+	const QsRenderImg &im = p.img[lo];
+	const int W = im.width, H = im.height, nc = im.ncomp, ntx = (W + QS_RENDER_TW - 1) / QS_RENDER_TW;
+	const int t = tile - im.tile_begin, x0 = (t % ntx) * QS_RENDER_TW, y0 = (t / ntx) * QS_RENDER_TH;
+	const int x1 = min(x0 + QS_RENDER_TW, W) - 1, y1 = min(y0 + QS_RENDER_TH, H) - 1;   /* last pixel of the tile */
+	if (threadIdx.x < nc) {
+		const int c = threadIdx.x;
+		/* components 1 and 2 of an up-sampled image: coef_up, at component 0's geometry */
+		const bool up = c > 0 && (im.up_mode == 1 || (im.up_mode == 2 && status[lo].y != 0));
+		const int k = up ? 0 : c;
+		QsRenderComp r;
+		r.coef = up ? im.coef_up[c - 1] : im.coef[c];
+		r.wblk = im.wblk[k]; r.cw = im.cw[k]; r.ch = im.ch[k]; r.hs = im.hs[k]; r.vs = im.vs[k];
+		const int rx = r.hs == 2 ? 1 : 0, ry = r.vs == 2 ? 1 : 0;     /* the fancy up-sampler's ring */
+		r.bx0 = max(x0 / r.hs - rx, 0) >> 3; r.nbx = (min(x1 / r.hs + rx, r.cw - 1) >> 3) - r.bx0 + 1;
+		r.by0 = max(y0 / r.vs - ry, 0) >> 3; r.nby = (min(y1 / r.vs + ry, r.ch - 1) >> 3) - r.by0 + 1;
+		g[c] = r;
+	}
+	for (int i = threadIdx.x; i < nc * 64; i += QS_RT_THREADS) qmul[i >> 6][i & 63] = im.q[i >> 6][i & 63];
+	__syncthreads();
+
+	/* islow IDCT of every block of the windows, one thread per block (as qs_idct_pass_kernel) */
+	const int nb0 = g[0].nbx * g[0].nby, nb1 = nc > 1 ? g[1].nbx * g[1].nby : 0, nb2 = nc > 2 ? g[2].nbx * g[2].nby : 0;
+	for (int k = threadIdx.x; k < nb0 + nb1 + nb2; k += QS_RT_THREADS) {
+		const int c = k < nb0 ? 0 : k < nb0 + nb1 ? 1 : 2;
+		const int j = k - (c == 0 ? 0 : c == 1 ? nb0 : nb0 + nb1);
+		const QsRenderComp &r = g[c];
+		const int lby = j / r.nbx, lbx = j - lby * r.nbx;
+		const int4 *src = (const int4 *)(r.coef + ((size_t)(r.by0 + lby) * r.wblk + r.bx0 + lbx) * 64);
+		int cf[64];
+#pragma unroll
+		for (int v8 = 0; v8 < 8; v8++) {
+			int4 v = __ldg(src + v8);
+			int w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+			for (int h = 0; h < 4; h++) {
+				cf[v8 * 8 + 2 * h] = (short)(w[h] & 0xffff) * qmul[c][v8 * 8 + 2 * h];
+				cf[v8 * 8 + 2 * h + 1] = (w[h] >> 16) * qmul[c][v8 * 8 + 2 * h + 1];
+			}
+		}
+		int ws[64];
+#pragma unroll
+		for (int x = 0; x < 8; x++) {
+			int in[8], o[8];
+#pragma unroll
+			for (int y = 0; y < 8; y++) in[y] = cf[y * 8 + x];
+			qs_islow_1d<1024>(in, o);
+#pragma unroll
+			for (int y = 0; y < 8; y++) ws[y * 8 + x] = o[y] >> 11;
+		}
+		uint32_t rlo[8], rhi[8];
+		qs_islow_rows(ws, rlo, rhi);
+		uint8_t *d = &pix[c][lby * 8 * QS_RS_W + lbx * 8];
+#pragma unroll
+		for (int y = 0; y < 8; y++) *(uint2 *)(d + y * QS_RS_W) = make_uint2(rlo[y], rhi[y]);
+	}
+	__syncthreads();
+
+	/* pixels: a warp renders a row of 128, four consecutive pixels per lane */
+	const QsSmemPx P0{pix[0], g[0].bx0 * 8, g[0].by0 * 8}, P1{pix[1], g[1].bx0 * 8, g[1].by0 * 8},
+			P2{pix[2], g[2].bx0 * 8, g[2].by0 * 8};
+	const int lane = threadIdx.x & 31, ox = x0 + lane * 4;
+	if (ox > x1) return;
+	const bool ycc = nc >= 3 && im.ycc;
+	for (int oy = y0 + (threadIdx.x >> 5); oy <= y1; oy += QS_RT_THREADS / 32) {
+		uint32_t px[4];
+#pragma unroll
+		for (int i = 0; i < 4; i++) {
+			const int x = min(ox + i, x1);
+			const int y = qs_upsample_at(P0, g[0].hs, g[0].vs, g[0].cw, g[0].ch, x, oy);
+			int c1 = y, c2 = y;
+			if (nc >= 3) {
+				c1 = qs_upsample_at(P1, g[1].hs, g[1].vs, g[1].cw, g[1].ch, x, oy);
+				c2 = qs_upsample_at(P2, g[2].hs, g[2].vs, g[2].cw, g[2].ch, x, oy);
+			}
+			px[i] = qs_rgb_pixel(y, c1, c2, ycc);
+		}
+		const bool full = ox + 3 <= x1;
+		if (layout == QS_RENDER_HWC) {
+			uint8_t *o = im.out + ((size_t)oy * W + ox) * 3;
+			if (full && !((uintptr_t)o & 3)) {
+				uint32_t *o4 = (uint32_t *)o;
+				o4[0] = px[0] | (px[1] << 24);
+				o4[1] = (px[1] >> 8) | (px[2] << 16);
+				o4[2] = (px[2] >> 16) | (px[3] << 8);
+			} else {
+				for (int i = 0; i < 4 && ox + i <= x1; i++) {
+					o[3 * i] = (uint8_t)px[i]; o[3 * i + 1] = (uint8_t)(px[i] >> 8); o[3 * i + 2] = (uint8_t)(px[i] >> 16);
+				}
+			}
+		} else {
+#pragma unroll
+			for (int k = 0; k < 3; k++) {
+				uint8_t *o = im.out + (size_t)k * W * H + (size_t)oy * W + ox;
+				if (full && !((uintptr_t)o & 3)) {
+					*(uint32_t *)o = __byte_perm(__byte_perm(px[0], px[1], 0x0040 + 0x0011 * k),
+							__byte_perm(px[2], px[3], 0x0040 + 0x0011 * k), 0x5410);
+				} else {
+					for (int i = 0; i < 4 && ox + i <= x1; i++) o[i] = (uint8_t)(px[i] >> (8 * k));
+				}
+			}
+		}
+	}
+}
+
+cudaError_t qs_launch_render_async(const QsRenderImg *imgs, int n, int tiles, const int2 *status, int layout,
+		cudaStream_t st) {
+	if (tiles <= 0) return cudaSuccess;
+	QsRenderPack pack;
+	memcpy(pack.img, imgs, (size_t)n * sizeof(QsRenderImg));
+	if (n < QS_RENDER_PACK) memset(pack.img + n, 0, (size_t)(QS_RENDER_PACK - n) * sizeof(QsRenderImg));
+	qs_render_async_kernel<<<tiles, QS_RT_THREADS, 0, st>>>(pack, n, status, layout);
+	return cudaGetLastError();
 }
 
 cudaError_t qs_launch_render_rgb(const uint8_t *const *planes, const int *strides, const int *cw, const int *ch,

@@ -42,4 +42,27 @@ typedef struct {
 typedef struct { QsStatusImg img[QS_MAX_JOBS]; } QsStatusPack;
 cudaError_t qs_launch_async_status(const QsStatusPack *p, int n, const int *flags, int2 *status, cudaStream_t st);
 
+/* per image of a stream-ordered render (qs_cuda.cu render_async); tiles of QS_RENDER_TW x
+ * QS_RENDER_TH output pixels, counted row by row from the image's tile_begin */
+#define QS_RENDER_TW 128
+#define QS_RENDER_TH 64
+typedef struct {
+	const int16_t *coef[3];      /* components 0..2 (1 and 2 unused for a grey image) */
+	const int16_t *coef_up[2];   /* up-sampled chroma at component 0's geometry, or NULL */
+	uint8_t *out;
+	int32_t width, height, tile_begin;
+	int32_t wblk[3], cw[3], ch[3];   /* cw / ch: libjpeg's downsampled_width / downsampled_height */
+	uint8_t hs[3], vs[3];        /* expansion factors max_samp / samp */
+	uint8_t ncomp, ycc;
+	uint8_t up_mode;             /* 0: coef, 1: coef_up (host flag), 2: status[i].upsampled decides */
+	uint8_t pad;
+	uint16_t q[3][64];           /* multipliers: the raw quant table where it de-quantizes, else ones */
+} QsRenderImg;
+#define QS_RENDER_PACK 60
+#define QS_RENDER_HWC 0
+#define QS_RENDER_CHW 1
+/* status: the launch's first image's {stop, upsampled}, or NULL when no image has up_mode 2 */
+cudaError_t qs_launch_render_async(const QsRenderImg *imgs, int n, int tiles, const int2 *status, int layout,
+		cudaStream_t st);
+
 #endif

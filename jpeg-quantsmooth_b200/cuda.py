@@ -125,6 +125,8 @@ def load():
     lib.jpegqs_cuda_async_workspace_bytes.argtypes = [C.c_int, C.POINTER(_Image), C.c_int, C.POINTER(C.c_size_t)]
     lib.jpegqs_cuda_run_async.argtypes = [C.c_void_p, C.c_int, C.POINTER(_Image), C.c_int, C.c_int, C.c_void_p,
                                           C.c_size_t, C.c_void_p, C.c_void_p]
+    lib.jpegqs_cuda_render_async.argtypes = [C.c_void_p, C.c_int, C.POINTER(_Image), C.c_void_p, C.c_int,
+                                             C.c_void_p, C.c_void_p]
     lib.jpegqs_cuda_tables.argtypes = [C.c_int, C.c_void_p]
     lib.jpegqs_cuda_orig_coef.argtypes = [C.c_int, C.c_int]
     _lib = lib
@@ -225,6 +227,13 @@ def async_workspace_bytes(images: Sequence[CoefImage], flags: int) -> int:
     if rc < 0:
         raise QsError(f"jpegqs_cuda_async_workspace_bytes: malformed image ({rc})")
     return int(out.value)
+
+
+def _stream_handle(stream) -> C.c_void_p:
+    """The cudaStream_t to pass for a torch.cuda.Stream.  torch's default stream is the legacy
+    stream, handle 0; the library reads NULL as the context's own stream, which is not ordered with
+    it, so the legacy stream goes in as cudaStreamLegacy (1)."""
+    return C.c_void_p(stream.cuda_stream or 1)
 
 
 def _check_tensor(t, shape, what: str):
@@ -464,12 +473,91 @@ class QsContext:
             status = torch.empty((n, 2), dtype=torch.int32, device=device)
             self._check(self.lib.jpegqs_cuda_run_async(self.h, n, arr, flags & 0x7f, niter, ws.data_ptr(),
                                                        size.value, status.data_ptr() if n else None,
-                                                       C.c_void_p(stream.cuda_stream)))
+                                                       _stream_handle(stream)))
         for i, im in enumerate(images):
             for c, comp in enumerate(im.comps):
                 if comp.quant is not None:
                     comp.quant = np.array(list(arr[i].comp[c].quant), dtype=np.uint16)
         return status, [tuple(u) if u is not None else None for u in ups]
+
+    # ---- stream-ordered render to RGB (include/jpegqs_cuda.h jpegqs_cuda_render_async) ----
+    def render_async(self, images: Sequence[CoefImage], coefs, status=None, up=None, layout: str = "hwc",
+                     out=None, stream=None):
+        """Decode device-resident coefficients to 8-bit RGB, as libjpeg would, without blocking the
+        calling thread.  The coefficient tensors are only read.
+
+        images, coefs, up: as for run_async; `status` and `up` are what run_async returned, so that
+        up-sampled chroma is read from `up` exactly where status[i, 1] is 1 on the device.  status
+        may also be a sequence of per-image booleans (the `upsampled` run_device and
+        run_batch_device report), or None: every image reads `coefs`.
+        layout: "hwc" gives uint8 [H, W, 3] per image, "chw" gives [3, H, W].  out: a sequence of
+        per-image uint8 CUDA tensors of that shape to write (a batched tensor's unbind(0) will do);
+        by default they are allocated on the stream.  stream: a torch.cuda.Stream (default: the
+        current one).  Capturable with torch.cuda.graph.  Returns the list of output tensors."""
+        import torch
+        n = len(images)
+        if layout not in ("hwc", "chw"):
+            raise ValueError(f"layout {layout!r}: expected 'hwc' or 'chw'")
+        if len(coefs) != n or (up is not None and len(up) != n) or (out is not None and len(out) != n):
+            raise ValueError("images, coefs, up and out must have one entry per image")
+        host_up = None
+        if status is not None and not isinstance(status, torch.Tensor):
+            host_up = [bool(u) for u in status]
+            if len(host_up) != n:
+                raise ValueError("status must have one entry per image")
+        tensors = []
+        for i, im in enumerate(images):
+            if len(coefs[i]) != len(im.comps):
+                raise ValueError(f"image {i}: {len(coefs[i])} coefficient tensors for {len(im.comps)} components")
+            for c, (comp, t) in enumerate(zip(im.comps, coefs[i])):
+                _check_tensor(t, (comp.hblk, comp.wblk, 64), f"coefs[{i}][{c}]")
+                tensors.append((f"coefs[{i}][{c}]", t))
+            given = up[i] if up is not None else None
+            if given is not None:
+                if len(given) != 2 or len(im.comps) < 3:
+                    raise ValueError(f"up[{i}]: expected two tensors for a three-component image")
+                y = im.comps[0]
+                for j, t in enumerate(given):
+                    _check_tensor(t, (y.hblk, y.wblk, 64), f"up[{i}][{j}]")
+                    tensors.append((f"up[{i}][{j}]", t))
+            if host_up is not None and host_up[i] and given is None:
+                raise ValueError(f"image {i} is up-sampled but up[{i}] is missing")
+        if isinstance(status, torch.Tensor):
+            if status.dtype != torch.int32 or tuple(status.shape) != (n, 2) or not status.is_contiguous():
+                raise ValueError(f"status: expected a contiguous int32 tensor [{n}, 2]")
+            tensors.append(("status", status))
+        shapes = [(im.height, im.width, 3) if layout == "hwc" else (3, im.height, im.width) for im in images]
+        if out is not None:
+            for i, t in enumerate(out):
+                if not isinstance(t, torch.Tensor):
+                    raise TypeError(f"out[{i}]: expected a torch.Tensor, got {type(t).__name__}")
+                if t.dtype != torch.uint8:
+                    raise TypeError(f"out[{i}]: dtype {t.dtype}, expected torch.uint8")
+                if tuple(t.shape) != shapes[i]:
+                    raise ValueError(f"out[{i}]: shape {tuple(t.shape)}, expected {shapes[i]}")
+                if not t.is_contiguous():
+                    raise ValueError(f"out[{i}]: not contiguous")
+                tensors.append((f"out[{i}]", t))
+        device = self.device if self.device >= 0 else torch.cuda.current_device()
+        for what, t in tensors:
+            if not t.is_cuda or t.device.index != device:
+                raise ValueError(f"{what}: on {t.device}, expected cuda:{device}")
+        stream = stream if stream is not None else torch.cuda.current_stream(device)
+        with torch.cuda.device(device), torch.cuda.stream(stream):
+            if out is None:
+                out = [torch.empty(s, dtype=torch.uint8, device=device) for s in shapes]
+            out = list(out)
+            coef_ptrs = [[t.data_ptr() for t in coefs[i]] for i in range(n)]
+            up_ptrs = [[None, up[i][0].data_ptr(), up[i][1].data_ptr()] if up is not None and up[i] is not None else []
+                       for i in range(n)]
+            arr = _image_array(images, coef_ptrs, up_ptrs)
+            for i in range(n):
+                arr[i].upsampled = int(bool(host_up and host_up[i]))
+            outs = (C.c_void_p * max(n, 1))(*[t.data_ptr() for t in out])
+            self._check(self.lib.jpegqs_cuda_render_async(
+                self.h, n, arr, status.data_ptr() if isinstance(status, torch.Tensor) else None,
+                0 if layout == "hwc" else 1, outs, _stream_handle(stream)))
+        return out
 
     # ---- one slab of a sharded image (include/jpegqs_cuda.h "one image sharded by MCU rows") ----
     def run_slab(self, link, slab: CoefImage, rank: int, world: int, row0: Sequence[int],
@@ -671,3 +759,15 @@ def run_async(images: Sequence[CoefImage], coefs, flags: int, niter: int, up=Non
     if not isinstance(first, torch.Tensor) or not first.is_cuda:
         raise ValueError("run_async: the coefficient tensors must be CUDA tensors")
     return default_context(first.device.index).run_async(images, coefs, flags, niter, up, stream)
+
+
+def render_async(images: Sequence[CoefImage], coefs, status=None, up=None, layout: str = "hwc", out=None,
+                 stream=None):
+    """QsContext.render_async on the default context of the tensors' device: decodes CUDA
+    coefficient tensors to uint8 RGB tensors ([H, W, 3] or [3, H, W]), enqueued on `stream`
+    (default: the current one) without waiting."""
+    import torch
+    first = next((t for ts in coefs for t in ts), None)
+    if not isinstance(first, torch.Tensor) or not first.is_cuda:
+        raise ValueError("render_async: the coefficient tensors must be CUDA tensors")
+    return default_context(first.device.index).render_async(images, coefs, status, up, layout, out, stream)
