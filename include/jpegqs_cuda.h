@@ -91,6 +91,8 @@ void jpegqs_cuda_kernel_stats(const jpegqs_cuda_ctx *ctx, float *idct_ms, int *i
  * key 7: blocks per slab wave for key 6; 0 = SM count x resident warps x 32 (tests force small values)
  * key 8: the two edge coefficients of an anti-diagonal ride along with up to two of its full
  *        coefficients in one "mixed" chunk instead of forming their own
+ * key 9: entropy-coded bytes per decode subsequence of jpegqs_cuda_decode_async (>= 32, default
+ *        512; tests force small values so that every file crosses many subsequence boundaries)
  * keys 0, 2 (lock-step level, warps per sub-partition) only exist in the measurement build
  * (make -C csrc experiments); the shipped library accepts their default values and answers
  * JPEGQS_ERR_UNSUPPORTED otherwise.  key 3: retired, ignored.  key 4: retired (a packed FP32x2
@@ -211,6 +213,91 @@ int jpegqs_cuda_run_async(jpegqs_cuda_ctx *ctx, int nimages, jpegqs_cuda_image *
 int jpegqs_cuda_render_async(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image *imgs,
 		const jpegqs_cuda_status *status_dev, int layout, uint8_t *const *out_dev, void *stream);
 
+/* ---- JPEG files to quantized coefficients -----------------------------------------------------
+ * The first stage of a device pipeline: JPEG bytes -> the coefficients jpeg_read_coefficients gives,
+ * as [hblk][wblk][64] int16 arrays, exactly what jpegqs_cuda_run_async and jpegqs_cuda_render_async
+ * take.  jpegqs_cuda_jpeg_parse reads the markers up to the first SOS on the host;
+ * jpegqs_cuda_decode_async decodes the entropy-coded data on the GPU for the files parse accepts,
+ * jpegqs_cuda_jpeg_read on host threads for all others.
+ *
+ * The scan a device decode needs: what is in force at the first SOS.  No libjpeg types. */
+typedef struct {
+	int32_t ncomp;                    /* components in the scan                                  */
+	int32_t comp[4];                  /* frame component index of scan component k (MCU order)  */
+	int32_t dc_tbl[4], ac_tbl[4];     /* table selectors (Td, Ta) of scan component k            */
+	int32_t dc_present[4], ac_present[4];  /* 1 = table slot defined by a DHT before the SOS     */
+	uint8_t dc_bits[4][17], dc_val[4][256];  /* DHT's BITS (index 1..16; 0 unused) and HUFFVAL  */
+	uint8_t ac_bits[4][17], ac_val[4][256];
+	uint32_t restart_interval;        /* DRI value in force, MCUs; 0 = no restart markers        */
+	uint64_t entropy_offset;          /* byte offset of the first entropy-coded byte in the file */
+	int32_t jpeg_color_space;         /* libjpeg's J_COLOR_SPACE guess (JCS_* values of jpeglib.h) */
+	int32_t sof;                      /* 0xC0 / 0xC1 / 0xC2: the frame's SOF marker             */
+} jpegqs_cuda_scan;
+
+/* Host-only, no device needed.  Fills img (ncomp, is_ycbcr, image size; per component wblk, hblk,
+ * sampling, has_qtbl, quant; coef / coef_up / rows / rows_up NULL) and scan from the markers before
+ * the first SOS, with the marker walk of the jpegqs tool's reader.  Returns
+ *   0                       the device decoder takes the file: SOF0 / SOF1, 8-bit samples, and the
+ *                           first scan holds all 1-4 components;
+ *   JPEGQS_ERR_UNSUPPORTED  img and scan filled, but only jpegqs_cuda_jpeg_read takes it (progressive
+ *                           files, sequential files with more than one scan, Huffman tables libjpeg
+ *                           would reject for a device decode: an all-ones code or a DC symbol > 15);
+ *   JPEGQS_ERR_ARG          what the reader rejects (jpegqs_cuda_last_error(NULL) has its message). */
+int jpegqs_cuda_jpeg_parse(const uint8_t *data, size_t len, jpegqs_cuda_image *img, jpegqs_cuda_scan *scan);
+/* Host decode of any file the jpegqs tool reads (its reader: several threads, libjpeg-compatible
+ * handling of damaged data) into img->comp[c].coef: HOST arrays [hblk][wblk][64] of the geometry
+ * jpegqs_cuda_jpeg_parse reports.  Returns the number of warnings (recoverable damage, >= 0) or
+ * JPEGQS_ERR_ARG (message in jpegqs_cuda_last_error(NULL)). */
+int jpegqs_cuda_jpeg_read(const uint8_t *data, size_t len, const jpegqs_cuda_image *img);
+
+/* Stream-ordered, graph-capturable decode of n files' entropy-coded data on the GPU.
+ *   - Inputs.  data_dev[i]: DEVICE memory holding file i from its first byte, data_len[i] bytes long.
+ *     imgs[i] / scans[i]: what jpegqs_cuda_jpeg_parse returned 0 for (the host structs are read during
+ *     the call only).  The entropy-coded segment starts at scans[i].entropy_offset; the device finds
+ *     its end, the first marker that is not RSTn (any marker when restart_interval is 0).  Bytes
+ *     after it are ignored.
+ *   - Output.  imgs[i].comp[c].coef: DEVICE pointers, 16-byte aligned, [hblk][wblk][64] int16:
+ *     the quantized coefficients jpeg_read_coefficients gives, natural order - run_async's input.
+ *     Blocks of the MCU padding (beyond wblk / hblk in an interleaved scan) are decoded and dropped.
+ *     DC predictors are int and stored as (JCOEF), as libjpeg does.
+ *   - Status.  status_dev[i] (device int32) is 0 when image i decoded cleanly, otherwise an OR of
+ *     the JPEGQS_DECODE_* bits below.  status 0 => the coefficients equal jpeg_read_coefficients'.  A
+ *     flagged image's coefficients are unspecified, but every write stays inside that image's arrays
+ *     and every loop is bounded by the data length; the other images are not affected.
+ *   - Argument errors change nothing: every check runs before the first enqueue and a failed one
+ *     returns JPEGQS_ERR_ARG with nothing enqueued.  Checked: NULL pointers (imgs, scans, data_dev and
+ *     its entries, data_len, status_dev, coef), a coef not 16-byte aligned, rows / rows_up set, a
+ *     workspace too small or not 256-byte aligned, entropy_offset >= data_len, ncomp outside 1..4 or
+ *     unequal to the scan's, scan components that are not a permutation of the frame's, selectors
+ *     naming absent or invalid tables, sampling factors outside 1..4 or more than 10 blocks per MCU,
+ *     and wblk / hblk other than libjpeg's width_in_blocks / height_in_blocks.  A CUDA error while
+ *     enqueueing returns JPEGQS_ERR_CUDA.
+ *   - The stream rules of run_async: no cudaMalloc, no synchronisation, no event record or query, no
+ *     host memory read after return.  Huffman tables and per-image descriptors travel as kernel
+ *     parameters.  Legal under cudaStreamCaptureModeGlobal: a replay decodes the current contents of
+ *     the same data, coef, workspace and status buffers, with the headers (geometry, tables,
+ *     restart interval, entropy offset) and data_len fixed at capture - so a captured graph decodes
+ *     the next file of a stream of same-header files.  Two calls on different streams with separate
+ *     workspaces may be in flight together.  jpegqs_cuda_last_launches counts the launches (ten per
+ *     group of up to 8 images; larger batches run as several groups, one after another).
+ *   - Workspace: all per-call device state (the unstuffed data, restart positions, per-subsequence
+ *     decoder states and counts, the derived Huffman look-up tables).  With A(x) = x rounded up to a
+ *     multiple of 256, L = data_len - entropy_offset, I = ceil(MCUs / restart_interval) (1 without
+ *     restarts; MCUs = blocks for a one-component scan), the size is the sum over images of
+ *       16384 + A(L + 8) + A(24 * ceil(L / 4096)) + 2 * A(4 * I) + A(96 * (floor(L / 32) + I))
+ *     It does not depend on tuning key 9 (it is sized for the smallest value, 32).
+ * Returns 0 or a negative error. */
+#define JPEGQS_DECODE_BAD_CODE   1    /* a bit pattern that is no Huffman code of the table        */
+#define JPEGQS_DECODE_TRUNCATED  2    /* a unit read past the end of its data / restart interval   */
+#define JPEGQS_DECODE_RESTART    4    /* a restart marker missing, extra or out of sequence        */
+#define JPEGQS_DECODE_AC_RUN     8    /* an AC coefficient placed past coefficient 63              */
+#define JPEGQS_DECODE_UNITS     16    /* the data does not hold the image's number of MCUs         */
+int jpegqs_cuda_decode_workspace_bytes(int n, const jpegqs_cuda_image *imgs, const jpegqs_cuda_scan *scans,
+		const size_t *data_len, size_t *bytes);
+int jpegqs_cuda_decode_async(jpegqs_cuda_ctx *ctx, int n, const jpegqs_cuda_image *imgs,
+		const jpegqs_cuda_scan *scans, const uint8_t *const *data_dev, const size_t *data_len,
+		void *workspace, size_t workspace_bytes, int32_t *status_dev, void *stream);
+
 /* ---- one image sharded by MCU rows over several GPUs (SURVEY.md 8e) ----------------------
  * Every rank - a device of this process, or another process on the same box - smooths one slab
  * of contiguous MCU rows and exchanges ONE pixel row per plane with each neighbour after every
@@ -330,6 +417,16 @@ int jpegqs_cuda_orig_coef(int coef, int q);
  * indices); idx = natural-order coefficient indices.  uniform: bit 0 = uniform chunks, bit 1 =
  * mixed chunks; quant == NULL gives the table-independent schedule.  Returns the chunk count (<= 64), or JPEGQS_ERR_ARG. */
 int jpegqs_cuda_chunk_schedule(const uint16_t *quant, int max_coefs, int uniform, uint8_t *out);
+/* jpegqs_cuda_decode_async's algorithm run on the CPU, for one file: the same unstuffing, the same
+ * subsequences of sub_bytes (tuning key 9) bytes, the same speculative decode, synchronisation rounds
+ * (block rounds of 128 subsequences, one grid round, the in-order chain check), placement and final
+ * decode, with the same block and unit decoders; threads run in sequence.  img->comp[c].coef are
+ * HOST arrays.  *status receives the JPEGQS_DECODE_* bits.  overrun (may be NULL, overrun_cap
+ * entries): per subsequence, in order, the units the synchronisation steps decoded past its end
+ * before the chain from its exit met the speculative decode of the next subsequence (0 where it
+ * met at once).  *nsub (may be NULL) receives the subsequence count.  Returns 0 or JPEGQS_ERR_ARG. */
+int jpegqs_cuda_decode_model(const jpegqs_cuda_image *img, const jpegqs_cuda_scan *scan, const uint8_t *data,
+		size_t data_len, int sub_bytes, int32_t *status, uint32_t *overrun, size_t overrun_cap, size_t *nsub);
 
 #ifdef __cplusplus
 }

@@ -39,7 +39,8 @@ def quality_to_flags(quality: int) -> int:
 def __getattr__(name):
     # the CUDA binding is imported lazily so that the host-only helpers
     # (synth, image) work on a machine without the built extension
-    if name in ("cuda", "do_quantsmooth", "run_async", "render_async", "async_workspace_bytes", "QsContext", "lib_path"):
+    if name in ("cuda", "do_quantsmooth", "run_async", "render_async", "async_workspace_bytes", "QsContext", "lib_path",
+                "parse_jpeg", "read_jpeg", "decode_async", "decode_workspace_bytes", "decode_model"):
         import importlib
         _cuda = importlib.import_module(__name__ + ".cuda")
         if name == "cuda":

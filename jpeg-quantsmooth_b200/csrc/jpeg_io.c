@@ -1,0 +1,91 @@
+/*
+ * jpeg_io.c - the host side of reading JPEG files into the library's layout
+ * (include/jpegqs_cuda.h "JPEG files to quantized coefficients"): the header parse that feeds
+ * jpegqs_cuda_decode_async, and the host decode for the files the device decoder does not take.
+ * Both use jpegcoef.c's reader; nothing here parses markers itself.
+ */
+#include <stdio.h>
+#include <stdlib.h>
+#include <string.h>
+#include "jpegcoef.h"
+#include "jpegqs_cuda.h"
+
+void qs_set_host_error(const char *msg);          /* qs_cuda.cu: jpegqs_cuda_last_error(NULL) */
+
+/* libjpeg's rule for a table it decodes with (jdhuff.c jpeg_make_d_derived_tbl): no all-ones code,
+ * DC symbols <= 15.  jpegcoef.c is more lenient; the device decoder relies on it. */
+static int table_ok(const unsigned char *bits, const unsigned char *val, int dc) {
+	int l, i, k = 0; long code = 0;
+	for (l = 1; l <= 16; l++) {
+		for (i = 0; i < bits[l]; i++, k++, code++) if (k >= 256 || (dc && val[k] > 15)) return 0;
+		if (code >= (1L << l)) return 0;
+		code <<= 1;
+	}
+	return 1;
+}
+
+static void fill_image(const jq_image *im, jpegqs_cuda_image *img) {
+	int c, k;
+	memset(img, 0, sizeof(*img));
+	img->ncomp = im->cinfo.num_components;
+	img->is_ycbcr = im->cinfo.jpeg_color_space == JCS_YCbCr;
+	img->image_width = im->cinfo.image_width; img->image_height = im->cinfo.image_height;
+	for (c = 0; c < img->ncomp; c++) {
+		const jpeg_component_info *ci = &im->cinfo.comp_info[c];
+		jpegqs_cuda_comp *o = &img->comp[c];
+		o->wblk = ci->width_in_blocks; o->hblk = ci->height_in_blocks;
+		o->h_samp = ci->h_samp_factor; o->v_samp = ci->v_samp_factor;
+		o->has_qtbl = ci->quant_table != NULL;
+		if (ci->quant_table) for (k = 0; k < 64; k++) o->quant[k] = ci->quant_table->quantval[k];
+	}
+}
+
+int jpegqs_cuda_jpeg_parse(const uint8_t *data, size_t len, jpegqs_cuda_image *img, jpegqs_cuda_scan *scan) {
+	jq_image im; jq_header h; char err[256]; int k, ok;
+	if (!data || !img || !scan) { qs_set_host_error("jpegqs_cuda_jpeg_parse: NULL argument"); return JPEGQS_ERR_ARG; }
+	if (jq_read_header(data, len, &im, &h, err)) { qs_set_host_error(err); return JPEGQS_ERR_ARG; }
+	fill_image(&im, img);
+	memset(scan, 0, sizeof(*scan));
+	scan->ncomp = h.ncomp;
+	for (k = 0; k < 4; k++) {
+		scan->comp[k] = h.ci[k]; scan->dc_tbl[k] = h.td[k]; scan->ac_tbl[k] = h.ta[k];
+		scan->dc_present[k] = h.dc_present[k]; scan->ac_present[k] = h.ac_present[k];
+		memcpy(scan->dc_bits[k], h.dc_bits[k], 17); memcpy(scan->dc_val[k], h.dc_val[k], 256);
+		memcpy(scan->ac_bits[k], h.ac_bits[k], 17); memcpy(scan->ac_val[k], h.ac_val[k], 256);
+	}
+	scan->restart_interval = (uint32_t)h.restart_interval;
+	scan->entropy_offset = h.entropy_offset;
+	scan->jpeg_color_space = (int32_t)im.cinfo.jpeg_color_space;
+	scan->sof = h.sof;
+	jq_free(&im);
+	ok = h.sof != 0xC2 && h.ncomp == img->ncomp && h.entropy_offset < len;
+	for (k = 0; ok && k < h.ncomp; k++)
+		ok = h.dc_present[h.td[k]] && h.ac_present[h.ta[k]] &&
+			table_ok(h.dc_bits[h.td[k]], h.dc_val[h.td[k]], 1) && table_ok(h.ac_bits[h.ta[k]], h.ac_val[h.ta[k]], 0);
+	if (!ok) { qs_set_host_error("jpegqs_cuda_jpeg_parse: only the host reader takes this file"); return JPEGQS_ERR_UNSUPPORTED; }
+	return 0;
+}
+
+int jpegqs_cuda_jpeg_read(const uint8_t *data, size_t len, const jpegqs_cuda_image *img) {
+	jq_image im; char err[256]; int c, warn; JDIMENSION y;
+	if (!data || !img) { qs_set_host_error("jpegqs_cuda_jpeg_read: NULL argument"); return JPEGQS_ERR_ARG; }
+	if (jq_read(data, len, 0, &im, err)) { qs_set_host_error(err); return JPEGQS_ERR_ARG; }
+	if (img->ncomp != im.cinfo.num_components) goto geometry;
+	for (c = 0; c < img->ncomp; c++) {
+		const jpeg_component_info *ci = &im.cinfo.comp_info[c];
+		if (!img->comp[c].coef || img->comp[c].wblk != ci->width_in_blocks || img->comp[c].hblk != ci->height_in_blocks)
+			goto geometry;
+	}
+	for (c = 0; c < img->ncomp; c++) {
+		const jpegqs_cuda_comp *o = &img->comp[c];
+		JBLOCKARRAY rows = im.cinfo.mem->access_virt_barray((j_common_ptr)&im.cinfo, im.coef_arrays[c], 0, o->hblk, FALSE);
+		for (y = 0; y < o->hblk; y++) memcpy(o->coef + (size_t)y * o->wblk * 64, rows[y], (size_t)o->wblk * sizeof(JBLOCK));
+	}
+	warn = im.warnings;
+	jq_free(&im);
+	return warn;
+geometry:
+	jq_free(&im);
+	qs_set_host_error("jpegqs_cuda_jpeg_read: the arrays do not match the file's geometry (or a coef is NULL)");
+	return JPEGQS_ERR_ARG;
+}

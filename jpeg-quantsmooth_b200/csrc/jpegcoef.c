@@ -864,10 +864,11 @@ static unsigned be16(const unsigned char *p) { return (unsigned)p[0] << 8 | p[1]
 
 /* defer: progressive scans are recorded and decoded side by side at the end (returns 1 if that did
  * not work out: the caller reads the file again with defer = 0) */
-static int jq_read_impl(const unsigned char *data, size_t len, int copy, jq_image *im, char *err, int defer) {
+static int jq_read_impl(const unsigned char *data, size_t len, int copy, jq_image *im, char *err, int defer,
+		jq_header *hdr) {
 	const unsigned char *p = data, *end = data + len;
 	jq_priv *pv; jq_dec *d; jq_marker **tail; int have_frame = 0, i, done = 0, adobe = -1;
-	jq_dscan *dsc = NULL; int ndsc = 0, retry = 0;
+	jq_dscan *dsc = NULL; int ndsc = 0, retry = 0, sof_code = 0;
 	memset(im, 0, sizeof(*im));
 	err[0] = 0;
 	if (len < 4 || p[0] != 0xFF || p[1] != 0xD8) { snprintf(err, 256, "not a JPEG file (no SOI)"); return -1; }
@@ -925,6 +926,7 @@ static int jq_read_impl(const unsigned char *data, size_t len, int copy, jq_imag
 			if (have_frame || seglen < 6) { snprintf(err, 256, "bad frame header"); goto fail; }
 			if (seg[0] != 8) { snprintf(err, 256, "%d-bit samples are not supported", seg[0]); goto fail; }
 			im->progressive = code == 0xC2;
+			sof_code = (int)code;
 			im->cinfo.image_height = be16(seg + 1); im->cinfo.image_width = be16(seg + 3);
 			nf = seg[5];
 			if (nf < 1 || nf > 4 || seglen < 6u + 3 * nf || !im->cinfo.image_width || !im->cinfo.image_height) {
@@ -951,6 +953,7 @@ static int jq_read_impl(const unsigned char *data, size_t len, int copy, jq_imag
 				/* libjpeg geometry (jdinput.c initial_setup): not padded to the MCU */
 				c->width_in_blocks = (im->cinfo.image_width * c->h_samp_factor + 8 * maxh - 1) / (8 * maxh);
 				c->height_in_blocks = (im->cinfo.image_height * c->v_samp_factor + 8 * maxv - 1) / (8 * maxv);
+				if (hdr) continue;                          /* header only: no arrays */
 				im->coef_arrays[i] = jq_request((j_common_ptr)&im->cinfo, JPOOL_IMAGE, TRUE,
 						d->mcux * c->h_samp_factor, d->mcuy * c->v_samp_factor, 1);
 				if (!im->coef_arrays[i]) { snprintf(err, 256, "out of memory"); goto fail; }
@@ -979,6 +982,20 @@ static int jq_read_impl(const unsigned char *data, size_t len, int copy, jq_imag
 			if (!im->progressive) { s.Ss = 0; s.Se = 63; s.Ah = s.Al = 0; }
 			if (s.Ss > s.Se || s.Se > 63 || s.Al > 13 || (s.Ss > 0 && ns != 1)) { snprintf(err, 256, "bad scan parameters"); goto fail; }
 			d->ri = im->restart_interval;
+			if (hdr) {                                  /* header only: stop before the entropy-coded data */
+				memset(hdr, 0, sizeof(*hdr));
+				hdr->sof = im->progressive ? 0xC2 : sof_code; hdr->ncomp = ns;
+				for (i = 0; i < ns; i++) { hdr->ci[i] = s.ci[i]; hdr->td[i] = s.td[i]; hdr->ta[i] = s.ta[i]; }
+				for (i = 0; i < 4; i++) {
+					hdr->dc_present[i] = d->dc[i].present; hdr->ac_present[i] = d->ac[i].present;
+					memcpy(hdr->dc_bits[i], d->dc[i].bits, 17); memcpy(hdr->dc_val[i], d->dc[i].val, 256);
+					memcpy(hdr->ac_bits[i], d->ac[i].bits, 17); memcpy(hdr->ac_val[i], d->ac[i].val, 256);
+				}
+				hdr->restart_interval = im->restart_interval;
+				hdr->entropy_offset = (size_t)(p - data);
+				done = 1;
+				continue;
+			}
 			if (defer && im->progressive) {                 /* record the scan, find the next marker */
 				const unsigned char *q = p; jq_dscan *c;
 				if (ndsc == JQ_MAX_DEFER) { retry = 1; goto fail; }
@@ -1037,11 +1054,19 @@ fail:
 
 int jq_read(const unsigned char *data, size_t len, int copy, jq_image *im, char *err) {
 	if (codec_thread_count() >= 2 && !getenv("JPEGQS_SERIAL_DECODE")) {
-		int rc = jq_read_impl(data, len, copy, im, err, 1);
+		int rc = jq_read_impl(data, len, copy, im, err, 1, NULL);
 		if (rc <= 0) return rc;
 		if (getenv("JPEGQS_CODEC_TRACE")) fprintf(stderr, "jpegcoef: reading the file again, scan after scan\n");
 	}
-	return jq_read_impl(data, len, copy, im, err, 0) ? -1 : 0;
+	return jq_read_impl(data, len, copy, im, err, 0, NULL) ? -1 : 0;
+}
+
+int jq_read_header(const unsigned char *data, size_t len, jq_image *im, jq_header *hdr, char *err) {
+	if (!hdr) { snprintf(err, 256, "no header record"); return -1; }
+	memset(hdr, 0, sizeof(*hdr));
+	if (jq_read_impl(data, len, 0, im, err, 0, hdr)) return -1;
+	if (!hdr->ncomp) { jq_free(im); snprintf(err, 256, "no scan found"); return -1; }
+	return 0;
 }
 
 /* ---------------------------------------------------------------- the writer */

@@ -54,6 +54,23 @@ int jq_write(jq_image *im, jvirt_barray_ptr *arrays, int optimize, unsigned char
 
 void jq_free(jq_image *im);
 
+/* What is in force at the first SOS: its component order and table selectors, the Huffman
+ * tables as DHT sent them (bits[0] unused), the restart interval and where the entropy-coded
+ * data starts. */
+typedef struct {
+	int sof;                             /* 0xC0, 0xC1 or 0xC2 */
+	int ncomp, ci[4], td[4], ta[4];      /* scan components (frame indices) and selectors */
+	int dc_present[4], ac_present[4];
+	unsigned char dc_bits[4][17], dc_val[4][256], ac_bits[4][17], ac_val[4][256];
+	int restart_interval;
+	size_t entropy_offset;
+} jq_header;
+
+/* jq_read's marker walk up to the first SOS: fills im->cinfo (frame, quant tables, colour space)
+ * and hdr without reading entropy-coded data and without allocating coefficient arrays.  Returns 0,
+ * or -1 with a message in err.  im must be released with jq_free. */
+int jq_read_header(const unsigned char *data, size_t len, jq_image *im, jq_header *hdr, char *err);
+
 /* worker threads of the codec: 0 = one per processor (at most 16).  The writer codes segments of
  * MCU rows on them; the reader decodes sequential (SOF0/SOF1) scans on them - restart intervals as
  * they are, scans without restart markers by speculative parsing of chunks that are stitched where

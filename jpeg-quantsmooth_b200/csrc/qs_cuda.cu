@@ -192,6 +192,7 @@ struct jpegqs_cuda_ctx {
 	/* optional per-kernel timing (bench.py's roofline line): event pairs around launches */
 	int profiling;
 	int tune_sync, tune_maxn, tune_wpg, tune_gs, tune_uni, tune_slabs, tune_wave, tune_merge;              /* kernel variant knobs (jpegqs_cuda_set_tuning) */
+	int tune_decode;                       /* key 9: entropy-coded bytes per decode subsequence */
 	std::vector<cudaEvent_t> ev_pool; size_t ev_used;
 	std::vector<int> ev_kind;              /* 0 = idct pass, 1 = smoothing pass, per pair */
 	float kernel_ms[2]; int kernel_launches[2];
@@ -275,6 +276,7 @@ extern "C" int jpegqs_cuda_create(int device, jpegqs_cuda_ctx **out) {
 	ctx->arena = NULL; ctx->arena_cap = ctx->arena_pos = 0; ctx->workspace = false; ctx->ev0 = ctx->ev1 = NULL;
 	ctx->last_ms = 0; ctx->launches = 0;
 	ctx->profiling = 0; ctx->ev_used = 0; ctx->tune_sync = 2; ctx->tune_maxn = 4; ctx->tune_wpg = 4; ctx->tune_gs = 1; ctx->tune_uni = 1; ctx->tune_merge = 1; ctx->tune_slabs = 1; ctx->tune_wave = 0;
+	ctx->tune_decode = 512;
 	ctx->kernel_ms[0] = ctx->kernel_ms[1] = 0; ctx->kernel_launches[0] = ctx->kernel_launches[1] = 0;
 	int rc = [&]() -> int {
 		CK(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking));
@@ -610,8 +612,20 @@ extern "C" int jpegqs_cuda_set_tuning(jpegqs_cuda_ctx *ctx, int key, int value) 
 	}
 	if (key == 6) { ctx->tune_slabs = value ? 1 : 0; return 0; }
 	if (key == 7) { if (value < 0) return JPEGQS_ERR_ARG; ctx->tune_wave = value; return 0; }
+	if (key == 9) { if (value < 32) return JPEGQS_ERR_ARG; ctx->tune_decode = value; return 0; }
 	return JPEGQS_ERR_ARG;
 }
+
+/* for qs_decode.cu: the context's device, stream and key 9; the launch count and message of a call */
+void qs_ctx_decode_info(jpegqs_cuda_ctx *ctx, int *device, cudaStream_t *stream, int *sub_bytes) {
+	*device = ctx->device; *stream = ctx->stream; *sub_bytes = ctx->tune_decode;
+}
+void qs_ctx_decode_done(jpegqs_cuda_ctx *ctx, int launches, const char *err) {
+	ctx->launches = launches;
+	if (err && err[0]) snprintf(ctx->err, sizeof(ctx->err), "%s", err);
+}
+/* for the host-only entry points (jpeg_io.c, qs_decode.cu): jpegqs_cuda_last_error(NULL) */
+extern "C" void qs_set_host_error(const char *msg) { snprintf(g_err, sizeof(g_err), "%s", msg); }
 extern "C" int jpegqs_cuda_chunk_schedule(const uint16_t *quant, int max_coefs, int uniform, uint8_t *out) {
 	if (max_coefs < 1 || max_coefs > 4 || !out) return JPEGQS_ERR_ARG;
 	uint16_t q[64];

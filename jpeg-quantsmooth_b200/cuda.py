@@ -14,7 +14,7 @@ from typing import List, Optional, Sequence
 
 import numpy as np
 
-from .image import CoefImage, JCS_YCbCr
+from .image import CoefImage, Component, JCS_YCbCr
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 MAX_COMP = 10
@@ -41,6 +41,16 @@ class _Image(C.Structure):
     _fields_ = [("ncomp", C.c_int32), ("is_ycbcr", C.c_int32),
                 ("image_width", C.c_uint32), ("image_height", C.c_uint32),
                 ("comp", _Comp * MAX_COMP), ("upsampled", C.c_int32)]
+
+
+class _Scan(C.Structure):
+    """jpegqs_cuda_scan: what is in force at a file's first SOS (include/jpegqs_cuda.h)."""
+    _fields_ = [("ncomp", C.c_int32), ("comp", C.c_int32 * 4), ("dc_tbl", C.c_int32 * 4), ("ac_tbl", C.c_int32 * 4),
+                ("dc_present", C.c_int32 * 4), ("ac_present", C.c_int32 * 4),
+                ("dc_bits", (C.c_uint8 * 17) * 4), ("dc_val", (C.c_uint8 * 256) * 4),
+                ("ac_bits", (C.c_uint8 * 17) * 4), ("ac_val", (C.c_uint8 * 256) * 4),
+                ("restart_interval", C.c_uint32), ("entropy_offset", C.c_uint64),
+                ("jpeg_color_space", C.c_int32), ("sof", C.c_int32)]
 
 
 class _Job(C.Structure):
@@ -127,6 +137,14 @@ def load():
                                           C.c_size_t, C.c_void_p, C.c_void_p]
     lib.jpegqs_cuda_render_async.argtypes = [C.c_void_p, C.c_int, C.POINTER(_Image), C.c_void_p, C.c_int,
                                              C.c_void_p, C.c_void_p]
+    lib.jpegqs_cuda_jpeg_parse.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(_Image), C.POINTER(_Scan)]
+    lib.jpegqs_cuda_jpeg_read.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(_Image)]
+    lib.jpegqs_cuda_decode_workspace_bytes.argtypes = [C.c_int, C.POINTER(_Image), C.POINTER(_Scan),
+                                                       C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
+    lib.jpegqs_cuda_decode_async.argtypes = [C.c_void_p, C.c_int, C.POINTER(_Image), C.POINTER(_Scan), C.c_void_p,
+                                             C.POINTER(C.c_size_t), C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
+    lib.jpegqs_cuda_decode_model.argtypes = [C.POINTER(_Image), C.POINTER(_Scan), C.c_char_p, C.c_size_t, C.c_int,
+                                             C.POINTER(C.c_int32), C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
     lib.jpegqs_cuda_tables.argtypes = [C.c_int, C.c_void_p]
     lib.jpegqs_cuda_orig_coef.argtypes = [C.c_int, C.c_int]
     _lib = lib
@@ -227,6 +245,92 @@ def async_workspace_bytes(images: Sequence[CoefImage], flags: int) -> int:
     if rc < 0:
         raise QsError(f"jpegqs_cuda_async_workspace_bytes: malformed image ({rc})")
     return int(out.value)
+
+
+# ---- JPEG files (include/jpegqs_cuda.h "JPEG files to quantized coefficients") ----
+DECODE_BAD_CODE, DECODE_TRUNCATED, DECODE_RESTART, DECODE_AC_RUN, DECODE_UNITS = 1, 2, 4, 8, 16
+DECODE_SUB_MIN, DECODE_SUB_DEFAULT = 32, 512
+
+
+def _placeholder(shape):
+    """An int16 array of this shape that costs no memory (all elements alias one zero)."""
+    return np.broadcast_to(np.zeros((), dtype=np.int16), shape)
+
+
+def _parse(data: bytes):
+    lib = load()
+    data = bytes(data)
+    ci, sc = _Image(), _Scan()
+    rc = lib.jpegqs_cuda_jpeg_parse(data, len(data), C.byref(ci), C.byref(sc))
+    if rc not in (0, -3):
+        raise QsError(f"parse_jpeg: {lib.jpegqs_cuda_last_error(None).decode()}")
+    comps = []
+    for c in range(ci.ncomp):
+        cc = ci.comp[c]
+        q = np.array(list(cc.quant), dtype=np.uint16) if cc.has_qtbl else None
+        comps.append(Component(coef=_placeholder((cc.hblk, cc.wblk, 64)), quant=q, h_samp=cc.h_samp,
+                               v_samp=cc.v_samp, quant_tbl_no=min(c, 1)))
+    image = CoefImage(width=ci.image_width, height=ci.image_height, colorspace=int(sc.jpeg_color_space), comps=comps)
+    return image, (sc if rc == 0 else None), sc
+
+
+def parse_jpeg(data: bytes):
+    """The header of a JPEG file, host-only: (CoefImage, scan).  The CoefImage carries the geometry,
+    sampling, quant tables and colour space; its arrays are placeholders of the right shape that
+    cost no memory.  scan (a jpegqs_cuda_scan) is what decode_async needs, or None when only
+    read_jpeg takes the file (progressive, several scans).  Raises QsError for what the reader
+    rejects (truncated headers, lossless / arithmetic / 12-bit files)."""
+    image, scan, _ = _parse(data)
+    return image, scan
+
+
+def read_jpeg(data: bytes) -> CoefImage:
+    """Host decode of any file the jpegqs tool reads, with its reader: the quantized coefficients
+    jpeg_read_coefficients gives, as numpy int16 [hblk, wblk, 64] arrays."""
+    lib = load()
+    data = bytes(data)
+    image, _, _ = _parse(data)
+    ci = _Image()
+    arrays = [np.zeros((c.hblk, c.wblk, 64), dtype=np.int16) for c in image.comps]
+    for c, a in zip(image.comps, arrays):
+        c.coef = a
+    _fill_image(ci, image, [a.ctypes.data for a in arrays], [])
+    rc = lib.jpegqs_cuda_jpeg_read(data, len(data), C.byref(ci))
+    if rc < 0:
+        raise QsError(f"read_jpeg: {lib.jpegqs_cuda_last_error(None).decode()}")
+    return image
+
+
+def decode_workspace_bytes(images: Sequence[CoefImage], scans, data_len: Sequence[int]) -> int:
+    """Device bytes of workspace decode_async needs (host-only)."""
+    lib = load()
+    n = len(images)
+    arr = _image_array(images)
+    sc = (_Scan * max(n, 1))(*scans)
+    lens = (C.c_size_t * max(n, 1))(*[int(x) for x in data_len])
+    out = C.c_size_t(0)
+    if lib.jpegqs_cuda_decode_workspace_bytes(n, arr, sc, lens, C.byref(out)) < 0:
+        raise QsError(lib.jpegqs_cuda_last_error(None).decode())
+    return int(out.value)
+
+
+def decode_model(image: CoefImage, scan, data: bytes, sub_bytes: int = DECODE_SUB_DEFAULT, out=None):
+    """decode_async's algorithm run on the CPU for one file (jpegqs_cuda_decode_model).  out: numpy
+    int16 arrays to write (default: new ones).  Returns (arrays, status, overrun), overrun the units
+    the synchronisation decoded past each subsequence's end."""
+    lib = load()
+    data = bytes(data)
+    if out is None:
+        out = [np.zeros((c.hblk, c.wblk, 64), dtype=np.int16) for c in image.comps]
+    ci = _Image()
+    _fill_image(ci, image, [a.ctypes.data for a in out], [])
+    cap = len(data) // DECODE_SUB_MIN + 1 + (image.comps[0].wblk * image.comps[0].hblk if scan.restart_interval else 1)
+    over = np.zeros(cap, dtype=np.uint32)
+    st, nsub = C.c_int32(0), C.c_size_t(0)
+    if lib.jpegqs_cuda_decode_model(C.byref(ci), C.byref(scan), data, len(data), sub_bytes, C.byref(st),
+                                    over.ctypes.data, cap, C.byref(nsub)) < 0:
+        raise QsError(lib.jpegqs_cuda_last_error(None).decode())
+    return out, int(st.value), over[:nsub.value]
 
 
 def _stream_handle(stream) -> C.c_void_p:
@@ -559,6 +663,66 @@ class QsContext:
                 0 if layout == "hwc" else 1, outs, _stream_handle(stream)))
         return out
 
+    # ---- JPEG bytes to coefficients (include/jpegqs_cuda.h jpegqs_cuda_decode_async) ----
+    def decode_async(self, images: Sequence[CoefImage], scans, data, out=None, stream=None):
+        """Decode JPEG files held in device memory to quantized coefficient tensors, without
+        blocking the calling thread.
+
+        images, scans: what parse_jpeg returned for each file (scan not None).  data[i]: a 1-D
+        contiguous uint8 CUDA tensor with file i's bytes.  out[i][c] (optional): int16 CUDA tensors
+        [hblk, wblk, 64] to write; by default they are allocated on the stream.  stream: a
+        torch.cuda.Stream (default: the current one).  Returns (coefs, status): coefs[i][c] the
+        tensors (run_async's and render_async's input), status an int32 device tensor [n], 0 where
+        image i decoded cleanly, else DECODE_* bits.  Capturable with torch.cuda.graph: a replay
+        decodes the current contents of the same data tensors."""
+        import torch
+        n = len(images)
+        if len(scans) != n or len(data) != n or (out is not None and len(out) != n):
+            raise ValueError("images, scans, data and out must have one entry per image")
+        tensors = []
+        for i, (im, sc) in enumerate(zip(images, scans)):
+            if sc is None or not isinstance(sc, _Scan):
+                raise ValueError(f"scans[{i}]: not a decodable scan (parse_jpeg gave None: use read_jpeg)")
+            t = data[i]
+            if not isinstance(t, torch.Tensor):
+                raise TypeError(f"data[{i}]: expected a torch.Tensor, got {type(t).__name__}")
+            if t.dtype != torch.uint8 or t.dim() != 1 or not t.is_contiguous():
+                raise ValueError(f"data[{i}]: expected a contiguous 1-D uint8 tensor")
+            if t.numel() <= sc.entropy_offset:
+                raise ValueError(f"data[{i}]: {t.numel()} bytes, the entropy-coded data starts at {sc.entropy_offset}")
+            tensors.append((f"data[{i}]", t))
+            if out is not None:
+                if len(out[i]) != len(im.comps):
+                    raise ValueError(f"out[{i}]: {len(out[i])} tensors for {len(im.comps)} components")
+                for c, (comp, o) in enumerate(zip(im.comps, out[i])):
+                    _check_tensor(o, (comp.hblk, comp.wblk, 64), f"out[{i}][{c}]")
+                    if o.data_ptr() % 16:
+                        raise ValueError(f"out[{i}][{c}]: not 16-byte aligned")
+                    tensors.append((f"out[{i}][{c}]", o))
+        device = self.device if self.device >= 0 else torch.cuda.current_device()
+        for what, t in tensors:
+            if not t.is_cuda or t.device.index != device:
+                raise ValueError(f"{what}: on {t.device}, expected cuda:{device}")
+        stream = stream if stream is not None else torch.cuda.current_stream(device)
+        with torch.cuda.device(device), torch.cuda.stream(stream):
+            if out is None:
+                out = [[torch.empty((c.hblk, c.wblk, 64), dtype=torch.int16, device=device) for c in im.comps]
+                       for im in images]
+            out = [list(o) for o in out]
+            arr = _image_array(images, [[t.data_ptr() for t in out[i]] for i in range(n)])
+            sc = (_Scan * max(n, 1))(*scans)
+            lens = (C.c_size_t * max(n, 1))(*[int(t.numel()) for t in data])
+            ptrs = (C.c_void_p * max(n, 1))(*[t.data_ptr() for t in data])
+            size = C.c_size_t(0)
+            if self.lib.jpegqs_cuda_decode_workspace_bytes(n, arr, sc, lens, C.byref(size)) < 0:
+                raise QsError(self.lib.jpegqs_cuda_last_error(None).decode())
+            # allocated on `stream`: reused only by work queued after this call's kernels
+            ws = torch.empty(max(size.value, 1), dtype=torch.uint8, device=device)
+            status = torch.empty((n,), dtype=torch.int32, device=device)
+            self._check(self.lib.jpegqs_cuda_decode_async(self.h, n, arr, sc, ptrs, lens, ws.data_ptr(), size.value,
+                                                          status.data_ptr() if n else None, _stream_handle(stream)))
+        return out, status
+
     # ---- one slab of a sharded image (include/jpegqs_cuda.h "one image sharded by MCU rows") ----
     def run_slab(self, link, slab: CoefImage, rank: int, world: int, row0: Sequence[int],
                  hblk_total: Sequence[int], flags: int, niter: int, coef_ptrs=None, up_ptrs=None, stream: int = 0):
@@ -759,6 +923,17 @@ def run_async(images: Sequence[CoefImage], coefs, flags: int, niter: int, up=Non
     if not isinstance(first, torch.Tensor) or not first.is_cuda:
         raise ValueError("run_async: the coefficient tensors must be CUDA tensors")
     return default_context(first.device.index).run_async(images, coefs, flags, niter, up, stream)
+
+
+def decode_async(images: Sequence[CoefImage], scans, data, out=None, stream=None):
+    """QsContext.decode_async on the default context of the data tensors' device: decodes JPEG
+    files in CUDA uint8 tensors to int16 coefficient tensors, enqueued on `stream` (default: the
+    current one) without waiting.  Returns (coefs, status [n] int32 device tensor)."""
+    import torch
+    first = next(iter(data), None)
+    if not isinstance(first, torch.Tensor) or not first.is_cuda:
+        raise ValueError("decode_async: the data tensors must be CUDA tensors")
+    return default_context(first.device.index).decode_async(images, scans, data, out, stream)
 
 
 def render_async(images: Sequence[CoefImage], coefs, status=None, up=None, layout: str = "hwc", out=None,
