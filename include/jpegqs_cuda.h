@@ -298,6 +298,103 @@ int jpegqs_cuda_decode_async(jpegqs_cuda_ctx *ctx, int n, const jpegqs_cuda_imag
 		const jpegqs_cuda_scan *scans, const uint8_t *const *data_dev, const size_t *data_len,
 		void *workspace, size_t workspace_bytes, int32_t *status_dev, void *stream);
 
+/* ---- quantized coefficients to JPEG files ----------------------------------------------------
+ * The last stage of a device pipeline: the coefficients decode_async / run_async leave on the GPU
+ * written as the sequential Huffman JPEG file the jpegqs tool writes for them (its writer, jpegcoef.c
+ * jq_write), byte for byte.
+ *
+ * The prefix: what jq_write puts before its first DQT - SOI, the JFIF APP0 (grayscale / YCbCr, with
+ * the input's version and density) or Adobe APP14 (RGB / CMYK / YCCK), then the input's APPn / COM
+ * markers copied at level `copy` (0 none, 1 COM, 2 COM + APPn; the tool's -c), markers between the
+ * scans of a progressive file included.  It depends on the input file only.  Host-only: walks the
+ * file's markers without decoding entropy-coded data.  *out_len receives the prefix length (out may
+ * be NULL to ask for it), *ncomp the frame's component count, comp_id / quant_tbl its component
+ * identifiers and quantization table numbers (entries past the component count 0).  Returns 0, or JPEGQS_ERR_ARG for what the
+ * tool's reader rejects or when the prefix does not fit cap (jpegqs_cuda_last_error(NULL)). */
+int jpegqs_cuda_jpeg_prefix(const uint8_t *data, size_t len, int copy, uint8_t *out, size_t cap, size_t *out_len,
+		int32_t *ncomp, int32_t comp_id[4], int32_t quant_tbl[4]);
+
+/* What the device writes in front of the entropy-coded data of image i besides the DQT, SOF, DHT and
+ * SOS segments: jpegqs_cuda_jpeg_prefix's output, in DEVICE memory, and the frame's identifiers. */
+typedef struct {
+	const uint8_t *prefix_dev;   /* DEVICE memory: the prefix bytes (host memory for encode_model) */
+	uint32_t prefix_len;
+	int32_t comp_id[4];          /* SOF / SOS component identifiers                                */
+	int32_t quant_tbl[4];        /* SOF quantization table numbers (0..3); DQT follows them        */
+} jpegqs_cuda_jpeg_head;
+
+/* Stream-ordered, graph-capturable encode of n images' coefficients to JPEG files on the GPU.
+ *   - What it writes.  For image i: heads[i]'s prefix, then what jq_write(..., optimize) writes for
+ *     these coefficients, geometry and quant tables: DQT for each table in use in component order
+ *     (16-bit, with SOF1, when a value exceeds 255), SOF0 / SOF1, DHT - with optimize 0 the T.81 K.3.3
+ *     tables, with optimize 1 optimal tables built from this image's symbol counts (T.81 K.2 with
+ *     jq_write's tie-breaking), two table pairs when there is more than one component - SOS, one
+ *     interleaved sequential scan without restart markers, EOI.  Blocks of the MCU padding code a DC
+ *     difference of 0 and no AC (libjpeg's jctrans.c), the last byte is filled with 1-bits, 0xFF
+ *     bytes are stuffed.  quant[] of a component with has_qtbl is written as its table (the values,
+ *     ones after run_async, are not applied to the coefficients).
+ *   - Inputs.  comp[].coef / coef_up: DEVICE pointers on the context's device, 16-byte aligned, of
+ *     libjpeg's wblk / hblk; rows / rows_up NULL.  1-4 components, sampling factors 1..4, at most 10
+ *     blocks per MCU, image size 1..65535.
+ *   - Chroma source, render_async's rule.  An image UPSAMPLE_UV can up-sample (YCbCr, three components,
+ *     chroma 1x1, luma not) is written "up-sampled" - components 1 and 2 from coef_up, all three
+ *     sampled 1x1 at the luma's block geometry, what do_quantsmooth leaves in cinfo - when
+ *       . run_status_dev != NULL: run_status_dev[i].upsampled != 0 on the device, for images whose two
+ *         coef_up pointers are set.  So one graph may hold decode -> run_async -> encode, and a replay
+ *         in which an image stops writes it at its sampling.  An image that can be up-sampled but was
+ *         given no coef_up is written as sampled; if the run status says it was up-sampled, its status
+ *         gets JPEGQS_ENCODE_NO_UP (the file is valid, but its chroma is not what the tool writes).
+ *       . run_status_dev == NULL: imgs[i].upsampled != 0 (coef_up then required).
+ *   - Output.  out_dev[i]: out_cap[i] bytes of device memory at any alignment.  len_dev[i] (device
+ *     uint64) receives the file length, status_dev[i] (device int32) 0 or an OR of the bits below.
+ *     On OVERFLOW len_dev[i] holds the length the file needs and nothing is written at or past
+ *     out_cap[i].  On RANGE the file is not valid (jq_write fails there with "coefficient out of range
+ *     for Huffman coding"); the writes stay inside out_cap[i] all the same.  A flagged image does not
+ *     affect the others.
+ *   - Bound.  jpegqs_cuda_encode_bound returns a capacity that never overflows: with U the blocks of
+ *     the scan (MCUs x blocks per MCU; the larger of the two geometries for an image that can be
+ *     up-sampled), prefix_len + 1680 + 2 * ceil(U * 1665 / 8) - a block codes to at most 1665 bits,
+ *     stuffing at most doubles the bytes, and DQT + SOF + DHT + SOS + EOI take at most 1680.
+ *   - Argument errors change nothing: every check runs before the first enqueue and a failed one
+ *     returns JPEGQS_ERR_ARG with nothing enqueued.  Checked: NULL pointers (imgs, heads, out_dev and
+ *     its entries, out_cap, len_dev, status_dev, workspace, coef, a prefix_dev of a non-empty prefix),
+ *     rows / rows_up set, coef / coef_up not 16-byte aligned, ncomp outside 1..4, sampling factors
+ *     outside 1..4, more than 10 blocks per MCU, wblk / hblk other than libjpeg's, an image size
+ *     outside 1..65535, comp_id outside 0..255 or quant_tbl outside 0..3, imgs[i].upsampled on an
+ *     image that cannot be up-sampled or without coef_up (run_status_dev NULL), a workspace too small
+ *     or not 256-byte aligned, and out_cap[i] < prefix_len.  A CUDA error while enqueueing returns
+ *     JPEGQS_ERR_CUDA.
+ *   - The stream rules of decode_async: no cudaMalloc, no synchronisation, no event record or query.
+ *     Descriptors, quant tables and the standard Huffman tables travel as kernel parameters; nothing
+ *     of imgs or heads is read after return.  Legal under cudaStreamCaptureModeGlobal: a replay
+ *     encodes the current contents of the same coefficient, prefix and status buffers with the
+ *     geometry, quant tables and identifiers fixed at capture.  Two calls on different streams with
+ *     separate workspaces may be in flight together.  jpegqs_cuda_last_launches counts the launches
+ *     (nine per group of up to 16 images, ten with optimize); larger batches run as several groups,
+ *     one after another on the stream.
+ *   - Workspace: all per-call device state.  With A(x) = x rounded up to a multiple of 256 and U as
+ *     for the bound, T = ceil(U / 256), W = ceil(U * 1665 / 32) + 2, the size is the sum over images of
+ *       32768 + A(2 * U) + A(8 * T) + A(4 * W) + A(4 * ceil(4 * W / 4096))
+ *     (descriptor, state and tables; bits per block; bits per tile; the unstuffed bits, sized for the
+ *     worst case; 0xFF counts per 4 KB).  It does not depend on optimize.  An 8K (7680 x 4320) 4:2:0
+ *     image that can be up-sampled has U = 1 555 200 and needs 324 MB, most of it the bit buffer.
+ * Returns 0 or a negative error. */
+#define JPEGQS_ENCODE_RANGE    1   /* a DC difference of category > 11 or an AC value of category > 10 */
+#define JPEGQS_ENCODE_OVERFLOW 2   /* the file does not fit out_cap; len_dev holds the size it needs   */
+#define JPEGQS_ENCODE_NO_UP    4   /* run status up-sampled, coef_up not given: written as sampled     */
+int jpegqs_cuda_encode_bound(const jpegqs_cuda_image *img, size_t prefix_len, size_t *bytes);
+int jpegqs_cuda_encode_workspace_bytes(int n, const jpegqs_cuda_image *imgs, int optimize, size_t *bytes);
+int jpegqs_cuda_encode_async(jpegqs_cuda_ctx *ctx, int n, const jpegqs_cuda_image *imgs,
+		const jpegqs_cuda_jpeg_head *heads, int optimize, const jpegqs_cuda_status *run_status_dev,
+		uint8_t *const *out_dev, const size_t *out_cap, uint64_t *len_dev, int32_t *status_dev,
+		void *workspace, size_t workspace_bytes, void *stream);
+/* jpegqs_cuda_encode_async's algorithm on the CPU for one image: the same unit, predictor, table,
+ * header and stuffing functions in the same order on one thread.  img->comp[c].coef / coef_up and
+ * head->prefix_dev are HOST memory; imgs->upsampled picks the geometry.  *len / *status as len_dev /
+ * status_dev.  Returns 0 or JPEGQS_ERR_ARG. */
+int jpegqs_cuda_encode_model(const jpegqs_cuda_image *img, const jpegqs_cuda_jpeg_head *head, int optimize,
+		uint8_t *out, size_t cap, uint64_t *len, int32_t *status);
+
 /* ---- one image sharded by MCU rows over several GPUs (SURVEY.md 8e) ----------------------
  * Every rank - a device of this process, or another process on the same box - smooths one slab
  * of contiguous MCU rows and exchanges ONE pixel row per plane with each neighbour after every

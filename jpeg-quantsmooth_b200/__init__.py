@@ -40,7 +40,8 @@ def __getattr__(name):
     # the CUDA binding is imported lazily so that the host-only helpers
     # (synth, image) work on a machine without the built extension
     if name in ("cuda", "do_quantsmooth", "run_async", "render_async", "async_workspace_bytes", "QsContext", "lib_path",
-                "parse_jpeg", "read_jpeg", "decode_async", "decode_workspace_bytes", "decode_model"):
+                "parse_jpeg", "read_jpeg", "decode_async", "decode_workspace_bytes", "decode_model",
+                "jpeg_prefix", "encode_bound", "encode_workspace_bytes", "encode_model", "encode_async"):
         import importlib
         _cuda = importlib.import_module(__name__ + ".cuda")
         if name == "cuda":

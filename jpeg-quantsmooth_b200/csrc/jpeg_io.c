@@ -89,3 +89,24 @@ geometry:
 	qs_set_host_error("jpegqs_cuda_jpeg_read: the arrays do not match the file's geometry (or a coef is NULL)");
 	return JPEGQS_ERR_ARG;
 }
+
+int jpegqs_cuda_jpeg_prefix(const uint8_t *data, size_t len, int copy, uint8_t *out, size_t cap, size_t *out_len,
+		int32_t *ncomp, int32_t comp_id[4], int32_t quant_tbl[4]) {
+	jq_image im; char err[256]; unsigned char *p = NULL; size_t n = 0; int k;
+	if (!data || !out_len || !ncomp || !comp_id || !quant_tbl) { qs_set_host_error("jpegqs_cuda_jpeg_prefix: NULL argument"); return JPEGQS_ERR_ARG; }
+	if (copy < 0 || copy > 2) { qs_set_host_error("jpegqs_cuda_jpeg_prefix: copy level outside 0..2"); return JPEGQS_ERR_ARG; }
+	if (jq_read_markers(data, len, copy, &im, err)) { qs_set_host_error(err); return JPEGQS_ERR_ARG; }
+	if (jq_prefix(&im, &p, &n)) { jq_free(&im); qs_set_host_error("jpegqs_cuda_jpeg_prefix: out of memory"); return JPEGQS_ERR_ARG; }
+	*out_len = n;
+	*ncomp = im.cinfo.num_components;
+	for (k = 0; k < 4; k++) {
+		int have = k < im.cinfo.num_components;
+		comp_id[k] = have ? im.comp_id[k] : 0;
+		quant_tbl[k] = have ? im.cinfo.comp_info[k].quant_tbl_no : 0;
+	}
+	jq_free(&im);
+	if (out && cap >= n) memcpy(out, p, n);
+	free(p);
+	if (out && cap < n) { qs_set_host_error("jpegqs_cuda_jpeg_prefix: the prefix does not fit out (*out_len holds its size)"); return JPEGQS_ERR_ARG; }
+	return 0;
+}

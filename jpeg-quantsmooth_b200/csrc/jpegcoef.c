@@ -865,7 +865,7 @@ static unsigned be16(const unsigned char *p) { return (unsigned)p[0] << 8 | p[1]
 /* defer: progressive scans are recorded and decoded side by side at the end (returns 1 if that did
  * not work out: the caller reads the file again with defer = 0) */
 static int jq_read_impl(const unsigned char *data, size_t len, int copy, jq_image *im, char *err, int defer,
-		jq_header *hdr) {
+		jq_header *hdr, int skip_data) {
 	const unsigned char *p = data, *end = data + len;
 	jq_priv *pv; jq_dec *d; jq_marker **tail; int have_frame = 0, i, done = 0, adobe = -1;
 	jq_dscan *dsc = NULL; int ndsc = 0, retry = 0, sof_code = 0;
@@ -953,7 +953,7 @@ static int jq_read_impl(const unsigned char *data, size_t len, int copy, jq_imag
 				/* libjpeg geometry (jdinput.c initial_setup): not padded to the MCU */
 				c->width_in_blocks = (im->cinfo.image_width * c->h_samp_factor + 8 * maxh - 1) / (8 * maxh);
 				c->height_in_blocks = (im->cinfo.image_height * c->v_samp_factor + 8 * maxv - 1) / (8 * maxv);
-				if (hdr) continue;                          /* header only: no arrays */
+				if (hdr || skip_data) continue;             /* header / markers only: no arrays */
 				im->coef_arrays[i] = jq_request((j_common_ptr)&im->cinfo, JPOOL_IMAGE, TRUE,
 						d->mcux * c->h_samp_factor, d->mcuy * c->v_samp_factor, 1);
 				if (!im->coef_arrays[i]) { snprintf(err, 256, "out of memory"); goto fail; }
@@ -994,6 +994,10 @@ static int jq_read_impl(const unsigned char *data, size_t len, int copy, jq_imag
 				hdr->restart_interval = im->restart_interval;
 				hdr->entropy_offset = (size_t)(p - data);
 				done = 1;
+				continue;
+			}
+			if (skip_data) {                            /* markers only: on to the next marker, as defer does */
+				while (p + 1 < end && !(p[0] == 0xFF && p[1] != 0 && p[1] != 0xFF && (p[1] & 0xF8) != 0xD0)) p++;
 				continue;
 			}
 			if (defer && im->progressive) {                 /* record the scan, find the next marker */
@@ -1054,19 +1058,23 @@ fail:
 
 int jq_read(const unsigned char *data, size_t len, int copy, jq_image *im, char *err) {
 	if (codec_thread_count() >= 2 && !getenv("JPEGQS_SERIAL_DECODE")) {
-		int rc = jq_read_impl(data, len, copy, im, err, 1, NULL);
+		int rc = jq_read_impl(data, len, copy, im, err, 1, NULL, 0);
 		if (rc <= 0) return rc;
 		if (getenv("JPEGQS_CODEC_TRACE")) fprintf(stderr, "jpegcoef: reading the file again, scan after scan\n");
 	}
-	return jq_read_impl(data, len, copy, im, err, 0, NULL) ? -1 : 0;
+	return jq_read_impl(data, len, copy, im, err, 0, NULL, 0) ? -1 : 0;
 }
 
 int jq_read_header(const unsigned char *data, size_t len, jq_image *im, jq_header *hdr, char *err) {
 	if (!hdr) { snprintf(err, 256, "no header record"); return -1; }
 	memset(hdr, 0, sizeof(*hdr));
-	if (jq_read_impl(data, len, 0, im, err, 0, hdr)) return -1;
+	if (jq_read_impl(data, len, 0, im, err, 0, hdr, 0)) return -1;
 	if (!hdr->ncomp) { jq_free(im); snprintf(err, 256, "no scan found"); return -1; }
 	return 0;
+}
+
+int jq_read_markers(const unsigned char *data, size_t len, int copy, jq_image *im, char *err) {
+	return jq_read_impl(data, len, copy, im, err, 0, NULL, 1) ? -1 : 0;
 }
 
 /* ---------------------------------------------------------------- the writer */
@@ -1509,9 +1517,53 @@ static void out_dht(jq_out *o, int tc_th, const jq_ehuff *h) {
 	for (i = 0; i < h->nval; i++) out_byte(o, h->val[i]);
 }
 
+/* SOI, then what libjpeg writes for every output file, whatever -c says (jcmarker.c write_file_header
+ * after jpeg_copy_critical_parameters -> jpeg_set_colorspace): a JFIF APP0 for grayscale / YCbCr with
+ * the source's version (if 1.x or 2.x) and density, an Adobe APP14 carrying the colour transform for
+ * RGB / CMYK / YCCK - without it a decoder would guess YCbCr / CMYK - and then the copied markers.
+ * Depends on the input file only: everything after it (DQT on) on the coefficients. */
+static void out_prefix(jq_out *o, const jq_image *im) {
+	J_COLOR_SPACE cs = im->cinfo.jpeg_color_space;
+	int jfif = cs == JCS_GRAYSCALE || cs == JCS_YCbCr, adobe = cs == JCS_RGB || cs == JCS_CMYK || cs == JCS_YCCK, i;
+	const jq_marker *m;
+	out_be16(o, 0xFFD8);
+	if (jfif) {
+		int major = 1, minor = 1, unit = 0, xd = 1, yd = 1;
+		if (im->saw_jfif) {                              /* jctrans.c jpeg_copy_critical_parameters */
+			if (im->jfif_major == 1 || im->jfif_major == 2) { major = im->jfif_major; minor = im->jfif_minor; }
+			unit = im->density_unit; xd = im->x_density; yd = im->y_density;
+		}
+		out_be16(o, 0xFFE0); out_be16(o, 16);
+		out_byte(o, 'J'); out_byte(o, 'F'); out_byte(o, 'I'); out_byte(o, 'F'); out_byte(o, 0);
+		out_byte(o, (unsigned)major); out_byte(o, (unsigned)minor); out_byte(o, (unsigned)unit);
+		out_be16(o, (unsigned)xd); out_be16(o, (unsigned)yd); out_byte(o, 0); out_byte(o, 0);
+	}
+	if (adobe) {
+		out_be16(o, 0xFFEE); out_be16(o, 14);
+		out_byte(o, 'A'); out_byte(o, 'd'); out_byte(o, 'o'); out_byte(o, 'b'); out_byte(o, 'e');
+		out_be16(o, 100); out_be16(o, 0); out_be16(o, 0);
+		out_byte(o, cs == JCS_YCCK ? 2u : 0u);           /* jcmarker.c emit_adobe_app14 (1 = YCbCr never gets here) */
+	}
+	for (m = im->markers; m; m = m->next) {              /* jcopy_markers_execute, quantsmooth.c:581-590 */
+		if (jfif && m->code == 0xE0 && m->len >= 5 && !memcmp(m->data, "JFIF", 5)) continue;   /* written above */
+		if (adobe && m->code == 0xEE && m->len >= 5 && !memcmp(m->data, "Adobe", 5)) continue;
+		out_byte(o, 0xFF); out_byte(o, (unsigned)m->code); out_be16(o, (unsigned)m->len + 2);
+		for (i = 0; i < (int)m->len; i++) out_byte(o, m->data[i]);
+	}
+}
+
+int jq_prefix(const jq_image *im, unsigned char **out, size_t *outlen) {
+	jq_out o;
+	memset(&o, 0, sizeof(o));
+	out_prefix(&o, im);
+	if (o.fail) { free(o.p); return -1; }
+	*out = o.p; *outlen = o.n;
+	return 0;
+}
+
 int jq_write(jq_image *im, jvirt_barray_ptr *arrays, int optimize, unsigned char **out, size_t *outlen, char *err) {
 	struct jpeg_decompress_struct *ci = &im->cinfo;
-	jq_out o; jq_ehuff *dc, *ac; jq_marker *m; int i, k, nt = ci->num_components > 1 ? 2 : 1, blocks = 0, sof = 0xC0;
+	jq_out o; jq_ehuff *dc, *ac; int i, k, nt = ci->num_components > 1 ? 2 : 1, blocks = 0, sof = 0xC0;
 	unsigned written_q = 0;
 	memset(&o, 0, sizeof(o)); err[0] = 0;
 	dc = (jq_ehuff*)calloc(2, sizeof(*dc)); ac = (jq_ehuff*)calloc(2, sizeof(*ac));
@@ -1527,38 +1579,7 @@ int jq_write(jq_image *im, jvirt_barray_ptr *arrays, int optimize, unsigned char
 	}
 	for (i = 0; i < nt; i++) { ehuff_codes(&dc[i]); ehuff_codes(&ac[i]); }
 
-	out_be16(&o, 0xFFD8);
-	{
-		/* What libjpeg writes for every output file, whatever -c says (jcmarker.c write_file_header
-		 * after jpeg_copy_critical_parameters -> jpeg_set_colorspace): a JFIF APP0 for grayscale /
-		 * YCbCr with the source's version (if 1.x or 2.x) and density, an Adobe APP14 carrying the
-		 * colour transform for RGB / CMYK / YCCK - without it a decoder would guess YCbCr / CMYK. */
-		J_COLOR_SPACE cs = ci->jpeg_color_space;
-		int jfif = cs == JCS_GRAYSCALE || cs == JCS_YCbCr, adobe = cs == JCS_RGB || cs == JCS_CMYK || cs == JCS_YCCK;
-		if (jfif) {
-			int major = 1, minor = 1, unit = 0, xd = 1, yd = 1;
-			if (im->saw_jfif) {                              /* jctrans.c jpeg_copy_critical_parameters */
-				if (im->jfif_major == 1 || im->jfif_major == 2) { major = im->jfif_major; minor = im->jfif_minor; }
-				unit = im->density_unit; xd = im->x_density; yd = im->y_density;
-			}
-			out_be16(&o, 0xFFE0); out_be16(&o, 16);
-			out_byte(&o, 'J'); out_byte(&o, 'F'); out_byte(&o, 'I'); out_byte(&o, 'F'); out_byte(&o, 0);
-			out_byte(&o, (unsigned)major); out_byte(&o, (unsigned)minor); out_byte(&o, (unsigned)unit);
-			out_be16(&o, (unsigned)xd); out_be16(&o, (unsigned)yd); out_byte(&o, 0); out_byte(&o, 0);
-		}
-		if (adobe) {
-			out_be16(&o, 0xFFEE); out_be16(&o, 14);
-			out_byte(&o, 'A'); out_byte(&o, 'd'); out_byte(&o, 'o'); out_byte(&o, 'b'); out_byte(&o, 'e');
-			out_be16(&o, 100); out_be16(&o, 0); out_be16(&o, 0);
-			out_byte(&o, cs == JCS_YCCK ? 2u : 0u);          /* jcmarker.c emit_adobe_app14 (1 = YCbCr never gets here) */
-		}
-		for (m = im->markers; m; m = m->next) {              /* jcopy_markers_execute, quantsmooth.c:581-590 */
-			if (jfif && m->code == 0xE0 && m->len >= 5 && !memcmp(m->data, "JFIF", 5)) continue;   /* written above */
-			if (adobe && m->code == 0xEE && m->len >= 5 && !memcmp(m->data, "Adobe", 5)) continue;
-			out_byte(&o, 0xFF); out_byte(&o, (unsigned)m->code); out_be16(&o, (unsigned)m->len + 2);
-			for (i = 0; i < (int)m->len; i++) out_byte(&o, m->data[i]);
-		}
-	}
+	out_prefix(&o, im);
 	for (k = 0; k < ci->num_components; k++) {           /* DQT for every table in use */
 		int tq = ci->comp_info[k].quant_tbl_no & 3, prec = 0;
 		JQUANT_TBL *t = ci->comp_info[k].quant_table ? ci->comp_info[k].quant_table : ci->quant_tbl_ptrs[tq];

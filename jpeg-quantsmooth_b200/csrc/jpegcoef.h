@@ -71,6 +71,16 @@ typedef struct {
  * or -1 with a message in err.  im must be released with jq_free. */
 int jq_read_header(const unsigned char *data, size_t len, jq_image *im, jq_header *hdr, char *err);
 
+/* jq_read's marker walk over the whole file without decoding any entropy-coded data (each scan is
+ * skipped to the next marker): fills im->cinfo, the colour space, the JFIF / Adobe fields and the
+ * markers copied at level `copy`, as jq_read does, but allocates no coefficient arrays.  Returns 0
+ * or -1 with a message in err.  im must be released with jq_free. */
+int jq_read_markers(const unsigned char *data, size_t len, int copy, jq_image *im, char *err);
+
+/* The bytes jq_write puts before its first DQT: SOI, the JFIF APP0 or Adobe APP14 of the colour
+ * space, the copied markers.  *out is malloc'd.  Returns 0 or -1 (out of memory). */
+int jq_prefix(const jq_image *im, unsigned char **out, size_t *outlen);
+
 /* worker threads of the codec: 0 = one per processor (at most 16).  The writer codes segments of
  * MCU rows on them; the reader decodes sequential (SOF0/SOF1) scans on them - restart intervals as
  * they are, scans without restart markers by speculative parsing of chunks that are stitched where

@@ -53,6 +53,12 @@ class _Scan(C.Structure):
                 ("jpeg_color_space", C.c_int32), ("sof", C.c_int32)]
 
 
+class _Head(C.Structure):
+    """jpegqs_cuda_jpeg_head: the prefix and frame identifiers of one encoded file (include/jpegqs_cuda.h)."""
+    _fields_ = [("prefix_dev", C.c_void_p), ("prefix_len", C.c_uint32), ("comp_id", C.c_int32 * 4),
+                ("quant_tbl", C.c_int32 * 4)]
+
+
 class _Job(C.Structure):
     _fields_ = [("coef", C.c_void_p), ("plane", C.c_void_p), ("plane2", C.c_void_p),
                 ("wblk", C.c_uint32), ("hblk", C.c_uint32), ("quant", C.c_uint16 * 64),
@@ -145,6 +151,15 @@ def load():
                                              C.POINTER(C.c_size_t), C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
     lib.jpegqs_cuda_decode_model.argtypes = [C.POINTER(_Image), C.POINTER(_Scan), C.c_char_p, C.c_size_t, C.c_int,
                                              C.POINTER(C.c_int32), C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
+    lib.jpegqs_cuda_jpeg_prefix.argtypes = [C.c_char_p, C.c_size_t, C.c_int, C.c_void_p, C.c_size_t,
+                                            C.POINTER(C.c_size_t), C.POINTER(C.c_int32), C.c_int32 * 4, C.c_int32 * 4]
+    lib.jpegqs_cuda_encode_bound.argtypes = [C.POINTER(_Image), C.c_size_t, C.POINTER(C.c_size_t)]
+    lib.jpegqs_cuda_encode_workspace_bytes.argtypes = [C.c_int, C.POINTER(_Image), C.c_int, C.POINTER(C.c_size_t)]
+    lib.jpegqs_cuda_encode_async.argtypes = [C.c_void_p, C.c_int, C.POINTER(_Image), C.POINTER(_Head), C.c_int,
+                                             C.c_void_p, C.c_void_p, C.POINTER(C.c_size_t), C.c_void_p, C.c_void_p,
+                                             C.c_void_p, C.c_size_t, C.c_void_p]
+    lib.jpegqs_cuda_encode_model.argtypes = [C.POINTER(_Image), C.POINTER(_Head), C.c_int, C.c_void_p, C.c_size_t,
+                                             C.POINTER(C.c_uint64), C.POINTER(C.c_int32)]
     lib.jpegqs_cuda_tables.argtypes = [C.c_int, C.c_void_p]
     lib.jpegqs_cuda_orig_coef.argtypes = [C.c_int, C.c_int]
     _lib = lib
@@ -331,6 +346,93 @@ def decode_model(image: CoefImage, scan, data: bytes, sub_bytes: int = DECODE_SU
                                     over.ctypes.data, cap, C.byref(nsub)) < 0:
         raise QsError(lib.jpegqs_cuda_last_error(None).decode())
     return out, int(st.value), over[:nsub.value]
+
+
+# ---- coefficients to JPEG files (include/jpegqs_cuda.h "quantized coefficients to JPEG files") ----
+ENCODE_RANGE, ENCODE_OVERFLOW, ENCODE_NO_UP = 1, 2, 4
+
+
+def jpeg_prefix(data: bytes, copy: int = 2):
+    """What the jpegqs tool's writer puts before its first DQT for this input file and marker copy
+    level (the tool's -c): SOI, the JFIF APP0 or Adobe APP14, the copied APPn / COM markers.  Host-only,
+    no entropy-coded data is decoded.  Returns (prefix bytes, component ids, quantization table
+    numbers), one id and one table number per component: the frame identifiers encode_async writes in
+    SOF / SOS and DQT, which a CoefImage does not carry."""
+    lib = load()
+    data = bytes(data)
+    ids, tbls, n, nc = (C.c_int32 * 4)(), (C.c_int32 * 4)(), C.c_size_t(0), C.c_int32(0)
+    if lib.jpegqs_cuda_jpeg_prefix(data, len(data), copy, None, 0, C.byref(n), C.byref(nc), ids, tbls) < 0:
+        raise QsError(f"jpeg_prefix: {lib.jpegqs_cuda_last_error(None).decode()}")
+    buf = (C.c_uint8 * max(n.value, 1))()
+    if lib.jpegqs_cuda_jpeg_prefix(data, len(data), copy, buf, n.value, C.byref(n), C.byref(nc), ids, tbls) < 0:
+        raise QsError(f"jpeg_prefix: {lib.jpegqs_cuda_last_error(None).decode()}")
+    return bytes(buf)[:n.value], tuple(ids[:nc.value]), tuple(tbls[:nc.value])
+
+
+def _head(prefix_ptr, prefix_len, comp_ids, quant_tbls, n):
+    h = _Head()
+    if len(comp_ids) != n or len(quant_tbls) != n:
+        raise ValueError(f"expected {n} component ids and quantization table numbers")
+    h.prefix_dev, h.prefix_len = prefix_ptr, prefix_len
+    for k in range(n):
+        h.comp_id[k], h.quant_tbl[k] = int(comp_ids[k]), int(quant_tbls[k])
+    return h
+
+
+def encode_bound(image: CoefImage, prefix_len: int) -> int:
+    """Output bytes encode_async can never exceed for this image and prefix length (host-only)."""
+    lib = load()
+    ci, out = _Image(), C.c_size_t(0)
+    _fill_image(ci, image, [None] * len(image.comps), [])
+    if lib.jpegqs_cuda_encode_bound(C.byref(ci), int(prefix_len), C.byref(out)) < 0:
+        raise QsError(lib.jpegqs_cuda_last_error(None).decode())
+    return int(out.value)
+
+
+def encode_workspace_bytes(images: Sequence[CoefImage], optimize: bool = False) -> int:
+    """Device bytes of workspace encode_async needs for these images (host-only)."""
+    lib = load()
+    arr, out = _image_array(images), C.c_size_t(0)
+    if lib.jpegqs_cuda_encode_workspace_bytes(len(images), arr, int(bool(optimize)), C.byref(out)) < 0:
+        raise QsError(lib.jpegqs_cuda_last_error(None).decode())
+    return int(out.value)
+
+
+def encode_model(image: CoefImage, arrays, prefix: bytes, comp_ids, quant_tbls, optimize: bool = False, up=None,
+                 capacity=None):
+    """encode_async's algorithm run on the CPU for one image (jpegqs_cuda_encode_model).  arrays: numpy
+    int16 [hblk, wblk, 64] per component; up: the two luma-sized arrays of up-sampled chroma, which
+    makes the model write the up-sampled geometry.  capacity: output bytes (default encode_bound).
+    Returns (file bytes, status).  On OVERFLOW the bytes are the first `capacity` bytes of the
+    file, which is not complete."""
+    lib = load()
+    nc = len(image.comps)
+    if len(arrays) != nc:
+        raise ValueError(f"{len(arrays)} arrays for {nc} components")
+    arrays = [np.ascontiguousarray(a, dtype=np.int16) for a in arrays]
+    for c, (comp, a) in enumerate(zip(image.comps, arrays)):
+        if a.shape != (comp.hblk, comp.wblk, 64):
+            raise ValueError(f"arrays[{c}]: shape {a.shape}, expected {(comp.hblk, comp.wblk, 64)}")
+    ups = [None, None]
+    if up is not None:
+        y = image.comps[0]
+        ups = [np.ascontiguousarray(a, dtype=np.int16) for a in up]
+        for a in ups:
+            if a.shape != (y.hblk, y.wblk, 64):
+                raise ValueError(f"up: shape {a.shape}, expected {(y.hblk, y.wblk, 64)}")
+    ci = _Image()
+    _fill_image(ci, image, [a.ctypes.data for a in arrays], [None] + [a.ctypes.data if a is not None else None for a in ups])
+    ci.upsampled = int(up is not None)
+    prefix = bytes(prefix)
+    pbuf = (C.c_uint8 * max(len(prefix), 1)).from_buffer_copy(prefix or b"\0")
+    head = _head(C.cast(pbuf, C.c_void_p), len(prefix), comp_ids, quant_tbls, nc)
+    cap = int(capacity) if capacity is not None else encode_bound(image, len(prefix))
+    out = np.zeros(max(cap, 1), dtype=np.uint8)
+    n, st = C.c_uint64(0), C.c_int32(0)
+    if lib.jpegqs_cuda_encode_model(C.byref(ci), C.byref(head), int(bool(optimize)), out.ctypes.data, cap,
+                                    C.byref(n), C.byref(st)) < 0:
+        raise QsError(lib.jpegqs_cuda_last_error(None).decode())
+    return out[:min(n.value, cap)].tobytes(), int(st.value)
 
 
 def _stream_handle(stream) -> C.c_void_p:
@@ -723,6 +825,119 @@ class QsContext:
                                                           status.data_ptr() if n else None, _stream_handle(stream)))
         return out, status
 
+    # ---- coefficients to JPEG bytes (include/jpegqs_cuda.h jpegqs_cuda_encode_async) ----
+    def encode_async(self, images: Sequence[CoefImage], coefs, heads, optimize: bool = False, status=None, up=None,
+                     out=None, capacity=None, stream=None):
+        """Write device-resident coefficients as JPEG files in device memory - the bytes the jpegqs
+        tool writes for them - without blocking the calling thread.  The coefficient tensors are
+        only read.
+
+        images, coefs, up, status: as for render_async (status / up what run_async returned, or
+        host booleans).  heads[i]: (prefix, comp_ids, quant_tbls) with prefix a 1-D contiguous uint8
+        CUDA tensor holding jpeg_prefix's bytes and the other two what jpeg_prefix returned.
+        optimize: optimal Huffman tables (the tool's -o).  out[i] (optional): 1-D uint8 CUDA tensors
+        to write, capacity[i] their usable bytes (default: their size); by default out[i] is
+        allocated on the stream at encode_bound's size.  stream: a torch.cuda.Stream (default: the
+        current one).  Returns (out, lengths, status): lengths an int64 device tensor [n] of file
+        lengths, status an int32 device tensor [n], 0 or ENCODE_RANGE / ENCODE_OVERFLOW /
+        ENCODE_NO_UP bits (NO_UP: status says image i was up-sampled but up[i] was not given, so it
+        was written at its own sampling).
+        Capturable with torch.cuda.graph: a replay encodes the current contents of the same tensors."""
+        import torch
+        n = len(images)
+        if len(coefs) != n or len(heads) != n or (up is not None and len(up) != n) or (out is not None and len(out) != n):
+            raise ValueError("images, coefs, heads, up and out must have one entry per image")
+        if capacity is not None and (out is None or len(capacity) != n):
+            raise ValueError("capacity needs out and one entry per image")
+        host_up = None
+        if status is not None and not isinstance(status, torch.Tensor):
+            host_up = [bool(u) for u in status]
+            if len(host_up) != n:
+                raise ValueError("status must have one entry per image")
+        tensors, prefixes = [], []
+        for i, im in enumerate(images):
+            if len(coefs[i]) != len(im.comps):
+                raise ValueError(f"image {i}: {len(coefs[i])} coefficient tensors for {len(im.comps)} components")
+            for c, (comp, t) in enumerate(zip(im.comps, coefs[i])):
+                _check_tensor(t, (comp.hblk, comp.wblk, 64), f"coefs[{i}][{c}]")
+                if t.data_ptr() % 16:
+                    raise ValueError(f"coefs[{i}][{c}]: not 16-byte aligned")
+                tensors.append((f"coefs[{i}][{c}]", t))
+            given = up[i] if up is not None else None
+            if given is not None:
+                if len(given) != 2 or len(im.comps) != 3:
+                    raise ValueError(f"up[{i}]: expected two tensors for a three-component image")
+                y = im.comps[0]
+                for j, t in enumerate(given):
+                    _check_tensor(t, (y.hblk, y.wblk, 64), f"up[{i}][{j}]")
+                    if t.data_ptr() % 16:
+                        raise ValueError(f"up[{i}][{j}]: not 16-byte aligned")
+                    tensors.append((f"up[{i}][{j}]", t))
+            if host_up is not None and host_up[i] and given is None:
+                raise ValueError(f"image {i} is up-sampled but up[{i}] is missing")
+            if len(heads[i]) != 3:
+                raise ValueError(f"heads[{i}]: expected (prefix tensor, comp_ids, quant_tbls)")
+            p, ids, tbls = heads[i]
+            if not isinstance(p, torch.Tensor) or p.dtype != torch.uint8 or p.dim() != 1 or not p.is_contiguous():
+                raise ValueError(f"heads[{i}]: the prefix must be a contiguous 1-D uint8 tensor")
+            if len(ids) != len(im.comps) or len(tbls) != len(im.comps):
+                raise ValueError(f"heads[{i}]: {len(im.comps)} component ids and table numbers expected")
+            tensors.append((f"heads[{i}] prefix", p))
+            prefixes.append(p)
+        if isinstance(status, torch.Tensor):
+            if status.dtype != torch.int32 or tuple(status.shape) != (n, 2) or not status.is_contiguous():
+                raise ValueError(f"status: expected a contiguous int32 tensor [{n}, 2]")
+            tensors.append(("status", status))
+        caps = None
+        if out is not None:
+            caps = []
+            for i, t in enumerate(out):
+                if not isinstance(t, torch.Tensor):
+                    raise TypeError(f"out[{i}]: expected a torch.Tensor, got {type(t).__name__}")
+                if t.dtype != torch.uint8 or t.dim() != 1 or not t.is_contiguous():
+                    raise ValueError(f"out[{i}]: expected a contiguous 1-D uint8 tensor")
+                cap = int(capacity[i]) if capacity is not None else t.numel()
+                if cap > t.numel() or cap < prefixes[i].numel():
+                    raise ValueError(f"out[{i}]: capacity {cap} outside [prefix length, {t.numel()}]")
+                caps.append(cap)
+                tensors.append((f"out[{i}]", t))
+        device = self.device if self.device >= 0 else torch.cuda.current_device()
+        for what, t in tensors:
+            if not t.is_cuda or t.device.index != device:
+                raise ValueError(f"{what}: on {t.device}, expected cuda:{device}")
+        up_ptrs = [[None, up[i][0].data_ptr(), up[i][1].data_ptr()] if up is not None and up[i] is not None else []
+                   for i in range(n)]
+        arr = _image_array(images, [[t.data_ptr() for t in coefs[i]] for i in range(n)], up_ptrs)
+        for i in range(n):
+            arr[i].upsampled = int(bool(host_up and host_up[i]))
+        if caps is None:
+            caps = []
+            for i in range(n):
+                b = C.c_size_t(0)
+                self._check(self.lib.jpegqs_cuda_encode_bound(C.byref(arr[i]), prefixes[i].numel(), C.byref(b)))
+                caps.append(int(b.value))
+        hs = (_Head * max(n, 1))()
+        for i, (p, ids, tbls) in enumerate(heads):
+            hs[i] = _head(p.data_ptr(), p.numel(), ids, tbls, len(images[i].comps))
+        stream = stream if stream is not None else torch.cuda.current_stream(device)
+        with torch.cuda.device(device), torch.cuda.stream(stream):
+            if out is None:
+                out = [torch.empty(c, dtype=torch.uint8, device=device) for c in caps]
+            out = list(out)
+            size = C.c_size_t(0)
+            self._check(self.lib.jpegqs_cuda_encode_workspace_bytes(n, arr, int(bool(optimize)), C.byref(size)))
+            # allocated on `stream`: reused only by work queued after this call's kernels
+            ws = torch.empty(max(size.value, 1), dtype=torch.uint8, device=device)
+            lengths = torch.empty((n,), dtype=torch.int64, device=device)
+            st = torch.empty((n,), dtype=torch.int32, device=device)
+            outs = (C.c_void_p * max(n, 1))(*[t.data_ptr() for t in out])
+            capa = (C.c_size_t * max(n, 1))(*caps)
+            self._check(self.lib.jpegqs_cuda_encode_async(
+                self.h, n, arr, hs, int(bool(optimize)), status.data_ptr() if isinstance(status, torch.Tensor) else None,
+                outs, capa, lengths.data_ptr() if n else None, st.data_ptr() if n else None, ws.data_ptr(), size.value,
+                _stream_handle(stream)))
+        return out, lengths, st
+
     # ---- one slab of a sharded image (include/jpegqs_cuda.h "one image sharded by MCU rows") ----
     def run_slab(self, link, slab: CoefImage, rank: int, world: int, row0: Sequence[int],
                  hblk_total: Sequence[int], flags: int, niter: int, coef_ptrs=None, up_ptrs=None, stream: int = 0):
@@ -946,3 +1161,16 @@ def render_async(images: Sequence[CoefImage], coefs, status=None, up=None, layou
     if not isinstance(first, torch.Tensor) or not first.is_cuda:
         raise ValueError("render_async: the coefficient tensors must be CUDA tensors")
     return default_context(first.device.index).render_async(images, coefs, status, up, layout, out, stream)
+
+
+def encode_async(images: Sequence[CoefImage], coefs, heads, optimize: bool = False, status=None, up=None, out=None,
+                 capacity=None, stream=None):
+    """QsContext.encode_async on the default context of the tensors' device: writes CUDA coefficient
+    tensors as JPEG files in CUDA uint8 tensors, enqueued on `stream` (default: the current one)
+    without waiting.  Returns (out, lengths [n] int64, status [n] int32), all on the device."""
+    import torch
+    first = next((t for ts in coefs for t in ts), None)
+    if not isinstance(first, torch.Tensor) or not first.is_cuda:
+        raise ValueError("encode_async: the coefficient tensors must be CUDA tensors")
+    return default_context(first.device.index).encode_async(images, coefs, heads, optimize, status, up, out,
+                                                            capacity, stream)

@@ -54,3 +54,38 @@ for sub_bytes in (32, 512):
     torch.cuda.synchronize()
     print("decode_async key 9 =", sub_bytes, "status", status.cpu().tolist(), flush=True)
 ctx.set_tuning(9, 512)
+
+
+# the JPEG encoder: good images of every kind, a RANGE image (AC 1024) and an OVERFLOW capacity (the
+# exact length minus 1) in one batch of more than one launch group (16 images), standard and optimal
+# tables; then decode -> run_async (q6) -> encode with the chroma source read from the run status
+from jpegqs_b200.image import CoefImage, Component, JCS_GRAYSCALE  # noqa: E402
+
+imgs, heads, hosts = [], [], []
+for f in good * 3:                                     # 18 good images
+    im = qs.read_jpeg(f)
+    pre, ids, tbls = qs.jpeg_prefix(f)
+    imgs.append(im); hosts.append((pre, ids, tbls))
+    heads.append((torch.frombuffer(bytearray(pre), dtype=torch.uint8).cuda(), ids, tbls))
+rb = np.zeros((2, 3, 64), np.int16)
+rb[1, 1, 5] = 1024
+imgs.append(CoefImage(width=24, height=16, colorspace=JCS_GRAYSCALE,
+                      comps=[Component(coef=rb, quant=np.ones(64, np.uint16))]))
+heads.append((torch.tensor([0xFF, 0xD8], dtype=torch.uint8, device="cuda"), (1,), (0,)))
+coefs = [[torch.from_numpy(np.ascontiguousarray(c.coef)).cuda() for c in im.comps] for im in imgs]
+for optimize in (False, True):
+    exact = len(qs.encode_model(imgs[0], [c.coef for c in imgs[0].comps], *hosts[0], optimize)[0])
+    caps = [exact - 1] + [qs.encode_bound(im, h[0].numel()) for im, h in zip(imgs[1:], heads[1:])]
+    outs = [torch.empty(c, dtype=torch.uint8, device="cuda") for c in caps]
+    out, lengths, status = ctx.encode_async(imgs, coefs, heads, optimize, out=outs, capacity=caps)
+    torch.cuda.synchronize()
+    print("encode_async optimize", int(optimize), "status", status.cpu().tolist(), flush=True)
+im, scan = qs.parse_jpeg(base)
+coefs, st = ctx.decode_async([im], [scan], [torch.frombuffer(bytearray(base), dtype=torch.uint8).cuda()])
+work = [im.clone()]
+rst, ups = ctx.run_async(work, coefs, 7, 1)
+pre, ids, tbls = qs.jpeg_prefix(base)
+out, lengths, status = ctx.encode_async(work, coefs, [(torch.frombuffer(bytearray(pre), dtype=torch.uint8).cuda(), ids, tbls)],
+                                        True, rst, ups)
+torch.cuda.synchronize()
+print("decode -> run_async -> encode_async: run", rst.cpu().tolist(), "encode status", status.cpu().tolist(), flush=True)
