@@ -298,6 +298,89 @@ int jpegqs_cuda_decode_async(jpegqs_cuda_ctx *ctx, int n, const jpegqs_cuda_imag
 		const jpegqs_cuda_scan *scans, const uint8_t *const *data_dev, const size_t *data_len,
 		void *workspace, size_t workspace_bytes, int32_t *status_dev, void *stream);
 
+/* ---- any scan script: progressive and multi-scan files ------------------------------------------
+ * jpegqs_cuda_decode_async takes files with one interleaved sequential scan.  The calls below take
+ * every file the jpegqs tool's reader takes - SOF0 / SOF1 / SOF2, Huffman, 8-bit samples, any scan
+ * script of up to JPEGQS_MAX_SCANS scans - and give the coefficients jpeg_read_coefficients gives.
+ *
+ * One scan as the host marker walk found it.  No libjpeg types. */
+#define JPEGQS_MAX_SCANS 64
+typedef struct {
+	int32_t ncomp;                    /* components in the scan (1 for progressive AC scans)     */
+	int32_t comp[4];                  /* frame component index of scan component k (MCU order)  */
+	int32_t dc_tbl[4], ac_tbl[4];     /* table selectors (Td, Ta) of scan component k            */
+	int32_t Ss, Se, Ah, Al;           /* spectral selection and successive approximation; a
+	                                   * sequential scan has 0, 63, 0, 0                         */
+	int32_t sof;                      /* the frame's SOF marker: 0xC0 / 0xC1 / 0xC2              */
+	int32_t dc_present[4], ac_present[4];  /* the Huffman tables in force at this SOS (a DHT may   */
+	uint8_t dc_bits[4][17], dc_val[4][256];  /* sit between scans): BITS (index 1..16) and HUFFVAL */
+	uint8_t ac_bits[4][17], ac_val[4][256];
+	uint32_t restart_interval;        /* DRI in force at this SOS; MCUs (blocks when ncomp = 1)  */
+	uint64_t offset;                  /* first entropy-coded byte of the scan                    */
+	uint64_t end;                     /* the next marker that is not RSTn, or the file's end when none
+	                                   * follows: the segment is [offset, end)                    */
+} jpegqs_cuda_scan_rec;
+
+/* Host-only.  Walks every marker of the file without decoding entropy-coded data: fills img as
+ * jpegqs_cuda_jpeg_parse does and scans[0 .. *nscans) (cap entries; *nscans is set whenever the
+ * walk succeeds, also when it exceeds cap).  Returns
+ *   0                       the file's scans are all in scans[] and jpegqs_cuda_decode_scans_async
+ *                           takes them;
+ *   JPEGQS_ERR_UNSUPPORTED  more scans than cap or JPEGQS_MAX_SCANS, a scan without a single
+ *                           entropy-coded byte (a file cut at an SOS), a selected Huffman table libjpeg
+ *                           would reject (an all-ones code, a DC symbol > 15), or a first scan
+ *                           (Ah = 0) after an AC refinement scan of the same component whose band
+ *                           overlaps it (not a T.81 scan script): jpegqs_cuda_jpeg_read takes these;
+ *   JPEGQS_ERR_ARG          what the reader rejects (message in jpegqs_cuda_last_error(NULL)),
+ *                           a scan using an undefined table included. */
+int jpegqs_cuda_jpeg_parse_scans(const uint8_t *data, size_t len, jpegqs_cuda_image *img,
+		jpegqs_cuda_scan_rec *scans, int cap, int *nscans);
+
+/* Stream-ordered, graph-capturable decode of n files of any scan script on the GPU.
+ *   - Inputs.  data_dev[i] / data_len[i] as for decode_async; imgs[i] and scans[i][0 .. nscans[i])
+ *     what jpegqs_cuda_jpeg_parse_scans returned 0 for (host structs, read during the call only).
+ *   - Output.  imgs[i].comp[c].coef: DEVICE pointers, 16-byte aligned, [hblk][wblk][64] int16.  The
+ *     call zeroes them first (coefficients no scan codes are 0), so a replay rewrites them whole.
+ *   - Status.  status_dev[i]: 0 or an OR of the JPEGQS_DECODE_* bits; status 0 => the coefficients
+ *     equal jpeg_read_coefficients'.  Every write stays inside image i's arrays.
+ *   - Schedule, per group of images (up to 16 images and 512 scans): zero the arrays; one byte pass
+ *     (unstuffing, RSTn) over every scan; every sequential, DC first and AC first scan through one set
+ *     of the speculative-subsequence launches of decode_async (in an AC first scan an end-of-band run
+ *     is one decoder step that counts all its blocks; a run that outlives its restart interval is cut
+ *     there); every DC refinement scan in one launch (one thread per block); AC refinement scans one
+ *     launch per level, one warp per restart interval.  The level of an AC refinement scan is one
+ *     more than the highest among the earlier AC refinement scans of its component whose bands
+ *     overlap.  Within a restart interval (the whole scan without restart markers) an AC refinement
+ *     scan is decoded serially: a file without restart markers decodes each such scan on one thread.
+ *   - Argument errors change nothing: every check runs before the first enqueue.  Checked besides
+ *     decode_async's image checks: nscans[i] outside 1..JPEGQS_MAX_SCANS, a scan's components not
+ *     distinct frame components, Ss / Se / Ah / Al outside T.81's ranges, an AC scan of several
+ *     components, offset / end outside data_len, a table the scan decodes with absent or invalid.
+ *   - The stream rules of decode_async: no allocation, synchronisation or event use; descriptors and
+ *     Huffman tables travel as kernel parameters (a store kernel per 24 scans writes them to the
+ *     workspace).  Under graph capture every scan's header, position, tables and restart interval
+ *     and data_len are fixed at capture: a replay decodes the current bytes of the same buffers, so
+ *     it decodes a file whose headers and scan positions are identical to the captured one's.
+ *     jpegqs_cuda_last_launches counts the launches.
+ *   - Workspace.  With A(x) = x rounded up to a multiple of 256, per scan L = end - offset and I =
+ *     ceil(MCUs / restart_interval) (1 without restarts; MCUs = blocks for a one-component scan), the
+ *     size is the sum over images and scans of
+ *       16384 + A(L + 8) + A(24 * ceil(L / 4096)) + 2 * A(4 * I) + S
+ *     with S = A(96 * (floor(L / 32) + I)) for sequential and first scans and S = 0 for refinement
+ *     scans.  It does not depend on tuning key 9.
+ * Returns 0 or a negative error. */
+int jpegqs_cuda_decode_scans_workspace_bytes(int n, const jpegqs_cuda_image *imgs,
+		const jpegqs_cuda_scan_rec *const *scans, const int *nscans, const size_t *data_len, size_t *bytes);
+int jpegqs_cuda_decode_scans_async(jpegqs_cuda_ctx *ctx, int n, const jpegqs_cuda_image *imgs,
+		const jpegqs_cuda_scan_rec *const *scans, const int *nscans, const uint8_t *const *data_dev,
+		const size_t *data_len, void *workspace, size_t workspace_bytes, int32_t *status_dev, void *stream);
+/* jpegqs_cuda_decode_scans_async's algorithm on one CPU thread, for one file: the same byte pass, the
+ * same subsequences of sub_bytes (>= 32) bytes, the same step decoders, placement, refinement
+ * decoders and scan order.  img->comp[c].coef are HOST arrays (zeroed by the call).  *status
+ * receives the JPEGQS_DECODE_* bits. */
+int jpegqs_cuda_decode_scans_model(const jpegqs_cuda_image *img, const jpegqs_cuda_scan_rec *scans, int nscans,
+		const uint8_t *data, size_t data_len, int sub_bytes, int32_t *status);
+
 /* ---- quantized coefficients to JPEG files ----------------------------------------------------
  * The last stage of a device pipeline: the coefficients decode_async / run_async leave on the GPU
  * written as the sequential Huffman JPEG file the jpegqs tool writes for them (its writer, jpegcoef.c

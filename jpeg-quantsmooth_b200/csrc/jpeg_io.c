@@ -66,6 +66,65 @@ int jpegqs_cuda_jpeg_parse(const uint8_t *data, size_t len, jpegqs_cuda_image *i
 	return 0;
 }
 
+/* the coefficients a scan codes, as a zig-zag band: a progressive DC scan codes coefficient 0 only */
+static void scan_band(const jq_scanrec *r, int prog, int *lo, int *hi) {
+	*lo = r->Ss; *hi = prog && r->Ss == 0 ? 0 : r->Se;
+}
+
+int jpegqs_cuda_jpeg_parse_scans(const uint8_t *data, size_t len, jpegqs_cuda_image *img,
+		jpegqs_cuda_scan_rec *scans, int cap, int *nscans) {
+	jq_image im; char err[256]; int n = 0, i, j, k, prog, unsupported = 0;
+	jq_scanrec *rec;
+	if (!data || !img || !nscans || cap < 0 || (cap && !scans)) { qs_set_host_error("jpegqs_cuda_jpeg_parse_scans: NULL argument"); return JPEGQS_ERR_ARG; }
+	rec = (jq_scanrec*)calloc(JPEGQS_MAX_SCANS, sizeof(*rec));
+	if (!rec) { qs_set_host_error("jpegqs_cuda_jpeg_parse_scans: out of memory"); return JPEGQS_ERR_ARG; }
+	if (jq_read_scans(data, len, &im, rec, JPEGQS_MAX_SCANS, &n, err)) { free(rec); qs_set_host_error(err); return JPEGQS_ERR_ARG; }
+	fill_image(&im, img);
+	prog = im.progressive;
+	jq_free(&im);
+	*nscans = n;
+	if (!n) { free(rec); qs_set_host_error("jpegqs_cuda_jpeg_parse_scans: no scan found"); return JPEGQS_ERR_ARG; }
+	if (n > JPEGQS_MAX_SCANS || n > cap) unsupported = 1;
+	for (i = 0; i < n && i < JPEGQS_MAX_SCANS; i++) {
+		const jq_scanrec *r = &rec[i];
+		int need_dc = !prog || (r->Ss == 0 && r->Ah == 0), need_ac = prog ? r->Ss > 0 : 1, lo, hi;
+		if (r->offset >= r->end) unsupported = 1;      /* no entropy-coded byte: a file cut at this SOS */
+		for (k = 0; k < r->ncomp; k++) {
+			if ((need_dc && !r->dc_present[r->td[k]]) || (need_ac && !r->ac_present[r->ta[k]])) {
+				free(rec); qs_set_host_error("jpegqs_cuda_jpeg_parse_scans: scan uses an undefined Huffman table"); return JPEGQS_ERR_ARG;
+			}
+			if ((need_dc && !table_ok(r->dc_bits[r->td[k]], r->dc_val[r->td[k]], 1)) ||
+					(need_ac && !table_ok(r->ac_bits[r->ta[k]], r->ac_val[r->ta[k]], 0))) unsupported = 1;
+		}
+		/* first scans (Ah = 0) of a component must code disjoint bands, and come before the
+		 * refinement scans of their band: the device runs all first scans before any refinement */
+		scan_band(r, prog, &lo, &hi);
+		for (j = 0; j < i && r->Ah == 0; j++) {
+			const jq_scanrec *e = &rec[j]; int elo, ehi, share = 0, a, b;
+			for (a = 0; a < r->ncomp; a++) for (b = 0; b < e->ncomp; b++) share |= r->ci[a] == e->ci[b];
+			scan_band(e, prog, &elo, &ehi);
+			if (share && lo <= ehi && elo <= hi) unsupported = 1;
+		}
+	}
+	for (i = 0; i < n && i < cap && i < JPEGQS_MAX_SCANS; i++) {
+		const jq_scanrec *r = &rec[i]; jpegqs_cuda_scan_rec *o = &scans[i];
+		memset(o, 0, sizeof(*o));
+		o->ncomp = r->ncomp;
+		for (k = 0; k < 4; k++) {
+			o->comp[k] = r->ci[k]; o->dc_tbl[k] = r->td[k]; o->ac_tbl[k] = r->ta[k];
+			o->dc_present[k] = r->dc_present[k]; o->ac_present[k] = r->ac_present[k];
+			memcpy(o->dc_bits[k], r->dc_bits[k], 17); memcpy(o->dc_val[k], r->dc_val[k], 256);
+			memcpy(o->ac_bits[k], r->ac_bits[k], 17); memcpy(o->ac_val[k], r->ac_val[k], 256);
+		}
+		o->Ss = r->Ss; o->Se = r->Se; o->Ah = r->Ah; o->Al = r->Al; o->sof = r->sof;
+		o->restart_interval = (uint32_t)r->restart_interval;
+		o->offset = r->offset; o->end = r->end;
+	}
+	free(rec);
+	if (unsupported) { qs_set_host_error("jpegqs_cuda_jpeg_parse_scans: only the host reader takes this file"); return JPEGQS_ERR_UNSUPPORTED; }
+	return 0;
+}
+
 int jpegqs_cuda_jpeg_read(const uint8_t *data, size_t len, const jpegqs_cuda_image *img) {
 	jq_image im; char err[256]; int c, warn; JDIMENSION y;
 	if (!data || !img) { qs_set_host_error("jpegqs_cuda_jpeg_read: NULL argument"); return JPEGQS_ERR_ARG; }

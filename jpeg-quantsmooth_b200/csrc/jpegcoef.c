@@ -864,8 +864,10 @@ static unsigned be16(const unsigned char *p) { return (unsigned)p[0] << 8 | p[1]
 
 /* defer: progressive scans are recorded and decoded side by side at the end (returns 1 if that did
  * not work out: the caller reads the file again with defer = 0) */
+typedef struct { jq_scanrec *recs; int cap, n; } jq_recs;      /* jq_read_scans' record of the scans */
+
 static int jq_read_impl(const unsigned char *data, size_t len, int copy, jq_image *im, char *err, int defer,
-		jq_header *hdr, int skip_data) {
+		jq_header *hdr, int skip_data, jq_recs *rec) {
 	const unsigned char *p = data, *end = data + len;
 	jq_priv *pv; jq_dec *d; jq_marker **tail; int have_frame = 0, i, done = 0, adobe = -1;
 	jq_dscan *dsc = NULL; int ndsc = 0, retry = 0, sof_code = 0;
@@ -997,7 +999,27 @@ static int jq_read_impl(const unsigned char *data, size_t len, int copy, jq_imag
 				continue;
 			}
 			if (skip_data) {                            /* markers only: on to the next marker, as defer does */
+				if (rec && rec->n < rec->cap) {
+					jq_scanrec *r = &rec->recs[rec->n];
+					memset(r, 0, sizeof(*r));
+					r->sof = im->progressive ? 0xC2 : sof_code;
+					r->ncomp = ns; r->Ss = s.Ss; r->Se = s.Se; r->Ah = s.Ah; r->Al = s.Al;
+					for (i = 0; i < ns; i++) { r->ci[i] = s.ci[i]; r->td[i] = s.td[i]; r->ta[i] = s.ta[i]; }
+					for (i = 0; i < 4; i++) {
+						r->dc_present[i] = d->dc[i].present; r->ac_present[i] = d->ac[i].present;
+						memcpy(r->dc_bits[i], d->dc[i].bits, 17); memcpy(r->dc_val[i], d->dc[i].val, 256);
+						memcpy(r->ac_bits[i], d->ac[i].bits, 17); memcpy(r->ac_val[i], d->ac[i].val, 256);
+					}
+					r->restart_interval = im->restart_interval;
+					r->offset = (size_t)(p - data);
+				}
 				while (p + 1 < end && !(p[0] == 0xFF && p[1] != 0 && p[1] != 0xFF && (p[1] & 0xF8) != 0xD0)) p++;
+				if (rec) {
+					/* the walk stops one byte short of the file's end when no marker follows (a file
+					 * cut inside entropy-coded data): that last byte is part of the segment */
+					if (rec->n < rec->cap) rec->recs[rec->n].end = p + 1 >= end ? len : (size_t)(p - data);
+					rec->n++;
+				}
 				continue;
 			}
 			if (defer && im->progressive) {                 /* record the scan, find the next marker */
@@ -1058,23 +1080,31 @@ fail:
 
 int jq_read(const unsigned char *data, size_t len, int copy, jq_image *im, char *err) {
 	if (codec_thread_count() >= 2 && !getenv("JPEGQS_SERIAL_DECODE")) {
-		int rc = jq_read_impl(data, len, copy, im, err, 1, NULL, 0);
+		int rc = jq_read_impl(data, len, copy, im, err, 1, NULL, 0, NULL);
 		if (rc <= 0) return rc;
 		if (getenv("JPEGQS_CODEC_TRACE")) fprintf(stderr, "jpegcoef: reading the file again, scan after scan\n");
 	}
-	return jq_read_impl(data, len, copy, im, err, 0, NULL, 0) ? -1 : 0;
+	return jq_read_impl(data, len, copy, im, err, 0, NULL, 0, NULL) ? -1 : 0;
 }
 
 int jq_read_header(const unsigned char *data, size_t len, jq_image *im, jq_header *hdr, char *err) {
 	if (!hdr) { snprintf(err, 256, "no header record"); return -1; }
 	memset(hdr, 0, sizeof(*hdr));
-	if (jq_read_impl(data, len, 0, im, err, 0, hdr, 0)) return -1;
+	if (jq_read_impl(data, len, 0, im, err, 0, hdr, 0, NULL)) return -1;
 	if (!hdr->ncomp) { jq_free(im); snprintf(err, 256, "no scan found"); return -1; }
 	return 0;
 }
 
 int jq_read_markers(const unsigned char *data, size_t len, int copy, jq_image *im, char *err) {
-	return jq_read_impl(data, len, copy, im, err, 0, NULL, 1) ? -1 : 0;
+	return jq_read_impl(data, len, copy, im, err, 0, NULL, 1, NULL) ? -1 : 0;
+}
+
+int jq_read_scans(const unsigned char *data, size_t len, jq_image *im, jq_scanrec *recs, int cap, int *nrec, char *err) {
+	jq_recs r; int rc;
+	r.recs = recs; r.cap = recs ? cap : 0; r.n = 0;
+	rc = jq_read_impl(data, len, 0, im, err, 0, NULL, 1, &r) ? -1 : 0;
+	*nrec = r.n;
+	return rc;
 }
 
 /* ---------------------------------------------------------------- the writer */

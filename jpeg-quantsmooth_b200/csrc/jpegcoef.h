@@ -77,6 +77,22 @@ int jq_read_header(const unsigned char *data, size_t len, jq_image *im, jq_heade
  * or -1 with a message in err.  im must be released with jq_free. */
 int jq_read_markers(const unsigned char *data, size_t len, int copy, jq_image *im, char *err);
 
+/* One scan as jq_read_scans records it: what jq_read's decoder would be handed at its SOS (the
+ * tables and restart interval in force), and its entropy-coded bytes [offset, end), end the next
+ * marker that is not RSTn (the file's end when none follows). */
+typedef struct {
+	int sof;                             /* the frame's SOF code: 0xC0, 0xC1 or 0xC2 */
+	int ncomp, ci[4], td[4], ta[4], Ss, Se, Ah, Al;
+	int dc_present[4], ac_present[4];
+	unsigned char dc_bits[4][17], dc_val[4][256], ac_bits[4][17], ac_val[4][256];
+	int restart_interval;
+	size_t offset, end;
+} jq_scanrec;
+
+/* jq_read_markers (copy 0) that also records the scans: recs[0 .. cap), *nrec = all scans found
+ * (may exceed cap).  Returns 0 or -1 with a message in err.  im must be released with jq_free. */
+int jq_read_scans(const unsigned char *data, size_t len, jq_image *im, jq_scanrec *recs, int cap, int *nrec, char *err);
+
 /* The bytes jq_write puts before its first DQT: SOI, the JFIF APP0 or Adobe APP14 of the colour
  * space, the copied markers.  *out is malloc'd.  Returns 0 or -1 (out of memory). */
 int jq_prefix(const jq_image *im, unsigned char **out, size_t *outlen);

@@ -53,6 +53,19 @@ class _Scan(C.Structure):
                 ("jpeg_color_space", C.c_int32), ("sof", C.c_int32)]
 
 
+class _ScanRec(C.Structure):
+    """jpegqs_cuda_scan_rec: one scan of a file as the host marker walk found it (include/jpegqs_cuda.h)."""
+    _fields_ = [("ncomp", C.c_int32), ("comp", C.c_int32 * 4), ("dc_tbl", C.c_int32 * 4), ("ac_tbl", C.c_int32 * 4),
+                ("Ss", C.c_int32), ("Se", C.c_int32), ("Ah", C.c_int32), ("Al", C.c_int32), ("sof", C.c_int32),
+                ("dc_present", C.c_int32 * 4), ("ac_present", C.c_int32 * 4),
+                ("dc_bits", (C.c_uint8 * 17) * 4), ("dc_val", (C.c_uint8 * 256) * 4),
+                ("ac_bits", (C.c_uint8 * 17) * 4), ("ac_val", (C.c_uint8 * 256) * 4),
+                ("restart_interval", C.c_uint32), ("offset", C.c_uint64), ("end", C.c_uint64)]
+
+
+MAX_SCANS = 64
+
+
 class _Head(C.Structure):
     """jpegqs_cuda_jpeg_head: the prefix and frame identifiers of one encoded file (include/jpegqs_cuda.h)."""
     _fields_ = [("prefix_dev", C.c_void_p), ("prefix_len", C.c_uint32), ("comp_id", C.c_int32 * 4),
@@ -151,6 +164,15 @@ def load():
                                              C.POINTER(C.c_size_t), C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
     lib.jpegqs_cuda_decode_model.argtypes = [C.POINTER(_Image), C.POINTER(_Scan), C.c_char_p, C.c_size_t, C.c_int,
                                              C.POINTER(C.c_int32), C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
+    lib.jpegqs_cuda_jpeg_parse_scans.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(_Image), C.POINTER(_ScanRec), C.c_int,
+                                                 C.POINTER(C.c_int)]
+    lib.jpegqs_cuda_decode_scans_workspace_bytes.argtypes = [C.c_int, C.POINTER(_Image), C.c_void_p, C.c_void_p,
+                                                             C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
+    lib.jpegqs_cuda_decode_scans_async.argtypes = [C.c_void_p, C.c_int, C.POINTER(_Image), C.c_void_p, C.c_void_p,
+                                                   C.c_void_p, C.POINTER(C.c_size_t), C.c_void_p, C.c_size_t, C.c_void_p,
+                                                   C.c_void_p]
+    lib.jpegqs_cuda_decode_scans_model.argtypes = [C.POINTER(_Image), C.POINTER(_ScanRec), C.c_int, C.c_char_p, C.c_size_t,
+                                                   C.c_int, C.POINTER(C.c_int32)]
     lib.jpegqs_cuda_jpeg_prefix.argtypes = [C.c_char_p, C.c_size_t, C.c_int, C.c_void_p, C.c_size_t,
                                             C.POINTER(C.c_size_t), C.POINTER(C.c_int32), C.c_int32 * 4, C.c_int32 * 4]
     lib.jpegqs_cuda_encode_bound.argtypes = [C.POINTER(_Image), C.c_size_t, C.POINTER(C.c_size_t)]
@@ -346,6 +368,65 @@ def decode_model(image: CoefImage, scan, data: bytes, sub_bytes: int = DECODE_SU
                                     over.ctypes.data, cap, C.byref(nsub)) < 0:
         raise QsError(lib.jpegqs_cuda_last_error(None).decode())
     return out, int(st.value), over[:nsub.value]
+
+
+def parse_jpeg_scans(data: bytes):
+    """Every marker of a JPEG file, host-only, no entropy-coded data decoded: (CoefImage, scans).  The
+    CoefImage is parse_jpeg's (placeholder arrays); scans is a ScanList of jpegqs_cuda_scan_rec, one per
+    scan, what decode_scans_async needs, or None when only read_jpeg takes the file (more than 64 scans,
+    tables libjpeg would reject, first scans after an overlapping refinement).  Raises QsError for
+    what the reader rejects."""
+    lib = load()
+    data = bytes(data)
+    image, _, _ = _parse(data)
+    ci, recs, n = _Image(), (_ScanRec * MAX_SCANS)(), C.c_int(0)
+    rc = lib.jpegqs_cuda_jpeg_parse_scans(data, len(data), C.byref(ci), recs, MAX_SCANS, C.byref(n))
+    if rc not in (0, -3):
+        raise QsError(f"parse_jpeg_scans: {lib.jpegqs_cuda_last_error(None).decode()}")
+    return image, (ScanList(recs[:n.value]) if rc == 0 else None)
+
+
+class ScanList(list):
+    """The jpegqs_cuda_scan_rec records of one file, in file order (parse_jpeg_scans)."""
+
+    def array(self):
+        return (_ScanRec * max(len(self), 1))(*self)
+
+
+def _scan_arrays(scans):
+    arrs = [s.array() for s in scans]
+    ptrs = (C.c_void_p * max(len(arrs), 1))(*[C.addressof(a) for a in arrs])
+    counts = (C.c_int * max(len(arrs), 1))(*[len(s) for s in scans])
+    return arrs, ptrs, counts
+
+
+def decode_scans_workspace_bytes(images: Sequence[CoefImage], scans, data_len: Sequence[int]) -> int:
+    """Device bytes of workspace decode_scans_async needs (host-only)."""
+    lib = load()
+    n = len(images)
+    arr = _image_array(images)
+    keep, ptrs, counts = _scan_arrays(scans)
+    lens = (C.c_size_t * max(n, 1))(*[int(x) for x in data_len])
+    out = C.c_size_t(0)
+    if lib.jpegqs_cuda_decode_scans_workspace_bytes(n, arr, ptrs, counts, lens, C.byref(out)) < 0:
+        raise QsError(lib.jpegqs_cuda_last_error(None).decode())
+    return int(out.value)
+
+
+def decode_scans_model(image: CoefImage, scans, data: bytes, sub_bytes: int = DECODE_SUB_DEFAULT, out=None):
+    """decode_scans_async's algorithm run on one CPU thread for one file (jpegqs_cuda_decode_scans_model).
+    out: numpy int16 arrays to write (default: new ones).  Returns (arrays, status)."""
+    lib = load()
+    data = bytes(data)
+    if out is None:
+        out = [np.zeros((c.hblk, c.wblk, 64), dtype=np.int16) for c in image.comps]
+    ci = _Image()
+    _fill_image(ci, image, [a.ctypes.data for a in out], [])
+    st = C.c_int32(0)
+    recs = ScanList(scans).array()
+    if lib.jpegqs_cuda_decode_scans_model(C.byref(ci), recs, len(scans), data, len(data), sub_bytes, C.byref(st)) < 0:
+        raise QsError(lib.jpegqs_cuda_last_error(None).decode())
+    return out, int(st.value)
 
 
 # ---- coefficients to JPEG files (include/jpegqs_cuda.h "quantized coefficients to JPEG files") ----
@@ -825,6 +906,61 @@ class QsContext:
                                                           status.data_ptr() if n else None, _stream_handle(stream)))
         return out, status
 
+    def decode_scans_async(self, images: Sequence[CoefImage], scans, data, out=None, stream=None):
+        """decode_async for files of any scan script (progressive, several scans): the same tensor and
+        stream conventions, scans[i] what parse_jpeg_scans returned for file i (not None).  The call
+        zeroes the output tensors itself.  Returns (coefs, status).  Capturable with torch.cuda.graph:
+        every scan's header, position and tables are fixed at capture, so a replay decodes the current
+        contents of the same data tensors as a file with identical headers."""
+        import torch
+        n = len(images)
+        if len(scans) != n or len(data) != n or (out is not None and len(out) != n):
+            raise ValueError("images, scans, data and out must have one entry per image")
+        tensors = []
+        for i, (im, sc) in enumerate(zip(images, scans)):
+            if not isinstance(sc, ScanList) or not sc:
+                raise ValueError(f"scans[{i}]: not a scan list (parse_jpeg_scans gave None: use read_jpeg)")
+            t = data[i]
+            if not isinstance(t, torch.Tensor):
+                raise TypeError(f"data[{i}]: expected a torch.Tensor, got {type(t).__name__}")
+            if t.dtype != torch.uint8 or t.dim() != 1 or not t.is_contiguous():
+                raise ValueError(f"data[{i}]: expected a contiguous 1-D uint8 tensor")
+            if t.numel() < max(r.end for r in sc):
+                raise ValueError(f"data[{i}]: {t.numel()} bytes, the last scan ends at {max(r.end for r in sc)}")
+            tensors.append((f"data[{i}]", t))
+            if out is not None:
+                if len(out[i]) != len(im.comps):
+                    raise ValueError(f"out[{i}]: {len(out[i])} tensors for {len(im.comps)} components")
+                for c, (comp, o) in enumerate(zip(im.comps, out[i])):
+                    _check_tensor(o, (comp.hblk, comp.wblk, 64), f"out[{i}][{c}]")
+                    if o.data_ptr() % 16:
+                        raise ValueError(f"out[{i}][{c}]: not 16-byte aligned")
+                    tensors.append((f"out[{i}][{c}]", o))
+        device = self.device if self.device >= 0 else torch.cuda.current_device()
+        for what, t in tensors:
+            if not t.is_cuda or t.device.index != device:
+                raise ValueError(f"{what}: on {t.device}, expected cuda:{device}")
+        stream = stream if stream is not None else torch.cuda.current_stream(device)
+        with torch.cuda.device(device), torch.cuda.stream(stream):
+            if out is None:
+                out = [[torch.empty((c.hblk, c.wblk, 64), dtype=torch.int16, device=device) for c in im.comps]
+                       for im in images]
+            out = [list(o) for o in out]
+            arr = _image_array(images, [[t.data_ptr() for t in out[i]] for i in range(n)])
+            keep, ptrs, counts = _scan_arrays(scans)
+            lens = (C.c_size_t * max(n, 1))(*[int(t.numel()) for t in data])
+            dptrs = (C.c_void_p * max(n, 1))(*[t.data_ptr() for t in data])
+            size = C.c_size_t(0)
+            if self.lib.jpegqs_cuda_decode_scans_workspace_bytes(n, arr, ptrs, counts, lens, C.byref(size)) < 0:
+                raise QsError(self.lib.jpegqs_cuda_last_error(None).decode())
+            # allocated on `stream`: reused only by work queued after this call's kernels
+            ws = torch.empty(max(size.value, 1), dtype=torch.uint8, device=device)
+            status = torch.empty((n,), dtype=torch.int32, device=device)
+            self._check(self.lib.jpegqs_cuda_decode_scans_async(self.h, n, arr, ptrs, counts, dptrs, lens, ws.data_ptr(),
+                                                                size.value, status.data_ptr() if n else None,
+                                                                _stream_handle(stream)))
+        return out, status
+
     # ---- coefficients to JPEG bytes (include/jpegqs_cuda.h jpegqs_cuda_encode_async) ----
     def encode_async(self, images: Sequence[CoefImage], coefs, heads, optimize: bool = False, status=None, up=None,
                      out=None, capacity=None, stream=None):
@@ -1138,6 +1274,17 @@ def run_async(images: Sequence[CoefImage], coefs, flags: int, niter: int, up=Non
     if not isinstance(first, torch.Tensor) or not first.is_cuda:
         raise ValueError("run_async: the coefficient tensors must be CUDA tensors")
     return default_context(first.device.index).run_async(images, coefs, flags, niter, up, stream)
+
+
+def decode_scans_async(images: Sequence[CoefImage], scans, data, out=None, stream=None):
+    """QsContext.decode_scans_async on the default context of the data tensors' device: decodes JPEG
+    files of any scan script in CUDA tensors to coefficient tensors; returns (coefs, status)."""
+    if not data:
+        raise ValueError("decode_scans_async: no images")
+    first = data[0]
+    if not getattr(first, "is_cuda", False):
+        raise ValueError("decode_scans_async: the data tensors must be CUDA tensors")
+    return default_context(first.device.index).decode_scans_async(images, scans, data, out, stream)
 
 
 def decode_async(images: Sequence[CoefImage], scans, data, out=None, stream=None):

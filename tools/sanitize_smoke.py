@@ -89,3 +89,39 @@ out, lengths, status = ctx.encode_async(work, coefs, [(torch.frombuffer(bytearra
                                         True, rst, ups)
 torch.cuda.synchronize()
 print("decode -> run_async -> encode_async: run", rst.cpu().tolist(), "encode status", status.cpu().tolist(), flush=True)
+
+
+# the scan decoder: progressive files of every kind (restart markers or not, grey, CMYK, untransformed
+# RGB), damaged ones beside them (truncated, bytes flipped, an RST removed, cut one byte after an SOS),
+# in a batch of more than one launch group (16 images), at the smallest subsequence size and the default
+pgood = [jpeg(90, 50, quality=75, progressive=True), jpeg(61, 43, quality=90, progressive=True, restart_marker_blocks=3),
+         jpeg(40, 24, "CMYK", quality=80, progressive=True), jpeg(33, 17, "L", quality=100, progressive=True),
+         jpeg(48, 32, quality=85, keep_rgb=True, subsampling=0, progressive=True),
+         jpeg(70, 30, quality=50, subsampling=1, optimize=True, progressive=True)]
+pbase, prst = pgood[0], pgood[1]
+pflip = bytearray(pbase)
+for p in range(qs.parse_jpeg_scans(pbase)[1][0].offset + 5, len(pbase) - 2, 41):
+    pflip[p] ^= 0x5A
+p = prst.index(b"\xff\xd1")
+last_sos = pbase.rindex(b"\xff\xda")
+pbad = [pbase[:len(pbase) * 2 // 3], bytes(pflip), prst[:p] + prst[p + 2:],
+        pbase[:last_sos + 2 + int.from_bytes(pbase[last_sos + 2:last_sos + 4], "big") + 1]]
+
+
+def device_scans(f):
+    """parse_jpeg_scans' records, or None for a file only the host reader takes or no reader takes"""
+    try:
+        return qs.parse_jpeg_scans(f)[1]
+    except qs.cuda.QsError:
+        return None
+
+
+pfiles = [f for f in pgood * 3 + pbad if device_scans(f) is not None]
+for sub_bytes in (32, 512):
+    ctx.set_tuning(9, sub_bytes)
+    parsed = [qs.parse_jpeg_scans(f) for f in pfiles]
+    data = [torch.frombuffer(bytearray(f), dtype=torch.uint8).cuda() for f in pfiles]
+    coefs, status = ctx.decode_scans_async([p[0] for p in parsed], [p[1] for p in parsed], data)
+    torch.cuda.synchronize()
+    print("decode_scans_async key 9 =", sub_bytes, len(pfiles), "images, status", status.cpu().tolist(), flush=True)
+ctx.set_tuning(9, 512)
