@@ -478,6 +478,65 @@ int jpegqs_cuda_encode_async(jpegqs_cuda_ctx *ctx, int n, const jpegqs_cuda_imag
 int jpegqs_cuda_encode_model(const jpegqs_cuda_image *img, const jpegqs_cuda_jpeg_head *head, int optimize,
 		uint8_t *out, size_t cap, uint64_t *len, int32_t *status);
 
+/* ---- JPEG file -> smoothed JPEG file, blocking --------------------------------------------------
+ * The jpegqs tool's transcode (read, do_quantsmooth, write) on the device: decode, smoothing and
+ * encode kernels on one stream, only the file's bytes crossing the bus.
+ *
+ * The route.  Host-only, no device needed, safe to call from any thread (it writes no error state).
+ * A file goes to the DEVICE only when all of these hold, else to the HOST (the tool's reader,
+ * do_quantsmooth and writer):
+ *   - the markers-only walk of the whole file meets no error and none of the reader's marker-level
+ *     warnings (bytes before a marker, no EOI), so the tool would exit 0 on it;
+ *   - jpegqs_cuda_jpeg_parse takes it (and it has one scan), or jpegqs_cuda_jpeg_parse_scans does;
+ *   - it is not a progressive file with an AC refinement scan without restart markers: the device
+ *     decodes such a scan on one thread, about 13x slower than the host reader (DESIGN.md 3.6.1);
+ *   - it has at most 4 components and, with several, at most 10 blocks per MCU (the encoder's limits).
+ * Returns JPEGQS_ROUTE_DEVICE, JPEGQS_ROUTE_HOST or JPEGQS_ERR_ARG (the reader rejects the file).
+ * *reason (may be NULL) receives a short static description for traces.  info (may be NULL) receives
+ * what the tool's -v line shows. */
+#define JPEGQS_ROUTE_HOST   0
+#define JPEGQS_ROUTE_DEVICE 1
+typedef struct {
+	uint32_t image_width, image_height;
+	int32_t ncomp, progressive;
+	int32_t restart_interval;          /* the last DRI of the file, as the reader reports it */
+} jpegqs_cuda_file_info;
+int jpegqs_cuda_transcode_route(const uint8_t *data, size_t len, const char **reason, jpegqs_cuda_file_info *info);
+
+/* The transcode.  data / len: a JPEG file in host memory.  flags, niter: do_quantsmooth's (flags &
+ * JPEGQS_FLAGS_MASK is used); optimize, copy: the tool's -o and -c.  The call routes the file itself,
+ * uploads it through pinned staging, runs decode_async (one sequential scan) or decode_scans_async,
+ * then run_async - unless do_quantsmooth would return early without touching the coefficients (niter
+ * <= 0 and UPSAMPLE_UV with nothing to up-sample) - then encode_async with the run status and the
+ * up-sampled chroma, so up-sampled and stopped images are written as the tool writes them, and waits.
+ * Returns
+ *   JPEGQS_TRANSCODE_OK        result->data / len hold the file the tool writes, byte for byte;
+ *   JPEGQS_TRANSCODE_FALLBACK  the host route must take this file: the route says HOST, the device
+ *                              decoder flagged the data (any JPEGQS_DECODE_* bit) or the encoder met
+ *                              a coefficient it cannot code (JPEGQS_ENCODE_RANGE).  The host route
+ *                              gives the reader's recovery, warning count and messages.
+ *                              result->reason says which;
+ *   < 0                        JPEGQS_ERR_ARG (arguments, a file the reader rejects) or
+ *                              JPEGQS_ERR_CUDA (jpegqs_cuda_last_error(ctx)).
+ * Output memory: result->data is allocated by the library with malloc(); release it with
+ * jpegqs_cuda_transcode_free (which is free()).  Device memory: the file, the coefficients, the
+ * up-sampled chroma, one workspace shared by the three stages (they run one after another on the
+ * stream) and the output belong to the context, only grow, and are kept between calls, so a run of
+ * files of similar sizes makes no cudaMalloc / cudaFree.  jpegqs_cuda_last_device_ms gives the
+ * smoothing kernels' time (CUDA events around run_async).  One calling thread per context, like the
+ * other blocking entry points. */
+#define JPEGQS_TRANSCODE_OK       0
+#define JPEGQS_TRANSCODE_FALLBACK 1
+typedef struct {
+	uint8_t *data; size_t len;         /* OK: the output file (malloc'd)                              */
+	int32_t smoothed;                  /* 1 = run_async ran (0: do_quantsmooth's early return)        */
+	int32_t stop, upsampled;           /* the run's status when it ran                                */
+	const char *reason;                /* FALLBACK: why, a static string; "" otherwise                */
+} jpegqs_cuda_transcode_result;
+int jpegqs_cuda_transcode(jpegqs_cuda_ctx *ctx, const uint8_t *data, size_t len, int flags, int niter,
+		int optimize, int copy, jpegqs_cuda_transcode_result *result);
+void jpegqs_cuda_transcode_free(void *p);
+
 /* ---- one image sharded by MCU rows over several GPUs (SURVEY.md 8e) ----------------------
  * Every rank - a device of this process, or another process on the same box - smooths one slab
  * of contiguous MCU rows and exchanges ONE pixel row per plane with each neighbour after every

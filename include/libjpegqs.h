@@ -25,6 +25,8 @@
 #define JPEGQS_H                       /* the reference's guard: both headers exclude each other */
 #endif
 
+#include <stddef.h>
+
 #ifdef __cplusplus
 extern "C" {
 #endif
@@ -83,6 +85,15 @@ JPEGQS_ATTR int do_quantsmooth(j_decompress_ptr srcinfo, jvirt_barray_ptr *coef_
 /* extension: create the CUDA context do_quantsmooth(flags) will use (device from the CPU field),
  * e.g. on a second thread while the caller still decodes its file; returns 0 or a negative value */
 JPEGQS_ATTR int jpegqs_warmup(int flags);
+
+/* extension: one JPEG file in memory to the file that reading it, do_quantsmooth(opts) and writing it
+ * (optimize, copy: the jpegqs tool's -o and -c) give, byte for byte, with the same -i lines on stderr -
+ * decoded, smoothed and encoded on the device do_quantsmooth(opts) uses (include/jpegqs_cuda.h
+ * jpegqs_cuda_transcode).  Returns 0 (*out: the file, malloc'd), 1 when the caller must take its
+ * own route for this file (nothing printed; *reason, a static string, says why: damaged data, a file
+ * the device route does not take) or a negative value, reported on stderr as do_quantsmooth does. */
+JPEGQS_ATTR int jpegqs_transcode(const unsigned char *data, size_t len, int copy, int optimize,
+		jpegqs_control_t *opts, unsigned char **out, size_t *outlen, const char **reason);
 
 #ifndef TRANSCODE_ONLY
 /* decode helpers; replace reference libjpegqs.h:50-55 / quantsmooth.h:2880-2904 */

@@ -42,7 +42,8 @@ def __getattr__(name):
     if name in ("cuda", "do_quantsmooth", "run_async", "render_async", "async_workspace_bytes", "QsContext", "lib_path",
                 "parse_jpeg", "read_jpeg", "decode_async", "decode_workspace_bytes", "decode_model",
                 "jpeg_prefix", "encode_bound", "encode_workspace_bytes", "encode_model", "encode_async",
-                "parse_jpeg_scans", "decode_scans_async", "decode_scans_workspace_bytes", "decode_scans_model"):
+                "parse_jpeg_scans", "decode_scans_async", "decode_scans_workspace_bytes", "decode_scans_model",
+                "transcode_route", "transcode"):
         import importlib
         _cuda = importlib.import_module(__name__ + ".cuda")
         if name == "cuda":

@@ -19,10 +19,10 @@
 #include <jpeglib.h>
 #include "libjpegqs.h"
 #include "jpegqs_cuda.h"
+#include "jpegcoef.h"
 
 #ifndef JPEGQS_NO_LOG
 #define WITH_LOG
-#define logfmt(...) fprintf(stderr, __VA_ARGS__)
 #include <sys/time.h>
 static int64_t now_usec(void) {
 	struct timeval tv; gettimeofday(&tv, NULL);
@@ -106,16 +106,18 @@ static jpegqs_cuda_multi *get_multi(void) {
 	return g_multi;
 }
 
-static jpegqs_cuda_ctx *get_ctx(int ordinal_plus1) {
+static jpegqs_cuda_ctx *get_ctx_quiet(int ordinal_plus1) {
 	int slot = ordinal_plus1 < 0 || ordinal_plus1 > QS_MAX_DEVICES ? 0 : ordinal_plus1;
-	if (!g_ctx[slot]) {
-		int rc = jpegqs_cuda_create(slot ? slot - 1 : -1, &g_ctx[slot]);
-		if (rc) {
-			fprintf(stderr, "jpegqs: CUDA back end unavailable: %s\n", jpegqs_cuda_last_error(NULL));
-			g_ctx[slot] = NULL;
-		}
-	}
+	if (!g_ctx[slot] && jpegqs_cuda_create(slot ? slot - 1 : -1, &g_ctx[slot])) g_ctx[slot] = NULL;
 	return g_ctx[slot];
+}
+static void report_unavailable(void) {
+	fprintf(stderr, "jpegqs: CUDA back end unavailable: %s\n", jpegqs_cuda_last_error(NULL));
+}
+static jpegqs_cuda_ctx *get_ctx(int ordinal_plus1) {
+	jpegqs_cuda_ctx *ctx = get_ctx_quiet(ordinal_plus1);
+	if (!ctx) report_unavailable();
+	return ctx;
 }
 
 /* Extension (include/libjpegqs.h): create the context do_quantsmooth(flags) will use.  CUDA
@@ -130,6 +132,123 @@ int jpegqs_warmup(int flags) {
 	ok = g_ctx[slot] != NULL;
 	pthread_mutex_unlock(&g_lock);
 	return ok ? 0 : JPEGQS_ERR_CUDA;
+}
+
+
+#ifdef WITH_LOG
+/* The -i lines (JPEGQS_INFO_*), the same for do_quantsmooth and jpegqs_transcode.  Before anything is
+ * touched: component tables and sampling, the quantization tables. */
+static void log_head(FILE *f, j_decompress_ptr srcinfo, int flags) {
+	jpeg_component_info *comp = srcinfo->comp_info; int ci, i, k;
+	if (flags & JPEGQS_INFO_COMP1)
+		for (ci = 0; ci < srcinfo->num_components; ci++)
+			fprintf(f, "component[%i] : table %i, samp %ix%i\n", ci, comp[ci].quant_tbl_no,
+					comp[ci].h_samp_factor, comp[ci].v_samp_factor);
+	if (flags & JPEGQS_INFO_QUANT)
+		for (i = 0; i < NUM_QUANT_TBLS; i++) {
+			JQUANT_TBL *t = srcinfo->quant_tbl_ptrs[i];
+			if (!t) continue;
+			fprintf(f, "quant[%i]:\n", i);
+			for (k = 0; k < DCTSIZE2; k++) {
+				fprintf(f, "%04x ", t->quantval[k]);
+				if ((k & 7) == 7) fprintf(f, "\n");
+			}
+		}
+}
+/* once the device is reached: the back end, the component sizes (quantsmooth.h:2569-2572) */
+static void log_device(FILE *f, j_decompress_ptr srcinfo, int flags, jpegqs_cuda_ctx *ctx, jpegqs_cuda_multi *multi) {
+	jpeg_component_info *comp = srcinfo->comp_info; int ci;
+	if (flags & JPEGQS_INFO_CPU) {
+		if (multi) fprintf(f, "SIMD type: CUDA sm_90a (%s x %d)\n", jpegqs_cuda_device_name(ctx), jpegqs_cuda_multi_devices(multi));
+		else fprintf(f, "SIMD type: CUDA sm_90a (%s)\n", jpegqs_cuda_device_name(ctx));
+	}
+	if (flags & JPEGQS_INFO_COMP2)
+		for (ci = 0; ci < srcinfo->num_components; ci++) if (comp[ci].quant_table)
+			fprintf(f, "component[%i] : size %ix%i\n", ci, comp[ci].width_in_blocks, comp[ci].height_in_blocks);
+}
+/* at the end of a run that did not stop */
+static void log_time(FILE *f, int flags, int64_t usec, jpegqs_cuda_ctx *ctx) {
+	if (flags & JPEGQS_INFO_TIME) {
+		fprintf(f, "quantsmooth: %.3fms\n", usec * 0.001);
+		fprintf(f, "quantsmooth (device kernels): %.3fms\n", jpegqs_cuda_last_device_ms(ctx));
+	}
+}
+#endif
+
+/* YCbCr with 1x1 chroma under JOINT_YUV / UPSAMPLE_UV: the chroma feed from a down-sampled luma */
+static int needs_downsample(j_decompress_ptr srcinfo, int flags) {
+	jpeg_component_info *comp = srcinfo->comp_info;
+	return flags & (JPEGQS_JOINT_YUV | JPEGQS_UPSAMPLE_UV) && srcinfo->jpeg_color_space == JCS_YCbCr &&
+			srcinfo->num_components >= 3 && comp[1].h_samp_factor == 1 && comp[1].v_samp_factor == 1 &&
+			comp[2].h_samp_factor == 1 && comp[2].v_samp_factor == 1;
+}
+/* 0: do_quantsmooth returns at once and touches nothing (quantsmooth.h:2447-2458) */
+static int smooths(j_decompress_ptr srcinfo, int flags, int niter) {
+	if (srcinfo->num_components < 1 || srcinfo->num_components > JPEGQS_CUDA_MAX_COMP) return 0;
+	if (niter > JPEGQS_ITER_MAX) niter = JPEGQS_ITER_MAX;
+	return niter > 0 || (flags & JPEGQS_UPSAMPLE_UV && needs_downsample(srcinfo, flags));
+}
+
+#ifdef WITH_LOG
+/* the buffered -i lines of a transcode reach stderr unless the file falls back to the host route,
+ * which prints them itself */
+static void log_flush(FILE **f, char **buf, size_t *len, int print) {
+	if (!*f) return;
+	fclose(*f); *f = NULL;
+	if (print && *len) fwrite(*buf, 1, *len, stderr);
+	free(*buf); *buf = NULL;
+}
+#endif
+
+/* Extension (include/libjpegqs.h): the jpegqs tool's device route.  The same context, lock, device
+ * selection and messages as do_quantsmooth, the same -i lines in the same order; the coefficients
+ * never leave the device (jpegqs_cuda_transcode). */
+JPEGQS_ATTR
+int jpegqs_transcode(const unsigned char *data, size_t len, int copy, int optimize, jpegqs_control_t *opts,
+		unsigned char **out, size_t *outlen, const char **reason) {
+	jq_image im; char err[256]; int flags = opts->flags, smooth, ret; jpegqs_cuda_ctx *ctx;
+	jpegqs_cuda_transcode_result res;
+#ifdef WITH_LOG
+	FILE *log; char *logbuf = NULL; size_t loglen = 0; int64_t t0;
+#endif
+	*out = NULL; *outlen = 0; *reason = "";
+	/* what do_quantsmooth would be handed: the frame, quant tables and colour space of the file */
+	if (jq_read_markers(data, len, 0, &im, err)) { *reason = "the reader rejects the file"; return JPEGQS_TRANSCODE_FALLBACK; }
+	smooth = smooths(&im.cinfo, flags, opts->niter);
+#ifdef WITH_LOG
+	log = open_memstream(&logbuf, &loglen);
+	if (!log) { jq_free(&im); *reason = "out of memory"; return JPEGQS_TRANSCODE_FALLBACK; }
+	log_head(log, &im.cinfo, flags);
+#endif
+	pthread_mutex_lock(&g_lock);
+	ctx = get_ctx_quiet((flags >> JPEGQS_CPU_SHIFT) & JPEGQS_CPU_MASK);
+	if (!ctx && !smooth) {
+		/* do_quantsmooth would not reach the device: the host route gives the file without one */
+		pthread_mutex_unlock(&g_lock);
+#ifdef WITH_LOG
+		log_flush(&log, &logbuf, &loglen, 0);
+#endif
+		jq_free(&im);
+		*reason = "no CUDA device, and nothing to smooth";
+		return JPEGQS_TRANSCODE_FALLBACK;
+	}
+#ifdef WITH_LOG
+	if (ctx && smooth) log_device(log, &im.cinfo, flags, ctx, NULL);
+	t0 = now_usec();
+#endif
+	if (!ctx) ret = JPEGQS_ERR_CUDA;
+	else ret = jpegqs_cuda_transcode(ctx, data, len, flags, opts->niter, optimize, copy, &res);
+#ifdef WITH_LOG
+	if (ret == JPEGQS_TRANSCODE_OK && smooth && !res.stop) log_time(log, flags, now_usec() - t0, ctx);
+	log_flush(&log, &logbuf, &loglen, ret != JPEGQS_TRANSCODE_FALLBACK);
+#endif
+	if (!ctx) report_unavailable();
+	else if (ret < 0) fprintf(stderr, "jpegqs: CUDA back end failed (%d): %s\n", ret, jpegqs_cuda_last_error(ctx));
+	pthread_mutex_unlock(&g_lock);
+	jq_free(&im);
+	if (ret == JPEGQS_TRANSCODE_FALLBACK) *reason = res.reason;
+	if (ret == JPEGQS_TRANSCODE_OK) { *out = res.data; *outlen = res.len; }
+	return ret;
 }
 
 /* Block-row table of one virtual array: libjpeg keeps a whole-image coefficient array in memory
@@ -170,40 +289,22 @@ JPEGQS_ATTR
 int do_quantsmooth(j_decompress_ptr srcinfo, jvirt_barray_ptr *coef_arrays, jpegqs_control_t *opts) {
 	jpegqs_cuda_image img; jpegqs_cuda_ctx *ctx; jpegqs_cuda_multi *multi = NULL;
 	jpeg_component_info *comp = srcinfo->comp_info;
-	int ci, i, ret, ncomp = srcinfo->num_components, niter = opts->niter;
-	int need_downsample = 0, flags = opts->flags, resident = 1, will_upsample;
+	int ci, i, ret, ncomp = srcinfo->num_components;
+	int need_downsample, flags = opts->flags, resident = 1, will_upsample;
 	int16_t **rows[JPEGQS_CUDA_MAX_COMP], **rows_up[2] = { NULL, NULL };
 	int16_t *flat[JPEGQS_CUDA_MAX_COMP], *flat_up[2] = { NULL, NULL };
 	jvirt_barray_ptr up[2] = { NULL, NULL };
 	JDIMENSION y;
 #ifdef WITH_LOG
 	int64_t t0 = 0;
-	if (flags & JPEGQS_INFO_COMP1)
-		for (ci = 0; ci < ncomp; ci++)
-			logfmt("component[%i] : table %i, samp %ix%i\n", ci, comp[ci].quant_tbl_no,
-					comp[ci].h_samp_factor, comp[ci].v_samp_factor);
-	if (flags & JPEGQS_INFO_QUANT)
-		for (i = 0; i < NUM_QUANT_TBLS; i++) {
-			JQUANT_TBL *t = srcinfo->quant_tbl_ptrs[i]; int k;
-			if (!t) continue;
-			logfmt("quant[%i]:\n", i);
-			for (k = 0; k < DCTSIZE2; k++) {
-				logfmt("%04x ", t->quantval[k]);
-				if ((k & 7) == 7) logfmt("\n");
-			}
-		}
+	log_head(stderr, srcinfo, flags);
 	if (flags & JPEGQS_INFO_TIME) t0 = now_usec();
 #endif
-#define LOG_COMP2 if (flags & JPEGQS_INFO_COMP2) for (ci = 0; ci < ncomp; ci++) if (comp[ci].quant_table) \
-	logfmt("component[%i] : size %ix%i\n", ci, comp[ci].width_in_blocks, comp[ci].height_in_blocks);
 	if (ncomp < 1 || ncomp > JPEGQS_CUDA_MAX_COMP) return 0;
 
 	/* same early exit as the reference (quantsmooth.h:2447-2458): nothing is touched */
-	if (flags & (JPEGQS_JOINT_YUV | JPEGQS_UPSAMPLE_UV) && srcinfo->jpeg_color_space == JCS_YCbCr &&
-			ncomp >= 3 && comp[1].h_samp_factor == 1 && comp[1].v_samp_factor == 1 &&
-			comp[2].h_samp_factor == 1 && comp[2].v_samp_factor == 1) need_downsample = 1;
-	if (niter > JPEGQS_ITER_MAX) niter = JPEGQS_ITER_MAX;
-	if (niter <= 0 && !(flags & JPEGQS_UPSAMPLE_UV && need_downsample)) return 0;
+	need_downsample = needs_downsample(srcinfo, flags);
+	if (!smooths(srcinfo, flags, opts->niter)) return 0;
 	will_upsample = need_downsample && flags & JPEGQS_UPSAMPLE_UV &&
 			(comp[0].h_samp_factor != 1 || comp[0].v_samp_factor != 1);
 
@@ -212,11 +313,7 @@ int do_quantsmooth(j_decompress_ptr srcinfo, jvirt_barray_ptr *coef_arrays, jpeg
 	ctx = multi ? jpegqs_cuda_multi_ctx(multi, 0) : get_ctx((flags >> JPEGQS_CPU_SHIFT) & JPEGQS_CPU_MASK);
 	if (!ctx) { pthread_mutex_unlock(&g_lock); return JPEGQS_ERR_CUDA; }
 #ifdef WITH_LOG
-	if (flags & JPEGQS_INFO_CPU) {
-		if (multi) logfmt("SIMD type: CUDA sm_90a (%s x %d)\n", jpegqs_cuda_device_name(ctx), jpegqs_cuda_multi_devices(multi));
-		else logfmt("SIMD type: CUDA sm_90a (%s)\n", jpegqs_cuda_device_name(ctx));
-	}
-	LOG_COMP2                                          /* quantsmooth.h:2569-2572 */
+	log_device(stderr, srcinfo, flags, ctx, multi);
 #endif
 
 	memset(&img, 0, sizeof(img));
@@ -337,10 +434,7 @@ int do_quantsmooth(j_decompress_ptr srcinfo, jvirt_barray_ptr *coef_arrays, jpeg
 	}
 #endif
 #ifdef WITH_LOG
-	if (!ret && flags & JPEGQS_INFO_TIME) {
-		logfmt("quantsmooth: %.3fms\n", (now_usec() - t0) * 0.001);
-		logfmt("quantsmooth (device kernels): %.3fms\n", jpegqs_cuda_last_device_ms(ctx));
-	}
+	if (!ret) log_time(stderr, flags, now_usec() - t0, ctx);
 #endif
 done:
 	for (ci = 0; ci < ncomp; ci++) { free(rows[ci]); free(flat[ci]); }

@@ -40,8 +40,21 @@ static void fill_image(const jq_image *im, jpegqs_cuda_image *img) {
 	}
 }
 
+/* jpegqs_cuda_jpeg_parse's rule for the first scan (the same fields in jq_header and jq_scanrec): not
+ * progressive, all frame components, at least one entropy-coded byte, tables libjpeg decodes with */
+#define FIRST_SCAN_OK(h, nframe, offset, len) first_scan_ok((h).sof, (h).ncomp, nframe, offset, len, (h).td, (h).ta, \
+		(h).dc_present, (h).ac_present, (h).dc_bits, (h).dc_val, (h).ac_bits, (h).ac_val)
+static int first_scan_ok(int sof, int ncomp, int nframe, size_t offset, size_t len, const int *td, const int *ta,
+		const int *dcp, const int *acp, unsigned char (*dcb)[17], unsigned char (*dcv)[256],
+		unsigned char (*acb)[17], unsigned char (*acv)[256]) {
+	int k, ok = sof != 0xC2 && ncomp == nframe && offset < len;
+	for (k = 0; ok && k < ncomp; k++)
+		ok = dcp[td[k]] && acp[ta[k]] && table_ok(dcb[td[k]], dcv[td[k]], 1) && table_ok(acb[ta[k]], acv[ta[k]], 0);
+	return ok;
+}
+
 int jpegqs_cuda_jpeg_parse(const uint8_t *data, size_t len, jpegqs_cuda_image *img, jpegqs_cuda_scan *scan) {
-	jq_image im; jq_header h; char err[256]; int k, ok;
+	jq_image im; jq_header h; char err[256]; int k;
 	if (!data || !img || !scan) { qs_set_host_error("jpegqs_cuda_jpeg_parse: NULL argument"); return JPEGQS_ERR_ARG; }
 	if (jq_read_header(data, len, &im, &h, err)) { qs_set_host_error(err); return JPEGQS_ERR_ARG; }
 	fill_image(&im, img);
@@ -58,11 +71,9 @@ int jpegqs_cuda_jpeg_parse(const uint8_t *data, size_t len, jpegqs_cuda_image *i
 	scan->jpeg_color_space = (int32_t)im.cinfo.jpeg_color_space;
 	scan->sof = h.sof;
 	jq_free(&im);
-	ok = h.sof != 0xC2 && h.ncomp == img->ncomp && h.entropy_offset < len;
-	for (k = 0; ok && k < h.ncomp; k++)
-		ok = h.dc_present[h.td[k]] && h.ac_present[h.ta[k]] &&
-			table_ok(h.dc_bits[h.td[k]], h.dc_val[h.td[k]], 1) && table_ok(h.ac_bits[h.ta[k]], h.ac_val[h.ta[k]], 0);
-	if (!ok) { qs_set_host_error("jpegqs_cuda_jpeg_parse: only the host reader takes this file"); return JPEGQS_ERR_UNSUPPORTED; }
+	if (!FIRST_SCAN_OK(h, img->ncomp, h.entropy_offset, len)) {
+		qs_set_host_error("jpegqs_cuda_jpeg_parse: only the host reader takes this file"); return JPEGQS_ERR_UNSUPPORTED;
+	}
 	return 0;
 }
 
@@ -71,30 +82,22 @@ static void scan_band(const jq_scanrec *r, int prog, int *lo, int *hi) {
 	*lo = r->Ss; *hi = prog && r->Ss == 0 ? 0 : r->Se;
 }
 
-int jpegqs_cuda_jpeg_parse_scans(const uint8_t *data, size_t len, jpegqs_cuda_image *img,
-		jpegqs_cuda_scan_rec *scans, int cap, int *nscans) {
-	jq_image im; char err[256]; int n = 0, i, j, k, prog, unsupported = 0;
-	jq_scanrec *rec;
-	if (!data || !img || !nscans || cap < 0 || (cap && !scans)) { qs_set_host_error("jpegqs_cuda_jpeg_parse_scans: NULL argument"); return JPEGQS_ERR_ARG; }
-	rec = (jq_scanrec*)calloc(JPEGQS_MAX_SCANS, sizeof(*rec));
-	if (!rec) { qs_set_host_error("jpegqs_cuda_jpeg_parse_scans: out of memory"); return JPEGQS_ERR_ARG; }
-	if (jq_read_scans(data, len, &im, rec, JPEGQS_MAX_SCANS, &n, err)) { free(rec); qs_set_host_error(err); return JPEGQS_ERR_ARG; }
-	fill_image(&im, img);
-	prog = im.progressive;
-	jq_free(&im);
-	*nscans = n;
-	if (!n) { free(rec); qs_set_host_error("jpegqs_cuda_jpeg_parse_scans: no scan found"); return JPEGQS_ERR_ARG; }
-	if (n > JPEGQS_MAX_SCANS || n > cap) unsupported = 1;
+/* jpegqs_cuda_jpeg_parse_scans' verdict on the recorded scans (n >= 1): 0, JPEGQS_ERR_UNSUPPORTED or
+ * JPEGQS_ERR_ARG, with the reason in *why */
+static int scans_check(const jq_scanrec *rec, int n, int prog, const char **why) {
+	int i, j, k, unsupported = 0;
+	*why = "only the host reader takes this file";
+	if (n > JPEGQS_MAX_SCANS) { *why = "more than 64 scans"; unsupported = 1; }
 	for (i = 0; i < n && i < JPEGQS_MAX_SCANS; i++) {
 		const jq_scanrec *r = &rec[i];
 		int need_dc = !prog || (r->Ss == 0 && r->Ah == 0), need_ac = prog ? r->Ss > 0 : 1, lo, hi;
-		if (r->offset >= r->end) unsupported = 1;      /* no entropy-coded byte: a file cut at this SOS */
+		if (r->offset >= r->end) { *why = "a scan without entropy-coded data"; unsupported = 1; }      /* a file cut at this SOS */
 		for (k = 0; k < r->ncomp; k++) {
 			if ((need_dc && !r->dc_present[r->td[k]]) || (need_ac && !r->ac_present[r->ta[k]])) {
-				free(rec); qs_set_host_error("jpegqs_cuda_jpeg_parse_scans: scan uses an undefined Huffman table"); return JPEGQS_ERR_ARG;
+				*why = "scan uses an undefined Huffman table"; return JPEGQS_ERR_ARG;
 			}
 			if ((need_dc && !table_ok(r->dc_bits[r->td[k]], r->dc_val[r->td[k]], 1)) ||
-					(need_ac && !table_ok(r->ac_bits[r->ta[k]], r->ac_val[r->ta[k]], 0))) unsupported = 1;
+					(need_ac && !table_ok(r->ac_bits[r->ta[k]], r->ac_val[r->ta[k]], 0))) { *why = "a Huffman table libjpeg rejects"; unsupported = 1; }
 		}
 		/* first scans (Ah = 0) of a component must code disjoint bands, and come before the
 		 * refinement scans of their band: the device runs all first scans before any refinement */
@@ -103,26 +106,120 @@ int jpegqs_cuda_jpeg_parse_scans(const uint8_t *data, size_t len, jpegqs_cuda_im
 			const jq_scanrec *e = &rec[j]; int elo, ehi, share = 0, a, b;
 			for (a = 0; a < r->ncomp; a++) for (b = 0; b < e->ncomp; b++) share |= r->ci[a] == e->ci[b];
 			scan_band(e, prog, &elo, &ehi);
-			if (share && lo <= ehi && elo <= hi) unsupported = 1;
+			if (share && lo <= ehi && elo <= hi) { *why = "overlapping first scans"; unsupported = 1; }
 		}
 	}
-	for (i = 0; i < n && i < cap && i < JPEGQS_MAX_SCANS; i++) {
-		const jq_scanrec *r = &rec[i]; jpegqs_cuda_scan_rec *o = &scans[i];
-		memset(o, 0, sizeof(*o));
-		o->ncomp = r->ncomp;
-		for (k = 0; k < 4; k++) {
-			o->comp[k] = r->ci[k]; o->dc_tbl[k] = r->td[k]; o->ac_tbl[k] = r->ta[k];
-			o->dc_present[k] = r->dc_present[k]; o->ac_present[k] = r->ac_present[k];
-			memcpy(o->dc_bits[k], r->dc_bits[k], 17); memcpy(o->dc_val[k], r->dc_val[k], 256);
-			memcpy(o->ac_bits[k], r->ac_bits[k], 17); memcpy(o->ac_val[k], r->ac_val[k], 256);
-		}
-		o->Ss = r->Ss; o->Se = r->Se; o->Ah = r->Ah; o->Al = r->Al; o->sof = r->sof;
-		o->restart_interval = (uint32_t)r->restart_interval;
-		o->offset = r->offset; o->end = r->end;
+	return unsupported ? JPEGQS_ERR_UNSUPPORTED : 0;
+}
+
+static void copy_rec(const jq_scanrec *r, jpegqs_cuda_scan_rec *o) {
+	int k;
+	memset(o, 0, sizeof(*o));
+	o->ncomp = r->ncomp;
+	for (k = 0; k < 4; k++) {
+		o->comp[k] = r->ci[k]; o->dc_tbl[k] = r->td[k]; o->ac_tbl[k] = r->ta[k];
+		o->dc_present[k] = r->dc_present[k]; o->ac_present[k] = r->ac_present[k];
+		memcpy(o->dc_bits[k], r->dc_bits[k], 17); memcpy(o->dc_val[k], r->dc_val[k], 256);
+		memcpy(o->ac_bits[k], r->ac_bits[k], 17); memcpy(o->ac_val[k], r->ac_val[k], 256);
 	}
+	o->Ss = r->Ss; o->Se = r->Se; o->Ah = r->Ah; o->Al = r->Al; o->sof = r->sof;
+	o->restart_interval = (uint32_t)r->restart_interval;
+	o->offset = r->offset; o->end = r->end;
+}
+
+int jpegqs_cuda_jpeg_parse_scans(const uint8_t *data, size_t len, jpegqs_cuda_image *img,
+		jpegqs_cuda_scan_rec *scans, int cap, int *nscans) {
+	jq_image im; char err[256]; int n = 0, i, prog, rc;
+	jq_scanrec *rec; const char *why;
+	if (!data || !img || !nscans || cap < 0 || (cap && !scans)) { qs_set_host_error("jpegqs_cuda_jpeg_parse_scans: NULL argument"); return JPEGQS_ERR_ARG; }
+	rec = (jq_scanrec*)calloc(JPEGQS_MAX_SCANS, sizeof(*rec));
+	if (!rec) { qs_set_host_error("jpegqs_cuda_jpeg_parse_scans: out of memory"); return JPEGQS_ERR_ARG; }
+	if (jq_read_scans(data, len, 0, &im, rec, JPEGQS_MAX_SCANS, &n, err)) { free(rec); qs_set_host_error(err); return JPEGQS_ERR_ARG; }
+	fill_image(&im, img);
+	prog = im.progressive;
+	jq_free(&im);
+	*nscans = n;
+	if (!n) { free(rec); qs_set_host_error("jpegqs_cuda_jpeg_parse_scans: no scan found"); return JPEGQS_ERR_ARG; }
+	rc = scans_check(rec, n, prog, &why);
+	if (rc == JPEGQS_ERR_ARG) { free(rec); qs_set_host_error("jpegqs_cuda_jpeg_parse_scans: scan uses an undefined Huffman table"); return rc; }
+	if (n > cap) rc = JPEGQS_ERR_UNSUPPORTED;
+	for (i = 0; i < n && i < cap && i < JPEGQS_MAX_SCANS; i++) copy_rec(&rec[i], &scans[i]);
 	free(rec);
-	if (unsupported) { qs_set_host_error("jpegqs_cuda_jpeg_parse_scans: only the host reader takes this file"); return JPEGQS_ERR_UNSUPPORTED; }
+	if (rc) { qs_set_host_error("jpegqs_cuda_jpeg_parse_scans: only the host reader takes this file"); return JPEGQS_ERR_UNSUPPORTED; }
 	return 0;
+}
+
+/* The route of a file through a transcode: jpegqs_cuda_transcode_route's rule, and what
+ * jpegqs_cuda_transcode needs of a DEVICE file, from one markers-only walk.  Every output but reason
+ * may be NULL.  On DEVICE: img filled (coef pointers NULL); *nscans = 0 and *scan filled when
+ * decode_async takes the file, else recs[0 .. *nscans) for decode_scans_async; head->comp_id /
+ * quant_tbl filled and *prefix (malloc'd, copy level `copy`) / *prefix_len set.  Writes no error
+ * state, so any thread may call it. */
+int qs_route_plan(const uint8_t *data, size_t len, int copy, jpegqs_cuda_file_info *info, jpegqs_cuda_image *img,
+		jpegqs_cuda_scan *scan, jpegqs_cuda_scan_rec *recs, int *nscans, jpegqs_cuda_jpeg_head *head,
+		uint8_t **prefix, size_t *prefix_len, const char **reason) {
+	jq_image im; char err[256]; jq_scanrec *rec; int n = 0, i, k, nc, blocks = 0, seq, route = JPEGQS_ROUTE_HOST;
+	const char *why = "", *check_why;
+	if (prefix) *prefix = NULL;
+	if (!data) { *reason = "no data"; return JPEGQS_ERR_ARG; }
+	rec = (jq_scanrec*)calloc(JPEGQS_MAX_SCANS, sizeof(*rec));
+	if (!rec) { *reason = "out of memory"; return JPEGQS_ERR_ARG; }
+	if (jq_read_scans(data, len, copy, &im, rec, JPEGQS_MAX_SCANS, &n, err)) { free(rec); *reason = "the reader rejects the file"; return JPEGQS_ERR_ARG; }
+	nc = im.cinfo.num_components;
+	for (i = 0; i < nc; i++) blocks += im.cinfo.comp_info[i].h_samp_factor * im.cinfo.comp_info[i].v_samp_factor;
+	if (info) {
+		info->image_width = im.cinfo.image_width; info->image_height = im.cinfo.image_height;
+		info->ncomp = nc; info->progressive = im.progressive; info->restart_interval = im.restart_interval;
+	}
+	/* the sequential decoder decodes the first scan only: a second scan would be lost */
+	seq = n == 1 && FIRST_SCAN_OK(rec[0], nc, rec[0].offset, len);
+	if (!n) why = "no scan";
+	else if (im.warnings) why = "marker-level damage (extraneous bytes or no EOI)";
+	else if (nc > 4) why = "more than 4 components";
+	else if (nc > 1 && blocks > 10) why = "more than 10 blocks per MCU";
+	else if (!seq && scans_check(rec, n, im.progressive, &check_why)) why = check_why;
+	else {
+		for (i = 0; i < n && i < JPEGQS_MAX_SCANS && !why[0]; i++)
+			if (im.progressive && rec[i].Ss > 0 && rec[i].Ah > 0 && !rec[i].restart_interval)
+				why = "progressive AC refinement scan without restart markers";
+		if (!why[0]) { route = JPEGQS_ROUTE_DEVICE; why = seq ? "sequential, one scan" : im.progressive ? "progressive" : "several scans"; }
+	}
+	if (route == JPEGQS_ROUTE_DEVICE) {
+		if (img) fill_image(&im, img);
+		if (nscans) *nscans = seq ? 0 : n;
+		if (scan && seq) {
+			const jq_scanrec *r = &rec[0];
+			memset(scan, 0, sizeof(*scan));
+			scan->ncomp = r->ncomp;
+			for (k = 0; k < 4; k++) {
+				scan->comp[k] = r->ci[k]; scan->dc_tbl[k] = r->td[k]; scan->ac_tbl[k] = r->ta[k];
+				scan->dc_present[k] = r->dc_present[k]; scan->ac_present[k] = r->ac_present[k];
+				memcpy(scan->dc_bits[k], r->dc_bits[k], 17); memcpy(scan->dc_val[k], r->dc_val[k], 256);
+				memcpy(scan->ac_bits[k], r->ac_bits[k], 17); memcpy(scan->ac_val[k], r->ac_val[k], 256);
+			}
+			scan->restart_interval = (uint32_t)r->restart_interval;
+			scan->entropy_offset = r->offset;
+			scan->jpeg_color_space = (int32_t)im.cinfo.jpeg_color_space;
+			scan->sof = r->sof;
+		}
+		if (recs && !seq) for (i = 0; i < n; i++) copy_rec(&rec[i], &recs[i]);
+		if (head) for (k = 0; k < 4; k++) {
+			head->comp_id[k] = k < nc ? im.comp_id[k] : 0;
+			head->quant_tbl[k] = k < nc ? im.cinfo.comp_info[k].quant_tbl_no : 0;
+		}
+		if (prefix && jq_prefix(&im, prefix, prefix_len)) { *prefix = NULL; route = JPEGQS_ERR_ARG; why = "out of memory"; }
+	}
+	jq_free(&im);
+	free(rec);
+	*reason = why;
+	return route;
+}
+
+int jpegqs_cuda_transcode_route(const uint8_t *data, size_t len, const char **reason, jpegqs_cuda_file_info *info) {
+	const char *why;
+	int rc = qs_route_plan(data, len, 0, info, NULL, NULL, NULL, NULL, NULL, NULL, NULL, &why);
+	if (reason) *reason = why;
+	return rc;
 }
 
 int jpegqs_cuda_jpeg_read(const uint8_t *data, size_t len, const jpegqs_cuda_image *img) {

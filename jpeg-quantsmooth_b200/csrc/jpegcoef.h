@@ -89,9 +89,9 @@ typedef struct {
 	size_t offset, end;
 } jq_scanrec;
 
-/* jq_read_markers (copy 0) that also records the scans: recs[0 .. cap), *nrec = all scans found
- * (may exceed cap).  Returns 0 or -1 with a message in err.  im must be released with jq_free. */
-int jq_read_scans(const unsigned char *data, size_t len, jq_image *im, jq_scanrec *recs, int cap, int *nrec, char *err);
+/* jq_read_markers that also records the scans: recs[0 .. cap), *nrec = all scans found (may exceed
+ * cap).  Returns 0 or -1 with a message in err.  im must be released with jq_free. */
+int jq_read_scans(const unsigned char *data, size_t len, int copy, jq_image *im, jq_scanrec *recs, int cap, int *nrec, char *err);
 
 /* The bytes jq_write puts before its first DQT: SOI, the JFIF APP0 or Adobe APP14 of the colour
  * space, the copied markers.  *out is malloc'd.  Returns 0 or -1 (out of memory). */

@@ -77,13 +77,18 @@ static int usage(const char *prog) {
 /* One "input output" pair moves through three stages: read + Huffman-decode, do_quantsmooth,
  * encode + write.  A single pair runs them in a row; --batch runs them as a pipeline (a reader
  * thread, the calling thread for the device work, a writer thread), so that with many files the
- * process moves at the pace of the slowest stage instead of their sum. */
+ * process moves at the pace of the slowest stage instead of their sum.
+ * The device route (jpegqs_transcode): when the file allows it, the reader only loads the bytes, the
+ * middle stage decodes, smooths and encodes on the device and the writer only writes the result -
+ * the same bytes, exit status and messages as the host codec around do_quantsmooth. */
 typedef struct {
 	const char *in_name, *out_name;
 	int state;                           /* stages completed: 0 none, 1 read, 2 smoothed, 3 written */
 	int rc;                              /* exit status of this pair so far (non-zero: later stages are skipped) */
 	int have_im;
 	jq_image im;
+	unsigned char *data; size_t len;     /* device route: the input file, then (out) the output file */
+	unsigned char *out; size_t outlen;
 	double t_read, t_smooth, t_write;    /* stage durations, ms */
 } qs_job;
 
@@ -91,29 +96,71 @@ typedef struct {
 	const char *prog;
 	jpegqs_control_t opts;
 	int copy, optimize, verbose, ppm, cpu;
+	const char *host_only;               /* why no pair takes the device route, NULL if pairs may */
+	int trace;                           /* JPEGQS_CODEC_TRACE: print the route of every pair */
 } qs_cfg;
+
+/* the reader's part of the host route: Huffman-decode the file (consumes data) */
+static void job_decode(const qs_cfg *g, qs_job *j, unsigned char *data, size_t len, int header_line) {
+	char err[256];
+	if (jq_read(data, len, g->copy, &j->im, err)) { fprintf(stderr, "%s: %s\n", g->prog, err); free(data); j->rc = 1; return; }
+	free(data);
+	j->have_im = 1;
+	if (g->verbose && header_line)
+		fprintf(stderr, "%s: %ux%u, %d component(s), %s, restart interval %d\n", j->in_name, j->im.cinfo.image_width,
+				j->im.cinfo.image_height, j->im.cinfo.num_components, j->im.progressive ? "progressive" : "sequential",
+				j->im.restart_interval);
+}
 
 static void job_read(const qs_cfg *g, qs_job *j) {
 	double t0 = now_ms();
-	FILE *f; unsigned char *data; size_t len = 0; char err[256];
+	FILE *f; unsigned char *data; size_t len = 0;
 	f = strcmp(j->in_name, "-") ? fopen(j->in_name, "rb") : stdin;
 	if (!f) { fprintf(stderr, "%s: can't open input file \"%s\"\n", g->prog, j->in_name); j->rc = 1; return; }
 	data = load_all(f, &len);
 	if (f != stdin) fclose(f);
 	if (!data) { fprintf(stderr, "%s: can't read input file \"%s\"\n", g->prog, j->in_name); j->rc = 1; return; }
-	if (jq_read(data, len, g->copy, &j->im, err)) { fprintf(stderr, "%s: %s\n", g->prog, err); free(data); j->rc = 1; return; }
-	free(data);
-	j->have_im = 1;
-	if (g->verbose)
-		fprintf(stderr, "%s: %ux%u, %d component(s), %s, restart interval %d\n", j->in_name, j->im.cinfo.image_width,
-				j->im.cinfo.image_height, j->im.cinfo.num_components, j->im.progressive ? "progressive" : "sequential",
-				j->im.restart_interval);
+#ifndef JPEGQS_NO_CUDA_RENDER
+	if (!g->host_only) {
+		jpegqs_cuda_file_info info; const char *why = "";
+		int route = jpegqs_cuda_transcode_route(data, len, &why, &info);
+		if (g->trace) fprintf(stderr, "jpegqs: %s: %s route (%s)\n", j->in_name, route == JPEGQS_ROUTE_DEVICE ? "device" : "host", why);
+		if (route == JPEGQS_ROUTE_DEVICE) {
+			j->data = data; j->len = len;
+			if (g->verbose)
+				fprintf(stderr, "%s: %ux%u, %d component(s), %s, restart interval %d\n", j->in_name, info.image_width,
+						info.image_height, info.ncomp, info.progressive ? "progressive" : "sequential", info.restart_interval);
+			j->t_read = now_ms() - t0;
+			return;
+		}
+	} else if (g->trace) fprintf(stderr, "jpegqs: %s: host route (%s)\n", j->in_name, g->host_only);
+#endif
+	job_decode(g, j, data, len, 1);
 	j->t_read = now_ms() - t0;
 }
 
 static void job_smooth(const qs_cfg *g, qs_job *j) {
 	double t0 = now_ms();
 	jpegqs_control_t opts = g->opts;
+#ifndef JPEGQS_NO_CUDA_RENDER
+	if (j->data) {                                      /* the device route */
+		const char *why = ""; unsigned char *data = j->data;
+		int rc = jpegqs_transcode(data, j->len, g->copy, g->optimize, &opts, &j->out, &j->outlen, &why);
+		if (rc != JPEGQS_TRANSCODE_FALLBACK) {
+			free(data); j->data = NULL;
+			if (rc < 0) j->rc = 2;
+			j->t_smooth = now_ms() - t0;
+			return;
+		}
+		/* damaged data (or a file the device route does not take after all): the host route gives
+		 * the reader's recovery, warning count and messages */
+		if (g->trace) fprintf(stderr, "jpegqs: %s: host route after all (%s)\n", j->in_name, why);
+		j->data = NULL;
+		job_decode(g, j, data, j->len, 0);
+		if (j->rc) return;
+		opts = g->opts;
+	}
+#endif
 	if (do_quantsmooth(&j->im.cinfo, j->im.coef_arrays, &opts) < 0) j->rc = 2;
 	j->t_smooth = now_ms() - t0;
 }
@@ -121,7 +168,7 @@ static void job_smooth(const qs_cfg *g, qs_job *j) {
 static void job_write(const qs_cfg *g, qs_job *j) {
 	double t0 = now_ms();
 	jq_image *im = &j->im;
-	FILE *f; unsigned char *out = NULL; size_t outlen = 0; char err[256]; int io_err = 0;
+	FILE *f; unsigned char *out = NULL; size_t outlen = 0; char err[256]; int io_err = 0, device = j->out != NULL;
 #ifdef JPEGQS_NO_CUDA_RENDER
 	if (g->ppm) { fprintf(stderr, "%s: --ppm needs the CUDA back end\n", g->prog); j->rc = 1; return; }
 #else
@@ -169,7 +216,8 @@ static void job_write(const qs_cfg *g, qs_job *j) {
 		free(rgb);
 	} else
 #endif
-	if (jq_write(im, im->coef_arrays, g->optimize, &out, &outlen, err)) {
+	if (device) { out = j->out; outlen = j->outlen; j->out = NULL; }     /* the device route wrote it */
+	else if (jq_write(im, im->coef_arrays, g->optimize, &out, &outlen, err)) {
 		fprintf(stderr, "%s: %s\n", g->prog, err); j->rc = 1; return;
 	}
 	/* the output is opened after the input was read, so it may name the same file */
@@ -180,14 +228,22 @@ static void job_write(const qs_cfg *g, qs_job *j) {
 	if (io_err) fprintf(stderr, "%s: error writing \"%s\"\n", g->prog, j->out_name);
 	free(out);
 	j->t_write = now_ms() - t0;
-	if (g->verbose) fprintf(stderr, "wall time: read + decode %.1f ms, do_quantsmooth %.1f ms (includes waiting for CUDA start-up), "
+	if (g->verbose && device)
+		fprintf(stderr, "wall time: read %.1f ms, device decode + do_quantsmooth + encode %.1f ms (includes waiting for "
+				"CUDA start-up), write %.1f ms\n", j->t_read, j->t_smooth, j->t_write);
+	else if (g->verbose) fprintf(stderr, "wall time: read + decode %.1f ms, do_quantsmooth %.1f ms (includes waiting for CUDA start-up), "
 			"encode + write %.1f ms\n", j->t_read, j->t_smooth, j->t_write);
 	/* the reference's exit status (quantsmooth.c:626): 2 when the codec met recoverable damage
-	 * (libjpeg's num_warnings), else 0 - do_quantsmooth's "stopped early" value is not an error */
-	j->rc = io_err ? 1 : im->warnings ? 2 : 0;
+	 * (libjpeg's num_warnings), else 0 - do_quantsmooth's "stopped early" value is not an error.
+	 * A file with any warning never finishes on the device route. */
+	j->rc = io_err ? 1 : !device && im->warnings ? 2 : 0;
 }
 
-static void job_release(qs_job *j) { if (j->have_im) { jq_free(&j->im); j->have_im = 0; } }
+static void job_release(qs_job *j) {
+	if (j->have_im) { jq_free(&j->im); j->have_im = 0; }
+	free(j->data); j->data = NULL;
+	free(j->out); j->out = NULL;
+}
 
 /* one input -> one output, the stages in a row; returns the process exit status for this pair */
 static int run_one(const qs_cfg *g, qs_job *j, int warm_ok) {
@@ -347,7 +403,13 @@ int main(int argc, char **argv) {
 	 * kernel image, seconds in a fresh process) is paid once; the exit status is the worst of the pairs */
 	{
 		qs_cfg g; qs_job *jobs; int n = (argc - i) / 2, k;
+		const char *gpus = getenv("JPEGQS_GPUS");
 		g.prog = argv[0]; g.opts = opts; g.copy = copy; g.optimize = optimize; g.verbose = verbose; g.ppm = ppm; g.cpu = cpu;
+		g.trace = getenv("JPEGQS_CODEC_TRACE") != NULL;
+		/* the device route where the pair reaches the device anyway (the warm-up's condition) and
+		 * its output is a JPEG file; JPEGQS_HOST_CODEC=1 keeps every pair on the host codec */
+		g.host_only = ppm ? "--ppm" : !(opts.niter > 0 || (opts.flags & JPEGQS_UPSAMPLE_UV)) ? "nothing to smooth" :
+				gpus && *gpus ? "JPEGQS_GPUS" : getenv("JPEGQS_HOST_CODEC") ? "JPEGQS_HOST_CODEC" : NULL;
 		jobs = (qs_job*)calloc((size_t)n, sizeof(qs_job));
 		if (!jobs) { fprintf(stderr, "%s: out of memory\n", argv[0]); return 1; }
 		for (k = 0; k < n; k++) { jobs[k].in_name = argv[i + 2 * k]; jobs[k].out_name = argv[i + 2 * k + 1]; }

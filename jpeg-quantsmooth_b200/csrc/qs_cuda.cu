@@ -196,10 +196,12 @@ struct jpegqs_cuda_ctx {
 	std::vector<cudaEvent_t> ev_pool; size_t ev_used;
 	std::vector<int> ev_kind;              /* 0 = idct pass, 1 = smoothing pass, per pair */
 	float kernel_ms[2]; int kernel_launches[2];
+	void *transcode;                       /* jpegqs_cuda_transcode's buffers (qs_transcode.cu), grow-only */
 	char err[512];
 };
 
 static char g_err[512] = "";
+void qs_transcode_release(void *state);          /* qs_transcode.cu */
 
 #define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { \
 	snprintf(ctx ? ctx->err : g_err, 512, "%s:%d: %s: %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); \
@@ -225,7 +227,9 @@ extern "C" void jpegqs_cuda_host_free(void *p) { if (p) cudaFreeHost(p); }
 extern "C" void jpegqs_cuda_destroy(jpegqs_cuda_ctx *ctx) {
 	if (!ctx) return;
 	cudaSetDevice(ctx->device);
-	if (ctx->stream) { cudaStreamSynchronize(ctx->stream); cudaStreamDestroy(ctx->stream); }
+	if (ctx->stream) cudaStreamSynchronize(ctx->stream);
+	qs_transcode_release(ctx->transcode);
+	if (ctx->stream) cudaStreamDestroy(ctx->stream);
 	delete ctx->up; delete ctx->down; delete ctx->pool;      /* joins the threads */
 	if (ctx->up_stream) { cudaStreamSynchronize(ctx->up_stream); cudaStreamDestroy(ctx->up_stream); }
 	if (ctx->down_stream) { cudaStreamSynchronize(ctx->down_stream); cudaStreamDestroy(ctx->down_stream); }
@@ -278,6 +282,7 @@ extern "C" int jpegqs_cuda_create(int device, jpegqs_cuda_ctx **out) {
 	ctx->profiling = 0; ctx->ev_used = 0; ctx->tune_sync = 2; ctx->tune_maxn = 4; ctx->tune_wpg = 4; ctx->tune_gs = 1; ctx->tune_uni = 1; ctx->tune_merge = 1; ctx->tune_slabs = 1; ctx->tune_wave = 0;
 	ctx->tune_decode = 512;
 	ctx->kernel_ms[0] = ctx->kernel_ms[1] = 0; ctx->kernel_launches[0] = ctx->kernel_launches[1] = 0;
+	ctx->transcode = NULL;
 	int rc = [&]() -> int {
 		CK(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking));
 		CK(cudaStreamCreateWithFlags(&ctx->up_stream, cudaStreamNonBlocking));
@@ -624,6 +629,9 @@ void qs_ctx_decode_done(jpegqs_cuda_ctx *ctx, int launches, const char *err) {
 	ctx->launches = launches;
 	if (err && err[0]) snprintf(ctx->err, sizeof(ctx->err), "%s", err);
 }
+/* jpegqs_cuda_transcode (qs_transcode.cu): its buffers, and the smoothing time it measured */
+void **qs_ctx_transcode_state(jpegqs_cuda_ctx *ctx) { return &ctx->transcode; }
+void qs_ctx_set_last_ms(jpegqs_cuda_ctx *ctx, float ms) { ctx->last_ms = ms; }
 /* for the host-only entry points (jpeg_io.c, qs_decode.cu): jpegqs_cuda_last_error(NULL) */
 extern "C" void qs_set_host_error(const char *msg) { snprintf(g_err, sizeof(g_err), "%s", msg); }
 extern "C" int jpegqs_cuda_chunk_schedule(const uint16_t *quant, int max_coefs, int uniform, uint8_t *out) {

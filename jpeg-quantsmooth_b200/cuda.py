@@ -72,6 +72,22 @@ class _Head(C.Structure):
                 ("quant_tbl", C.c_int32 * 4)]
 
 
+class _FileInfo(C.Structure):
+    """jpegqs_cuda_file_info: what the jpegqs tool's -v line shows of a file (include/jpegqs_cuda.h)."""
+    _fields_ = [("image_width", C.c_uint32), ("image_height", C.c_uint32), ("ncomp", C.c_int32),
+                ("progressive", C.c_int32), ("restart_interval", C.c_int32)]
+
+
+class _TranscodeResult(C.Structure):
+    """jpegqs_cuda_transcode_result (include/jpegqs_cuda.h)."""
+    _fields_ = [("data", C.c_void_p), ("len", C.c_size_t), ("smoothed", C.c_int32), ("stop", C.c_int32),
+                ("upsampled", C.c_int32), ("reason", C.c_char_p)]
+
+
+ROUTE_HOST, ROUTE_DEVICE = 0, 1
+TRANSCODE_OK, TRANSCODE_FALLBACK = 0, 1
+
+
 class _Job(C.Structure):
     _fields_ = [("coef", C.c_void_p), ("plane", C.c_void_p), ("plane2", C.c_void_p),
                 ("wblk", C.c_uint32), ("hblk", C.c_uint32), ("quant", C.c_uint16 * 64),
@@ -182,6 +198,10 @@ def load():
                                              C.c_void_p, C.c_size_t, C.c_void_p]
     lib.jpegqs_cuda_encode_model.argtypes = [C.POINTER(_Image), C.POINTER(_Head), C.c_int, C.c_void_p, C.c_size_t,
                                              C.POINTER(C.c_uint64), C.POINTER(C.c_int32)]
+    lib.jpegqs_cuda_transcode_route.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(C.c_char_p), C.POINTER(_FileInfo)]
+    lib.jpegqs_cuda_transcode.argtypes = [C.c_void_p, C.c_char_p, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int,
+                                          C.POINTER(_TranscodeResult)]
+    lib.jpegqs_cuda_transcode_free.argtypes = [C.c_void_p]
     lib.jpegqs_cuda_tables.argtypes = [C.c_int, C.c_void_p]
     lib.jpegqs_cuda_orig_coef.argtypes = [C.c_int, C.c_int]
     _lib = lib
@@ -386,6 +406,28 @@ def parse_jpeg_scans(data: bytes):
     return image, (ScanList(recs[:n.value]) if rc == 0 else None)
 
 
+def _file_bytes(data, what: str) -> bytes:
+    if not isinstance(data, (bytes, bytearray, memoryview)):
+        raise TypeError(f"{what}: data must be bytes-like, not {type(data).__name__}")
+    return bytes(data)
+
+
+def transcode_route(data: bytes):
+    """Where the jpegqs tool transcodes this file, host-only: ("device", reason) or ("host", reason).
+    The rule of jpegqs_cuda_transcode_route (include/jpegqs_cuda.h): the device when the whole file
+    walks without a marker-level warning, one of the device decoders takes it, it is not a progressive
+    file with an AC refinement scan without restart markers, and the encoder takes its geometry.
+    Raises TypeError for data that is not bytes-like and QsError for a file the reader rejects."""
+    lib = load()
+    data = _file_bytes(data, "transcode_route")
+    why = C.c_char_p()
+    rc = lib.jpegqs_cuda_transcode_route(data, len(data), C.byref(why), None)
+    reason = (why.value or b"").decode()
+    if rc < 0:
+        raise QsError(f"transcode_route: {reason}")
+    return ("device" if rc == ROUTE_DEVICE else "host"), reason
+
+
 class ScanList(list):
     """The jpegqs_cuda_scan_rec records of one file, in file order (parse_jpeg_scans)."""
 
@@ -588,6 +630,23 @@ class QsContext:
         a, b, c, d = C.c_float(), C.c_int(), C.c_float(), C.c_int()
         self.lib.jpegqs_cuda_kernel_stats(self.h, C.byref(a), C.byref(b), C.byref(c), C.byref(d))
         return a.value, b.value, c.value, d.value
+
+    def transcode(self, data: bytes, flags: int, niter: int, optimize: bool = False, copy: int = 2):
+        """One JPEG file to the file the jpegqs tool writes for it (read, do_quantsmooth(flags, niter),
+        write with -o optimize and -c copy), decoded, smoothed and encoded on this context's device
+        (jpegqs_cuda_transcode).  Returns (bytes, None), or (None, reason) when the file must take the
+        host route: transcode_route says so, the device decoder flagged damaged data or the encoder met
+        a coefficient it cannot code.  Device buffers stay with the context and only grow."""
+        data = _file_bytes(data, "transcode")
+        res = _TranscodeResult()
+        rc = self._check(self.lib.jpegqs_cuda_transcode(self.h, data, len(data), int(flags), int(niter), int(bool(optimize)),
+                                                        int(copy), C.byref(res)))
+        if rc == TRANSCODE_FALLBACK:
+            return None, (res.reason or b"").decode()
+        try:
+            return C.string_at(res.data, res.len), None
+        finally:
+            self.lib.jpegqs_cuda_transcode_free(res.data)
 
     # ---- whole image, host buffers (the call a user of the reference makes) ----
     def do_quantsmooth(self, image: CoefImage, flags: int, niter: int, progprec: int = 0,
@@ -1321,3 +1380,9 @@ def encode_async(images: Sequence[CoefImage], coefs, heads, optimize: bool = Fal
         raise ValueError("encode_async: the coefficient tensors must be CUDA tensors")
     return default_context(first.device.index).encode_async(images, coefs, heads, optimize, status, up, out,
                                                             capacity, stream)
+
+
+def transcode(data: bytes, flags: int, niter: int, optimize: bool = False, copy: int = 2, device: int = -1):
+    """QsContext.transcode on the default context of `device`: (bytes, None), or (None, reason) for a
+    file the host route must take."""
+    return default_context(device).transcode(data, flags, niter, optimize, copy)
