@@ -530,12 +530,39 @@ int jpegqs_cuda_transcode_route(const uint8_t *data, size_t len, const char **re
 typedef struct {
 	uint8_t *data; size_t len;         /* OK: the output file (malloc'd)                              */
 	int32_t smoothed;                  /* 1 = run_async ran (0: do_quantsmooth's early return)        */
-	int32_t stop, upsampled;           /* the run's status when it ran                                */
+	int32_t stop, upsampled;           /* the run's status when it ran (0 when the decoder flagged the
+	                                      data: the run then went over unspecified coefficients)      */
 	const char *reason;                /* FALLBACK: why, a static string; "" otherwise                */
 } jpegqs_cuda_transcode_result;
 int jpegqs_cuda_transcode(jpegqs_cuda_ctx *ctx, const uint8_t *data, size_t len, int flags, int niter,
 		int optimize, int copy, jpegqs_cuda_transcode_result *result);
 void jpegqs_cuda_transcode_free(void *p);
+
+/* The transcode of n files in shared launches (jpegqs_cuda_transcode is the batch of one).
+ *   - Per file.  rc[i] and results[i] are exactly what jpegqs_cuda_transcode returns for file i alone:
+ *     JPEGQS_TRANSCODE_OK, JPEGQS_TRANSCODE_FALLBACK or JPEGQS_ERR_ARG for a file the reader rejects
+ *     (jpegqs_cuda_last_error(ctx) names the last such file), with the same bytes, smoothed, stop,
+ *     upsampled and reason.  A file that falls back or stops never changes another file's result.
+ *   - Return.  0, or a negative error for bad arguments (ctx, data, len, rc or results NULL, a data[i]
+ *     NULL, n < 0, copy outside 0..2: nothing is done) or a CUDA failure.  On a negative return every
+ *     results[i].data is NULL.  n == 0 returns 0 and touches nothing.
+ *   - Sub-batches.  Consecutive device-route files are grouped while the sum of their needs stays
+ *     within max_device_bytes: file + prefix, coefficients (+ up-sampled chroma), the encoder's bound
+ *     for the output, and one workspace shared by the stages - the largest of the decoders', run_async's
+ *     and the encoder's workspace for the group and of the packed output (the bounds again, each
+ *     rounded up to 16 bytes).  A file bigger than the budget runs alone; at most 1024 files go in one
+ *     sub-batch.  max_device_bytes 0: half of the device memory free at call time plus what the
+ *     context's transcode buffers already hold.  The buffers belong to the context and only grow.
+ *   - Per sub-batch, on the context's stream: one upload of all files and prefixes from pinned
+ *     staging; one decode_async over the single-scan files and one decode_scans_async over the others;
+ *     one run_async over the files that smooth (do_quantsmooth's early return is decided per file, and
+ *     the files that return early get run status 0); one encode_async over all; one packing kernel
+ *     that copies the clean files into one buffer; the status records back, a synchronisation, exactly
+ *     the packed bytes back, a synchronisation.
+ *   - jpegqs_cuda_last_device_ms gives the run_async time of the last sub-batch that smoothed. */
+int jpegqs_cuda_transcode_batch(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int optimize, int copy, size_t max_device_bytes, int *rc,
+		jpegqs_cuda_transcode_result *results);
 
 /* ---- one image sharded by MCU rows over several GPUs (SURVEY.md 8e) ----------------------
  * Every rank - a device of this process, or another process on the same box - smooths one slab

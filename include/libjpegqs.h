@@ -94,6 +94,16 @@ JPEGQS_ATTR int jpegqs_warmup(int flags);
  * the device route does not take) or a negative value, reported on stderr as do_quantsmooth does. */
 JPEGQS_ATTR int jpegqs_transcode(const unsigned char *data, size_t len, int copy, int optimize,
 		jpegqs_control_t *opts, unsigned char **out, size_t *outlen, const char **reason);
+/* extension: jpegqs_transcode for n files in shared device launches (jpegqs_cuda_transcode_batch).
+ * rc[i], out[i], outlen[i] and reason[i] are what jpegqs_transcode returns for file i alone.  Each
+ * file's -i lines and error messages are those of jpegqs_transcode; a file's time line shows the wall
+ * time of the whole call.  log NULL: they reach stderr, file by file in their order; otherwise log[i]
+ * receives file i's text (malloc'd, NULL when there is none, always NULL for a file that falls back)
+ * for the caller to print and free - so a caller can print them in order with the host route's
+ * output for the files that fall back.  Returns 0. */
+JPEGQS_ATTR int jpegqs_transcode_batch(int n, const unsigned char *const *data, const size_t *len, int copy,
+		int optimize, jpegqs_control_t *opts, unsigned char **out, size_t *outlen, int *rc, const char **reason,
+		char **log);
 
 #ifndef TRANSCODE_ONLY
 /* decode helpers; replace reference libjpegqs.h:50-55 / quantsmooth.h:2880-2904 */

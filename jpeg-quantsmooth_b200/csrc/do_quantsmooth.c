@@ -189,66 +189,101 @@ static int smooths(j_decompress_ptr srcinfo, int flags, int niter) {
 	return niter > 0 || (flags & JPEGQS_UPSAMPLE_UV && needs_downsample(srcinfo, flags));
 }
 
+/* Extension (include/libjpegqs.h): the jpegqs tool's device route, n files in shared launches
+ * (jpegqs_cuda_transcode_batch).  The same context, lock, device selection and messages as
+ * do_quantsmooth, and for each file the same -i lines in the same order as a call for that file
+ * alone, files in their order.  The time line of a file gives the wall time of the whole call and the
+ * device-kernel line the run_async time of its last sub-batch (jpegqs_cuda_last_device_ms): with the
+ * default device budget one call is one sub-batch unless its files need more than half the device's
+ * free memory.  A file that falls back prints nothing.  The coefficients never leave the device. */
+JPEGQS_ATTR
+int jpegqs_transcode_batch(int n, const unsigned char *const *data, const size_t *len, int copy, int optimize,
+		jpegqs_control_t *opts, unsigned char **out, size_t *outlen, int *rc, const char **reason, char **log) {
+	jq_image im; char err[256]; int flags = opts->flags, i, m = 0, ret = 0; jpegqs_cuda_ctx *ctx;
+	int *smooth, *idx, *brc; FILE **f; char **buf; size_t *blen; const unsigned char **bdata; size_t *blens;
+	jpegqs_cuda_transcode_result *res;
 #ifdef WITH_LOG
-/* the buffered -i lines of a transcode reach stderr unless the file falls back to the host route,
- * which prints them itself */
-static void log_flush(FILE **f, char **buf, size_t *len, int print) {
-	if (!*f) return;
-	fclose(*f); *f = NULL;
-	if (print && *len) fwrite(*buf, 1, *len, stderr);
-	free(*buf); *buf = NULL;
-}
+	int64_t t0 = 0, usec = 0;
 #endif
+	if (n <= 0) return 0;
+	smooth = (int*)calloc((size_t)n, sizeof(int)); idx = (int*)calloc((size_t)n, sizeof(int)); brc = (int*)calloc((size_t)n, sizeof(int));
+	f = (FILE**)calloc((size_t)n, sizeof(FILE*)); buf = (char**)calloc((size_t)n, sizeof(char*)); blen = (size_t*)calloc((size_t)n, sizeof(size_t));
+	bdata = (const unsigned char**)calloc((size_t)n, sizeof(*bdata)); blens = (size_t*)calloc((size_t)n, sizeof(size_t));
+	res = (jpegqs_cuda_transcode_result*)calloc((size_t)n, sizeof(*res));
+	if (!smooth || !idx || !brc || !f || !buf || !blen || !bdata || !blens || !res) {
+		for (i = 0; i < n; i++) { out[i] = NULL; outlen[i] = 0; rc[i] = JPEGQS_TRANSCODE_FALLBACK; reason[i] = "out of memory"; if (log) log[i] = NULL; }
+		ret = JPEGQS_TRANSCODE_FALLBACK; goto done;
+	}
+	for (i = 0; i < n; i++) {
+		out[i] = NULL; outlen[i] = 0; reason[i] = ""; rc[i] = JPEGQS_TRANSCODE_OK; if (log) log[i] = NULL;
+		/* what do_quantsmooth would be handed: the frame, quant tables and colour space of the file */
+		if (jq_read_markers(data[i], len[i], 0, &im, err)) { reason[i] = "the reader rejects the file"; rc[i] = JPEGQS_TRANSCODE_FALLBACK; continue; }
+		smooth[i] = smooths(&im.cinfo, flags, opts->niter);
+		f[i] = open_memstream(&buf[i], &blen[i]);
+		if (!f[i]) { jq_free(&im); reason[i] = "out of memory"; rc[i] = JPEGQS_TRANSCODE_FALLBACK; continue; }
+#ifdef WITH_LOG
+		log_head(f[i], &im.cinfo, flags);
+#endif
+		idx[m] = i; bdata[m] = data[i]; blens[m] = len[i]; m++;
+		jq_free(&im);
+	}
+	pthread_mutex_lock(&g_lock);
+	ctx = get_ctx_quiet((flags >> JPEGQS_CPU_SHIFT) & JPEGQS_CPU_MASK);
+	if (!ctx) {
+		for (i = 0; i < m; i++) {
+			int k = idx[i];
+			/* do_quantsmooth would not reach the device: the host route gives the file without one */
+			if (!smooth[k]) { rc[k] = JPEGQS_TRANSCODE_FALLBACK; reason[k] = "no CUDA device, and nothing to smooth"; continue; }
+			rc[k] = JPEGQS_ERR_CUDA;
+			fprintf(f[k], "jpegqs: CUDA back end unavailable: %s\n", jpegqs_cuda_last_error(NULL));
+		}
+	} else if (m) {
+		int r;
+#ifdef WITH_LOG
+		for (i = 0; i < m; i++) {
+			if (!smooth[idx[i]]) continue;
+			if (jq_read_markers(data[idx[i]], len[idx[i]], 0, &im, err)) continue;
+			log_device(f[idx[i]], &im.cinfo, flags, ctx, NULL);
+			jq_free(&im);
+		}
+		t0 = now_usec();
+#endif
+		r = jpegqs_cuda_transcode_batch(ctx, m, bdata, blens, flags, opts->niter, optimize, copy, 0, brc, res);
+#ifdef WITH_LOG
+		usec = now_usec() - t0;
+#endif
+		for (i = 0; i < m; i++) {
+			int k = idx[i];
+			rc[k] = r < 0 ? r : brc[i];
+			if (rc[k] == JPEGQS_TRANSCODE_FALLBACK) { reason[k] = res[i].reason; continue; }
+			if (rc[k] < 0) { fprintf(f[k], "jpegqs: CUDA back end failed (%d): %s\n", rc[k], jpegqs_cuda_last_error(ctx)); continue; }
+#ifdef WITH_LOG
+			if (smooth[k] && !res[i].stop) log_time(f[k], flags, usec, ctx);
+#endif
+			out[k] = res[i].data; outlen[k] = res[i].len;
+		}
+	}
+	for (i = 0; i < m; i++) {
+		int k = idx[i];
+		fclose(f[k]); f[k] = NULL;
+		if (rc[k] == JPEGQS_TRANSCODE_FALLBACK || !blen[k]) { free(buf[k]); buf[k] = NULL; }
+		if (!log) { if (buf[k]) fwrite(buf[k], 1, blen[k], stderr); free(buf[k]); }
+		else log[k] = buf[k];
+		buf[k] = NULL;
+	}
+	pthread_mutex_unlock(&g_lock);
+done:
+	free(smooth); free(idx); free(brc); free(f); free(buf); free(blen); free(bdata); free(blens); free(res);
+	return ret;
+}
 
-/* Extension (include/libjpegqs.h): the jpegqs tool's device route.  The same context, lock, device
- * selection and messages as do_quantsmooth, the same -i lines in the same order; the coefficients
- * never leave the device (jpegqs_cuda_transcode). */
+/* Extension (include/libjpegqs.h): one file, the batch of one. */
 JPEGQS_ATTR
 int jpegqs_transcode(const unsigned char *data, size_t len, int copy, int optimize, jpegqs_control_t *opts,
 		unsigned char **out, size_t *outlen, const char **reason) {
-	jq_image im; char err[256]; int flags = opts->flags, smooth, ret; jpegqs_cuda_ctx *ctx;
-	jpegqs_cuda_transcode_result res;
-#ifdef WITH_LOG
-	FILE *log; char *logbuf = NULL; size_t loglen = 0; int64_t t0;
-#endif
-	*out = NULL; *outlen = 0; *reason = "";
-	/* what do_quantsmooth would be handed: the frame, quant tables and colour space of the file */
-	if (jq_read_markers(data, len, 0, &im, err)) { *reason = "the reader rejects the file"; return JPEGQS_TRANSCODE_FALLBACK; }
-	smooth = smooths(&im.cinfo, flags, opts->niter);
-#ifdef WITH_LOG
-	log = open_memstream(&logbuf, &loglen);
-	if (!log) { jq_free(&im); *reason = "out of memory"; return JPEGQS_TRANSCODE_FALLBACK; }
-	log_head(log, &im.cinfo, flags);
-#endif
-	pthread_mutex_lock(&g_lock);
-	ctx = get_ctx_quiet((flags >> JPEGQS_CPU_SHIFT) & JPEGQS_CPU_MASK);
-	if (!ctx && !smooth) {
-		/* do_quantsmooth would not reach the device: the host route gives the file without one */
-		pthread_mutex_unlock(&g_lock);
-#ifdef WITH_LOG
-		log_flush(&log, &logbuf, &loglen, 0);
-#endif
-		jq_free(&im);
-		*reason = "no CUDA device, and nothing to smooth";
-		return JPEGQS_TRANSCODE_FALLBACK;
-	}
-#ifdef WITH_LOG
-	if (ctx && smooth) log_device(log, &im.cinfo, flags, ctx, NULL);
-	t0 = now_usec();
-#endif
-	if (!ctx) ret = JPEGQS_ERR_CUDA;
-	else ret = jpegqs_cuda_transcode(ctx, data, len, flags, opts->niter, optimize, copy, &res);
-#ifdef WITH_LOG
-	if (ret == JPEGQS_TRANSCODE_OK && smooth && !res.stop) log_time(log, flags, now_usec() - t0, ctx);
-	log_flush(&log, &logbuf, &loglen, ret != JPEGQS_TRANSCODE_FALLBACK);
-#endif
-	if (!ctx) report_unavailable();
-	else if (ret < 0) fprintf(stderr, "jpegqs: CUDA back end failed (%d): %s\n", ret, jpegqs_cuda_last_error(ctx));
-	pthread_mutex_unlock(&g_lock);
-	jq_free(&im);
-	if (ret == JPEGQS_TRANSCODE_FALLBACK) *reason = res.reason;
-	if (ret == JPEGQS_TRANSCODE_OK) { *out = res.data; *outlen = res.len; }
-	return ret;
+	int rc = 0;
+	jpegqs_transcode_batch(1, &data, &len, copy, optimize, opts, out, outlen, &rc, reason, NULL);
+	return rc;
 }
 
 /* Block-row table of one virtual array: libjpeg keeps a whole-image coefficient array in memory

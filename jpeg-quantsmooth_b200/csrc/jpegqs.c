@@ -89,6 +89,7 @@ typedef struct {
 	jq_image im;
 	unsigned char *data; size_t len;     /* device route: the input file, then (out) the output file */
 	unsigned char *out; size_t outlen;
+	size_t held;                         /* --batch: bytes counted against the readers' look-ahead */
 	double t_read, t_smooth, t_write;    /* stage durations, ms */
 } qs_job;
 
@@ -112,7 +113,8 @@ static void job_decode(const qs_cfg *g, qs_job *j, unsigned char *data, size_t l
 				j->im.restart_interval);
 }
 
-static void job_read(const qs_cfg *g, qs_job *j) {
+/* host_wait (may be NULL): called before a host-route pair is Huffman-decoded (the pipeline's depth) */
+static void job_read(const qs_cfg *g, qs_job *j, void (*host_wait)(void *arg), void *arg) {
 	double t0 = now_ms();
 	FILE *f; unsigned char *data; size_t len = 0;
 	f = strcmp(j->in_name, "-") ? fopen(j->in_name, "rb") : stdin;
@@ -135,34 +137,57 @@ static void job_read(const qs_cfg *g, qs_job *j) {
 		}
 	} else if (g->trace) fprintf(stderr, "jpegqs: %s: host route (%s)\n", j->in_name, g->host_only);
 #endif
+	if (host_wait) host_wait(arg);
 	job_decode(g, j, data, len, 1);
 	j->t_read = now_ms() - t0;
 }
 
-static void job_smooth(const qs_cfg *g, qs_job *j) {
-	double t0 = now_ms();
+/* the host route's middle stage: do_quantsmooth on the coefficients the reader decoded */
+static void job_host_smooth(const qs_cfg *g, qs_job *j, double t0) {
 	jpegqs_control_t opts = g->opts;
+	if (do_quantsmooth(&j->im.cinfo, j->im.coef_arrays, &opts) < 0) j->rc = 2;
+	j->t_smooth = now_ms() - t0;
+}
+
 #ifndef JPEGQS_NO_CUDA_RENDER
-	if (j->data) {                                      /* the device route */
-		const char *why = ""; unsigned char *data = j->data;
-		int rc = jpegqs_transcode(data, j->len, g->copy, g->optimize, &opts, &j->out, &j->outlen, &why);
-		if (rc != JPEGQS_TRANSCODE_FALLBACK) {
-			free(data); j->data = NULL;
-			if (rc < 0) j->rc = 2;
-			j->t_smooth = now_ms() - t0;
-			return;
+#define QS_BATCH_MAX 256                 /* device pairs per jpegqs_transcode_batch call */
+/* the device route of m consecutive pairs in one call (jpegqs_transcode_batch); their -i lines are
+ * printed pair by pair, and a pair that falls back takes the host route in its place, so stderr is
+ * that of the pairs one after another */
+static void job_smooth_device(const qs_cfg *g, qs_job *jobs, int m) {
+	double t0 = now_ms(), t;
+	const unsigned char *data[QS_BATCH_MAX]; size_t len[QS_BATCH_MAX]; unsigned char *out[QS_BATCH_MAX];
+	size_t outlen[QS_BATCH_MAX]; int rc[QS_BATCH_MAX], k; const char *why[QS_BATCH_MAX]; char *log[QS_BATCH_MAX];
+	jpegqs_control_t opts = g->opts;
+	for (k = 0; k < m; k++) { data[k] = jobs[k].data; len[k] = jobs[k].len; }
+	jpegqs_transcode_batch(m, data, len, g->copy, g->optimize, &opts, out, outlen, rc, why, log);
+	t = now_ms() - t0;
+	for (k = 0; k < m; k++) {
+		qs_job *j = &jobs[k]; unsigned char *d = j->data;
+		j->data = NULL;
+		if (rc[k] != JPEGQS_TRANSCODE_FALLBACK) {
+			if (log[k]) { fputs(log[k], stderr); free(log[k]); }
+			free(d);
+			j->out = out[k]; j->outlen = outlen[k];
+			if (rc[k] < 0) j->rc = 2;
+			j->t_smooth = t;
+			continue;
 		}
 		/* damaged data (or a file the device route does not take after all): the host route gives
 		 * the reader's recovery, warning count and messages */
-		if (g->trace) fprintf(stderr, "jpegqs: %s: host route after all (%s)\n", j->in_name, why);
-		j->data = NULL;
-		job_decode(g, j, data, j->len, 0);
-		if (j->rc) return;
-		opts = g->opts;
+		if (g->trace) fprintf(stderr, "jpegqs: %s: host route after all (%s)\n", j->in_name, why[k]);
+		t0 = now_ms();
+		job_decode(g, j, d, j->len, 0);
+		if (!j->rc) job_host_smooth(g, j, t0);
 	}
+}
 #endif
-	if (do_quantsmooth(&j->im.cinfo, j->im.coef_arrays, &opts) < 0) j->rc = 2;
-	j->t_smooth = now_ms() - t0;
+
+static void job_smooth(const qs_cfg *g, qs_job *j) {
+#ifndef JPEGQS_NO_CUDA_RENDER
+	if (j->data) { job_smooth_device(g, j, 1); return; }
+#endif
+	job_host_smooth(g, j, now_ms());
 }
 
 static void job_write(const qs_cfg *g, qs_job *j) {
@@ -256,7 +281,7 @@ static int run_one(const qs_cfg *g, qs_job *j, int warm_ok) {
 		warm = !pthread_create(&warm_th, NULL, warmup_thread, &wflags);
 #endif
 	(void)warm_ok;
-	job_read(g, j);
+	job_read(g, j, NULL, NULL);
 	if (!j->rc) job_smooth(g, j);
 #ifndef JPEGQS_NO_CUDA_RENDER
 	if (warm) pthread_join(warm_th, NULL);
@@ -270,32 +295,56 @@ static int run_one(const qs_cfg *g, qs_job *j, int warm_ok) {
 #ifndef JPEGQS_NO_CUDA_RENDER
 /* --batch pipeline.  Reading and writing a file take longer than smoothing it, so several reader
  * threads (JPEGQS_BATCH_READERS, default 3) and writer threads (JPEGQS_BATCH_WRITERS, default 2)
- * work on different files at once while the calling thread keeps the device busy.  Readers stay
- * at most `depth` pairs ahead of the last written one (an 8K image is 100 MB of coefficients) and
- * do not open an input that an earlier, unfinished pair is going to write. */
+ * work on different files at once while the calling thread keeps the device busy.  A reader does not
+ * open an input that an earlier, unfinished pair is going to write.  How far readers run ahead:
+ *   - a host-route pair is Huffman-decoded only once the pair `depth` places before it is written
+ *     (an 8K image is 100 MB of coefficients);
+ *   - a file is loaded once that pair is written, or while fewer than QS_AHEAD_PAIRS pairs before it
+ *     are unwritten and the device-route pairs among them hold less than QS_AHEAD_BYTES of file
+ *     bytes.  Device-route pairs hold only their bytes, so many of them can be read ahead, and the
+ *     calling thread transcodes every read device-route pair that follows the next one in one call. */
 #define QS_MAX_READERS 16
+#define QS_AHEAD_PAIRS 128
+#define QS_AHEAD_BYTES ((size_t)256 << 20)
 typedef struct {
-	const qs_cfg *g; qs_job *jobs; int n, next, wnext, depth;
+	const qs_cfg *g; qs_job *jobs; int n, next, wnext, depth, written;
+	size_t held;                         /* file bytes of device-route pairs read and not yet written */
 	pthread_mutex_t mu; pthread_cond_t cv;
 } qs_pipe;
 
 static void pipe_advance(qs_pipe *p, qs_job *j, int state) {
-	pthread_mutex_lock(&p->mu); j->state = state; pthread_cond_broadcast(&p->cv); pthread_mutex_unlock(&p->mu);
+	pthread_mutex_lock(&p->mu);
+	j->state = state;
+	if (state == 3) { p->written++; p->held -= j->held; j->held = 0; }
+	pthread_cond_broadcast(&p->cv); pthread_mutex_unlock(&p->mu);
 }
 static void pipe_wait(qs_pipe *p, qs_job *j, int state) {
 	pthread_mutex_lock(&p->mu);
 	while (j->state < state) pthread_cond_wait(&p->cv, &p->mu);
 	pthread_mutex_unlock(&p->mu);
 }
+typedef struct { qs_pipe *p; qs_job *j; } qs_back;
+static void wait_back(void *arg) { qs_back *b = (qs_back*)arg; pipe_wait(b->p, b->j, 3); }
 static void *pipe_reader(void *arg) {
 	qs_pipe *p = (qs_pipe*)arg; int i, k;
 	for (;;) {
 		pthread_mutex_lock(&p->mu); i = p->next++; pthread_mutex_unlock(&p->mu);
 		if (i >= p->n) break;
-		if (i >= p->depth) pipe_wait(p, &p->jobs[i - p->depth], 3);
+		if (i >= p->depth) {
+			qs_job *back = &p->jobs[i - p->depth];
+			pthread_mutex_lock(&p->mu);
+			while (back->state < 3 && (i - p->written >= QS_AHEAD_PAIRS || p->held >= QS_AHEAD_BYTES)) pthread_cond_wait(&p->cv, &p->mu);
+			pthread_mutex_unlock(&p->mu);
+		}
 		for (k = 0; k < i; k++)
 			if (strcmp(p->jobs[k].out_name, "-") && !strcmp(p->jobs[k].out_name, p->jobs[i].in_name)) pipe_wait(p, &p->jobs[k], 3);
-		job_read(p->g, &p->jobs[i]);
+		{
+			qs_back back = { p, i >= p->depth ? &p->jobs[i - p->depth] : NULL };
+			job_read(p->g, &p->jobs[i], back.j ? wait_back : NULL, &back);
+		}
+		pthread_mutex_lock(&p->mu);
+		if (p->jobs[i].data) { p->jobs[i].held = p->jobs[i].len; p->held += p->jobs[i].len; }
+		pthread_mutex_unlock(&p->mu);
 		pipe_advance(p, &p->jobs[i], 1);
 	}
 	return NULL;
@@ -316,7 +365,7 @@ static void *pipe_writer(void *arg) {
 }
 /* returns the worst exit status of the pairs, -1 if no thread could be started (nothing done) */
 static int run_pipeline(const qs_cfg *g, qs_job *jobs, int n) {
-	qs_pipe p; pthread_t rd[QS_MAX_READERS], wr[QS_MAX_READERS]; int i, worst = 0, nrd = 3, nwr = 2, started = 0, writers = 0;
+	qs_pipe p; pthread_t rd[QS_MAX_READERS], wr[QS_MAX_READERS]; int i, k, m, worst = 0, nrd = 3, nwr = 2, started = 0, writers = 0;
 	const char *env = getenv("JPEGQS_BATCH_READERS");
 	if (env && atoi(env) > 0) nrd = atoi(env);
 	env = getenv("JPEGQS_BATCH_WRITERS");
@@ -327,19 +376,28 @@ static int run_pipeline(const qs_cfg *g, qs_job *jobs, int n) {
 	if (nwr > n) nwr = n;
 	/* stdin is read and stdout written in the order of the pairs: one thread on that side then */
 	for (i = 0; i < n; i++) { if (!strcmp(jobs[i].in_name, "-")) nrd = 1; if (!strcmp(jobs[i].out_name, "-")) nwr = 1; }
-	p.g = g; p.jobs = jobs; p.n = n; p.next = 0; p.wnext = 0; p.depth = nrd + nwr + 1;
+	p.g = g; p.jobs = jobs; p.n = n; p.next = 0; p.wnext = 0; p.depth = nrd + nwr + 1; p.written = 0; p.held = 0;
 	pthread_mutex_init(&p.mu, NULL); pthread_cond_init(&p.cv, NULL);
 	for (i = 0; i < nrd; i++) { if (pthread_create(&rd[started], NULL, pipe_reader, &p)) break; started++; }
 	if (!started) { pthread_cond_destroy(&p.cv); pthread_mutex_destroy(&p.mu); return -1; }
 	for (i = 0; i < nwr; i++) { if (pthread_create(&wr[writers], NULL, pipe_writer, &p)) break; writers++; }
-	for (i = 0; i < n; i++) {
+	for (i = 0; i < n; i += m) {
 		pipe_wait(&p, &jobs[i], 1);
-		if (!jobs[i].rc) job_smooth(g, &jobs[i]);
-		if (writers) pipe_advance(&p, &jobs[i], 2);
-		else {                                          /* no writer thread: write from here */
-			if (!jobs[i].rc) job_write(g, &jobs[i]);
-			job_release(&jobs[i]);
-			pipe_advance(&p, &jobs[i], 3);
+		m = 1;
+		if (!jobs[i].rc && jobs[i].data) {
+			/* the device-route pairs right after this one that are already read go in the same call */
+			pthread_mutex_lock(&p.mu);
+			while (i + m < n && m < QS_BATCH_MAX && jobs[i + m].state >= 1 && !jobs[i + m].rc && jobs[i + m].data) m++;
+			pthread_mutex_unlock(&p.mu);
+			job_smooth_device(g, &jobs[i], m);
+		} else if (!jobs[i].rc) job_smooth(g, &jobs[i]);
+		for (k = i; k < i + m; k++) {
+			if (writers) pipe_advance(&p, &jobs[k], 2);
+			else {                                      /* no writer thread: write from here */
+				if (!jobs[k].rc) job_write(g, &jobs[k]);
+				job_release(&jobs[k]);
+				pipe_advance(&p, &jobs[k], 3);
+			}
 		}
 	}
 	for (i = 0; i < started; i++) pthread_join(rd[i], NULL);

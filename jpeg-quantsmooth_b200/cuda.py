@@ -202,6 +202,9 @@ def load():
     lib.jpegqs_cuda_transcode.argtypes = [C.c_void_p, C.c_char_p, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int,
                                           C.POINTER(_TranscodeResult)]
     lib.jpegqs_cuda_transcode_free.argtypes = [C.c_void_p]
+    lib.jpegqs_cuda_transcode_batch.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_size_t), C.c_int,
+                                                C.c_int, C.c_int, C.c_int, C.c_size_t, C.POINTER(C.c_int),
+                                                C.POINTER(_TranscodeResult)]
     lib.jpegqs_cuda_tables.argtypes = [C.c_int, C.c_void_p]
     lib.jpegqs_cuda_orig_coef.argtypes = [C.c_int, C.c_int]
     _lib = lib
@@ -647,6 +650,42 @@ class QsContext:
             return C.string_at(res.data, res.len), None
         finally:
             self.lib.jpegqs_cuda_transcode_free(res.data)
+
+    def transcode_batch(self, datas, flags: int, niter: int, optimize: bool = False, copy: int = 2,
+                        max_device_bytes: int = 0):
+        """Many JPEG files, each to what transcode gives for it alone, in shared launches
+        (jpegqs_cuda_transcode_batch): a list of (bytes, None) or (None, reason), in the order of datas.
+        max_device_bytes bounds the device memory of one sub-batch (0: half of what is free plus what
+        the context already holds).  Raises QsError naming the index of a file the reader rejects,
+        ValueError for copy outside 0..2 or a negative max_device_bytes, TypeError for a non-bytes entry."""
+        if isinstance(datas, (bytes, bytearray, memoryview, str)) or not hasattr(datas, "__len__"):
+            raise TypeError("transcode_batch: datas must be a sequence of bytes-like files")
+        files = [_file_bytes(d, f"transcode_batch: file {i}") for i, d in enumerate(datas)]
+        if int(copy) not in (0, 1, 2):
+            raise ValueError(f"transcode_batch: copy must be 0, 1 or 2, not {copy}")
+        if int(max_device_bytes) < 0:
+            raise ValueError("transcode_batch: max_device_bytes must be >= 0")
+        n = len(files)
+        if not n:
+            return []
+        ptrs = (C.c_char_p * n)(*files)
+        lens = (C.c_size_t * n)(*[len(d) for d in files])
+        rc = (C.c_int * n)()
+        res = (_TranscodeResult * n)()
+        self._check(self.lib.jpegqs_cuda_transcode_batch(self.h, n, ptrs, lens, int(flags), int(niter), int(bool(optimize)),
+                                                         int(copy), int(max_device_bytes), rc, res))
+        out, bad = [], None
+        for i in range(n):
+            if rc[i] == TRANSCODE_OK:
+                out.append((C.string_at(res[i].data, res[i].len), None))
+                self.lib.jpegqs_cuda_transcode_free(res[i].data)
+            elif rc[i] == TRANSCODE_FALLBACK:
+                out.append((None, (res[i].reason or b"").decode()))
+            elif bad is None:
+                bad = i
+        if bad is not None:
+            raise QsError(f"transcode_batch: file {bad}: {self.lib.jpegqs_cuda_last_error(self.h).decode()}")
+        return out
 
     # ---- whole image, host buffers (the call a user of the reference makes) ----
     def do_quantsmooth(self, image: CoefImage, flags: int, niter: int, progprec: int = 0,
@@ -1386,3 +1425,10 @@ def transcode(data: bytes, flags: int, niter: int, optimize: bool = False, copy:
     """QsContext.transcode on the default context of `device`: (bytes, None), or (None, reason) for a
     file the host route must take."""
     return default_context(device).transcode(data, flags, niter, optimize, copy)
+
+
+def transcode_batch(datas, flags: int, niter: int, optimize: bool = False, copy: int = 2, max_device_bytes: int = 0,
+                    device: int = -1):
+    """QsContext.transcode_batch on the default context of `device`: a list of (bytes, None) or
+    (None, reason), one per file."""
+    return default_context(device).transcode_batch(datas, flags, niter, optimize, copy, max_device_bytes)
