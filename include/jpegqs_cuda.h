@@ -564,6 +564,52 @@ int jpegqs_cuda_transcode_batch(jpegqs_cuda_ctx *ctx, int n, const uint8_t *cons
 		int flags, int niter, int optimize, int copy, size_t max_device_bytes, int *rc,
 		jpegqs_cuda_transcode_result *results);
 
+/* ---- JPEG files -> smoothed pixels, blocking, many files per launch -----------------------------
+ * What the jpegqs tool's --ppm writes after its P5 / P6 header, for n files in host memory: libjpeg's
+ * islow, fancy-up-sampled pixels of the coefficients do_quantsmooth(flags, niter) leaves, so
+ * up-sampled and stopped images come out as the tool renders them.
+ *   - Output size.  out[i] holds exactly image_width * image_height * channels bytes, where width,
+ *     height and ncomp are what jpegqs_cuda_transcode_route puts in its info for file i and channels
+ *     is 1 for ncomp 1 (grey) and 3 for ncomp 3 (RGB).  layout JPEGQS_RENDER_HWC or _CHW (the same
+ *     bytes for a grey file).  out_on_device 1: out[i] is device memory on the context's device, at
+ *     any byte alignment; 0: host memory, filled from one download per sub-batch.  Either way the
+ *     call blocks and the outputs are complete when it returns.
+ *   - Per file, rc[i]: 0; JPEGQS_ERR_ARG for a file the reader rejects (jpegqs_cuda_last_error(ctx)
+ *     names the last such file); JPEGQS_ERR_UNSUPPORTED for a component count other than 1 or 3 or a
+ *     sampling render_async does not render (--ppm fails on these with "render failed (-3)").  out[i]
+ *     is then untouched.  A file that fails never changes another file's result.
+ *   - Route.  jpegqs_cuda_transcode_route's, unchanged.  DEVICE files are uploaded and decoded by
+ *     decode_async / decode_scans_async in shared launches; HOST files are read by
+ *     jpegqs_cuda_jpeg_read into pinned staging, on the calling thread while the device decodes; a
+ *     DEVICE file the device decoder flags is read again by jpegqs_cuda_jpeg_read, as the tool does
+ *     when a transcode falls back, so its warnings and recovery are the reader's.
+ *   - Per sub-batch, on the context's stream: one upload of the DEVICE files; the decoder launches;
+ *     the host reads; the decoder statuses back and a synchronisation; the re-reads; one upload of
+ *     the host-decoded coefficients; one run_async over the files that smooth (do_quantsmooth's early
+ *     return decided per file, as in transcode_batch); one render of every file, reading the run
+ *     status and the up-sampled chroma; the run statuses back (with the pixels when out_on_device is
+ *     0) and a synchronisation.
+ *   - Sub-batches, as transcode_batch's: consecutive files while the sum of their needs stays within
+ *     max_device_bytes (0: half of the free device memory plus what the context's buffers hold), at
+ *     most 1024 files, a bigger file alone.  The needs: the file, the coefficients and up-sampled
+ *     chroma, the shared workspace (the decoders' and run_async's) and, with host outputs, the
+ *     pixels.  A re-read file takes its coefficient bytes once more.  The buffers belong to the
+ *     context and only grow.  jpegqs_cuda_last_device_ms gives the run_async time of the last
+ *     sub-batch that smoothed.
+ *   - Return.  0, or a negative error for bad arguments (ctx, data, len, out, rc or results NULL, an
+ *     entry of data or out NULL, n < 0, a layout other than HWC / CHW, out_on_device other than 0 / 1:
+ *     nothing is done and rc / results are untouched) or a CUDA failure.  n == 0 returns 0. */
+typedef struct {
+	int32_t channels;        /* 1 (grey) or 3 (RGB)                                               */
+	int32_t host_decoded;    /* 1: the host reader decoded the entropy-coded data                  */
+	int32_t warnings;        /* the host reader's warning count (the tool would exit 2 if > 0)     */
+	int32_t smoothed, stop, upsampled;   /* as jpegqs_cuda_transcode_result                       */
+	const char *reason;      /* host_decoded: why (a static string), "" otherwise                  */
+} jpegqs_cuda_pixels_result;
+int jpegqs_cuda_pixels_batch(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int layout, int out_on_device, uint8_t *const *out, size_t max_device_bytes,
+		int *rc, jpegqs_cuda_pixels_result *results);
+
 /* ---- one image sharded by MCU rows over several GPUs (SURVEY.md 8e) ----------------------
  * Every rank - a device of this process, or another process on the same box - smooths one slab
  * of contiguous MCU rows and exchanges ONE pixel row per plane with each neighbour after every

@@ -151,7 +151,7 @@ int jpegqs_cuda_jpeg_parse_scans(const uint8_t *data, size_t len, jpegqs_cuda_im
 
 /* The route of a file through a transcode: jpegqs_cuda_transcode_route's rule, and what
  * jpegqs_cuda_transcode needs of a DEVICE file, from one markers-only walk.  Every output but reason
- * may be NULL.  On DEVICE: img filled (coef pointers NULL); *nscans = 0 and *scan filled when
+ * may be NULL.  On DEVICE and HOST: img filled (coef pointers NULL).  On DEVICE: *nscans = 0 and *scan filled when
  * decode_async takes the file, else recs[0 .. *nscans) for decode_scans_async; head->comp_id /
  * quant_tbl filled and *prefix (malloc'd, copy level `copy`) / *prefix_len set.  Writes no error
  * state, so any thread may call it. */
@@ -184,8 +184,8 @@ int qs_route_plan(const uint8_t *data, size_t len, int copy, jpegqs_cuda_file_in
 				why = "progressive AC refinement scan without restart markers";
 		if (!why[0]) { route = JPEGQS_ROUTE_DEVICE; why = seq ? "sequential, one scan" : im.progressive ? "progressive" : "several scans"; }
 	}
+	if (img) fill_image(&im, img);
 	if (route == JPEGQS_ROUTE_DEVICE) {
-		if (img) fill_image(&im, img);
 		if (nscans) *nscans = seq ? 0 : n;
 		if (scan && seq) {
 			const jq_scanrec *r = &rec[0];

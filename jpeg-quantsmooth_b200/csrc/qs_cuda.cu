@@ -2096,12 +2096,29 @@ extern "C" int jpegqs_cuda_render_rgb(jpegqs_cuda_ctx *ctx, const jpegqs_cuda_im
 }
 
 /* ---- stream-ordered render of device-resident images (see the header) ----------------------- */
-extern "C" int jpegqs_cuda_render_async(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image *imgs,
-		const jpegqs_cuda_status *status_dev, int layout, uint8_t *const *out_dev, void *stream) {
-	if (!ctx) return JPEGQS_ERR_ARG;
-	const char *bad = nimages < 0 || (nimages && (!imgs || !out_dev)) ? "images or outputs missing"
-			: layout != JPEGQS_RENDER_HWC && layout != JPEGQS_RENDER_CHW ? "unknown layout" : NULL;
+/* what the render kernel takes: 1 or 3 components whose sampling ratios are integral (libjpeg cannot
+ * decode others either); sampling factors outside 1..4 are not rendered */
+int qs_render_takes(const jpegqs_cuda_image *im) {
+	if (im->ncomp != 1 && im->ncomp != 3) return 0;
+	int maxh = 1, maxv = 1;
+	for (int c = 0; c < im->ncomp; c++) {
+		const jpegqs_cuda_comp *cc = &im->comp[c];
+		if (cc->h_samp < 1 || cc->h_samp > 4 || cc->v_samp < 1 || cc->v_samp > 4) return 0;
+		maxh = std::max(maxh, cc->h_samp); maxv = std::max(maxv, cc->v_samp);
+	}
+	for (int c = 0; c < im->ncomp; c++)
+		if (maxh % im->comp[c].h_samp || maxv % im->comp[c].v_samp) return 0;
+	return 1;
+}
+
+/* jpegqs_cuda_render_async with the layout checked by the caller; grey_store != 0 writes 1-component
+ * images with one byte per pixel (either layout: the single plane).  Consecutive images of one store
+ * mode share a launch. */
+int qs_render_images(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image *imgs,
+		const jpegqs_cuda_status *status_dev, int layout, int grey_store, uint8_t *const *out_dev, void *stream) {
+	const char *bad = nimages < 0 || (nimages && (!imgs || !out_dev)) ? "images or outputs missing" : NULL;
 	std::vector<QsRenderImg> d(bad ? 0 : nimages);
+	std::vector<int> store(d.size());
 	int unsupported = 0;
 	for (int i = 0; i < nimages && !bad && !unsupported; i++) {
 		const jpegqs_cuda_image *im = &imgs[i];
@@ -2117,9 +2134,10 @@ extern "C" int jpegqs_cuda_render_async(jpegqs_cuda_ctx *ctx, int nimages, const
 			else { maxh = std::max(maxh, cc->h_samp); maxv = std::max(maxv, cc->v_samp); }
 		}
 		if (!out_dev[i]) bad = "output NULL";
-		for (int c = 0; c < im->ncomp && !bad && !unsupported; c++) {
+		if (!bad && !qs_render_takes(im)) { unsupported = 1; break; }
+		store[i] = grey_store && im->ncomp == 1 ? QS_RENDER_GREY : layout;
+		for (int c = 0; c < im->ncomp && !bad; c++) {
 			const jpegqs_cuda_comp *cc = &im->comp[c];
-			if (maxh % cc->h_samp || maxv % cc->v_samp) { unsupported = 1; break; }   /* libjpeg cannot either */
 			r.cw[c] = (int)(((uint64_t)im->image_width * cc->h_samp + maxh - 1) / maxh);
 			r.ch[c] = (int)(((uint64_t)im->image_height * cc->v_samp + maxv - 1) / maxv);
 			/* the blocks must hold every real sample: the kernel reads up to column cw - 1, row ch - 1 */
@@ -2154,16 +2172,27 @@ extern "C" int jpegqs_cuda_render_async(jpegqs_cuda_ctx *ctx, int nimages, const
 	CK(cudaSetDevice(ctx->device));
 	cudaStream_t st = stream ? (cudaStream_t)stream : ctx->stream;
 	ctx->launches = 0;
-	/* the descriptors travel as kernel parameters: QS_RENDER_PACK images per launch */
-	for (int i0 = 0; i0 < nimages; i0 += QS_RENDER_PACK) {
-		int n = std::min(QS_RENDER_PACK, nimages - i0), tiles = 0;
-		for (int i = 0; i < n; i++) {
-			QsRenderImg &r = d[i0 + i];
+	/* the descriptors travel as kernel parameters: QS_RENDER_PACK images of one store mode per launch */
+	for (int i0 = 0; i0 < nimages;) {
+		int n = 0, tiles = 0;
+		for (; n < QS_RENDER_PACK && i0 + n < nimages && store[i0 + n] == store[i0]; n++) {
+			QsRenderImg &r = d[i0 + n];
 			r.tile_begin = tiles;
 			tiles += ((r.width + QS_RENDER_TW - 1) / QS_RENDER_TW) * ((r.height + QS_RENDER_TH - 1) / QS_RENDER_TH);
 		}
-		CK(qs_launch_render_async(d.data() + i0, n, tiles, status_dev ? (const int2 *)(status_dev + i0) : NULL, layout, st));
+		CK(qs_launch_render_async(d.data() + i0, n, tiles, status_dev ? (const int2 *)(status_dev + i0) : NULL, store[i0], st));
 		if (tiles) ctx->launches++;
+		i0 += n;
 	}
 	return 0;
+}
+
+extern "C" int jpegqs_cuda_render_async(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image *imgs,
+		const jpegqs_cuda_status *status_dev, int layout, uint8_t *const *out_dev, void *stream) {
+	if (!ctx) return JPEGQS_ERR_ARG;
+	if (!(nimages < 0 || (nimages && (!imgs || !out_dev))) && layout != JPEGQS_RENDER_HWC && layout != JPEGQS_RENDER_CHW) {
+		snprintf(ctx->err, sizeof(ctx->err), "render_async: unknown layout");
+		return JPEGQS_ERR_ARG;
+	}
+	return qs_render_images(ctx, nimages, imgs, status_dev, layout, 0, out_dev, stream);
 }

@@ -1832,8 +1832,11 @@ struct QsSmemPx {
 
 struct QsRenderComp { const int16_t *coef; int wblk, bx0, by0, nbx, nby, cw, ch, hs, vs; };
 
+/* STORE: QS_RENDER_HWC / QS_RENDER_CHW (three bytes per pixel), or QS_RENDER_GREY (one byte per pixel,
+ * the CHW store of plane 0 only; for 1-component images) */
+template <int STORE>
 __global__ void __launch_bounds__(QS_RT_THREADS, 2) qs_render_async_kernel(const __grid_constant__ QsRenderPack p,
-		int n, const int2 *__restrict__ status, int layout) {
+		int n, const int2 *__restrict__ status) {
 	__shared__ __align__(16) uint8_t pix[3][QS_RS_H * QS_RS_W];
 	__shared__ int qmul[3][64];
 	__shared__ QsRenderComp g[3];
@@ -1920,7 +1923,7 @@ __global__ void __launch_bounds__(QS_RT_THREADS, 2) qs_render_async_kernel(const
 			px[i] = qs_rgb_pixel(y, c1, c2, ycc);
 		}
 		const bool full = ox + 3 <= x1;
-		if (layout == QS_RENDER_HWC) {
+		if (STORE == QS_RENDER_HWC) {
 			uint8_t *o = im.out + ((size_t)oy * W + ox) * 3;
 			if (full && !((uintptr_t)o & 3)) {
 				uint32_t *o4 = (uint32_t *)o;
@@ -1934,7 +1937,7 @@ __global__ void __launch_bounds__(QS_RT_THREADS, 2) qs_render_async_kernel(const
 			}
 		} else {
 #pragma unroll
-			for (int k = 0; k < 3; k++) {
+			for (int k = 0; k < (STORE == QS_RENDER_GREY ? 1 : 3); k++) {
 				uint8_t *o = im.out + (size_t)k * W * H + (size_t)oy * W + ox;
 				if (full && !((uintptr_t)o & 3)) {
 					*(uint32_t *)o = __byte_perm(__byte_perm(px[0], px[1], 0x0040 + 0x0011 * k),
@@ -1947,13 +1950,16 @@ __global__ void __launch_bounds__(QS_RT_THREADS, 2) qs_render_async_kernel(const
 	}
 }
 
-cudaError_t qs_launch_render_async(const QsRenderImg *imgs, int n, int tiles, const int2 *status, int layout,
+cudaError_t qs_launch_render_async(const QsRenderImg *imgs, int n, int tiles, const int2 *status, int store,
 		cudaStream_t st) {
 	if (tiles <= 0) return cudaSuccess;
 	QsRenderPack pack;
 	memcpy(pack.img, imgs, (size_t)n * sizeof(QsRenderImg));
 	if (n < QS_RENDER_PACK) memset(pack.img + n, 0, (size_t)(QS_RENDER_PACK - n) * sizeof(QsRenderImg));
-	qs_render_async_kernel<<<tiles, QS_RT_THREADS, 0, st>>>(pack, n, status, layout);
+	if (store == QS_RENDER_HWC) qs_render_async_kernel<QS_RENDER_HWC><<<tiles, QS_RT_THREADS, 0, st>>>(pack, n, status);
+	else if (store == QS_RENDER_CHW) qs_render_async_kernel<QS_RENDER_CHW><<<tiles, QS_RT_THREADS, 0, st>>>(pack, n, status);
+	else if (store == QS_RENDER_GREY) qs_render_async_kernel<QS_RENDER_GREY><<<tiles, QS_RT_THREADS, 0, st>>>(pack, n, status);
+	else return cudaErrorInvalidValue;
 	return cudaGetLastError();
 }
 

@@ -59,10 +59,13 @@ typedef struct {
 	uint16_t q[3][64];           /* multipliers: the raw quant table where it de-quantizes, else ones */
 } QsRenderImg;
 #define QS_RENDER_PACK 60
+/* store modes of the render kernel: the two public layouts, and one byte per pixel for 1-component
+ * images (qs_render_images' grey store) */
 #define QS_RENDER_HWC 0
 #define QS_RENDER_CHW 1
+#define QS_RENDER_GREY 2
 /* status: the launch's first image's {stop, upsampled}, or NULL when no image has up_mode 2 */
-cudaError_t qs_launch_render_async(const QsRenderImg *imgs, int n, int tiles, const int2 *status, int layout,
+cudaError_t qs_launch_render_async(const QsRenderImg *imgs, int n, int tiles, const int2 *status, int store,
 		cudaStream_t st);
 
 #endif

@@ -5,6 +5,8 @@
  * decode, smoothing and encode kernels are those of qs_decode.cu, qs_scans.cu, qs_kernels.cu and
  * qs_encode.cu, reached through their public entry points; the one kernel here packs the encoded
  * files into one buffer so that a sub-batch comes back in one copy.
+ * jpegqs_cuda_pixels_batch: the same files to the smoothed pixels the tool's --ppm writes, through
+ * the same plans, sub-batches and decoder launches, the host reader, run_async and the fused render.
  */
 #include <cuda_runtime.h>
 #include <stdio.h>
@@ -26,6 +28,9 @@ void qs_ctx_set_last_ms(jpegqs_cuda_ctx *ctx, float ms);
 extern "C" int qs_route_plan(const uint8_t *data, size_t len, int copy, jpegqs_cuda_file_info *info, jpegqs_cuda_image *img,
 		jpegqs_cuda_scan *scan, jpegqs_cuda_scan_rec *recs, int *nscans, jpegqs_cuda_jpeg_head *head,
 		uint8_t **prefix, size_t *prefix_len, const char **reason);
+int qs_render_takes(const jpegqs_cuda_image *im);                     /* qs_cuda.cu */
+int qs_render_images(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image *imgs,
+		const jpegqs_cuda_status *status_dev, int layout, int grey_store, uint8_t *const *out_dev, void *stream);
 
 /* ---- the packing kernel -------------------------------------------------------------------------
  * After encode_async, file k of a sub-batch sits at the start of its bound-sized slot.  One launch
@@ -111,9 +116,11 @@ struct QsBuf { void *p; size_t cap; };
 struct QsTranscode {
 	QsBuf in_dev, coef_dev, ws_dev, out_dev;   /* descriptors + files + prefixes; coefficients + up-sampled
 	                                              chroma; the workspace the three stages share, then the
-	                                              packed files; the output slots */
+	                                              packed files; the output slots (pixels: run statuses +
+	                                              rendered pixels) */
 	QsBuf stat_dev;                            /* per-file status words and the records of the packing kernel */
 	QsBuf in_host, out_host, stat_host;        /* pinned staging of the upload and the two downloads */
+	QsBuf hcoef_dev, hcoef_host;               /* pixels: the host-decoded files' coefficients and their staging */
 	cudaEvent_t ev0, ev1;                      /* around run_async: jpegqs_cuda_last_device_ms */
 	int sms;
 	jpegqs_cuda_scan_rec recs[JPEGQS_MAX_SCANS];
@@ -126,9 +133,11 @@ void qs_transcode_release(void *state) {
 	QsTranscode *t = (QsTranscode*)state;
 	if (!t) return;
 	cudaFree(t->in_dev.p); cudaFree(t->coef_dev.p); cudaFree(t->ws_dev.p); cudaFree(t->out_dev.p); cudaFree(t->stat_dev.p);
+	cudaFree(t->hcoef_dev.p);
 	if (t->in_host.p) cudaFreeHost(t->in_host.p);
 	if (t->out_host.p) cudaFreeHost(t->out_host.p);
 	if (t->stat_host.p) cudaFreeHost(t->stat_host.p);
+	if (t->hcoef_host.p) cudaFreeHost(t->hcoef_host.p);
 	if (t->ev0) cudaEventDestroy(t->ev0);
 	if (t->ev1) cudaEventDestroy(t->ev1);
 	delete t;
@@ -144,14 +153,17 @@ static cudaError_t grow_dev(QsBuf *b, size_t need) {
 	if (e == cudaSuccess) b->cap = cap;
 	return e;
 }
-static cudaError_t grow_host(QsBuf *b, size_t need) {
+/* keep: leading bytes of the old contents carried over into a new allocation */
+static cudaError_t grow_host(QsBuf *b, size_t need, size_t keep = 0) {
 	if (need <= b->cap) return cudaSuccess;
-	if (b->p) cudaFreeHost(b->p);
-	b->p = NULL; b->cap = 0;
+	void *p = NULL;
 	size_t cap = align256(need + need / 8 + (1 << 16));
-	cudaError_t e = cudaMallocHost(&b->p, cap);
-	if (e == cudaSuccess) b->cap = cap;
-	return e;
+	cudaError_t e = cudaMallocHost(&p, cap);
+	if (e != cudaSuccess) return e;
+	if (keep) memcpy(p, b->p, keep);
+	if (b->p) cudaFreeHost(b->p);
+	b->p = p; b->cap = cap;
+	return cudaSuccess;
 }
 
 extern "C" void jpegqs_cuda_transcode_free(void *p) { free(p); }
@@ -161,56 +173,221 @@ struct QsPlan {
 	jpegqs_cuda_image img; jpegqs_cuda_scan scan; jpegqs_cuda_jpeg_head head;
 	std::vector<jpegqs_cuda_scan_rec> recs;    /* empty: one sequential scan (decode_async) */
 	uint8_t *prefix; size_t plen;
+	int go;                                    /* the file takes part in the sub-batches */
+	int host;                                  /* pixels: the host reader decodes it */
 	int smooth, can_up;
-	size_t in_bytes, coef_bytes, up_bytes, cap;
+	size_t in_bytes, coef_bytes, up_bytes, cap, pix;
 	size_t ws_dec, ws_run, ws_enc;             /* this file's share of each stage's workspace */
+	size_t fixed, packed;                      /* its share of the buffers outside the workspace; of the packed output */
 };
 
-/* bytes a sub-batch of these files needs: file + prefix + descriptor, coefficients (+ up-sampled
- * chroma), output slot, and the shared workspace - the largest of the three stages' and of the packed
- * output's.  Each stage's workspace formula is a sum over files (run_async's constant is counted per
- * file here, so this bounds the exact group figure from above). */
+/* bytes a sub-batch of these files needs: each file's fixed share (the batch decides what that
+ * holds), and the shared workspace - the largest of the decoders', run_async's and the encoder's and of
+ * the packed output.  Each stage's workspace formula is a sum over files (run_async's constant is
+ * counted per file here, so this bounds the exact group figure from above). */
 struct QsNeed {
 	size_t fixed, dec, run, enc, packed;
 	size_t total() const { size_t w = dec; if (run > w) w = run; if (enc > w) w = enc; if (packed > w) w = packed; return fixed + w; }
-	void add(const QsPlan &p) {
-		fixed += p.in_bytes + sizeof(QsPackDesc) + p.coef_bytes + p.up_bytes + align256(p.cap);
-		dec += p.ws_dec; run += p.ws_run; enc += p.ws_enc; packed += align16(p.cap);
+	void add(const QsPlan &p) { fixed += p.fixed; dec += p.ws_dec; run += p.ws_run; enc += p.ws_enc; packed += p.packed; }
+};
+
+/* The context's batch state (created on first use), its device and stream. */
+static int batch_state(jpegqs_cuda_ctx *ctx, cudaStream_t *st, QsTranscode **out) {
+	char msg[256];
+	int device, sub_bytes;
+	cudaError_t e;
+	qs_ctx_decode_info(ctx, &device, st, &sub_bytes);
+	QsTranscode **slot = (QsTranscode**)qs_ctx_transcode_state(ctx);
+	if ((e = cudaSetDevice(device)) != cudaSuccess) goto fail;
+	if (!*slot) {
+		QsTranscode *t = new QsTranscode();
+		memset(t, 0, sizeof(*t));
+		*slot = t;
+		if ((e = cudaEventCreate(&t->ev0)) != cudaSuccess || (e = cudaEventCreate(&t->ev1)) != cudaSuccess ||
+				(e = cudaDeviceGetAttribute(&t->sms, cudaDevAttrMultiProcessorCount, device)) != cudaSuccess) goto fail;
+	}
+	*out = *slot;
+	return 0;
+fail:
+	snprintf(msg, sizeof(msg), "%s:%d: batch state: %s", __FILE__, __LINE__, cudaGetErrorString(e));
+	qs_ctx_decode_done(ctx, 0, msg);
+	return JPEGQS_ERR_CUDA;
+}
+
+/* File i's route from one markers-only walk (qs_route_plan): img for every file the reader takes; for a
+ * DEVICE file its scans, the upload (file + prefix) and the decoder workspace; with prefix != 0 the
+ * head and prefix of copy level `copy`.  *route: the route, or JPEGQS_ERR_ARG with *why the reader's
+ * complaint.  Returns 0 or a negative error of the workspace formulas. */
+static int plan_route(QsPlan &p, const uint8_t *data, size_t len, int copy, int prefix, jpegqs_cuda_scan_rec *recs,
+		int *route, const char **why) {
+	int nscans = 0;
+	memset(&p.head, 0, sizeof(p.head));
+	*route = qs_route_plan(data, len, copy, NULL, &p.img, &p.scan, recs, &nscans, prefix ? &p.head : NULL,
+			prefix ? &p.prefix : NULL, prefix ? &p.plen : NULL, why);
+	if (*route != JPEGQS_ROUTE_DEVICE) return 0;
+	p.recs.assign(recs, recs + nscans);
+	p.in_bytes = align256(len) + align256(p.plen);
+	if (p.recs.empty()) return jpegqs_cuda_decode_workspace_bytes(1, &p.img, &p.scan, &len, &p.ws_dec);
+	const jpegqs_cuda_scan_rec *r = p.recs.data();
+	return jpegqs_cuda_decode_scans_workspace_bytes(1, &p.img, &r, &nscans, &len, &p.ws_dec);
+}
+
+/* do_quantsmooth's early return (csrc/do_quantsmooth.c): nothing to smooth and nothing to up-sample
+ * leaves the coefficients and the quant tables as read.  Then the coefficient and up-sampled chroma
+ * bytes and run_async's workspace share. */
+static int plan_run(QsPlan &p, int flags, int niter) {
+	const jpegqs_cuda_comp *c = p.img.comp;
+	int need_downsample = (flags & (QS_JOINT_YUV | QS_UPSAMPLE_UV)) && p.img.is_ycbcr && p.img.ncomp >= 3 &&
+			c[1].h_samp == 1 && c[1].v_samp == 1 && c[2].h_samp == 1 && c[2].v_samp == 1;
+	p.smooth = !((niter > QS_ITER_MAX ? QS_ITER_MAX : niter) <= 0 && !((flags & QS_UPSAMPLE_UV) && need_downsample));
+	p.can_up = p.smooth && need_downsample && (flags & QS_UPSAMPLE_UV) && (c[0].h_samp != 1 || c[0].v_samp != 1);
+	p.coef_bytes = 0; p.up_bytes = 0;
+	for (int k = 0; k < p.img.ncomp; k++) p.coef_bytes += align256((size_t)c[k].wblk * c[k].hblk * 128);
+	if (p.can_up) p.up_bytes = 2 * align256((size_t)c[0].wblk * c[0].hblk * 128);
+	p.ws_run = 0;
+	if (p.smooth) return jpegqs_cuda_async_workspace_bytes(1, &p.img, flags & QS_FLAGS_MASK, &p.ws_run);
+	return 0;
+}
+
+/* the budget: 0 = half of what is free on the device now plus what these buffers already hold */
+static cudaError_t batch_budget(const QsTranscode *t, size_t max_device_bytes, size_t *budget) {
+	*budget = max_device_bytes;
+	if (max_device_bytes) return cudaSuccess;
+	size_t fr = 0, tot = 0;
+	cudaError_t e = cudaMemGetInfo(&fr, &tot);
+	*budget = (fr + t->in_dev.cap + t->coef_dev.cap + t->ws_dev.cap + t->out_dev.cap + t->stat_dev.cap + t->hcoef_dev.cap) / 2;
+	return e;
+}
+
+/* the next sub-batch: consecutive files that go, from *i0 on, while their needs stay within the budget
+ * (a file bigger than the budget goes alone), at most QS_PACK_MAX files; empty at the end */
+static std::vector<int> next_group(const std::vector<QsPlan> &plans, int n, int *i0, size_t budget) {
+	std::vector<int> files;
+	QsNeed need = {0, 0, 0, 0, 0};
+	int i = *i0;
+	for (; i < n && (int)files.size() < QS_PACK_MAX; i++) {
+		if (!plans[i].go) continue;
+		QsNeed with = need; with.add(plans[i]);
+		if (!files.empty() && with.total() > budget) break;
+		need = with; files.push_back(i);
+	}
+	*i0 = i;
+	return files;
+}
+
+/* One sub-batch: its files in the order of the later stages, their images, and the positions (in
+ * that order) of the files each device decoder takes. */
+struct QsGroup {
+	std::vector<int> order;
+	std::vector<jpegqs_cuda_image> eimg;
+	std::vector<int> seq_k, scan_k;
+	std::vector<const uint8_t*> data_dev;
+	void set(const std::vector<QsPlan> &plans, const std::vector<int> &ord) {
+		order = ord;
+		const size_t m = ord.size();
+		eimg.resize(m); data_dev.assign(m, NULL); seq_k.clear(); scan_k.clear();
+		for (size_t k = 0; k < m; k++) {
+			const QsPlan &p = plans[ord[k]];
+			eimg[k] = p.img;
+			if (!p.host) (p.recs.empty() ? seq_k : scan_k).push_back((int)k);
+		}
 	}
 };
+
+/* the exact workspace of the two decoders for the group's device-decoded files (the larger one) */
+static int group_decode_ws(const QsGroup &g, const std::vector<QsPlan> &plans, const size_t *len, size_t *ws) {
+	size_t w; int r;
+	*ws = 0;
+	if (!g.seq_k.empty()) {
+		std::vector<jpegqs_cuda_image> im; std::vector<jpegqs_cuda_scan> sc; std::vector<size_t> ln;
+		for (int k : g.seq_k) { im.push_back(g.eimg[k]); sc.push_back(plans[g.order[k]].scan); ln.push_back(len[g.order[k]]); }
+		if ((r = jpegqs_cuda_decode_workspace_bytes((int)im.size(), im.data(), sc.data(), ln.data(), &w)) < 0) return r;
+		if (w > *ws) *ws = w;
+	}
+	if (!g.scan_k.empty()) {
+		std::vector<jpegqs_cuda_image> im; std::vector<const jpegqs_cuda_scan_rec*> sc; std::vector<int> ns; std::vector<size_t> ln;
+		for (int k : g.scan_k) {
+			const QsPlan &p = plans[g.order[k]];
+			im.push_back(g.eimg[k]); sc.push_back(p.recs.data()); ns.push_back((int)p.recs.size()); ln.push_back(len[g.order[k]]);
+		}
+		if ((r = jpegqs_cuda_decode_scans_workspace_bytes((int)im.size(), im.data(), sc.data(), ns.data(), ln.data(), &w)) < 0) return r;
+		if (w > *ws) *ws = w;
+	}
+	return 0;
+}
+
+/* the device-decoded files' bytes (file | prefix, each 256-byte aligned) into the pinned staging from
+ * offset io on; records where each file will be on the device.  Returns the end offset. */
+static size_t group_stage(QsGroup &g, const std::vector<QsPlan> &plans, const uint8_t *const *data, const size_t *len,
+		uint8_t *in_host, const uint8_t *in_dev, size_t io) {
+	for (size_t k = 0; k < g.order.size(); k++) {
+		const QsPlan &p = plans[g.order[k]]; const size_t L = len[g.order[k]];
+		if (p.host) continue;
+		memcpy(in_host + io, data[g.order[k]], L);
+		if (p.plen) memcpy(in_host + io + align256(L), p.prefix, p.plen);
+		g.data_dev[k] = in_dev + io;
+		io += p.in_bytes;
+	}
+	return io;
+}
+
+/* a component's coefficient arrays from cp on, 256-byte aligned; returns the next free byte */
+static char *place_coefs(jpegqs_cuda_image &im, char *cp) {
+	for (int q = 0; q < im.ncomp; q++) { im.comp[q].coef = (int16_t*)cp; cp += align256((size_t)im.comp[q].wblk * im.comp[q].hblk * 128); }
+	return cp;
+}
+static char *place_up(jpegqs_cuda_image &im, const QsPlan &p, char *cp) {
+	if (p.can_up) for (int q = 1; q <= 2; q++) { im.comp[q].coef_up = (int16_t*)cp; cp += p.up_bytes / 2; }
+	return cp;
+}
+
+/* decode_async over the single-scan files and decode_scans_async over the others: statuses to dec[] in
+ * that order */
+static int group_decode(jpegqs_cuda_ctx *ctx, const QsGroup &g, const std::vector<QsPlan> &plans, const size_t *len,
+		void *ws, size_t ws_cap, int32_t *dec, cudaStream_t st) {
+	int r;
+	if (!g.seq_k.empty()) {
+		std::vector<jpegqs_cuda_image> im; std::vector<jpegqs_cuda_scan> sc; std::vector<const uint8_t*> dd; std::vector<size_t> ln;
+		for (int k : g.seq_k) { im.push_back(g.eimg[k]); sc.push_back(plans[g.order[k]].scan); dd.push_back(g.data_dev[k]); ln.push_back(len[g.order[k]]); }
+		if ((r = jpegqs_cuda_decode_async(ctx, (int)im.size(), im.data(), sc.data(), dd.data(), ln.data(), ws, ws_cap, dec, st)) < 0) return r;
+	}
+	if (!g.scan_k.empty()) {
+		std::vector<jpegqs_cuda_image> im; std::vector<const jpegqs_cuda_scan_rec*> sc; std::vector<int> ns;
+		std::vector<const uint8_t*> dd; std::vector<size_t> ln;
+		for (int k : g.scan_k) {
+			const QsPlan &p = plans[g.order[k]];
+			im.push_back(g.eimg[k]); sc.push_back(p.recs.data()); ns.push_back((int)p.recs.size());
+			dd.push_back(g.data_dev[k]); ln.push_back(len[g.order[k]]);
+		}
+		if ((r = jpegqs_cuda_decode_scans_async(ctx, (int)im.size(), im.data(), sc.data(), ns.data(), dd.data(), ln.data(),
+				ws, ws_cap, dec + g.seq_k.size(), st)) < 0) return r;
+	}
+	return 0;
+}
+
+#define TK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { \
+	snprintf(msg, sizeof(msg), "%s:%d: %s: %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); \
+	qs_ctx_decode_done(ctx, 0, msg); ret = JPEGQS_ERR_CUDA; goto fail; } } while (0)
+#define TQ(call) do { int r_ = (call); if (r_ < 0) { ret = r_; goto fail; } } while (0)
 
 /* the batch; `who` names the entry point in error messages */
 static int transcode_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint8_t *const *data, const size_t *len,
 		int flags, int niter, int optimize, int copy, size_t max_device_bytes, int *rc, jpegqs_cuda_transcode_result *results) {
 	char msg[512];
-	int device, sub_bytes; cudaStream_t st;
+	cudaStream_t st;
 	std::vector<QsPlan> plans((size_t)n);
 	for (int i = 0; i < n; i++) plans[i].prefix = NULL;
 	int ret = 0;
-#define TK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { \
-	snprintf(msg, sizeof(msg), "%s:%d: %s: %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); \
-	qs_ctx_decode_done(ctx, 0, msg); ret = JPEGQS_ERR_CUDA; goto fail; } } while (0)
-#define TQ(call) do { int r_ = (call); if (r_ < 0) { ret = r_; goto fail; } } while (0)
 	{
-	qs_ctx_decode_info(ctx, &device, &st, &sub_bytes);
-	QsTranscode **slot = (QsTranscode**)qs_ctx_transcode_state(ctx);
-	TK(cudaSetDevice(device));
-	if (!*slot) {
-		QsTranscode *t = new QsTranscode();
-		memset(t, 0, sizeof(*t));
-		*slot = t;
-		TK(cudaEventCreate(&t->ev0)); TK(cudaEventCreate(&t->ev1));
-		TK(cudaDeviceGetAttribute(&t->sms, cudaDevAttrMultiProcessorCount, device));
-	}
-	QsTranscode *t = *slot;
+	QsTranscode *t = NULL;
+	TQ(batch_state(ctx, &st, &t));
 	const int rflags = flags & QS_FLAGS_MASK;
 
 	/* every file's route, and everything the stages need of it, from one markers-only walk */
 	for (int i = 0; i < n; i++) {
 		QsPlan &p = plans[i];
-		int nscans = 0; const char *why;
-		memset(&p.head, 0, sizeof(p.head));
-		int route = qs_route_plan(data[i], len[i], copy, NULL, &p.img, &p.scan, t->recs, &nscans, &p.head, &p.prefix, &p.plen, &why);
+		int route; const char *why;
+		TQ(plan_route(p, data[i], len[i], copy, 1, t->recs, &route, &why));
 		if (route < 0) {
 			if (n == 1) snprintf(msg, sizeof(msg), "%s: %s", who, why);
 			else snprintf(msg, sizeof(msg), "%s: file %d: %s", who, i, why);
@@ -219,51 +396,22 @@ static int transcode_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const u
 		}
 		if (route != JPEGQS_ROUTE_DEVICE) { results[i].reason = why; rc[i] = JPEGQS_TRANSCODE_FALLBACK; continue; }
 		rc[i] = JPEGQS_TRANSCODE_OK;
-		p.recs.assign(t->recs, t->recs + nscans);
-
-		/* do_quantsmooth's early return (csrc/do_quantsmooth.c): nothing to smooth and nothing to
-		 * up-sample leaves the coefficients and the quant tables as read */
-		const jpegqs_cuda_comp *c = p.img.comp;
-		int need_downsample = (flags & (QS_JOINT_YUV | QS_UPSAMPLE_UV)) && p.img.is_ycbcr && p.img.ncomp >= 3 &&
-				c[1].h_samp == 1 && c[1].v_samp == 1 && c[2].h_samp == 1 && c[2].v_samp == 1;
-		p.smooth = !((niter > QS_ITER_MAX ? QS_ITER_MAX : niter) <= 0 && !((flags & QS_UPSAMPLE_UV) && need_downsample));
-		p.can_up = p.smooth && need_downsample && (flags & QS_UPSAMPLE_UV) && (c[0].h_samp != 1 || c[0].v_samp != 1);
-		p.in_bytes = align256(len[i]) + align256(p.plen);
-		p.coef_bytes = 0; p.up_bytes = 0;
-		for (int k = 0; k < p.img.ncomp; k++) p.coef_bytes += align256((size_t)c[k].wblk * c[k].hblk * 128);
-		if (p.can_up) p.up_bytes = 2 * align256((size_t)c[0].wblk * c[0].hblk * 128);
-		if (p.recs.empty()) TQ(jpegqs_cuda_decode_workspace_bytes(1, &p.img, &p.scan, &len[i], &p.ws_dec));
-		else {
-			const jpegqs_cuda_scan_rec *r = p.recs.data();
-			TQ(jpegqs_cuda_decode_scans_workspace_bytes(1, &p.img, &r, &nscans, &len[i], &p.ws_dec));
-		}
-		p.ws_run = 0;
-		if (p.smooth) TQ(jpegqs_cuda_async_workspace_bytes(1, &p.img, rflags, &p.ws_run));
+		TQ(plan_run(p, flags, niter));
 		TQ(jpegqs_cuda_encode_workspace_bytes(1, &p.img, optimize, &p.ws_enc));
 		TQ(jpegqs_cuda_encode_bound(&p.img, p.plen, &p.cap));
+		/* file + prefix + descriptor, coefficients (+ up-sampled chroma), output slot */
+		p.fixed = p.in_bytes + sizeof(QsPackDesc) + p.coef_bytes + p.up_bytes + align256(p.cap);
+		p.packed = align16(p.cap);
+		p.go = 1;
 	}
 
-	/* the budget: 0 = half of what is free on the device now plus what these buffers already hold */
-	size_t budget = max_device_bytes;
-	if (!budget) {
-		size_t fr = 0, tot = 0;
-		TK(cudaMemGetInfo(&fr, &tot));
-		budget = (fr + t->in_dev.cap + t->coef_dev.cap + t->ws_dev.cap + t->out_dev.cap + t->stat_dev.cap) / 2;
-	}
+	size_t budget;
+	TK(batch_budget(t, max_device_bytes, &budget));
 
 	/* sub-batches: consecutive device files while their needs stay within the budget */
 	int i0 = 0;
 	while (i0 < n) {
-		std::vector<int> files;
-		QsNeed need = {0, 0, 0, 0, 0};
-		int i = i0;
-		for (; i < n && (int)files.size() < QS_PACK_MAX; i++) {
-			if (rc[i] != JPEGQS_TRANSCODE_OK) continue;
-			QsNeed with = need; with.add(plans[i]);
-			if (!files.empty() && with.total() > budget) break;
-			need = with; files.push_back(i);
-		}
-		i0 = i;
+		std::vector<int> files = next_group(plans, n, &i0, budget);
 		if (files.empty()) continue;
 		const int m = (int)files.size();
 
@@ -273,30 +421,16 @@ static int transcode_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const u
 		for (int f : files) if (plans[f].smooth) order.push_back(f);
 		const int ms = (int)order.size();
 		for (int f : files) if (!plans[f].smooth) order.push_back(f);
-		std::vector<jpegqs_cuda_image> eimg(m);
+		QsGroup g; g.set(plans, order);
+		std::vector<jpegqs_cuda_image> &eimg = g.eimg;
 		std::vector<jpegqs_cuda_jpeg_head> heads(m);
 		std::vector<uint8_t*> out_ptr(m);
 		std::vector<size_t> caps(m);
 		std::vector<QsPackDesc> desc(m);
-		std::vector<int> seq_k, scan_k;                       /* encode positions of each decoder's files */
-		for (int k = 0; k < m; k++) (plans[order[k]].recs.empty() ? seq_k : scan_k).push_back(k);
 
 		/* exact workspace of each stage for this group; the packed output shares the workspace */
 		size_t ws = 0, w, in_total = align256((size_t)m * sizeof(QsPackDesc)), coef_total = 0, out_total = 0, packed = 0;
-		for (int k = 0; k < m; k++) eimg[k] = plans[order[k]].img;
-		if (!seq_k.empty()) {
-			std::vector<jpegqs_cuda_image> im; std::vector<jpegqs_cuda_scan> sc; std::vector<size_t> ln;
-			for (int k : seq_k) { im.push_back(eimg[k]); sc.push_back(plans[order[k]].scan); ln.push_back(len[order[k]]); }
-			TQ(jpegqs_cuda_decode_workspace_bytes((int)im.size(), im.data(), sc.data(), ln.data(), &w)); if (w > ws) ws = w;
-		}
-		if (!scan_k.empty()) {
-			std::vector<jpegqs_cuda_image> im; std::vector<const jpegqs_cuda_scan_rec*> sc; std::vector<int> ns; std::vector<size_t> ln;
-			for (int k : scan_k) {
-				const QsPlan &p = plans[order[k]];
-				im.push_back(eimg[k]); sc.push_back(p.recs.data()); ns.push_back((int)p.recs.size()); ln.push_back(len[order[k]]);
-			}
-			TQ(jpegqs_cuda_decode_scans_workspace_bytes((int)im.size(), im.data(), sc.data(), ns.data(), ln.data(), &w)); if (w > ws) ws = w;
-		}
+		TQ(group_decode_ws(g, plans, len, &ws));
 		if (ms) { TQ(jpegqs_cuda_async_workspace_bytes(ms, eimg.data(), rflags, &w)); if (w > ws) ws = w; }
 		TQ(jpegqs_cuda_encode_workspace_bytes(m, eimg.data(), optimize, &w)); if (w > ws) ws = w;
 		for (int k = 0; k < m; k++) {
@@ -320,46 +454,25 @@ static int transcode_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const u
 		uint8_t *in_dev = (uint8_t*)t->in_dev.p, *in_host = (uint8_t*)t->in_host.p, *sd = (uint8_t*)t->stat_dev.p;
 		char *cp = (char*)t->coef_dev.p;
 		size_t io = align256((size_t)m * sizeof(QsPackDesc)), oo = 0;
-		std::vector<const uint8_t*> data_dev(m);
+		group_stage(g, plans, data, len, in_host, in_dev, io);
 		for (int k = 0; k < m; k++) {
-			QsPlan &p = plans[order[k]]; const size_t L = len[order[k]];
-			jpegqs_cuda_image &im = eimg[k]; const jpegqs_cuda_comp *c = im.comp;
-			for (int q = 0; q < im.ncomp; q++) { im.comp[q].coef = (int16_t*)cp; cp += align256((size_t)c[q].wblk * c[q].hblk * 128); }
-			if (p.can_up) for (int q = 1; q <= 2; q++) { im.comp[q].coef_up = (int16_t*)cp; cp += p.up_bytes / 2; }
-			memcpy(in_host + io, data[order[k]], L);
-			memcpy(in_host + io + align256(L), p.prefix, p.plen);
-			data_dev[k] = in_dev + io;
-			heads[k] = p.head; heads[k].prefix_dev = in_dev + io + align256(L); heads[k].prefix_len = (uint32_t)p.plen;
-			io += p.in_bytes;
+			QsPlan &p = plans[order[k]];
+			cp = place_up(eimg[k], p, place_coefs(eimg[k], cp));
+			heads[k] = p.head; heads[k].prefix_dev = g.data_dev[k] + align256(len[order[k]]); heads[k].prefix_len = (uint32_t)p.plen;
 			out_ptr[k] = (uint8_t*)t->out_dev.p + oo; caps[k] = p.cap;
 			memset(&desc[k], 0, sizeof(desc[k]));
 			desc[k].slot = oo; desc[k].cap = p.cap;
 			oo += align256(p.cap);
 		}
-		for (size_t q = 0; q < seq_k.size(); q++) desc[seq_k[q]].dec_idx = (int32_t)q;
-		for (size_t q = 0; q < scan_k.size(); q++) desc[scan_k[q]].dec_idx = (int32_t)(seq_k.size() + q);
+		for (size_t q = 0; q < g.seq_k.size(); q++) desc[g.seq_k[q]].dec_idx = (int32_t)q;
+		for (size_t q = 0; q < g.scan_k.size(); q++) desc[g.scan_k[q]].dec_idx = (int32_t)(g.seq_k.size() + q);
 		memcpy(in_host, desc.data(), (size_t)m * sizeof(QsPackDesc));
 		TK(cudaMemcpyAsync(in_dev, in_host, in_total, cudaMemcpyHostToDevice, st));
 
 		int32_t *dec = (int32_t*)(sd + st_dec), *enc = (int32_t*)(sd + st_enc);
 		jpegqs_cuda_status *run = (jpegqs_cuda_status*)(sd + st_run);
 		uint64_t *lens = (uint64_t*)(sd + st_len);
-		if (!seq_k.empty()) {
-			std::vector<jpegqs_cuda_image> im; std::vector<jpegqs_cuda_scan> sc; std::vector<const uint8_t*> dd; std::vector<size_t> ln;
-			for (int k : seq_k) { im.push_back(eimg[k]); sc.push_back(plans[order[k]].scan); dd.push_back(data_dev[k]); ln.push_back(len[order[k]]); }
-			TQ(jpegqs_cuda_decode_async(ctx, (int)im.size(), im.data(), sc.data(), dd.data(), ln.data(), t->ws_dev.p, t->ws_dev.cap, dec, st));
-		}
-		if (!scan_k.empty()) {
-			std::vector<jpegqs_cuda_image> im; std::vector<const jpegqs_cuda_scan_rec*> sc; std::vector<int> ns;
-			std::vector<const uint8_t*> dd; std::vector<size_t> ln;
-			for (int k : scan_k) {
-				const QsPlan &p = plans[order[k]];
-				im.push_back(eimg[k]); sc.push_back(p.recs.data()); ns.push_back((int)p.recs.size());
-				dd.push_back(data_dev[k]); ln.push_back(len[order[k]]);
-			}
-			TQ(jpegqs_cuda_decode_scans_async(ctx, (int)im.size(), im.data(), sc.data(), ns.data(), dd.data(), ln.data(),
-					t->ws_dev.p, t->ws_dev.cap, dec + seq_k.size(), st));
-		}
+		TQ(group_decode(ctx, g, plans, len, t->ws_dev.p, t->ws_dev.cap, dec, st));
 		if (ms) {
 			TK(cudaEventRecord(t->ev0, st));
 			TQ(jpegqs_cuda_run_async(ctx, ms, eimg.data(), rflags, niter, t->ws_dev.p, t->ws_dev.cap, run, st));
@@ -422,8 +535,6 @@ static int transcode_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const u
 fail:
 	for (int i = 0; i < n; i++) { free(plans[i].prefix); free(results[i].data); results[i].data = NULL; results[i].len = 0; }
 	return ret;
-#undef TK
-#undef TQ
 }
 
 extern "C" int jpegqs_cuda_transcode_batch(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
@@ -454,4 +565,209 @@ extern "C" int jpegqs_cuda_transcode(jpegqs_cuda_ctx *ctx, const uint8_t *data, 
 	int rc = 0;
 	int ret = transcode_batch(ctx, "jpegqs_cuda_transcode", 1, &data, &len, flags, niter, optimize, copy, 0, &rc, result);
 	return ret < 0 ? ret : rc;
+}
+
+/* ---- JPEG files to smoothed pixels (jpegqs_cuda_pixels_batch) ------------------------------------- */
+/* the host reader's decode of file f into the pinned staging at offset off; the warning count or
+ * JPEGQS_ERR_ARG */
+static int host_read(const QsPlan &p, const uint8_t *data, size_t len, uint8_t *staging, size_t off) {
+	jpegqs_cuda_image im = p.img;
+	place_coefs(im, (char*)staging + off);
+	return jpegqs_cuda_jpeg_read(data, len, &im);
+}
+
+static int pixels_batch(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len, int flags, int niter,
+		int layout, int on_device, uint8_t *const *out, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results) {
+	static const char who[] = "jpegqs_cuda_pixels_batch";
+	char msg[512];
+	cudaStream_t st;
+	std::vector<QsPlan> plans((size_t)n);
+	int ret = 0;
+	{
+	QsTranscode *t = NULL;
+	TQ(batch_state(ctx, &st, &t));
+	const int rflags = flags & QS_FLAGS_MASK;
+
+	for (int i = 0; i < n; i++) {
+		QsPlan &p = plans[i];
+		int route; const char *why;
+		p.prefix = NULL; p.plen = 0;
+		TQ(plan_route(p, data[i], len[i], 0, 0, t->recs, &route, &why));
+		if (route < 0) {
+			snprintf(msg, sizeof(msg), "%s: file %d: %s", who, i, why);
+			qs_ctx_decode_done(ctx, 0, msg);
+			rc[i] = JPEGQS_ERR_ARG; continue;
+		}
+		if (!qs_render_takes(&p.img)) { rc[i] = JPEGQS_ERR_UNSUPPORTED; continue; }
+		p.host = route != JPEGQS_ROUTE_DEVICE;
+		if (p.host) { p.in_bytes = 0; p.ws_dec = 0; results[i].host_decoded = 1; results[i].reason = why; }
+		results[i].channels = p.img.ncomp;
+		TQ(plan_run(p, flags, niter));
+		p.pix = (size_t)p.img.image_width * p.img.image_height * p.img.ncomp;
+		/* file, coefficients (+ up-sampled chroma), the rendered pixels when they come back to the host */
+		p.fixed = p.in_bytes + p.coef_bytes + p.up_bytes + (on_device ? 0 : align256(p.pix));
+		p.ws_enc = 0; p.packed = 0;
+		p.go = 1;
+	}
+
+	size_t budget;
+	TK(batch_budget(t, max_device_bytes, &budget));
+
+	int i0 = 0;
+	while (i0 < n) {
+		std::vector<int> files = next_group(plans, n, &i0, budget);
+		if (files.empty()) continue;
+		const int m = (int)files.size();
+		QsGroup g; g.set(plans, files);
+
+		/* workspace: the decoders' and run_async's over every file that may smooth (a bound when a host
+		 * read fails); device buffers: the uploaded files, the device-decoded files' coefficients and
+		 * every file's up-sampled chroma, the decoder statuses */
+		size_t ws = 0, w, in_total = 0, coef_total = 0;
+		TQ(group_decode_ws(g, plans, len, &ws));
+		{
+			std::vector<jpegqs_cuda_image> sm;
+			for (int k = 0; k < m; k++) if (plans[files[k]].smooth) sm.push_back(g.eimg[k]);
+			if (!sm.empty()) { TQ(jpegqs_cuda_async_workspace_bytes((int)sm.size(), sm.data(), rflags, &w)); if (w > ws) ws = w; }
+		}
+		for (int f : files) in_total += plans[f].in_bytes, coef_total += (plans[f].host ? 0 : plans[f].coef_bytes) + plans[f].up_bytes;
+		const int ndec = (int)(g.seq_k.size() + g.scan_k.size());
+		TK(grow_dev(&t->in_dev, in_total));
+		TK(grow_dev(&t->coef_dev, coef_total + 256));
+		TK(grow_dev(&t->ws_dev, ws));
+		TK(grow_dev(&t->stat_dev, 4 * (size_t)m));
+		TK(grow_host(&t->in_host, in_total));
+		TK(grow_host(&t->stat_host, 4 * (size_t)m));
+
+		/* 1-2: the files up, the decoders enqueued, their statuses down */
+		group_stage(g, plans, data, len, (uint8_t*)t->in_host.p, (const uint8_t*)t->in_dev.p, 0);
+		char *cp = (char*)t->coef_dev.p;
+		for (int k = 0; k < m; k++) {
+			const QsPlan &p = plans[files[k]];
+			if (!p.host) cp = place_coefs(g.eimg[k], cp);
+			cp = place_up(g.eimg[k], p, cp);
+		}
+		int32_t *dec = (int32_t*)t->stat_dev.p;
+		if (in_total) TK(cudaMemcpyAsync(t->in_dev.p, t->in_host.p, in_total, cudaMemcpyHostToDevice, st));
+		TQ(group_decode(ctx, g, plans, len, t->ws_dev.p, t->ws_dev.cap, dec, st));
+		if (ndec) TK(cudaMemcpyAsync(t->stat_host.p, dec, 4 * (size_t)ndec, cudaMemcpyDeviceToHost, st));
+
+		/* 3: the host-route files read while the device decodes, into the staging of the host-decoded
+		 * coefficients (hoff: each file's offset there) */
+		std::vector<size_t> hoff(m, 0);
+		std::vector<char> alive(m, 1);
+		size_t hb = 0;
+		for (int k = 0; k < m; k++) if (plans[files[k]].host) { hoff[k] = hb; hb += plans[files[k]].coef_bytes; }
+		TK(grow_host(&t->hcoef_host, hb));
+		for (int k = 0; k < m; k++) {
+			const int f = files[k];
+			if (!plans[f].host) continue;
+			int r = host_read(plans[f], data[f], len[f], (uint8_t*)t->hcoef_host.p, hoff[k]);
+			if (r < 0) {
+				snprintf(msg, sizeof(msg), "%s: file %d: %s", who, f, jpegqs_cuda_last_error(NULL));
+				qs_ctx_decode_done(ctx, 0, msg);
+				rc[f] = JPEGQS_ERR_ARG; alive[k] = 0; continue;
+			}
+			results[f].warnings = r;
+		}
+		TK(cudaStreamSynchronize(st));
+
+		/* 4-5: a file the device decoder flagged is read again on the host, as the tool reads it */
+		const int32_t *dh = (const int32_t*)t->stat_host.p;
+		std::vector<int> dpos;                         /* decoder status index -> group position */
+		for (int k : g.seq_k) dpos.push_back(k);
+		for (int k : g.scan_k) dpos.push_back(k);
+		for (int q = 0; q < ndec; q++) {
+			if (!dh[q]) continue;
+			const int k = dpos[q], f = files[k];
+			const size_t keep = hb;
+			hoff[k] = hb; hb += plans[f].coef_bytes;
+			TK(grow_host(&t->hcoef_host, hb, keep));
+			results[f].host_decoded = 1; results[f].reason = "the device decoder flagged the data";
+			plans[f].host = 1;
+			int r = host_read(plans[f], data[f], len[f], (uint8_t*)t->hcoef_host.p, hoff[k]);
+			if (r < 0) {
+				snprintf(msg, sizeof(msg), "%s: file %d: %s", who, f, jpegqs_cuda_last_error(NULL));
+				qs_ctx_decode_done(ctx, 0, msg);
+				rc[f] = JPEGQS_ERR_ARG; alive[k] = 0; continue;
+			}
+			results[f].warnings = r;
+		}
+		/* 6: the host-decoded coefficients up in one copy */
+		if (hb) {
+			TK(grow_dev(&t->hcoef_dev, hb));
+			for (int k = 0; k < m; k++) if (plans[files[k]].host) place_coefs(g.eimg[k], (char*)t->hcoef_dev.p + hoff[k]);
+			TK(cudaMemcpyAsync(t->hcoef_dev.p, t->hcoef_host.p, hb, cudaMemcpyHostToDevice, st));
+		}
+
+		/* 7: run_async over the files that smooth, then one render over all.  Order: the colour files
+		 * that smooth, the grey files that smooth, the grey files that do not, the colour files that do
+		 * not - run_async's images are a prefix, and the grey store's images are consecutive, so the
+		 * render takes at most three launches per 60 images */
+		std::vector<int> rk;                           /* render order -> group position */
+		for (int pass = 0; pass < 4; pass++)
+			for (int k = 0; k < m; k++) {
+				const QsPlan &p = plans[files[k]];
+				if (alive[k] && p.smooth == (pass < 2) && (p.img.ncomp == 1) == (pass == 1 || pass == 2)) rk.push_back(k);
+			}
+		const int nr = (int)rk.size();
+		int ms = 0;
+		std::vector<jpegqs_cuda_image> rimg(nr);
+		for (int j = 0; j < nr; j++) { rimg[j] = g.eimg[rk[j]]; if (plans[files[rk[j]]].smooth) ms++; }
+		const size_t st_bytes = align256(sizeof(jpegqs_cuda_status) * (size_t)(nr ? nr : 1));
+		std::vector<size_t> poff(nr);
+		size_t pix_total = st_bytes;
+		for (int j = 0; j < nr; j++) { poff[j] = pix_total; if (!on_device) pix_total += align256(plans[files[rk[j]]].pix); }
+		TK(grow_dev(&t->out_dev, pix_total));
+		TK(grow_host(&t->out_host, pix_total));
+		jpegqs_cuda_status *run = (jpegqs_cuda_status*)t->out_dev.p;
+		std::vector<uint8_t*> outs(nr);
+		for (int j = 0; j < nr; j++) outs[j] = on_device ? out[files[rk[j]]] : (uint8_t*)t->out_dev.p + poff[j];
+		if (ms) {
+			TK(cudaEventRecord(t->ev0, st));
+			TQ(jpegqs_cuda_run_async(ctx, ms, rimg.data(), rflags, niter, t->ws_dev.p, t->ws_dev.cap, run, st));
+			TK(cudaEventRecord(t->ev1, st));
+		}
+		if (ms < nr) TK(cudaMemsetAsync(run + ms, 0, (size_t)(nr - ms) * sizeof(jpegqs_cuda_status), st));
+		if (nr) TQ(qs_render_images(ctx, nr, rimg.data(), run, layout, 1, outs.data(), st));
+		/* the run statuses, and the pixels in the same copy when they come back to the host */
+		if (nr) TK(cudaMemcpyAsync(t->out_host.p, t->out_dev.p, pix_total, cudaMemcpyDeviceToHost, st));
+		TK(cudaStreamSynchronize(st));
+		if (ms) {
+			float ms_run = 0;
+			TK(cudaEventElapsedTime(&ms_run, t->ev0, t->ev1));
+			qs_ctx_set_last_ms(ctx, ms_run);
+		}
+		const jpegqs_cuda_status *rs = (const jpegqs_cuda_status*)t->out_host.p;
+		for (int j = 0; j < nr; j++) {
+			const int f = files[rk[j]];
+			results[f].smoothed = plans[f].smooth; results[f].stop = rs[j].stop; results[f].upsampled = rs[j].upsampled;
+			if (!on_device) memcpy(out[f], (const uint8_t*)t->out_host.p + poff[j], plans[f].pix);
+		}
+	}
+	return 0;
+	}
+fail:
+	return ret;
+}
+#undef TK
+#undef TQ
+
+extern "C" int jpegqs_cuda_pixels_batch(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int layout, int out_on_device, uint8_t *const *out, size_t max_device_bytes, int *rc,
+		jpegqs_cuda_pixels_result *results) {
+	static const char who[] = "jpegqs_cuda_pixels_batch";
+	char msg[160];
+	if (!ctx) return JPEGQS_ERR_ARG;
+	if (n < 0) { qs_ctx_decode_done(ctx, 0, "jpegqs_cuda_pixels_batch: negative file count"); return JPEGQS_ERR_ARG; }
+	if (!n) return 0;
+	if (!data || !len || !out || !rc || !results) { qs_ctx_decode_done(ctx, 0, "jpegqs_cuda_pixels_batch: NULL argument"); return JPEGQS_ERR_ARG; }
+	for (int i = 0; i < n; i++) if (!data[i] || !out[i]) {
+		snprintf(msg, sizeof(msg), "%s: file %d: NULL %s", who, i, data[i] ? "output" : "data");
+		qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG;
+	}
+	if (layout != JPEGQS_RENDER_HWC && layout != JPEGQS_RENDER_CHW) { qs_ctx_decode_done(ctx, 0, "jpegqs_cuda_pixels_batch: unknown layout"); return JPEGQS_ERR_ARG; }
+	if (out_on_device != 0 && out_on_device != 1) { qs_ctx_decode_done(ctx, 0, "jpegqs_cuda_pixels_batch: out_on_device must be 0 or 1"); return JPEGQS_ERR_ARG; }
+	for (int i = 0; i < n; i++) { memset(&results[i], 0, sizeof(results[i])); results[i].reason = ""; rc[i] = 0; }
+	return pixels_batch(ctx, n, data, len, flags, niter, layout, out_on_device, out, max_device_bytes, rc, results);
 }

@@ -84,6 +84,12 @@ class _TranscodeResult(C.Structure):
                 ("upsampled", C.c_int32), ("reason", C.c_char_p)]
 
 
+class _PixelsResult(C.Structure):
+    """jpegqs_cuda_pixels_result (include/jpegqs_cuda.h)."""
+    _fields_ = [("channels", C.c_int32), ("host_decoded", C.c_int32), ("warnings", C.c_int32),
+                ("smoothed", C.c_int32), ("stop", C.c_int32), ("upsampled", C.c_int32), ("reason", C.c_char_p)]
+
+
 ROUTE_HOST, ROUTE_DEVICE = 0, 1
 TRANSCODE_OK, TRANSCODE_FALLBACK = 0, 1
 
@@ -205,6 +211,9 @@ def load():
     lib.jpegqs_cuda_transcode_batch.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_size_t), C.c_int,
                                                 C.c_int, C.c_int, C.c_int, C.c_size_t, C.POINTER(C.c_int),
                                                 C.POINTER(_TranscodeResult)]
+    lib.jpegqs_cuda_pixels_batch.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_size_t), C.c_int,
+                                             C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p), C.c_size_t,
+                                             C.POINTER(C.c_int), C.POINTER(_PixelsResult)]
     lib.jpegqs_cuda_tables.argtypes = [C.c_int, C.c_void_p]
     lib.jpegqs_cuda_orig_coef.argtypes = [C.c_int, C.c_int]
     _lib = lib
@@ -686,6 +695,66 @@ class QsContext:
         if bad is not None:
             raise QsError(f"transcode_batch: file {bad}: {self.lib.jpegqs_cuda_last_error(self.h).decode()}")
         return out
+
+    def decode_pixels(self, datas, flags: int, niter: int, layout: str = "hwc", device: str = "cuda",
+                      max_device_bytes: int = 0):
+        """Many JPEG files to the smoothed pixels the jpegqs tool's --ppm writes for them (islow, fancy
+        up-sampling, after do_quantsmooth(flags, niter)), in shared launches (jpegqs_cuda_pixels_batch).
+        Returns, in the order of datas, one record per file:
+            (pixels, warnings, host_decoded, smoothed, stop, upsampled, reason)
+        pixels is a uint8 tensor [H, W, C] for layout "hwc" or [C, H, W] for "chw", C = 1 for a grey
+        file and 3 for a colour one; on cuda:<this context's device> for device="cuda", a CPU tensor for
+        device="cpu".  warnings: the host reader's warning count (0 for a file the device decoded);
+        host_decoded / reason: whether and why the host reader decoded the file.  Raises TypeError for a
+        non-bytes entry or a bare bytes object, ValueError for an unknown layout or device or a negative
+        max_device_bytes, and QsError naming the index of a file the reader rejects or the render
+        cannot take (1 or 3 components, integral sampling ratios)."""
+        if isinstance(datas, (bytes, bytearray, memoryview, str)) or not hasattr(datas, "__len__"):
+            raise TypeError("decode_pixels: datas must be a sequence of bytes-like files")
+        files = [_file_bytes(d, f"decode_pixels: file {i}") for i, d in enumerate(datas)]
+        if layout not in ("hwc", "chw"):
+            raise ValueError(f"decode_pixels: layout {layout!r}: expected 'hwc' or 'chw'")
+        if device not in ("cuda", "cpu"):
+            raise ValueError(f"decode_pixels: device {device!r}: expected 'cuda' or 'cpu'")
+        if int(max_device_bytes) < 0:
+            raise ValueError("decode_pixels: max_device_bytes must be >= 0")
+        n = len(files)
+        if not n:
+            return []
+        import torch
+        # the output size rule of jpegqs_cuda_pixels_batch: transcode_route's width, height and ncomp
+        shapes = []
+        for i, d in enumerate(files):
+            info = _FileInfo()
+            if self.lib.jpegqs_cuda_transcode_route(d, len(d), None, C.byref(info)) < 0:
+                raise QsError(f"decode_pixels: file {i}: the reader rejects the file")
+            if info.ncomp not in (1, 3):
+                raise QsError(f"decode_pixels: file {i}: {info.ncomp} components; the render takes 1 or 3")
+            c, h, w = info.ncomp, info.image_height, info.image_width
+            shapes.append((h, w, c) if layout == "hwc" else (c, h, w))
+        if device == "cuda":
+            dev = self.device if self.device >= 0 else torch.cuda.current_device()
+            outs = [torch.empty(s, dtype=torch.uint8, device=dev) for s in shapes]
+            # the call writes on the context's stream: the memory must be free on the current one
+            torch.cuda.current_stream(dev).synchronize()
+        else:
+            outs = [torch.empty(s, dtype=torch.uint8) for s in shapes]
+        ptrs = (C.c_char_p * n)(*files)
+        lens = (C.c_size_t * n)(*[len(d) for d in files])
+        optrs = (C.c_void_p * n)(*[t.data_ptr() for t in outs])
+        rc = (C.c_int * n)()
+        res = (_PixelsResult * n)()
+        self._check(self.lib.jpegqs_cuda_pixels_batch(self.h, n, ptrs, lens, int(flags), int(niter),
+                                                      0 if layout == "hwc" else 1, int(device == "cuda"), optrs,
+                                                      int(max_device_bytes), rc, res))
+        for i in range(n):
+            if rc[i] == -2:
+                raise QsError(f"decode_pixels: file {i}: {self.lib.jpegqs_cuda_last_error(self.h).decode()}")
+            if rc[i] < 0:
+                raise QsError(f"decode_pixels: file {i}: the render takes 1 or 3 components with integral "
+                              "sampling ratios only")
+        return [(outs[i], res[i].warnings, res[i].host_decoded, res[i].smoothed, res[i].stop, res[i].upsampled,
+                 (res[i].reason or b"").decode()) for i in range(n)]
 
     # ---- whole image, host buffers (the call a user of the reference makes) ----
     def do_quantsmooth(self, image: CoefImage, flags: int, niter: int, progprec: int = 0,
@@ -1432,3 +1501,10 @@ def transcode_batch(datas, flags: int, niter: int, optimize: bool = False, copy:
     """QsContext.transcode_batch on the default context of `device`: a list of (bytes, None) or
     (None, reason), one per file."""
     return default_context(device).transcode_batch(datas, flags, niter, optimize, copy, max_device_bytes)
+
+
+def decode_pixels(datas, flags: int, niter: int, layout: str = "hwc", device: str = "cuda", max_device_bytes: int = 0,
+                  gpu: int = -1):
+    """QsContext.decode_pixels on the default context of CUDA device `gpu`: one record (pixels, warnings,
+    host_decoded, smoothed, stop, upsampled, reason) per file."""
+    return default_context(gpu).decode_pixels(datas, flags, niter, layout, device, max_device_bytes)
