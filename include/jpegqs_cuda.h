@@ -213,6 +213,34 @@ int jpegqs_cuda_run_async(jpegqs_cuda_ctx *ctx, int nimages, jpegqs_cuda_image *
 int jpegqs_cuda_render_async(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image *imgs,
 		const jpegqs_cuda_status *status_dev, int layout, uint8_t *const *out_dev, void *stream);
 
+/* ---- the same render at 1/2, 1/4 or 1/8 size: libjpeg's scaled decode -----------------------
+ * jpegqs_cuda_render_async is this call with scale_denom 1; everything above holds, except:
+ *   - Output.  out_dev[i]: ceil(image_width / d) * ceil(image_height / d) * 3 bytes, d = scale_denom.
+ *   - Pixels.  What jpeg_read_scanlines gives for the coefficients with scale_num 1, scale_denom d,
+ *     JDCT_ISLOW, do_fancy_upsampling TRUE and JCS_RGB output.  The image never exists at full size:
+ *       . each component gets libjpeg's DCT scaled size (jpeg_calc_output_dimensions): 8 / d, doubled
+ *         while the sampling ratios allow, so chroma is scaled up by its IDCT rather than up-sampled
+ *         where possible (4:2:0 at 1/2: luma 4x4, chroma 8x8, no up-sampling);
+ *       . blocks of scaled size 4, 2 and 1 go through libjpeg's reduced IDCTs (jidctred.c
+ *         jpeg_idct_4x4 / 2x2 / 1x1), size 8 through the islow IDCT;
+ *       . downsampled_width / height and the up-sampling ratios are computed at the scaled sizes;
+ *         fancy up-sampling is used where libjpeg uses it: not at d = 8 (smallest scaled size 1), and
+ *         h2v1 / h2v2 replicate when the scaled downsampled_width is 2 or less.
+ *   - Checked as well: scale_denom outside {1, 2, 4, 8} returns JPEGQS_ERR_ARG with nothing enqueued,
+ *     and the blocks must cover the samples at the scaled geometry (wblk * size >= downsampled_width).
+ * Returns 0 or a negative error. */
+int jpegqs_cuda_render_scaled_async(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image *imgs,
+		const jpegqs_cuda_status *status_dev, int layout, int scale_denom, uint8_t *const *out_dev, void *stream);
+
+/* jpegqs_cuda_render_scaled_async's algorithm on the calling thread, for one image (host-only, no
+ * device needed): the same reduced IDCTs, up-sampling and colour conversion.  comp[].coef / coef_up
+ * are HOST arrays; upsampled != 0 reads components 1 and 2 from coef_up, as a host-flagged up-sampled
+ * image.  out: ceil(image_width / d) * ceil(image_height / d) * 3 bytes in layout HWC or CHW (a grey
+ * image gives R = G = B).  Returns 0, JPEGQS_ERR_ARG (NULL img or out, unknown layout, scale_denom
+ * outside {1, 2, 4, 8}, the geometry checks of render_async) or JPEGQS_ERR_UNSUPPORTED (what
+ * render_async does not render); jpegqs_cuda_last_error(NULL) says why. */
+int jpegqs_cuda_render_model(const jpegqs_cuda_image *img, int upsampled, int layout, int scale_denom, uint8_t *out);
+
 /* ---- JPEG files to quantized coefficients -----------------------------------------------------
  * The first stage of a device pipeline: JPEG bytes -> the coefficients jpeg_read_coefficients gives,
  * as [hblk][wblk][64] int16 arrays, exactly what jpegqs_cuda_run_async and jpegqs_cuda_render_async
@@ -609,6 +637,23 @@ typedef struct {
 int jpegqs_cuda_pixels_batch(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
 		int flags, int niter, int layout, int out_on_device, uint8_t *const *out, size_t max_device_bytes,
 		int *rc, jpegqs_cuda_pixels_result *results);
+
+/* The same files at 1/2, 1/4 or 1/8 size (jpegqs_cuda_pixels_batch is this call with scale_denom 1):
+ * the routes, sub-batches, warnings, host_decoded, smoothed, stop and upsampled are those of the
+ * unscaled call, and only the render differs - jpegqs_cuda_render_scaled_async's.
+ *   - Output size.  out[i] holds exactly ceil(width / d) * ceil(height / d) * channels bytes, d =
+ *     scale_denom, with width, height and channels as for jpegqs_cuda_pixels_batch.  A 1920 x 1080
+ *     colour file at d = 4 gives 480 x 270 x 3 bytes.  With host outputs each file's share of the
+ *     sub-batch budget and of the download is its scaled size.
+ *   - Pixels.  Byte for byte what libjpeg's jpeg_read_scanlines gives with scale_num 1, scale_denom d,
+ *     JDCT_ISLOW and fancy up-sampling, JCS_RGB (JCS_GRAYSCALE for a grey file), for the coefficients
+ *     the render reads at d = 1: for a file that smooths, those of the file jpegqs writes for the same
+ *     flags and niter; for a file do_quantsmooth returns early on, those of the input file.
+ *   - Return.  As jpegqs_cuda_pixels_batch's, and a scale_denom outside {1, 2, 4, 8} is a bad argument
+ *     (JPEGQS_ERR_ARG, nothing done). */
+int jpegqs_cuda_pixels_batch_scaled(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int layout, int scale_denom, int out_on_device, uint8_t *const *out,
+		size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results);
 
 /* ---- one image sharded by MCU rows over several GPUs (SURVEY.md 8e) ----------------------
  * Every rank - a device of this process, or another process on the same box - smooths one slab

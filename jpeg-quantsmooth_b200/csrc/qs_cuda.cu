@@ -2111,55 +2111,79 @@ int qs_render_takes(const jpegqs_cuda_image *im) {
 	return 1;
 }
 
-/* jpegqs_cuda_render_async with the layout checked by the caller; grey_store != 0 writes 1-component
- * images with one byte per pixel (either layout: the single plane).  Consecutive images of one store
- * mode share a launch. */
+/* one image's render descriptor at scale 1 / scale_denom, writing to out.  Returns 1 for an image the
+ * render does not take, else 0 with bad set on a malformed one.  host: coef / coef_up are host arrays
+ * (render_model), so their alignment does not matter.
+ *
+ * The scaled geometry is libjpeg's (jdmaster.c jpeg_calc_output_dimensions, scale_num 1): the output is
+ * ceil(image_width / d) x ceil(image_height / d); the smallest DCT scaled size is m = 8 / d, and a
+ * component's size doubles from m while max_samp * m stays a multiple of samp * size * 2 in both
+ * directions - chroma is scaled up by its IDCT instead of by the up-sampler where the ratios allow it
+ * (4:2:0 at 1/2: luma 4x4, chroma 8x8 with no up-sampling).  downsampled_width / height are
+ * ceil(image_width * samp * size / (max_samp * 8)), and the up-sampler expands by
+ * max_samp * m / (samp * size), an integer by construction. */
+static int qs_render_desc(const jpegqs_cuda_image *im, int scale_denom, int status_given, int host, uint8_t *out,
+		QsRenderImg &r, const char *&bad) {
+	memset(&r, 0, sizeof(r));
+	if (im->ncomp != 1 && im->ncomp != 3) return 1;
+	int maxh = 1, maxv = 1;
+	for (int c = 0; c < im->ncomp && !bad; c++) {
+		const jpegqs_cuda_comp *cc = &im->comp[c];
+		if (cc->h_samp < 1 || cc->h_samp > 4 || cc->v_samp < 1 || cc->v_samp > 4) bad = "sampling factor outside 1..4";
+		else if (!cc->coef || cc->rows || cc->rows_up) bad = "coef NULL, or host block-row tables";
+		else if (!host && ((uintptr_t)cc->coef | (c ? (uintptr_t)cc->coef_up : 0)) & 15) bad = "coef or coef_up not 16-byte aligned";
+		else { maxh = std::max(maxh, cc->h_samp); maxv = std::max(maxv, cc->v_samp); }
+	}
+	if (!out) bad = "output NULL";
+	if (bad) return 0;
+	if (!qs_render_takes(im)) return 1;
+	const int m = 8 / scale_denom;
+	for (int c = 0; c < im->ncomp && !bad; c++) {
+		const jpegqs_cuda_comp *cc = &im->comp[c];
+		int ss = m;
+		while (ss < 8 && (maxh * m) % (cc->h_samp * ss * 2) == 0 && (maxv * m) % (cc->v_samp * ss * 2) == 0) ss *= 2;
+		const int lss = ss == 8 ? 3 : ss == 4 ? 2 : ss == 2 ? 1 : 0;
+		r.cw[c] = (int)(((uint64_t)im->image_width * cc->h_samp * ss + maxh * 8 - 1) / (maxh * 8));
+		r.ch[c] = (int)(((uint64_t)im->image_height * cc->v_samp * ss + maxv * 8 - 1) / (maxv * 8));
+		/* the blocks must hold every real sample: the kernel reads up to column cw - 1, row ch - 1 */
+		if ((uint64_t)cc->wblk * ss < (uint64_t)r.cw[c] || (uint64_t)cc->hblk * ss < (uint64_t)r.ch[c]) bad = "blocks do not cover the image";
+		r.coef[c] = cc->coef; r.wblk[c] = (int32_t)cc->wblk;
+		r.hs[c] = (uint8_t)(maxh * m / (cc->h_samp * ss)); r.vs[c] = (uint8_t)(maxv * m / (cc->v_samp * ss));
+		if (scale_denom > 1) r.lss |= (uint8_t)(lss << (2 * c));
+		int val = 0;
+		for (int k = 0; k < 64; k++) val |= cc->quant[k];
+		bool deq = cc->has_qtbl && val > 1;             /* render_rgb's rule: still quantized */
+		for (int k = 0; k < 64; k++) r.q[c][k] = deq ? cc->quant[k] : 1;
+	}
+	if (bad) return 0;
+	if (im->ncomp == 3) {
+		r.coef_up[0] = im->comp[1].coef_up; r.coef_up[1] = im->comp[2].coef_up;
+		if (status_given) r.up_mode = r.coef_up[0] && r.coef_up[1] ? 2 : 0;
+		else if (im->upsampled) {
+			if (!r.coef_up[0] || !r.coef_up[1]) bad = "upsampled without coef_up";
+			r.up_mode = 1;
+		}
+	}
+	r.width = (int32_t)((im->image_width + scale_denom - 1) / scale_denom);
+	r.height = (int32_t)((im->image_height + scale_denom - 1) / scale_denom);
+	r.out = out; r.ncomp = (uint8_t)im->ncomp; r.ycc = im->is_ycbcr ? 1 : 0;
+	return 0;
+}
+
+/* jpegqs_cuda_render_scaled_async with the layout and scale checked by the caller; grey_store != 0 writes
+ * 1-component images with one byte per pixel (either layout: the single plane).  Consecutive images of
+ * one store mode share a launch. */
 int qs_render_images(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image *imgs,
-		const jpegqs_cuda_status *status_dev, int layout, int grey_store, uint8_t *const *out_dev, void *stream) {
+		const jpegqs_cuda_status *status_dev, int layout, int grey_store, int scale_denom, uint8_t *const *out_dev,
+		void *stream) {
 	const char *bad = nimages < 0 || (nimages && (!imgs || !out_dev)) ? "images or outputs missing" : NULL;
 	std::vector<QsRenderImg> d(bad ? 0 : nimages);
 	std::vector<int> store(d.size());
 	int unsupported = 0;
 	for (int i = 0; i < nimages && !bad && !unsupported; i++) {
 		const jpegqs_cuda_image *im = &imgs[i];
-		QsRenderImg &r = d[i];
-		memset(&r, 0, sizeof(r));
-		if (im->ncomp != 1 && im->ncomp != 3) { unsupported = 1; break; }
-		int maxh = 1, maxv = 1;
-		for (int c = 0; c < im->ncomp && !bad; c++) {
-			const jpegqs_cuda_comp *cc = &im->comp[c];
-			if (cc->h_samp < 1 || cc->h_samp > 4 || cc->v_samp < 1 || cc->v_samp > 4) bad = "sampling factor outside 1..4";
-			else if (!cc->coef || cc->rows || cc->rows_up) bad = "coef NULL, or host block-row tables";
-			else if (((uintptr_t)cc->coef | (c ? (uintptr_t)cc->coef_up : 0)) & 15) bad = "coef or coef_up not 16-byte aligned";
-			else { maxh = std::max(maxh, cc->h_samp); maxv = std::max(maxv, cc->v_samp); }
-		}
-		if (!out_dev[i]) bad = "output NULL";
-		if (!bad && !qs_render_takes(im)) { unsupported = 1; break; }
+		unsupported = qs_render_desc(im, scale_denom, status_dev != NULL, 0, out_dev[i], d[i], bad);
 		store[i] = grey_store && im->ncomp == 1 ? QS_RENDER_GREY : layout;
-		for (int c = 0; c < im->ncomp && !bad; c++) {
-			const jpegqs_cuda_comp *cc = &im->comp[c];
-			r.cw[c] = (int)(((uint64_t)im->image_width * cc->h_samp + maxh - 1) / maxh);
-			r.ch[c] = (int)(((uint64_t)im->image_height * cc->v_samp + maxv - 1) / maxv);
-			/* the blocks must hold every real sample: the kernel reads up to column cw - 1, row ch - 1 */
-			if ((uint64_t)cc->wblk * 8 < (uint64_t)r.cw[c] || (uint64_t)cc->hblk * 8 < (uint64_t)r.ch[c]) bad = "blocks do not cover the image";
-			r.coef[c] = cc->coef; r.wblk[c] = (int32_t)cc->wblk;
-			r.hs[c] = (uint8_t)(maxh / cc->h_samp); r.vs[c] = (uint8_t)(maxv / cc->v_samp);
-			int val = 0;
-			for (int k = 0; k < 64; k++) val |= cc->quant[k];
-			bool deq = cc->has_qtbl && val > 1;             /* render_rgb's rule: still quantized */
-			for (int k = 0; k < 64; k++) r.q[c][k] = deq ? cc->quant[k] : 1;
-		}
-		if (bad || unsupported) break;
-		if (im->ncomp == 3) {
-			r.coef_up[0] = im->comp[1].coef_up; r.coef_up[1] = im->comp[2].coef_up;
-			if (status_dev) r.up_mode = r.coef_up[0] && r.coef_up[1] ? 2 : 0;
-			else if (im->upsampled) {
-				if (!r.coef_up[0] || !r.coef_up[1]) bad = "upsampled without coef_up";
-				r.up_mode = 1;
-			}
-		}
-		r.out = out_dev[i]; r.width = (int32_t)im->image_width; r.height = (int32_t)im->image_height;
-		r.ncomp = (uint8_t)im->ncomp; r.ycc = im->is_ycbcr ? 1 : 0;
 	}
 	if (unsupported) {
 		snprintf(ctx->err, sizeof(ctx->err), "render_async: 1 or 3 components with integral sampling ratios only");
@@ -2180,19 +2204,57 @@ int qs_render_images(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image 
 			r.tile_begin = tiles;
 			tiles += ((r.width + QS_RENDER_TW - 1) / QS_RENDER_TW) * ((r.height + QS_RENDER_TH - 1) / QS_RENDER_TH);
 		}
-		CK(qs_launch_render_async(d.data() + i0, n, tiles, status_dev ? (const int2 *)(status_dev + i0) : NULL, store[i0], st));
+		CK(qs_launch_render_async(d.data() + i0, n, tiles, status_dev ? (const int2 *)(status_dev + i0) : NULL, store[i0],
+				scale_denom, st));
 		if (tiles) ctx->launches++;
 		i0 += n;
 	}
 	return 0;
 }
 
-extern "C" int jpegqs_cuda_render_async(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image *imgs,
-		const jpegqs_cuda_status *status_dev, int layout, uint8_t *const *out_dev, void *stream) {
+static int qs_scale_ok(int scale_denom) {
+	return scale_denom == 1 || scale_denom == 2 || scale_denom == 4 || scale_denom == 8;
+}
+
+extern "C" int jpegqs_cuda_render_scaled_async(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image *imgs,
+		const jpegqs_cuda_status *status_dev, int layout, int scale_denom, uint8_t *const *out_dev, void *stream) {
 	if (!ctx) return JPEGQS_ERR_ARG;
 	if (!(nimages < 0 || (nimages && (!imgs || !out_dev))) && layout != JPEGQS_RENDER_HWC && layout != JPEGQS_RENDER_CHW) {
 		snprintf(ctx->err, sizeof(ctx->err), "render_async: unknown layout");
 		return JPEGQS_ERR_ARG;
 	}
-	return qs_render_images(ctx, nimages, imgs, status_dev, layout, 0, out_dev, stream);
+	if (!qs_scale_ok(scale_denom)) {
+		snprintf(ctx->err, sizeof(ctx->err), "render_async: scale_denom must be 1, 2, 4 or 8");
+		return JPEGQS_ERR_ARG;
+	}
+	return qs_render_images(ctx, nimages, imgs, status_dev, layout, 0, scale_denom, out_dev, stream);
+}
+
+extern "C" int jpegqs_cuda_render_async(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image *imgs,
+		const jpegqs_cuda_status *status_dev, int layout, uint8_t *const *out_dev, void *stream) {
+	return jpegqs_cuda_render_scaled_async(ctx, nimages, imgs, status_dev, layout, 1, out_dev, stream);
+}
+
+extern "C" int jpegqs_cuda_render_model(const jpegqs_cuda_image *img, int upsampled, int layout, int scale_denom,
+		uint8_t *out) {
+	const char *bad = !img || !out ? "NULL argument" : layout != JPEGQS_RENDER_HWC && layout != JPEGQS_RENDER_CHW ?
+			"unknown layout" : !qs_scale_ok(scale_denom) ? "scale_denom must be 1, 2, 4 or 8" : NULL;
+	QsRenderImg r;
+	int unsupported = 0;
+	if (!bad) {
+		jpegqs_cuda_image im = *img;
+		im.upsampled = upsampled ? 1 : 0;
+		unsupported = qs_render_desc(&im, scale_denom, 0, 1, out, r, bad);
+	}
+	if (unsupported) {
+		qs_set_host_error("jpegqs_cuda_render_model: 1 or 3 components with integral sampling ratios only");
+		return JPEGQS_ERR_UNSUPPORTED;
+	}
+	if (bad) {
+		char m[160]; snprintf(m, sizeof(m), "jpegqs_cuda_render_model: %s", bad);
+		qs_set_host_error(m);
+		return JPEGQS_ERR_ARG;
+	}
+	qs_render_host(&r, layout, scale_denom);
+	return 0;
 }

@@ -22,6 +22,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <limits.h>
+#include <string.h>
+#include <vector>
 #include "qs_common.h"
 #include "qs_kernels.h"
 
@@ -100,7 +102,7 @@ __device__ __forceinline__ int qs_cvtt_x86(float x) {
  * exactly one of t0/t1 below, so adding RND there once is the same integer sum as adding it to
  * each of the eight outputs - and it is free inside the IMAD that forms (in0 +- in4) << 13. */
 template <int RND>
-__device__ __forceinline__ void qs_islow_1d(const int *in, int *out) {
+__host__ __device__ __forceinline__ void qs_islow_1d(const int *in, int *out) {
 	int z1, z2, z3, z4, z5, e0, e1, e2, e3, t0, t1, t2, t3, a, b;
 	z2 = in[2]; z3 = in[6];
 	z1 = (z2 + z3) * 4433;
@@ -121,16 +123,23 @@ __device__ __forceinline__ void qs_islow_1d(const int *in, int *out) {
 }
 
 /* four int32 -> four saturated bytes b0 | b1<<8 | b2<<16 | b3<<24 */
-__device__ __forceinline__ uint32_t qs_pack_sat_u8(int b0, int b1, int b2, int b3) {
+__host__ __device__ __forceinline__ uint32_t qs_pack_sat_u8(int b0, int b1, int b2, int b3) {
+#ifdef __CUDA_ARCH__
 	uint32_t t, r;
 	asm("cvt.pack.sat.u8.s32.b32 %0, %1, %2, 0;" : "=r"(t) : "r"(b3), "r"(b2));
 	asm("cvt.pack.sat.u8.s32.b32 %0, %1, %2, %3;" : "=r"(r) : "r"(b1), "r"(b0), "r"(t));
 	return r;
+#else
+	const int b[4] = {b0, b1, b2, b3};
+	uint32_t r = 0;
+	for (int k = 0; k < 4; k++) r |= (uint32_t)(b[k] < 0 ? 0 : b[k] > 255 ? 255 : b[k]) << (8 * k);
+	return r;
+#endif
 }
 
 /* second pass over a 64-int workspace (already column-transformed and descaled):
  * rows -> packed pixels lo[y] = px[y][0..3], hi[y] = px[y][4..7] */
-__device__ __forceinline__ void qs_islow_rows(const int *ws, uint32_t *lo, uint32_t *hi) {
+__host__ __device__ __forceinline__ void qs_islow_rows(const int *ws, uint32_t *lo, uint32_t *hi) {
 #pragma unroll
 	for (int y = 0; y < 8; y++) {
 		int o[8];
@@ -1751,10 +1760,13 @@ struct QsPlanePx {
 
 /* One up-sampled sample at output pixel (ox, oy) of a component whose expansion factors are
  * hs x vs and whose real (not block padded) size is cw x ch; px(x, y) reads its sample (x, y).
- * Edges replicate the last real sample, column cw - 1 / row ch - 1, as libjpeg does. */
-template <class Px>
-__device__ __forceinline__ int qs_upsample_at(const Px &px, int hs, int vs, int cw, int ch, int ox, int oy) {
+ * Edges replicate the last real sample, column cw - 1 / row ch - 1, as libjpeg does.  FANCY false:
+ * replication only - libjpeg's jinit_upsampler turns fancy up-sampling off when the smallest DCT
+ * scaled size is 1 (scale 1/8), because its main controller has no context rows then. */
+template <bool FANCY = true, class Px>
+__host__ __device__ __forceinline__ int qs_upsample_at(const Px &px, int hs, int vs, int cw, int ch, int ox, int oy) {
 	if (hs == 1 && vs == 1) return px(ox, oy);
+	if (!FANCY) return px(min(ox / hs, cw - 1), min(oy / vs, ch - 1));
 	if (hs == 2 && vs == 1 && cw > 2) {                 /* h2v1_fancy_upsample */
 		int x = ox >> 1, v = px(x, oy);
 		if (ox & 1) return x == cw - 1 ? v : (v * 3 + px(x + 1, oy) + 2) >> 2;
@@ -1781,7 +1793,7 @@ __device__ __forceinline__ int qs_upsample_at(const Px &px, int hs, int vs, int 
 /* one output pixel, r | g << 8 | b << 16: YCbCr -> RGB with the fixed-point tables of jdcolor.c
  * (build_ycc_rgb_table / ycc_rgb_convert, SCALEBITS 16) when ycc, the three samples as they are
  * otherwise (a grey image passes its sample three times) */
-__device__ __forceinline__ uint32_t qs_rgb_pixel(int y, int c1, int c2, bool ycc) {
+__host__ __device__ __forceinline__ uint32_t qs_rgb_pixel(int y, int c1, int c2, bool ycc) {
 	int r = y, g = c1, b = c2;
 	if (ycc) {
 		int cb = c1 - 128, cr = c2 - 128;
@@ -1806,6 +1818,117 @@ __global__ void qs_render_rgb_kernel(QsRenderArgs a, uint8_t *__restrict__ rgb) 
 }
 
 /* ------------------------------------------------------------------------------------------
+ * Scaled decode (DESIGN.md section 3.9): libjpeg's reduced-size IDCTs, jidctred.c jpeg_idct_4x4,
+ * jpeg_idct_2x2 and jpeg_idct_1x1, restated from the published algorithm.  They are the LL&M
+ * butterfly of the islow IDCT with the terms the smaller output does not need left out, in
+ * fixed point with CONST_BITS 13 and PASS1_BITS 2: jpeg_idct_4x4 reads no row or column 4,
+ * jpeg_idct_2x2 only rows / columns 0, 1, 3, 5 and 7, jpeg_idct_1x1 only the DC term.
+ * The descale of every output is DESCALE(x, n) = (x + 2^(n-1)) >> n.  libjpeg-turbo runs SSE2
+ * versions of the 4x4 and 2x2 ones; they saturate where the C range-limit table wraps (a sample
+ * beyond [-384, 383] before the +128), so these clamp, as the islow render does (section 6 f2).
+ * jpeg_idct_1x1 has no SIMD version: it keeps the table's wrap.
+ * ------------------------------------------------------------------------------------------ */
+__host__ __device__ __forceinline__ int qs_descale(int x, int n) { return (x + (1 << (n - 1))) >> n; }
+
+/* one 1-D pass of jpeg_idct_4x4 over in[0..7] (in[4] is not read): out[0..3] before the descale */
+__host__ __device__ __forceinline__ void qs_red4_1d(const int *in, int *out) {
+	const int t0 = in[0] * (1 << 14);                       /* << (CONST_BITS + 1) */
+	const int t2 = in[2] * 15137 - in[6] * 6270;            /* FIX(1.847759065), FIX(0.765366865) */
+	const int t10 = t0 + t2, t12 = t0 - t2;
+	const int z1 = in[7], z2 = in[5], z3 = in[3], z4 = in[1];
+	/* FIX(0.211164243), FIX(1.451774981), FIX(2.172734803), FIX(1.061594337) */
+	const int o0 = -z1 * 1730 + z2 * 11893 - z3 * 17799 + z4 * 8697;
+	/* FIX(0.509795579), FIX(0.601344887), FIX(0.899976223), FIX(2.562915447) */
+	const int o2 = -z1 * 4176 - z2 * 4926 + z3 * 7373 + z4 * 20995;
+	out[0] = t10 + o2; out[3] = t10 - o2; out[1] = t12 + o0; out[2] = t12 - o0;
+}
+
+/* one 1-D pass of jpeg_idct_2x2 over in[0, 1, 3, 5, 7]: out[0..1] before the descale */
+__host__ __device__ __forceinline__ void qs_red2_1d(const int *in, int *out) {
+	const int t10 = in[0] * (1 << 15);                      /* << (CONST_BITS + 2) */
+	/* FIX(0.720959822), FIX(0.850430095), FIX(1.272758580), FIX(3.624509785) */
+	const int t0 = -in[7] * 5906 + in[5] * 6967 - in[3] * 10426 + in[1] * 29692;
+	out[0] = t10 + t0; out[1] = t10 - t0;
+}
+
+/* libjpeg's post-IDCT range limit (prepare_range_limit_table): the low 10 bits of x as a signed value,
+ * plus 128, clamped to [0, 255] */
+__host__ __device__ __forceinline__ int qs_range_limit(int x) {
+	x &= 1023;
+	return x < 128 ? x + 128 : x < 512 ? 255 : x < 896 ? 0 : x - 896;
+}
+
+__host__ __device__ __forceinline__ void qs_store_u32(uint8_t *d, uint32_t v) {
+#ifdef __CUDA_ARCH__
+	*(uint32_t *)d = v;
+#else
+	memcpy(d, &v, 4);
+#endif
+}
+
+/* the ss x ss samples of one block at DCT scaled size ss into dst (row stride `stride`).  cf: the 64
+ * de-quantized coefficients in natural order (only cf[0] is read for ss 1).  ss 8 is the islow IDCT of
+ * the full-size render. */
+__host__ __device__ __forceinline__ void qs_idct_scaled(const int *cf, int ss, uint8_t *dst, int stride) {
+	if (ss == 8) {
+		int ws[64];
+#pragma unroll
+		for (int x = 0; x < 8; x++) {
+			int in[8], o[8];
+#pragma unroll
+			for (int y = 0; y < 8; y++) in[y] = cf[y * 8 + x];
+			qs_islow_1d<1024>(in, o);
+#pragma unroll
+			for (int y = 0; y < 8; y++) ws[y * 8 + x] = o[y] >> 11;
+		}
+		uint32_t rlo[8], rhi[8];
+		qs_islow_rows(ws, rlo, rhi);
+#pragma unroll
+		for (int y = 0; y < 8; y++) { qs_store_u32(dst + y * stride, rlo[y]); qs_store_u32(dst + y * stride + 4, rhi[y]); }
+	} else if (ss == 4) {
+		int ws[32];                                         /* [4 rows][8 columns]; column 4 unused */
+#pragma unroll
+		for (int x = 0; x < 8; x++) {
+			if (x == 4) { for (int y = 0; y < 4; y++) ws[y * 8 + x] = 0; continue; }
+			int in[8], o[4];
+#pragma unroll
+			for (int y = 0; y < 8; y++) in[y] = cf[y * 8 + x];
+			qs_red4_1d(in, o);
+#pragma unroll
+			for (int y = 0; y < 4; y++) ws[y * 8 + x] = qs_descale(o[y], 12);   /* CONST_BITS - PASS1_BITS + 1 */
+		}
+#pragma unroll
+		for (int y = 0; y < 4; y++) {
+			int o[4];
+			qs_red4_1d(ws + y * 8, o);
+			qs_store_u32(dst + y * stride, qs_pack_sat_u8(qs_descale(o[0], 19) + 128, qs_descale(o[1], 19) + 128,
+					qs_descale(o[2], 19) + 128, qs_descale(o[3], 19) + 128));        /* CONST_BITS + PASS1_BITS + 3 + 1 */
+		}
+	} else if (ss == 2) {
+		int ws[16];                                         /* [2 rows][8 columns]; columns 2, 4, 6 unused */
+#pragma unroll
+		for (int x = 0; x < 8; x++) {
+			if (x == 2 || x == 4 || x == 6) { ws[x] = ws[8 + x] = 0; continue; }
+			int in[8], o[2];
+#pragma unroll
+			for (int y = 0; y < 8; y++) in[y] = cf[y * 8 + x];
+			qs_red2_1d(in, o);
+			ws[x] = qs_descale(o[0], 13); ws[8 + x] = qs_descale(o[1], 13);       /* CONST_BITS - PASS1_BITS + 2 */
+		}
+#pragma unroll
+		for (int y = 0; y < 2; y++) {
+			int o[2];
+			qs_red2_1d(ws + y * 8, o);
+			const int a = qs_descale(o[0], 20) + 128, b = qs_descale(o[1], 20) + 128;   /* CONST_BITS + PASS1_BITS + 3 + 2 */
+			dst[y * stride] = (uint8_t)(a < 0 ? 0 : a > 255 ? 255 : a);
+			dst[y * stride + 1] = (uint8_t)(b < 0 ? 0 : b > 255 ? 255 : b);
+		}
+	} else {
+		dst[0] = (uint8_t)qs_range_limit(qs_descale(cf[0], 3));
+	}
+}
+
+/* ------------------------------------------------------------------------------------------
  * Stream-ordered render (qs_cuda.cu jpegqs_cuda_render_async): coefficients -> islow IDCT ->
  * libjpeg's up-sampling -> colour conversion -> pixels in one launch per batch; no sample plane
  * goes through global memory.  A CTA renders one QS_RENDER_TW x QS_RENDER_TH tile of output
@@ -1814,6 +1937,10 @@ __global__ void qs_render_rgb_kernel(QsRenderArgs a, uint8_t *__restrict__ rgb) 
  * from there.  Per component the window is at most 16 x 8 blocks: 16 x 8 at full resolution, 10 x 6
  * with 2:1 sub-sampling and its ring, fewer for 3:1 and 4:1 (which replicate and need no ring).
  * Coefficients are only read; de-quantization happens in registers, in int32 (jidctint.c).
+ * Scaled decode (D = scale_denom 2, 4 or 8): the tile is still 128 x 64 output pixels and the windows
+ * hold samples at each component's DCT scaled size (QsRenderImg.lss), so a tile reads up to D^2 times
+ * the blocks; each block gives ss x ss samples through qs_idct_scaled.  D = 1 is the code above,
+ * unchanged.
  * ------------------------------------------------------------------------------------------ */
 #define QS_RT_THREADS 256
 #define QS_RS_W 128
@@ -1833,13 +1960,15 @@ struct QsSmemPx {
 struct QsRenderComp { const int16_t *coef; int wblk, bx0, by0, nbx, nby, cw, ch, hs, vs; };
 
 /* STORE: QS_RENDER_HWC / QS_RENDER_CHW (three bytes per pixel), or QS_RENDER_GREY (one byte per pixel,
- * the CHW store of plane 0 only; for 1-component images) */
-template <int STORE>
+ * the CHW store of plane 0 only; for 1-component images).  D: the scale denominator (1, 2, 4, 8); the
+ * descriptors then hold the scaled geometry (qs_render_images). */
+template <int STORE, int D>
 __global__ void __launch_bounds__(QS_RT_THREADS, 2) qs_render_async_kernel(const __grid_constant__ QsRenderPack p,
 		int n, const int2 *__restrict__ status) {
 	__shared__ __align__(16) uint8_t pix[3][QS_RS_H * QS_RS_W];
 	__shared__ int qmul[3][64];
 	__shared__ QsRenderComp g[3];
+	__shared__ int glss[3];                              /* D > 1: log2 of each window's DCT scaled size */
 	const int tile = blockIdx.x;
 	int lo = 0, hi = n - 1;
 	while (lo < hi) {                                    /* last image with tile_begin <= tile */
@@ -1859,14 +1988,17 @@ __global__ void __launch_bounds__(QS_RT_THREADS, 2) qs_render_async_kernel(const
 		r.coef = up ? im.coef_up[c - 1] : im.coef[c];
 		r.wblk = im.wblk[k]; r.cw = im.cw[k]; r.ch = im.ch[k]; r.hs = im.hs[k]; r.vs = im.vs[k];
 		const int rx = r.hs == 2 ? 1 : 0, ry = r.vs == 2 ? 1 : 0;     /* the fancy up-sampler's ring */
-		r.bx0 = max(x0 / r.hs - rx, 0) >> 3; r.nbx = (min(x1 / r.hs + rx, r.cw - 1) >> 3) - r.bx0 + 1;
-		r.by0 = max(y0 / r.vs - ry, 0) >> 3; r.nby = (min(y1 / r.vs + ry, r.ch - 1) >> 3) - r.by0 + 1;
+		const int lss = D == 1 ? 3 : (im.lss >> (2 * k)) & 3;
+		r.bx0 = max(x0 / r.hs - rx, 0) >> lss; r.nbx = (min(x1 / r.hs + rx, r.cw - 1) >> lss) - r.bx0 + 1;
+		r.by0 = max(y0 / r.vs - ry, 0) >> lss; r.nby = (min(y1 / r.vs + ry, r.ch - 1) >> lss) - r.by0 + 1;
 		g[c] = r;
+		if (D > 1) glss[c] = lss;
 	}
 	for (int i = threadIdx.x; i < nc * 64; i += QS_RT_THREADS) qmul[i >> 6][i & 63] = im.q[i >> 6][i & 63];
 	__syncthreads();
 
-	/* islow IDCT of every block of the windows, one thread per block (as qs_idct_pass_kernel) */
+	/* islow IDCT (D > 1: each window's scaled IDCT) of every block of the windows, one thread per block
+	 * (as qs_idct_pass_kernel) */
 	const int nb0 = g[0].nbx * g[0].nby, nb1 = nc > 1 ? g[1].nbx * g[1].nby : 0, nb2 = nc > 2 ? g[2].nbx * g[2].nby : 0;
 	for (int k = threadIdx.x; k < nb0 + nb1 + nb2; k += QS_RT_THREADS) {
 		const int c = k < nb0 ? 0 : k < nb0 + nb1 ? 1 : 2;
@@ -1874,6 +2006,13 @@ __global__ void __launch_bounds__(QS_RT_THREADS, 2) qs_render_async_kernel(const
 		const QsRenderComp &r = g[c];
 		const int lby = j / r.nbx, lbx = j - lby * r.nbx;
 		const int4 *src = (const int4 *)(r.coef + ((size_t)(r.by0 + lby) * r.wblk + r.bx0 + lbx) * 64);
+		if constexpr (D > 1) {
+			if (glss[c] == 0) {                             /* jpeg_idct_1x1: the DC term only */
+				int cf0 = __ldg((const short *)src) * qmul[c][0];
+				qs_idct_scaled(&cf0, 1, &pix[c][lby * QS_RS_W + lbx], QS_RS_W);
+				continue;
+			}
+		}
 		int cf[64];
 #pragma unroll
 		for (int v8 = 0; v8 < 8; v8++) {
@@ -1885,27 +2024,33 @@ __global__ void __launch_bounds__(QS_RT_THREADS, 2) qs_render_async_kernel(const
 				cf[v8 * 8 + 2 * h + 1] = (w[h] >> 16) * qmul[c][v8 * 8 + 2 * h + 1];
 			}
 		}
-		int ws[64];
+		if constexpr (D > 1) {
+			const int lss = glss[c];
+			qs_idct_scaled(cf, 1 << lss, &pix[c][((lby * QS_RS_W) + lbx) << lss], QS_RS_W);
+		} else {
+			int ws[64];
 #pragma unroll
-		for (int x = 0; x < 8; x++) {
-			int in[8], o[8];
+			for (int x = 0; x < 8; x++) {
+				int in[8], o[8];
 #pragma unroll
-			for (int y = 0; y < 8; y++) in[y] = cf[y * 8 + x];
-			qs_islow_1d<1024>(in, o);
+				for (int y = 0; y < 8; y++) in[y] = cf[y * 8 + x];
+				qs_islow_1d<1024>(in, o);
 #pragma unroll
-			for (int y = 0; y < 8; y++) ws[y * 8 + x] = o[y] >> 11;
+				for (int y = 0; y < 8; y++) ws[y * 8 + x] = o[y] >> 11;
+			}
+			uint32_t rlo[8], rhi[8];
+			qs_islow_rows(ws, rlo, rhi);
+			uint8_t *d = &pix[c][lby * 8 * QS_RS_W + lbx * 8];
+#pragma unroll
+			for (int y = 0; y < 8; y++) *(uint2 *)(d + y * QS_RS_W) = make_uint2(rlo[y], rhi[y]);
 		}
-		uint32_t rlo[8], rhi[8];
-		qs_islow_rows(ws, rlo, rhi);
-		uint8_t *d = &pix[c][lby * 8 * QS_RS_W + lbx * 8];
-#pragma unroll
-		for (int y = 0; y < 8; y++) *(uint2 *)(d + y * QS_RS_W) = make_uint2(rlo[y], rhi[y]);
 	}
 	__syncthreads();
 
 	/* pixels: a warp renders a row of 128, four consecutive pixels per lane */
-	const QsSmemPx P0{pix[0], g[0].bx0 * 8, g[0].by0 * 8}, P1{pix[1], g[1].bx0 * 8, g[1].by0 * 8},
-			P2{pix[2], g[2].bx0 * 8, g[2].by0 * 8};
+	const int ls0 = D == 1 ? 3 : glss[0], ls1 = D == 1 ? 3 : glss[1], ls2 = D == 1 ? 3 : glss[2];
+	const QsSmemPx P0{pix[0], g[0].bx0 << ls0, g[0].by0 << ls0}, P1{pix[1], g[1].bx0 << ls1, g[1].by0 << ls1},
+			P2{pix[2], g[2].bx0 << ls2, g[2].by0 << ls2};
 	const int lane = threadIdx.x & 31, ox = x0 + lane * 4;
 	if (ox > x1) return;
 	const bool ycc = nc >= 3 && im.ycc;
@@ -1914,11 +2059,11 @@ __global__ void __launch_bounds__(QS_RT_THREADS, 2) qs_render_async_kernel(const
 #pragma unroll
 		for (int i = 0; i < 4; i++) {
 			const int x = min(ox + i, x1);
-			const int y = qs_upsample_at(P0, g[0].hs, g[0].vs, g[0].cw, g[0].ch, x, oy);
+			const int y = qs_upsample_at<D != 8>(P0, g[0].hs, g[0].vs, g[0].cw, g[0].ch, x, oy);
 			int c1 = y, c2 = y;
 			if (nc >= 3) {
-				c1 = qs_upsample_at(P1, g[1].hs, g[1].vs, g[1].cw, g[1].ch, x, oy);
-				c2 = qs_upsample_at(P2, g[2].hs, g[2].vs, g[2].cw, g[2].ch, x, oy);
+				c1 = qs_upsample_at<D != 8>(P1, g[1].hs, g[1].vs, g[1].cw, g[1].ch, x, oy);
+				c2 = qs_upsample_at<D != 8>(P2, g[2].hs, g[2].vs, g[2].cw, g[2].ch, x, oy);
 			}
 			px[i] = qs_rgb_pixel(y, c1, c2, ycc);
 		}
@@ -1950,17 +2095,83 @@ __global__ void __launch_bounds__(QS_RT_THREADS, 2) qs_render_async_kernel(const
 	}
 }
 
-cudaError_t qs_launch_render_async(const QsRenderImg *imgs, int n, int tiles, const int2 *status, int store,
+template <int D>
+static void qs_launch_render_scaled(const QsRenderPack &pack, int n, int tiles, const int2 *status, int store,
 		cudaStream_t st) {
+	if (store == QS_RENDER_HWC) qs_render_async_kernel<QS_RENDER_HWC, D><<<tiles, QS_RT_THREADS, 0, st>>>(pack, n, status);
+	else if (store == QS_RENDER_CHW) qs_render_async_kernel<QS_RENDER_CHW, D><<<tiles, QS_RT_THREADS, 0, st>>>(pack, n, status);
+	else qs_render_async_kernel<QS_RENDER_GREY, D><<<tiles, QS_RT_THREADS, 0, st>>>(pack, n, status);
+}
+
+cudaError_t qs_launch_render_async(const QsRenderImg *imgs, int n, int tiles, const int2 *status, int store,
+		int scale_denom, cudaStream_t st) {
 	if (tiles <= 0) return cudaSuccess;
+	if (store != QS_RENDER_HWC && store != QS_RENDER_CHW && store != QS_RENDER_GREY) return cudaErrorInvalidValue;
 	QsRenderPack pack;
 	memcpy(pack.img, imgs, (size_t)n * sizeof(QsRenderImg));
 	if (n < QS_RENDER_PACK) memset(pack.img + n, 0, (size_t)(QS_RENDER_PACK - n) * sizeof(QsRenderImg));
-	if (store == QS_RENDER_HWC) qs_render_async_kernel<QS_RENDER_HWC><<<tiles, QS_RT_THREADS, 0, st>>>(pack, n, status);
-	else if (store == QS_RENDER_CHW) qs_render_async_kernel<QS_RENDER_CHW><<<tiles, QS_RT_THREADS, 0, st>>>(pack, n, status);
-	else if (store == QS_RENDER_GREY) qs_render_async_kernel<QS_RENDER_GREY><<<tiles, QS_RT_THREADS, 0, st>>>(pack, n, status);
-	else return cudaErrorInvalidValue;
+	switch (scale_denom) {
+	case 1: qs_launch_render_scaled<1>(pack, n, tiles, status, store, st); break;
+	case 2: qs_launch_render_scaled<2>(pack, n, tiles, status, store, st); break;
+	case 4: qs_launch_render_scaled<4>(pack, n, tiles, status, store, st); break;
+	case 8: qs_launch_render_scaled<8>(pack, n, tiles, status, store, st); break;
+	default: return cudaErrorInvalidValue;
+	}
 	return cudaGetLastError();
+}
+
+/* sample (x, y) of a host plane of `stride` samples per row */
+struct QsHostPx {
+	const uint8_t *s; int stride;
+	__host__ __device__ int operator()(int x, int y) const { return s[(size_t)y * stride + x]; }
+};
+
+template <int D>
+static void qs_render_host_d(const QsRenderImg &im, int store) {
+	const int nc = im.ncomp, W = im.width, H = im.height;
+	std::vector<uint8_t> plane[3];
+	QsHostPx px[3];
+	int hs[3], vs[3], cw[3], ch[3];
+	for (int c = 0; c < nc; c++) {
+		const bool up = c > 0 && im.up_mode == 1;
+		const int k = up ? 0 : c, lss = D == 1 ? 3 : (im.lss >> (2 * k)) & 3, ss = 1 << lss;
+		const int16_t *coef = up ? im.coef_up[c - 1] : im.coef[c];
+		hs[c] = im.hs[k]; vs[c] = im.vs[k]; cw[c] = im.cw[k]; ch[c] = im.ch[k];
+		/* the blocks that hold the real samples (the render reads no others) */
+		const int nbx = (cw[c] + ss - 1) >> lss, nby = (ch[c] + ss - 1) >> lss, stride = nbx * ss;
+		plane[c].assign((size_t)stride * nby * ss, 0);
+		for (int by = 0; by < nby; by++)
+			for (int bx = 0; bx < nbx; bx++) {
+				const int16_t *b = coef + ((size_t)by * im.wblk[k] + bx) * 64;
+				int cf[64];
+				for (int i = 0; i < 64; i++) cf[i] = b[i] * im.q[c][i];
+				qs_idct_scaled(cf, ss, plane[c].data() + ((size_t)by * ss * stride + (size_t)bx * ss), stride);
+			}
+		px[c] = QsHostPx{plane[c].data(), stride};
+	}
+	const bool ycc = nc >= 3 && im.ycc;
+	for (int oy = 0; oy < H; oy++)
+		for (int ox = 0; ox < W; ox++) {
+			const int y = qs_upsample_at<D != 8>(px[0], hs[0], vs[0], cw[0], ch[0], ox, oy);
+			int c1 = y, c2 = y;
+			if (nc >= 3) {
+				c1 = qs_upsample_at<D != 8>(px[1], hs[1], vs[1], cw[1], ch[1], ox, oy);
+				c2 = qs_upsample_at<D != 8>(px[2], hs[2], vs[2], cw[2], ch[2], ox, oy);
+			}
+			const uint32_t v = qs_rgb_pixel(y, c1, c2, ycc);
+			const size_t i = (size_t)oy * W + ox;
+			if (store == QS_RENDER_HWC) for (int j = 0; j < 3; j++) im.out[3 * i + j] = (uint8_t)(v >> (8 * j));
+			else for (int j = 0; j < (store == QS_RENDER_GREY ? 1 : 3); j++) im.out[(size_t)j * W * H + i] = (uint8_t)(v >> (8 * j));
+		}
+}
+
+void qs_render_host(const QsRenderImg *im, int store, int scale_denom) {
+	switch (scale_denom) {
+	case 1: qs_render_host_d<1>(*im, store); break;
+	case 2: qs_render_host_d<2>(*im, store); break;
+	case 4: qs_render_host_d<4>(*im, store); break;
+	default: qs_render_host_d<8>(*im, store); break;
+	}
 }
 
 cudaError_t qs_launch_render_rgb(const uint8_t *const *planes, const int *strides, const int *cw, const int *ch,

@@ -55,7 +55,8 @@ typedef struct {
 	uint8_t hs[3], vs[3];        /* expansion factors max_samp / samp */
 	uint8_t ncomp, ycc;
 	uint8_t up_mode;             /* 0: coef, 1: coef_up (host flag), 2: status[i].upsampled decides */
-	uint8_t pad;
+	uint8_t lss;                 /* scale_denom > 1: bits 2c..2c+1 hold log2 of component c's DCT scaled
+	                                size; width, height, cw, ch, hs and vs are then the scaled ones */
 	uint16_t q[3][64];           /* multipliers: the raw quant table where it de-quantizes, else ones */
 } QsRenderImg;
 #define QS_RENDER_PACK 60
@@ -64,8 +65,12 @@ typedef struct {
 #define QS_RENDER_HWC 0
 #define QS_RENDER_CHW 1
 #define QS_RENDER_GREY 2
-/* status: the launch's first image's {stop, upsampled}, or NULL when no image has up_mode 2 */
+/* status: the launch's first image's {stop, upsampled}, or NULL when no image has up_mode 2;
+ * scale_denom: 1, 2, 4 or 8 */
 cudaError_t qs_launch_render_async(const QsRenderImg *imgs, int n, int tiles, const int2 *status, int store,
-		cudaStream_t st);
+		int scale_denom, cudaStream_t st);
+/* the same render of one image on the calling thread: host coefficient and output pointers, up_mode 0
+ * or 1 */
+void qs_render_host(const QsRenderImg *im, int store, int scale_denom);
 
 #endif

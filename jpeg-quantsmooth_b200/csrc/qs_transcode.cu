@@ -30,7 +30,8 @@ extern "C" int qs_route_plan(const uint8_t *data, size_t len, int copy, jpegqs_c
 		uint8_t **prefix, size_t *prefix_len, const char **reason);
 int qs_render_takes(const jpegqs_cuda_image *im);                     /* qs_cuda.cu */
 int qs_render_images(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image *imgs,
-		const jpegqs_cuda_status *status_dev, int layout, int grey_store, uint8_t *const *out_dev, void *stream);
+		const jpegqs_cuda_status *status_dev, int layout, int grey_store, int scale_denom, uint8_t *const *out_dev,
+		void *stream);
 
 /* ---- the packing kernel -------------------------------------------------------------------------
  * After encode_async, file k of a sub-batch sits at the start of its bound-sized slot.  One launch
@@ -576,9 +577,9 @@ static int host_read(const QsPlan &p, const uint8_t *data, size_t len, uint8_t *
 	return jpegqs_cuda_jpeg_read(data, len, &im);
 }
 
-static int pixels_batch(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len, int flags, int niter,
-		int layout, int on_device, uint8_t *const *out, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results) {
-	static const char who[] = "jpegqs_cuda_pixels_batch";
+static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int layout, int scale_denom, int on_device, uint8_t *const *out, size_t max_device_bytes, int *rc,
+		jpegqs_cuda_pixels_result *results) {
 	char msg[512];
 	cudaStream_t st;
 	std::vector<QsPlan> plans((size_t)n);
@@ -603,7 +604,9 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data,
 		if (p.host) { p.in_bytes = 0; p.ws_dec = 0; results[i].host_decoded = 1; results[i].reason = why; }
 		results[i].channels = p.img.ncomp;
 		TQ(plan_run(p, flags, niter));
-		p.pix = (size_t)p.img.image_width * p.img.image_height * p.img.ncomp;
+		/* the output at scale 1 / scale_denom: ceil(width / d) x ceil(height / d) x channels */
+		p.pix = (size_t)((p.img.image_width + scale_denom - 1) / scale_denom) * ((p.img.image_height + scale_denom - 1) / scale_denom)
+				* p.img.ncomp;
 		/* file, coefficients (+ up-sampled chroma), the rendered pixels when they come back to the host */
 		p.fixed = p.in_bytes + p.coef_bytes + p.up_bytes + (on_device ? 0 : align256(p.pix));
 		p.ws_enc = 0; p.packed = 0;
@@ -729,7 +732,7 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data,
 			TK(cudaEventRecord(t->ev1, st));
 		}
 		if (ms < nr) TK(cudaMemsetAsync(run + ms, 0, (size_t)(nr - ms) * sizeof(jpegqs_cuda_status), st));
-		if (nr) TQ(qs_render_images(ctx, nr, rimg.data(), run, layout, 1, outs.data(), st));
+		if (nr) TQ(qs_render_images(ctx, nr, rimg.data(), run, layout, 1, scale_denom, outs.data(), st));
 		/* the run statuses, and the pixels in the same copy when they come back to the host */
 		if (nr) TK(cudaMemcpyAsync(t->out_host.p, t->out_dev.p, pix_total, cudaMemcpyDeviceToHost, st));
 		TK(cudaStreamSynchronize(st));
@@ -753,21 +756,39 @@ fail:
 #undef TK
 #undef TQ
 
-extern "C" int jpegqs_cuda_pixels_batch(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
-		int flags, int niter, int layout, int out_on_device, uint8_t *const *out, size_t max_device_bytes, int *rc,
-		jpegqs_cuda_pixels_result *results) {
-	static const char who[] = "jpegqs_cuda_pixels_batch";
-	char msg[160];
+static int pixels_entry(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int layout, int scale_denom, int out_on_device, uint8_t *const *out, size_t max_device_bytes,
+		int *rc, jpegqs_cuda_pixels_result *results) {
+	char msg[200];
 	if (!ctx) return JPEGQS_ERR_ARG;
-	if (n < 0) { qs_ctx_decode_done(ctx, 0, "jpegqs_cuda_pixels_batch: negative file count"); return JPEGQS_ERR_ARG; }
+	if (n < 0) { snprintf(msg, sizeof(msg), "%s: negative file count", who); qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG; }
 	if (!n) return 0;
-	if (!data || !len || !out || !rc || !results) { qs_ctx_decode_done(ctx, 0, "jpegqs_cuda_pixels_batch: NULL argument"); return JPEGQS_ERR_ARG; }
+	if (!data || !len || !out || !rc || !results) { snprintf(msg, sizeof(msg), "%s: NULL argument", who); qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG; }
 	for (int i = 0; i < n; i++) if (!data[i] || !out[i]) {
 		snprintf(msg, sizeof(msg), "%s: file %d: NULL %s", who, i, data[i] ? "output" : "data");
 		qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG;
 	}
-	if (layout != JPEGQS_RENDER_HWC && layout != JPEGQS_RENDER_CHW) { qs_ctx_decode_done(ctx, 0, "jpegqs_cuda_pixels_batch: unknown layout"); return JPEGQS_ERR_ARG; }
-	if (out_on_device != 0 && out_on_device != 1) { qs_ctx_decode_done(ctx, 0, "jpegqs_cuda_pixels_batch: out_on_device must be 0 or 1"); return JPEGQS_ERR_ARG; }
+	if (layout != JPEGQS_RENDER_HWC && layout != JPEGQS_RENDER_CHW) { snprintf(msg, sizeof(msg), "%s: unknown layout", who); qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG; }
+	if (scale_denom != 1 && scale_denom != 2 && scale_denom != 4 && scale_denom != 8) {
+		snprintf(msg, sizeof(msg), "%s: scale_denom must be 1, 2, 4 or 8", who); qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG;
+	}
+	if (out_on_device != 0 && out_on_device != 1) {
+		snprintf(msg, sizeof(msg), "%s: out_on_device must be 0 or 1", who); qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG;
+	}
 	for (int i = 0; i < n; i++) { memset(&results[i], 0, sizeof(results[i])); results[i].reason = ""; rc[i] = 0; }
-	return pixels_batch(ctx, n, data, len, flags, niter, layout, out_on_device, out, max_device_bytes, rc, results);
+	return pixels_batch(ctx, who, n, data, len, flags, niter, layout, scale_denom, out_on_device, out, max_device_bytes, rc, results);
+}
+
+extern "C" int jpegqs_cuda_pixels_batch_scaled(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int layout, int scale_denom, int out_on_device, uint8_t *const *out, size_t max_device_bytes,
+		int *rc, jpegqs_cuda_pixels_result *results) {
+	return pixels_entry(ctx, "jpegqs_cuda_pixels_batch_scaled", n, data, len, flags, niter, layout, scale_denom, out_on_device,
+			out, max_device_bytes, rc, results);
+}
+
+extern "C" int jpegqs_cuda_pixels_batch(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int layout, int out_on_device, uint8_t *const *out, size_t max_device_bytes, int *rc,
+		jpegqs_cuda_pixels_result *results) {
+	return pixels_entry(ctx, "jpegqs_cuda_pixels_batch", n, data, len, flags, niter, layout, 1, out_on_device, out,
+			max_device_bytes, rc, results);
 }

@@ -178,6 +178,9 @@ def load():
                                           C.c_size_t, C.c_void_p, C.c_void_p]
     lib.jpegqs_cuda_render_async.argtypes = [C.c_void_p, C.c_int, C.POINTER(_Image), C.c_void_p, C.c_int,
                                              C.c_void_p, C.c_void_p]
+    lib.jpegqs_cuda_render_scaled_async.argtypes = [C.c_void_p, C.c_int, C.POINTER(_Image), C.c_void_p, C.c_int,
+                                                    C.c_int, C.c_void_p, C.c_void_p]
+    lib.jpegqs_cuda_render_model.argtypes = [C.POINTER(_Image), C.c_int, C.c_int, C.c_int, C.c_void_p]
     lib.jpegqs_cuda_jpeg_parse.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(_Image), C.POINTER(_Scan)]
     lib.jpegqs_cuda_jpeg_read.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(_Image)]
     lib.jpegqs_cuda_decode_workspace_bytes.argtypes = [C.c_int, C.POINTER(_Image), C.POINTER(_Scan),
@@ -214,6 +217,9 @@ def load():
     lib.jpegqs_cuda_pixels_batch.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_size_t), C.c_int,
                                              C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p), C.c_size_t,
                                              C.POINTER(C.c_int), C.POINTER(_PixelsResult)]
+    lib.jpegqs_cuda_pixels_batch_scaled.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_size_t),
+                                                    C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p),
+                                                    C.c_size_t, C.POINTER(C.c_int), C.POINTER(_PixelsResult)]
     lib.jpegqs_cuda_tables.argtypes = [C.c_int, C.c_void_p]
     lib.jpegqs_cuda_orig_coef.argtypes = [C.c_int, C.c_int]
     _lib = lib
@@ -272,6 +278,21 @@ class PinnedArray:
             self.close()
         except Exception:
             pass
+
+
+SCALE_DENOMS = (1, 2, 4, 8)
+
+
+def _scale_denom(d, who: str) -> int:
+    if isinstance(d, bool) or not isinstance(d, (int, np.integer)) or int(d) not in SCALE_DENOMS:
+        raise ValueError(f"{who}: scale_denom {d!r}: expected 1, 2, 4 or 8")
+    return int(d)
+
+
+def _scaled_shape(width: int, height: int, channels: int, layout: str, d: int):
+    """libjpeg's output size at scale 1/d: ceil(width / d) x ceil(height / d)"""
+    w, h = -(-int(width) // d), -(-int(height) // d)
+    return (h, w, channels) if layout == "hwc" else (channels, h, w)
 
 
 def _fill_image(ci: _Image, image: CoefImage, coef_ptrs: Sequence[int], up_ptrs: Sequence[Optional[int]]):
@@ -381,6 +402,37 @@ def decode_workspace_bytes(images: Sequence[CoefImage], scans, data_len: Sequenc
     if lib.jpegqs_cuda_decode_workspace_bytes(n, arr, sc, lens, C.byref(out)) < 0:
         raise QsError(lib.jpegqs_cuda_last_error(None).decode())
     return int(out.value)
+
+
+def render_model(image: CoefImage, upsampled=False, layout: str = "hwc", scale_denom: int = 1):
+    """render_async's algorithm on one CPU thread for one image (jpegqs_cuda_render_model): libjpeg's
+    islow / reduced IDCTs, up-sampling and colour conversion at scale 1/scale_denom.  upsampled: None /
+    False reads the image's own arrays; otherwise a pair of int16 numpy arrays [hblk, wblk, 64] at
+    component 0's geometry, read for components 1 and 2.  Returns a uint8 numpy array [H, W, 3] ("hwc")
+    or [3, H, W] ("chw"), H = ceil(height / d) and W = ceil(width / d)."""
+    if layout not in ("hwc", "chw"):
+        raise ValueError(f"render_model: layout {layout!r}: expected 'hwc' or 'chw'")
+    d = _scale_denom(scale_denom, "render_model")
+    lib = load()
+    arrays = [np.ascontiguousarray(c.coef, dtype=np.int16) for c in image.comps]
+    for c, a in zip(image.comps, arrays):
+        if a.shape != (c.hblk, c.wblk, 64):
+            raise ValueError(f"render_model: a coefficient array of shape {a.shape}, expected {(c.hblk, c.wblk, 64)}")
+    ups = []
+    if upsampled is not None and upsampled is not False:
+        if len(upsampled) != 2 or len(image.comps) != 3:
+            raise ValueError("render_model: upsampled must be two arrays for a three-component image")
+        y = image.comps[0]
+        ups = [np.ascontiguousarray(u, dtype=np.int16) for u in upsampled]
+        if any(u.shape != (y.hblk, y.wblk, 64) for u in ups):
+            raise ValueError(f"render_model: up-sampled arrays must have component 0's shape {(y.hblk, y.wblk, 64)}")
+    ci = _Image()
+    _fill_image(ci, image, [a.ctypes.data for a in arrays], [None] + [u.ctypes.data for u in ups] if ups else [])
+    out = np.zeros(_scaled_shape(image.width, image.height, 3, layout, d), dtype=np.uint8)
+    rc = lib.jpegqs_cuda_render_model(C.byref(ci), int(bool(ups)), 0 if layout == "hwc" else 1, d, out.ctypes.data)
+    if rc < 0:
+        raise QsError(f"render_model: {lib.jpegqs_cuda_last_error(None).decode()} ({rc})")
+    return out
 
 
 def decode_model(image: CoefImage, scan, data: bytes, sub_bytes: int = DECODE_SUB_DEFAULT, out=None):
@@ -697,7 +749,7 @@ class QsContext:
         return out
 
     def decode_pixels(self, datas, flags: int, niter: int, layout: str = "hwc", device: str = "cuda",
-                      max_device_bytes: int = 0):
+                      max_device_bytes: int = 0, scale_denom: int = 1):
         """Many JPEG files to the smoothed pixels the jpegqs tool's --ppm writes for them (islow, fancy
         up-sampling, after do_quantsmooth(flags, niter)), in shared launches (jpegqs_cuda_pixels_batch).
         Returns, in the order of datas, one record per file:
@@ -708,7 +760,10 @@ class QsContext:
         host_decoded / reason: whether and why the host reader decoded the file.  Raises TypeError for a
         non-bytes entry or a bare bytes object, ValueError for an unknown layout or device or a negative
         max_device_bytes, and QsError naming the index of a file the reader rejects or the render
-        cannot take (1 or 3 components, integral sampling ratios)."""
+        cannot take (1 or 3 components, integral sampling ratios).
+        scale_denom 2, 4 or 8: libjpeg's scaled decode of the same coefficients at 1/d size
+        (jpegqs_cuda_pixels_batch_scaled); pixels are then [ceil(H/d), ceil(W/d), C] or
+        [C, ceil(H/d), ceil(W/d)].  ValueError for any other value than 1, 2, 4 or 8."""
         if isinstance(datas, (bytes, bytearray, memoryview, str)) or not hasattr(datas, "__len__"):
             raise TypeError("decode_pixels: datas must be a sequence of bytes-like files")
         files = [_file_bytes(d, f"decode_pixels: file {i}") for i, d in enumerate(datas)]
@@ -718,6 +773,7 @@ class QsContext:
             raise ValueError(f"decode_pixels: device {device!r}: expected 'cuda' or 'cpu'")
         if int(max_device_bytes) < 0:
             raise ValueError("decode_pixels: max_device_bytes must be >= 0")
+        scale = _scale_denom(scale_denom, "decode_pixels")
         n = len(files)
         if not n:
             return []
@@ -731,7 +787,7 @@ class QsContext:
             if info.ncomp not in (1, 3):
                 raise QsError(f"decode_pixels: file {i}: {info.ncomp} components; the render takes 1 or 3")
             c, h, w = info.ncomp, info.image_height, info.image_width
-            shapes.append((h, w, c) if layout == "hwc" else (c, h, w))
+            shapes.append(_scaled_shape(w, h, c, layout, scale))
         if device == "cuda":
             dev = self.device if self.device >= 0 else torch.cuda.current_device()
             outs = [torch.empty(s, dtype=torch.uint8, device=dev) for s in shapes]
@@ -744,9 +800,14 @@ class QsContext:
         optrs = (C.c_void_p * n)(*[t.data_ptr() for t in outs])
         rc = (C.c_int * n)()
         res = (_PixelsResult * n)()
-        self._check(self.lib.jpegqs_cuda_pixels_batch(self.h, n, ptrs, lens, int(flags), int(niter),
-                                                      0 if layout == "hwc" else 1, int(device == "cuda"), optrs,
-                                                      int(max_device_bytes), rc, res))
+        if scale == 1:
+            self._check(self.lib.jpegqs_cuda_pixels_batch(self.h, n, ptrs, lens, int(flags), int(niter),
+                                                          0 if layout == "hwc" else 1, int(device == "cuda"), optrs,
+                                                          int(max_device_bytes), rc, res))
+        else:
+            self._check(self.lib.jpegqs_cuda_pixels_batch_scaled(self.h, n, ptrs, lens, int(flags), int(niter),
+                                                                 0 if layout == "hwc" else 1, scale, int(device == "cuda"),
+                                                                 optrs, int(max_device_bytes), rc, res))
         for i in range(n):
             if rc[i] == -2:
                 raise QsError(f"decode_pixels: file {i}: {self.lib.jpegqs_cuda_last_error(self.h).decode()}")
@@ -936,7 +997,7 @@ class QsContext:
 
     # ---- stream-ordered render to RGB (include/jpegqs_cuda.h jpegqs_cuda_render_async) ----
     def render_async(self, images: Sequence[CoefImage], coefs, status=None, up=None, layout: str = "hwc",
-                     out=None, stream=None):
+                     out=None, stream=None, scale_denom: int = 1):
         """Decode device-resident coefficients to 8-bit RGB, as libjpeg would, without blocking the
         calling thread.  The coefficient tensors are only read.
 
@@ -947,11 +1008,14 @@ class QsContext:
         layout: "hwc" gives uint8 [H, W, 3] per image, "chw" gives [3, H, W].  out: a sequence of
         per-image uint8 CUDA tensors of that shape to write (a batched tensor's unbind(0) will do);
         by default they are allocated on the stream.  stream: a torch.cuda.Stream (default: the
-        current one).  Capturable with torch.cuda.graph.  Returns the list of output tensors."""
+        current one).  scale_denom 2, 4 or 8: libjpeg's scaled decode (jpegqs_cuda_render_scaled_async),
+        H and W then being ceil(height / d) and ceil(width / d).  Capturable with torch.cuda.graph.
+        Returns the list of output tensors."""
         import torch
         n = len(images)
         if layout not in ("hwc", "chw"):
             raise ValueError(f"layout {layout!r}: expected 'hwc' or 'chw'")
+        d = _scale_denom(scale_denom, "render_async")
         if len(coefs) != n or (up is not None and len(up) != n) or (out is not None and len(out) != n):
             raise ValueError("images, coefs, up and out must have one entry per image")
         host_up = None
@@ -980,7 +1044,7 @@ class QsContext:
             if status.dtype != torch.int32 or tuple(status.shape) != (n, 2) or not status.is_contiguous():
                 raise ValueError(f"status: expected a contiguous int32 tensor [{n}, 2]")
             tensors.append(("status", status))
-        shapes = [(im.height, im.width, 3) if layout == "hwc" else (3, im.height, im.width) for im in images]
+        shapes = [_scaled_shape(im.width, im.height, 3, layout, d) for im in images]
         if out is not None:
             for i, t in enumerate(out):
                 if not isinstance(t, torch.Tensor):
@@ -1008,9 +1072,13 @@ class QsContext:
             for i in range(n):
                 arr[i].upsampled = int(bool(host_up and host_up[i]))
             outs = (C.c_void_p * max(n, 1))(*[t.data_ptr() for t in out])
-            self._check(self.lib.jpegqs_cuda_render_async(
-                self.h, n, arr, status.data_ptr() if isinstance(status, torch.Tensor) else None,
-                0 if layout == "hwc" else 1, outs, _stream_handle(stream)))
+            st = status.data_ptr() if isinstance(status, torch.Tensor) else None
+            if d == 1:
+                self._check(self.lib.jpegqs_cuda_render_async(self.h, n, arr, st, 0 if layout == "hwc" else 1, outs,
+                                                              _stream_handle(stream)))
+            else:
+                self._check(self.lib.jpegqs_cuda_render_scaled_async(self.h, n, arr, st, 0 if layout == "hwc" else 1, d,
+                                                                     outs, _stream_handle(stream)))
         return out
 
     # ---- JPEG bytes to coefficients (include/jpegqs_cuda.h jpegqs_cuda_decode_async) ----
@@ -1466,15 +1534,15 @@ def decode_async(images: Sequence[CoefImage], scans, data, out=None, stream=None
 
 
 def render_async(images: Sequence[CoefImage], coefs, status=None, up=None, layout: str = "hwc", out=None,
-                 stream=None):
+                 stream=None, scale_denom: int = 1):
     """QsContext.render_async on the default context of the tensors' device: decodes CUDA
-    coefficient tensors to uint8 RGB tensors ([H, W, 3] or [3, H, W]), enqueued on `stream`
-    (default: the current one) without waiting."""
+    coefficient tensors to uint8 RGB tensors ([H, W, 3] or [3, H, W], at 1/scale_denom size),
+    enqueued on `stream` (default: the current one) without waiting."""
     import torch
     first = next((t for ts in coefs for t in ts), None)
     if not isinstance(first, torch.Tensor) or not first.is_cuda:
         raise ValueError("render_async: the coefficient tensors must be CUDA tensors")
-    return default_context(first.device.index).render_async(images, coefs, status, up, layout, out, stream)
+    return default_context(first.device.index).render_async(images, coefs, status, up, layout, out, stream, scale_denom)
 
 
 def encode_async(images: Sequence[CoefImage], coefs, heads, optimize: bool = False, status=None, up=None, out=None,
@@ -1504,7 +1572,7 @@ def transcode_batch(datas, flags: int, niter: int, optimize: bool = False, copy:
 
 
 def decode_pixels(datas, flags: int, niter: int, layout: str = "hwc", device: str = "cuda", max_device_bytes: int = 0,
-                  gpu: int = -1):
+                  gpu: int = -1, scale_denom: int = 1):
     """QsContext.decode_pixels on the default context of CUDA device `gpu`: one record (pixels, warnings,
-    host_decoded, smoothed, stop, upsampled, reason) per file."""
-    return default_context(gpu).decode_pixels(datas, flags, niter, layout, device, max_device_bytes)
+    host_decoded, smoothed, stop, upsampled, reason) per file, at 1/scale_denom size."""
+    return default_context(gpu).decode_pixels(datas, flags, niter, layout, device, max_device_bytes, scale_denom)
