@@ -655,6 +655,50 @@ int jpegqs_cuda_pixels_batch_scaled(jpegqs_cuda_ctx *ctx, int n, const uint8_t *
 		int flags, int niter, int layout, int scale_denom, int out_on_device, uint8_t *const *out,
 		size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results);
 
+/* ---- the same files cropped and resized: Pillow's Image.resize, byte for byte --------------------
+ * File i's output is exactly what Pillow gives for
+ *     Image.fromarray(P).crop((left, top, right, bottom)).resize((width, height), filter)
+ * where P is what jpegqs_cuda_pixels_batch_scaled gives for the file at the same scale_denom, as an
+ * 'RGB' picture, or 'L' for a grey file.  The filters are Pillow's convolution filters, numbered as
+ * its Image.Resampling; NEAREST (0) takes another code path in Pillow and is rejected.
+ *   - Output size.  out[i] holds exactly width * height * channels bytes in layout HWC or CHW, with
+ *     channels as for jpegqs_cuda_pixels_batch.  With host outputs each file's share of the budget and
+ *     of the download is its resized size.
+ *   - Everything else - routes, sub-batches, warnings, host_decoded, smoothed, stop, upsampled - is
+ *     pixels_batch_scaled's for the same files.
+ *   - Arithmetic.  Pillow's (Resample.c): per axis, weights computed in double on the host and rounded
+ *     to int32 with 22 fractional bits; a horizontal pass over the rows the vertical pass reads, into
+ *     an 8-bit intermediate, then the vertical pass; each output byte is clip8(2^21 + sum src * k).
+ *   - Per sub-batch: the render writes each file's 1/scale_denom picture (HWC) to a context buffer;
+ *     one upload carries the resize descriptors and weight tables; two launches over all the files
+ *     write the outputs.  The budget counts the picture, the intermediate and the tables of each file,
+ *     and with host outputs the resized bytes.
+ *   - Per file, rc[i]: as pixels_batch_scaled's, and JPEGQS_ERR_ARG for a crop outside the file's
+ *     1/scale_denom picture, or an empty one (jpegqs_cuda_last_error(ctx) names the file); out[i] is
+ *     then untouched and no other file changes.
+ *   - Return.  As pixels_batch_scaled's; also JPEGQS_ERR_ARG with nothing done for boxes NULL, a
+ *     filter other than the five below, or a width or height outside 1..65535. */
+#define JPEGQS_RESIZE_LANCZOS  1   /* Pillow's Image.Resampling values */
+#define JPEGQS_RESIZE_BILINEAR 2
+#define JPEGQS_RESIZE_BICUBIC  3
+#define JPEGQS_RESIZE_BOX      4
+#define JPEGQS_RESIZE_HAMMING  5
+typedef struct {
+	int32_t left, top, right, bottom;  /* crop in the 1/scale_denom picture; all 0: the whole picture */
+	int32_t width, height;             /* output size */
+} jpegqs_cuda_resize_box;
+int jpegqs_cuda_pixels_batch_resized(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int layout, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
+		int out_on_device, uint8_t *const *out, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results);
+
+/* The resize of jpegqs_cuda_pixels_batch_resized on the calling thread, for one picture (host-only, no
+ * device needed): the same weight tables and per-pixel arithmetic.  src: width x height x channels
+ * bytes, HWC; channels 1 or 3.  out: box->width * box->height * channels bytes in layout HWC or CHW.
+ * Returns 0, or JPEGQS_ERR_ARG (NULL pointer, bad size, channels, layout or filter, a crop outside
+ * the picture or empty); jpegqs_cuda_last_error(NULL) says why. */
+int jpegqs_cuda_resize_model(const uint8_t *src, int width, int height, int channels, int layout, int filter,
+		const jpegqs_cuda_resize_box *box, uint8_t *out);
+
 /* ---- one image sharded by MCU rows over several GPUs (SURVEY.md 8e) ----------------------
  * Every rank - a device of this process, or another process on the same box - smooths one slab
  * of contiguous MCU rows and exchanges ONE pixel row per plane with each neighbour after every

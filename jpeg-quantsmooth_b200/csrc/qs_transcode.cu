@@ -6,7 +6,8 @@
  * qs_encode.cu, reached through their public entry points; the one kernel here packs the encoded
  * files into one buffer so that a sub-batch comes back in one copy.
  * jpegqs_cuda_pixels_batch: the same files to the smoothed pixels the tool's --ppm writes, through
- * the same plans, sub-batches and decoder launches, the host reader, run_async and the fused render.
+ * the same plans, sub-batches and decoder launches, the host reader, run_async and the fused render;
+ * jpegqs_cuda_pixels_batch_resized adds qs_resize.cu's crop and resize after the render.
  */
 #include <cuda_runtime.h>
 #include <stdio.h>
@@ -15,6 +16,7 @@
 #include <vector>
 #include "jpegqs_cuda.h"
 #include "qs_common.h"
+#include "qs_resize.h"
 
 /* include/libjpegqs.h's JPEGQS_FLAGS_MASK and JPEGQS_ITER_MAX (that header needs <jpeglib.h>) */
 #define QS_FLAGS_MASK 0x7f
@@ -122,6 +124,8 @@ struct QsTranscode {
 	QsBuf stat_dev;                            /* per-file status words and the records of the packing kernel */
 	QsBuf in_host, out_host, stat_host;        /* pinned staging of the upload and the two downloads */
 	QsBuf hcoef_dev, hcoef_host;               /* pixels: the host-decoded files' coefficients and their staging */
+	QsBuf rs_dev, rs_host;                     /* resized pixels: descriptors + weight tables, intermediates,
+	                                              rendered pictures; the staging of the descriptors and tables */
 	cudaEvent_t ev0, ev1;                      /* around run_async: jpegqs_cuda_last_device_ms */
 	int sms;
 	jpegqs_cuda_scan_rec recs[JPEGQS_MAX_SCANS];
@@ -134,11 +138,12 @@ void qs_transcode_release(void *state) {
 	QsTranscode *t = (QsTranscode*)state;
 	if (!t) return;
 	cudaFree(t->in_dev.p); cudaFree(t->coef_dev.p); cudaFree(t->ws_dev.p); cudaFree(t->out_dev.p); cudaFree(t->stat_dev.p);
-	cudaFree(t->hcoef_dev.p);
+	cudaFree(t->hcoef_dev.p); cudaFree(t->rs_dev.p);
 	if (t->in_host.p) cudaFreeHost(t->in_host.p);
 	if (t->out_host.p) cudaFreeHost(t->out_host.p);
 	if (t->stat_host.p) cudaFreeHost(t->stat_host.p);
 	if (t->hcoef_host.p) cudaFreeHost(t->hcoef_host.p);
+	if (t->rs_host.p) cudaFreeHost(t->rs_host.p);
 	if (t->ev0) cudaEventDestroy(t->ev0);
 	if (t->ev1) cudaEventDestroy(t->ev1);
 	delete t;
@@ -256,7 +261,8 @@ static cudaError_t batch_budget(const QsTranscode *t, size_t max_device_bytes, s
 	if (max_device_bytes) return cudaSuccess;
 	size_t fr = 0, tot = 0;
 	cudaError_t e = cudaMemGetInfo(&fr, &tot);
-	*budget = (fr + t->in_dev.cap + t->coef_dev.cap + t->ws_dev.cap + t->out_dev.cap + t->stat_dev.cap + t->hcoef_dev.cap) / 2;
+	*budget = (fr + t->in_dev.cap + t->coef_dev.cap + t->ws_dev.cap + t->out_dev.cap + t->stat_dev.cap + t->hcoef_dev.cap +
+			t->rs_dev.cap) / 2;
 	return e;
 }
 
@@ -577,12 +583,15 @@ static int host_read(const QsPlan &p, const uint8_t *data, size_t len, uint8_t *
 	return jpegqs_cuda_jpeg_read(data, len, &im);
 }
 
+/* boxes != NULL: each file's picture is cropped and resized (qs_resize.cu) with filter */
 static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint8_t *const *data, const size_t *len,
-		int flags, int niter, int layout, int scale_denom, int on_device, uint8_t *const *out, size_t max_device_bytes, int *rc,
-		jpegqs_cuda_pixels_result *results) {
+		int flags, int niter, int layout, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes, int on_device,
+		uint8_t *const *out, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results) {
 	char msg[512];
 	cudaStream_t st;
 	std::vector<QsPlan> plans((size_t)n);
+	std::vector<QsResizePlan> rsp(boxes ? (size_t)n : 0);
+	std::vector<size_t> pic(boxes ? (size_t)n : 0);  /* resized files: the rendered picture's bytes */
 	int ret = 0;
 	{
 	QsTranscode *t = NULL;
@@ -600,15 +609,30 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 			rc[i] = JPEGQS_ERR_ARG; continue;
 		}
 		if (!qs_render_takes(&p.img)) { rc[i] = JPEGQS_ERR_UNSUPPORTED; continue; }
+		/* the picture at scale 1 / scale_denom: ceil(width / d) x ceil(height / d) x channels */
+		const int pw = (int)((p.img.image_width + scale_denom - 1) / scale_denom);
+		const int ph = (int)((p.img.image_height + scale_denom - 1) / scale_denom);
+		p.pix = (size_t)pw * ph * p.img.ncomp;
+		if (boxes) {
+			const char *bad = qs_resize_plan(pw, ph, boxes[i], filter, rsp[i]);
+			if (bad) {
+				snprintf(msg, sizeof(msg), "%s: file %d: %s (picture %d x %d)", who, i, bad, pw, ph);
+				qs_ctx_decode_done(ctx, 0, msg);
+				rc[i] = JPEGQS_ERR_ARG; continue;
+			}
+			pic[i] = p.pix;
+			p.pix = (size_t)boxes[i].width * boxes[i].height * p.img.ncomp;
+		}
 		p.host = route != JPEGQS_ROUTE_DEVICE;
 		if (p.host) { p.in_bytes = 0; p.ws_dec = 0; results[i].host_decoded = 1; results[i].reason = why; }
 		results[i].channels = p.img.ncomp;
 		TQ(plan_run(p, flags, niter));
-		/* the output at scale 1 / scale_denom: ceil(width / d) x ceil(height / d) x channels */
-		p.pix = (size_t)((p.img.image_width + scale_denom - 1) / scale_denom) * ((p.img.image_height + scale_denom - 1) / scale_denom)
-				* p.img.ncomp;
-		/* file, coefficients (+ up-sampled chroma), the rendered pixels when they come back to the host */
+		/* file, coefficients (+ up-sampled chroma), the output pixels when they come back to the host;
+		 * resized: also the rendered picture, the intermediate, the tables and the descriptor */
 		p.fixed = p.in_bytes + p.coef_bytes + p.up_bytes + (on_device ? 0 : align256(p.pix));
+		if (boxes)
+			p.fixed += align256(pic[i]) + align256((size_t)rsp[i].mid_h * rsp[i].out_w * p.img.ncomp) +
+					align256(rsp[i].tab.size() * sizeof(int32_t)) + align256(sizeof(QsResizeDesc));
 		p.ws_enc = 0; p.packed = 0;
 		p.go = 1;
 	}
@@ -726,13 +750,44 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 		jpegqs_cuda_status *run = (jpegqs_cuda_status*)t->out_dev.p;
 		std::vector<uint8_t*> outs(nr);
 		for (int j = 0; j < nr; j++) outs[j] = on_device ? out[files[rk[j]]] : (uint8_t*)t->out_dev.p + poff[j];
+		/* resized: the render writes each picture into rs_dev, which holds the descriptors and tables (one
+		 * upload from rs_host), then the intermediates, then the pictures; the resize writes outs */
+		uint32_t hblocks = 0, vblocks = 0;
+		if (boxes && nr) {
+			size_t up = align256(sizeof(QsResizeDesc) * (size_t)nr), all;
+			std::vector<size_t> toff(nr), moff(nr), qoff(nr);
+			for (int j = 0; j < nr; j++) { toff[j] = up; up += align256(rsp[files[rk[j]]].tab.size() * sizeof(int32_t)); }
+			all = up;
+			for (int j = 0; j < nr; j++) {
+				const QsResizePlan &r = rsp[files[rk[j]]];
+				moff[j] = all; all += align256((size_t)r.mid_h * r.out_w * rimg[j].ncomp);
+			}
+			for (int j = 0; j < nr; j++) { qoff[j] = all; all += align256(pic[files[rk[j]]]); }
+			TK(grow_dev(&t->rs_dev, all));
+			TK(grow_host(&t->rs_host, up));
+			uint8_t *rd = (uint8_t*)t->rs_dev.p, *rh = (uint8_t*)t->rs_host.p;
+			QsResizeDesc *desc = (QsResizeDesc*)rh;
+			for (int j = 0; j < nr; j++) {
+				const int f = files[rk[j]];
+				const QsResizePlan &r = rsp[f];
+				const int pw = (int)((rimg[j].image_width + scale_denom - 1) / scale_denom);
+				qs_resize_desc(r, pw, rimg[j].ncomp, layout == JPEGQS_RENDER_CHW, desc[j]);
+				memcpy(rh + toff[j], r.tab.data(), r.tab.size() * sizeof(int32_t));
+				desc[j].src = rd + qoff[j]; desc[j].mid = rd + moff[j]; desc[j].out = outs[j];
+				desc[j].tab = (const int32_t*)(rd + toff[j]);
+				outs[j] = rd + qoff[j];
+			}
+			qs_resize_number(desc, nr, &hblocks, &vblocks);
+			TK(cudaMemcpyAsync(rd, rh, up, cudaMemcpyHostToDevice, st));
+		}
 		if (ms) {
 			TK(cudaEventRecord(t->ev0, st));
 			TQ(jpegqs_cuda_run_async(ctx, ms, rimg.data(), rflags, niter, t->ws_dev.p, t->ws_dev.cap, run, st));
 			TK(cudaEventRecord(t->ev1, st));
 		}
 		if (ms < nr) TK(cudaMemsetAsync(run + ms, 0, (size_t)(nr - ms) * sizeof(jpegqs_cuda_status), st));
-		if (nr) TQ(qs_render_images(ctx, nr, rimg.data(), run, layout, 1, scale_denom, outs.data(), st));
+		if (nr) TQ(qs_render_images(ctx, nr, rimg.data(), run, boxes ? JPEGQS_RENDER_HWC : layout, 1, scale_denom, outs.data(), st));
+		if (boxes && nr) TK(qs_launch_resize((const QsResizeDesc*)t->rs_dev.p, nr, hblocks, vblocks, st));
 		/* the run statuses, and the pixels in the same copy when they come back to the host */
 		if (nr) TK(cudaMemcpyAsync(t->out_host.p, t->out_dev.p, pix_total, cudaMemcpyDeviceToHost, st));
 		TK(cudaStreamSynchronize(st));
@@ -756,9 +811,10 @@ fail:
 #undef TK
 #undef TQ
 
+/* resize != 0: jpegqs_cuda_pixels_batch_resized, with filter and boxes */
 static int pixels_entry(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint8_t *const *data, const size_t *len,
-		int flags, int niter, int layout, int scale_denom, int out_on_device, uint8_t *const *out, size_t max_device_bytes,
-		int *rc, jpegqs_cuda_pixels_result *results) {
+		int flags, int niter, int layout, int scale_denom, int resize, int filter, const jpegqs_cuda_resize_box *boxes,
+		int out_on_device, uint8_t *const *out, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results) {
 	char msg[200];
 	if (!ctx) return JPEGQS_ERR_ARG;
 	if (n < 0) { snprintf(msg, sizeof(msg), "%s: negative file count", who); qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG; }
@@ -775,20 +831,39 @@ static int pixels_entry(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 	if (out_on_device != 0 && out_on_device != 1) {
 		snprintf(msg, sizeof(msg), "%s: out_on_device must be 0 or 1", who); qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG;
 	}
+	if (resize) {
+		if (!boxes) { snprintf(msg, sizeof(msg), "%s: boxes NULL", who); qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG; }
+		if (!qs_resize_filter_ok(filter)) {
+			snprintf(msg, sizeof(msg), "%s: filter %d: expected LANCZOS (1), BILINEAR (2), BICUBIC (3), BOX (4) or HAMMING (5)", who, filter);
+			qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG;
+		}
+		for (int i = 0; i < n; i++) if (boxes[i].width < 1 || boxes[i].width > 65535 || boxes[i].height < 1 || boxes[i].height > 65535) {
+			snprintf(msg, sizeof(msg), "%s: file %d: output size %d x %d outside 1..65535", who, i, boxes[i].width, boxes[i].height);
+			qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG;
+		}
+	}
 	for (int i = 0; i < n; i++) { memset(&results[i], 0, sizeof(results[i])); results[i].reason = ""; rc[i] = 0; }
-	return pixels_batch(ctx, who, n, data, len, flags, niter, layout, scale_denom, out_on_device, out, max_device_bytes, rc, results);
+	return pixels_batch(ctx, who, n, data, len, flags, niter, layout, scale_denom, filter, resize ? boxes : NULL, out_on_device, out,
+			max_device_bytes, rc, results);
+}
+
+extern "C" int jpegqs_cuda_pixels_batch_resized(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int layout, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes, int out_on_device,
+		uint8_t *const *out, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results) {
+	return pixels_entry(ctx, "jpegqs_cuda_pixels_batch_resized", n, data, len, flags, niter, layout, scale_denom, 1, filter, boxes,
+			out_on_device, out, max_device_bytes, rc, results);
 }
 
 extern "C" int jpegqs_cuda_pixels_batch_scaled(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
 		int flags, int niter, int layout, int scale_denom, int out_on_device, uint8_t *const *out, size_t max_device_bytes,
 		int *rc, jpegqs_cuda_pixels_result *results) {
-	return pixels_entry(ctx, "jpegqs_cuda_pixels_batch_scaled", n, data, len, flags, niter, layout, scale_denom, out_on_device,
-			out, max_device_bytes, rc, results);
+	return pixels_entry(ctx, "jpegqs_cuda_pixels_batch_scaled", n, data, len, flags, niter, layout, scale_denom, 0, 0, NULL,
+			out_on_device, out, max_device_bytes, rc, results);
 }
 
 extern "C" int jpegqs_cuda_pixels_batch(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
 		int flags, int niter, int layout, int out_on_device, uint8_t *const *out, size_t max_device_bytes, int *rc,
 		jpegqs_cuda_pixels_result *results) {
-	return pixels_entry(ctx, "jpegqs_cuda_pixels_batch", n, data, len, flags, niter, layout, 1, out_on_device, out,
+	return pixels_entry(ctx, "jpegqs_cuda_pixels_batch", n, data, len, flags, niter, layout, 1, 0, 0, NULL, out_on_device, out,
 			max_device_bytes, rc, results);
 }

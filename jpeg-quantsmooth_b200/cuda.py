@@ -94,6 +94,11 @@ ROUTE_HOST, ROUTE_DEVICE = 0, 1
 TRANSCODE_OK, TRANSCODE_FALLBACK = 0, 1
 
 
+class _ResizeBox(C.Structure):
+    _fields_ = [("left", C.c_int32), ("top", C.c_int32), ("right", C.c_int32), ("bottom", C.c_int32),
+                ("width", C.c_int32), ("height", C.c_int32)]
+
+
 class _Job(C.Structure):
     _fields_ = [("coef", C.c_void_p), ("plane", C.c_void_p), ("plane2", C.c_void_p),
                 ("wblk", C.c_uint32), ("hblk", C.c_uint32), ("quant", C.c_uint16 * 64),
@@ -220,6 +225,12 @@ def load():
     lib.jpegqs_cuda_pixels_batch_scaled.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_size_t),
                                                     C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p),
                                                     C.c_size_t, C.POINTER(C.c_int), C.POINTER(_PixelsResult)]
+    lib.jpegqs_cuda_pixels_batch_resized.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_size_t),
+                                                     C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(_ResizeBox),
+                                                     C.c_int, C.POINTER(C.c_void_p), C.c_size_t, C.POINTER(C.c_int),
+                                                     C.POINTER(_PixelsResult)]
+    lib.jpegqs_cuda_resize_model.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                             C.POINTER(_ResizeBox), C.c_void_p]
     lib.jpegqs_cuda_tables.argtypes = [C.c_int, C.c_void_p]
     lib.jpegqs_cuda_orig_coef.argtypes = [C.c_int, C.c_int]
     _lib = lib
@@ -293,6 +304,68 @@ def _scaled_shape(width: int, height: int, channels: int, layout: str, d: int):
     """libjpeg's output size at scale 1/d: ceil(width / d) x ceil(height / d)"""
     w, h = -(-int(width) // d), -(-int(height) // d)
     return (h, w, channels) if layout == "hwc" else (channels, h, w)
+
+
+# Pillow's convolution filters, by name, with its Image.Resampling numbers (NEAREST, 0, is not one)
+RESIZE_FILTERS = {"lanczos": 1, "bilinear": 2, "bicubic": 3, "box": 4, "hamming": 5}
+
+
+def _resize_filter(f, who: str) -> int:
+    """a filter name, or Pillow's Image.Resampling value of one of the five convolution filters"""
+    if isinstance(f, str) and f.lower() in RESIZE_FILTERS:
+        return RESIZE_FILTERS[f.lower()]
+    if not isinstance(f, (str, bool)) and isinstance(f, (int, np.integer)) and int(f) in RESIZE_FILTERS.values():
+        return int(f)
+    raise ValueError(f"{who}: filter {f!r}: expected one of {', '.join(RESIZE_FILTERS)} (Pillow's BOX, BILINEAR, "
+                     "HAMMING, BICUBIC, LANCZOS; NEAREST is not supported)")
+
+
+def _int_tuple(v, k: int):
+    if isinstance(v, (str, bytes)) or not hasattr(v, "__len__") or len(v) != k:
+        return None
+    if any(isinstance(x, bool) or not isinstance(x, (int, np.integer)) for x in v):
+        return None
+    return tuple(int(x) for x in v)
+
+
+def _resize_boxes(n: int, size, crop, who: str):
+    """Per file, (size, crop): size (width, height) or None, crop (left, top, right, bottom) or None,
+    checked for form; ValueError names the file index"""
+    def one_size(v, i):
+        t = _int_tuple(v, 2)
+        if t is None or not (1 <= t[0] <= 65535 and 1 <= t[1] <= 65535):
+            raise ValueError(f"{who}: file {i}: size {v!r}: expected (width, height), each in 1..65535")
+        return t
+    if size is None:
+        sizes = [None] * n
+    elif _int_tuple(size, 2) is not None:
+        sizes = [one_size(size, i) for i in range(n)]
+    elif isinstance(size, (list, tuple)) and len(size) == n:
+        sizes = [one_size(v, i) for i, v in enumerate(size)]
+    else:
+        raise ValueError(f"{who}: size must be (width, height) or a list of {n} of them")
+    if crop is None:
+        crops = [None] * n
+    elif isinstance(crop, (list, tuple)) and len(crop) == n:
+        crops = []
+        for i, v in enumerate(crop):
+            t = None if v is None else _int_tuple(v, 4)
+            if v is not None and (t is None or min(t) < 0 or t[0] >= t[2] or t[1] >= t[3]):
+                raise ValueError(f"{who}: file {i}: crop {v!r}: expected (left, top, right, bottom) with "
+                                 "0 <= left < right and 0 <= top < bottom")
+            crops.append(t)
+    else:
+        raise ValueError(f"{who}: crop must be None or a list of {n} (left, top, right, bottom) boxes or None")
+    return sizes, crops
+
+
+def _resize_box(pw: int, ph: int, size, crop, i: int, who: str) -> _ResizeBox:
+    """the C box of file i, whose picture is pw x ph: crop None is the whole picture; size None is the crop's"""
+    left, top, right, bottom = crop if crop is not None else (0, 0, pw, ph)
+    if right > pw or bottom > ph:
+        raise ValueError(f"{who}: file {i}: crop {crop!r} outside the {pw} x {ph} picture")
+    w, h = size if size is not None else (right - left, bottom - top)
+    return _ResizeBox(left, top, right, bottom, w, h)
 
 
 def _fill_image(ci: _Image, image: CoefImage, coef_ptrs: Sequence[int], up_ptrs: Sequence[Optional[int]]):
@@ -433,6 +506,36 @@ def render_model(image: CoefImage, upsampled=False, layout: str = "hwc", scale_d
     if rc < 0:
         raise QsError(f"render_model: {lib.jpegqs_cuda_last_error(None).decode()} ({rc})")
     return out
+
+
+def resize_model(pixels, size, crop=None, filter="bicubic", layout: str = "hwc"):
+    """The device resize on one CPU thread (jpegqs_cuda_resize_model): byte for byte Pillow's
+    Image.fromarray(pixels).crop(crop).resize(size, filter).  pixels: uint8 [H, W] (grey, 'L') or
+    [H, W, C] with C 1 or 3, as decode_pixels gives them in layout "hwc".  size (width, height) and
+    crop (left, top, right, bottom) or None follow Pillow's conventions; filter as decode_pixels'.
+    Returns [height, width] for a 2-D input, else [height, width, C] ("hwc") or [C, height, width]
+    ("chw").  ValueError for a bad argument."""
+    if layout not in ("hwc", "chw"):
+        raise ValueError(f"resize_model: layout {layout!r}: expected 'hwc' or 'chw'")
+    a = np.asarray(pixels)
+    if a.dtype != np.uint8 or a.ndim not in (2, 3) or (a.ndim == 3 and a.shape[2] not in (1, 3)) or 0 in a.shape:
+        raise ValueError(f"resize_model: pixels must be uint8 [H, W] or [H, W, 1|3], not {a.dtype} {a.shape}")
+    a = np.ascontiguousarray(a)
+    fcode = _resize_filter(filter, "resize_model")
+    if size is None:
+        raise ValueError("resize_model: size (width, height) is required")
+    sizes, crops = _resize_boxes(1, size, None if crop is None else [crop], "resize_model")
+    h, w = a.shape[:2]
+    c = 1 if a.ndim == 2 else a.shape[2]
+    box = _resize_box(w, h, sizes[0], crops[0], 0, "resize_model")
+    shape = (box.height, box.width, c) if layout == "hwc" else (c, box.height, box.width)
+    out = np.zeros(shape, dtype=np.uint8)
+    lib = load()
+    rc = lib.jpegqs_cuda_resize_model(a.ctypes.data, w, h, c, 0 if layout == "hwc" else 1, fcode, C.byref(box),
+                                      out.ctypes.data)
+    if rc < 0:
+        raise ValueError(f"resize_model: {lib.jpegqs_cuda_last_error(None).decode()} ({rc})")
+    return out.reshape(box.height, box.width) if a.ndim == 2 else out
 
 
 def decode_model(image: CoefImage, scan, data: bytes, sub_bytes: int = DECODE_SUB_DEFAULT, out=None):
@@ -749,7 +852,7 @@ class QsContext:
         return out
 
     def decode_pixels(self, datas, flags: int, niter: int, layout: str = "hwc", device: str = "cuda",
-                      max_device_bytes: int = 0, scale_denom: int = 1):
+                      max_device_bytes: int = 0, scale_denom: int = 1, size=None, crop=None, filter="bicubic"):
         """Many JPEG files to the smoothed pixels the jpegqs tool's --ppm writes for them (islow, fancy
         up-sampling, after do_quantsmooth(flags, niter)), in shared launches (jpegqs_cuda_pixels_batch).
         Returns, in the order of datas, one record per file:
@@ -763,7 +866,16 @@ class QsContext:
         cannot take (1 or 3 components, integral sampling ratios).
         scale_denom 2, 4 or 8: libjpeg's scaled decode of the same coefficients at 1/d size
         (jpegqs_cuda_pixels_batch_scaled); pixels are then [ceil(H/d), ceil(W/d), C] or
-        [C, ceil(H/d), ceil(W/d)].  ValueError for any other value than 1, 2, 4 or 8."""
+        [C, ceil(H/d), ceil(W/d)].  ValueError for any other value than 1, 2, 4 or 8.
+        size / crop / filter: each file's pixels cropped and resized on the device, byte for byte
+        Pillow's Image.fromarray(P).crop(crop).resize(size, filter) of the picture P the call gives
+        without them (jpegqs_cuda_pixels_batch_resized).  The conventions are Pillow's, not torch's:
+        size is (width, height), for every file or a list with one per file; crop is None or a list
+        with one (left, top, right, bottom) box or None per file, in the 1/scale_denom picture.  filter
+        is "bicubic" (Image.resize's default), "bilinear", "lanczos", "box" or "hamming", or Pillow's
+        Image.Resampling value of one of them; NEAREST is not supported.  A crop without size returns
+        the crop as it is.  Pixels are then [height, width, C] or [C, height, width].  ValueError
+        naming the file index for a bad size, crop or filter, before anything runs."""
         if isinstance(datas, (bytes, bytearray, memoryview, str)) or not hasattr(datas, "__len__"):
             raise TypeError("decode_pixels: datas must be a sequence of bytes-like files")
         files = [_file_bytes(d, f"decode_pixels: file {i}") for i, d in enumerate(datas)]
@@ -775,9 +887,12 @@ class QsContext:
             raise ValueError("decode_pixels: max_device_bytes must be >= 0")
         scale = _scale_denom(scale_denom, "decode_pixels")
         n = len(files)
+        resize = size is not None or crop is not None
+        if resize:
+            fcode = _resize_filter(filter, "decode_pixels")
+            sizes, crops = _resize_boxes(n, size, crop, "decode_pixels")
         if not n:
             return []
-        import torch
         # the output size rule of jpegqs_cuda_pixels_batch: transcode_route's width, height and ncomp
         shapes = []
         for i, d in enumerate(files):
@@ -788,6 +903,14 @@ class QsContext:
                 raise QsError(f"decode_pixels: file {i}: {info.ncomp} components; the render takes 1 or 3")
             c, h, w = info.ncomp, info.image_height, info.image_width
             shapes.append(_scaled_shape(w, h, c, layout, scale))
+        if resize:
+            boxes = (_ResizeBox * n)()
+            for i, s in enumerate(shapes):
+                ph, pw = (s[0], s[1]) if layout == "hwc" else (s[1], s[2])
+                boxes[i] = _resize_box(pw, ph, sizes[i], crops[i], i, "decode_pixels")
+                c = 1 if s[2 if layout == "hwc" else 0] == 1 else 3
+                shapes[i] = (boxes[i].height, boxes[i].width, c) if layout == "hwc" else (c, boxes[i].height, boxes[i].width)
+        import torch
         if device == "cuda":
             dev = self.device if self.device >= 0 else torch.cuda.current_device()
             outs = [torch.empty(s, dtype=torch.uint8, device=dev) for s in shapes]
@@ -800,7 +923,12 @@ class QsContext:
         optrs = (C.c_void_p * n)(*[t.data_ptr() for t in outs])
         rc = (C.c_int * n)()
         res = (_PixelsResult * n)()
-        if scale == 1:
+        if resize:
+            self._check(self.lib.jpegqs_cuda_pixels_batch_resized(self.h, n, ptrs, lens, int(flags), int(niter),
+                                                                  0 if layout == "hwc" else 1, scale, fcode, boxes,
+                                                                  int(device == "cuda"), optrs, int(max_device_bytes), rc,
+                                                                  res))
+        elif scale == 1:
             self._check(self.lib.jpegqs_cuda_pixels_batch(self.h, n, ptrs, lens, int(flags), int(niter),
                                                           0 if layout == "hwc" else 1, int(device == "cuda"), optrs,
                                                           int(max_device_bytes), rc, res))
@@ -1572,7 +1700,10 @@ def transcode_batch(datas, flags: int, niter: int, optimize: bool = False, copy:
 
 
 def decode_pixels(datas, flags: int, niter: int, layout: str = "hwc", device: str = "cuda", max_device_bytes: int = 0,
-                  gpu: int = -1, scale_denom: int = 1):
+                  gpu: int = -1, scale_denom: int = 1, size=None, crop=None, filter="bicubic"):
     """QsContext.decode_pixels on the default context of CUDA device `gpu`: one record (pixels, warnings,
-    host_decoded, smoothed, stop, upsampled, reason) per file, at 1/scale_denom size."""
-    return default_context(gpu).decode_pixels(datas, flags, niter, layout, device, max_device_bytes, scale_denom)
+    host_decoded, smoothed, stop, upsampled, reason) per file, at 1/scale_denom size, cropped and resized
+    as Pillow would with size / crop / filter ((width, height) and (left, top, right, bottom), Pillow's
+    conventions)."""
+    return default_context(gpu).decode_pixels(datas, flags, niter, layout, device, max_device_bytes, scale_denom,
+                                              size, crop, filter)
