@@ -699,6 +699,93 @@ int jpegqs_cuda_pixels_batch_resized(jpegqs_cuda_ctx *ctx, int n, const uint8_t 
 int jpegqs_cuda_resize_model(const uint8_t *src, int width, int height, int channels, int layout, int filter,
 		const jpegqs_cuda_resize_box *box, uint8_t *out);
 
+/* ---- 8-bit pictures -> JPEG files: Pillow's Image.save, byte for byte ---------------------------
+ * Picture i's file is exactly what Pillow (with its libjpeg-turbo) writes for
+ *     Image.fromarray(P).save(f, "JPEG", quality=quality, subsampling=subsampling, optimize=optimize)
+ * where P is the picture as an 'RGB' (channels 3) or 'L' (channels 1) image.  That is plain libjpeg:
+ * jpeg_set_defaults, jpeg_set_quality(quality, force_baseline TRUE), luma sampling 1x1 / 2x1 / 2x2 for
+ * subsampling 0 / 1 / 2 (4:4:4, 4:2:2, 4:2:0, Pillow's numbering; grey pictures ignore it), chroma 1x1,
+ * optimize_coding = optimize, islow DCT, component ids 1, 2, 3, quantization table 0 for luma and 1 for
+ * both chroma components, and the JFIF 1.01 APP0 with density unit 0 and density 1:1.
+ *   - The compressor kernel restates jccolor.c's rgb_ycc_convert (16-bit fixed point), jcsample.c's
+ *     fullsize / h2v1 / h2v2 down-sampling (alternating biases 0,1 and 1,2), jcprepct.c's edges (the
+ *     right edge repeats the last full-resolution column before down-sampling; the bottom edge repeats
+ *     the last down-sampled row), jfdctint.c's jpeg_fdct_islow on sample - 128 and jcdctmgr.c's
+ *     quantization (sign(t) * ((|t| + 4q) / (8q))).  Geometry is libjpeg's: downsampled width =
+ *     ceil(W * h / max_h), width in blocks = ceil(downsampled width / 8), and the same for heights.
+ *   - jpegqs_cuda_encode_async then writes the coefficients, so the files are its output for them.
+ *   - Grey pictures: the samples do not depend on subsampling, but Pillow sets the luma sampling factors
+ *     whatever the component count, so the SOF of a grey file saved with 4:2:2 / 4:2:0 says 2x1 / 2x2
+ *     (its single-component scan is coded block by block all the same); so does this one. */
+typedef struct {
+	int32_t quality;       /* 1..100                                                               */
+	int32_t subsampling;   /* 0 = 4:4:4, 1 = 4:2:2, 2 = 4:2:0 (Pillow's numbers); ignored for grey   */
+	int32_t optimize;      /* 0 / 1: optimal Huffman tables                                        */
+} jpegqs_cuda_jpeg_params;
+typedef struct {
+	const uint8_t *pixels_dev; /* DEVICE memory (host memory for compress_model), HWC, any alignment  */
+	int32_t width, height;     /* 1..65535                                                         */
+	int32_t channels;          /* 1 (grey) or 3 (RGB)                                              */
+	size_t row_bytes;          /* bytes from one row to the next, >= width * channels              */
+} jpegqs_cuda_pixels_in;
+
+/* Stream-ordered, graph-capturable compression of n device pictures with one params for all.
+ *   - Per group of up to 32 pictures, one compressor launch turns every component into quantized
+ *     coefficients in the workspace; then jpegqs_cuda_encode_async writes them with the scaled tables
+ *     and the JFIF prefix (the compressor kernel copies the prefix from its parameters into the
+ *     workspace).  jpegqs_cuda_last_launches counts both.
+ *   - Output.  out_dev[i]: out_cap[i] bytes of device memory at any alignment; len_dev[i] (device
+ *     uint64) and status_dev[i] (device int32) as encode_async's: 0, or JPEGQS_ENCODE_OVERFLOW with
+ *     len_dev[i] the length the file needs and nothing written at or past out_cap[i].  RANGE cannot
+ *     occur for 8-bit samples.
+ *   - Bound.  jpegqs_cuda_compress_bound: encode_bound with a 20-byte prefix, 20 + 1680 +
+ *     2 * ceil(U * 1665 / 8), with U = MCUs x blocks per MCU: ceil(W/8) * ceil(H/8) for grey,
+ *     3 * ceil(W/8) * ceil(H/8) for 4:4:4, 4 * ceil(W/16) * ceil(H/8) for 4:2:2 and
+ *     6 * ceil(W/16) * ceil(H/16) for 4:2:0.
+ *   - Workspace.  With A(x) = x rounded up to a multiple of 256, jpegqs_cuda_compress_workspace_bytes is
+ *     256 (the prefix) plus, per picture, sum over components of A(128 * wblk * hblk) (the
+ *     coefficients) plus encode_workspace_bytes' term for the picture's geometry:
+ *       32768 + A(2 * U) + A(8 * T) + A(4 * Wd) + A(4 * ceil(4 * Wd / 4096)),
+ *     T = ceil(U / 256), Wd = ceil(U * 1665 / 32) + 2.  The workspace is 256-byte aligned.
+ *   - Argument errors change nothing: every check runs before the first enqueue and a failed one
+ *     returns JPEGQS_ERR_ARG with nothing enqueued.  Checked: NULL pointers (pics, params, out_dev and
+ *     its entries, out_cap, len_dev, status_dev, workspace, pixels_dev), quality outside 1..100,
+ *     subsampling outside 0..2, optimize other than 0 / 1, width or height outside 1..65535, channels
+ *     other than 1 or 3, row_bytes < width * channels, out_cap[i] < 20, a workspace too small or not
+ *     256-byte aligned.
+ *   - encode_async's stream rules: no cudaMalloc, no synchronisation; descriptors, tables and the
+ *     prefix travel as kernel parameters and nothing of pics or params is read after return.  A
+ *     replay of a captured call compresses the current contents of the same pixel buffers. */
+int jpegqs_cuda_compress_bound(const jpegqs_cuda_pixels_in *pic, const jpegqs_cuda_jpeg_params *params, size_t *bytes);
+int jpegqs_cuda_compress_workspace_bytes(int n, const jpegqs_cuda_pixels_in *pics, const jpegqs_cuda_jpeg_params *params,
+		size_t *bytes);
+int jpegqs_cuda_compress_async(jpegqs_cuda_ctx *ctx, int n, const jpegqs_cuda_pixels_in *pics,
+		const jpegqs_cuda_jpeg_params *params, uint8_t *const *out_dev, const size_t *out_cap, uint64_t *len_dev,
+		int32_t *status_dev, void *workspace, size_t workspace_bytes, void *stream);
+/* The same per-block functions and encode_model on the calling thread, for one picture whose pixels_dev
+ * is HOST memory (no device needed).  *len / *status as len_dev / status_dev.  Returns 0 or
+ * JPEGQS_ERR_ARG (the checks of compress_async; cap < 20); jpegqs_cuda_last_error(NULL) says why. */
+int jpegqs_cuda_compress_model(const jpegqs_cuda_pixels_in *pic, const jpegqs_cuda_jpeg_params *params,
+		uint8_t *out, size_t cap, uint64_t *len, int32_t *status);
+
+/* JPEG files in, JPEG files out: each file's picture as jpegqs_cuda_pixels_batch_resized gives it (boxes
+ * given) or jpegqs_cuda_pixels_batch_scaled (boxes NULL), written as Pillow's Image.save(quality,
+ * subsampling, optimize) writes it (compress_async's files).  A grey file gives a grey JPEG.
+ *   - Per sub-batch, after the render (and resize) into the context's buffers: compress_async over the
+ *     pictures, then the packing kernel of transcode_batch; only the packed files and the statuses
+ *     come back.
+ *   - out[i] receives a malloc'd file of out_len[i] bytes (release it with jpegqs_cuda_transcode_free),
+ *     or NULL for a file that fails.  rc[i], routes, warnings and results[i] are those of the pixel
+ *     call for the same files; a bad file or a bad crop fails alone.
+ *   - The budget counts, per file, what the pixel call counts with host outputs, plus the compressor's
+ *     workspace share (coefficients and encoder workspace) and the bound, twice (slot and packed copy).
+ *   - Return.  As pixels_batch_resized's (0, or a negative error with nothing done for bad arguments:
+ *     also params NULL or out of range, out_len NULL); on a negative return every out[i] is NULL. */
+int jpegqs_cuda_pixels_batch_jpeg(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
+		const jpegqs_cuda_jpeg_params *params, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results,
+		uint8_t **out, size_t *out_len);
+
 /* ---- one image sharded by MCU rows over several GPUs (SURVEY.md 8e) ----------------------
  * Every rank - a device of this process, or another process on the same box - smooths one slab
  * of contiguous MCU rows and exchanges ONE pixel row per plane with each neighbour after every

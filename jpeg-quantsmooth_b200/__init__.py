@@ -43,7 +43,8 @@ def __getattr__(name):
                 "parse_jpeg", "read_jpeg", "decode_async", "decode_workspace_bytes", "decode_model",
                 "jpeg_prefix", "encode_bound", "encode_workspace_bytes", "encode_model", "encode_async",
                 "parse_jpeg_scans", "decode_scans_async", "decode_scans_workspace_bytes", "decode_scans_model",
-                "transcode_route", "transcode", "transcode_batch", "decode_pixels", "render_model", "resize_model"):
+                "transcode_route", "transcode", "transcode_batch", "decode_pixels", "render_model", "resize_model",
+                "compress_model", "compress_bound", "compress_async", "reencode"):
         import importlib
         _cuda = importlib.import_module(__name__ + ".cuda")
         if name == "cuda":

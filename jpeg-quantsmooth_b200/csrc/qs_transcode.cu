@@ -126,6 +126,9 @@ struct QsTranscode {
 	QsBuf hcoef_dev, hcoef_host;               /* pixels: the host-decoded files' coefficients and their staging */
 	QsBuf rs_dev, rs_host;                     /* resized pixels: descriptors + weight tables, intermediates,
 	                                              rendered pictures; the staging of the descriptors and tables */
+	QsBuf jp_dev, jp_host;                     /* JPEG outputs: packing descriptors, lengths, statuses, records
+	                                              and the encoder's output slots; the staging of descriptors
+	                                              and records */
 	cudaEvent_t ev0, ev1;                      /* around run_async: jpegqs_cuda_last_device_ms */
 	int sms;
 	jpegqs_cuda_scan_rec recs[JPEGQS_MAX_SCANS];
@@ -138,7 +141,8 @@ void qs_transcode_release(void *state) {
 	QsTranscode *t = (QsTranscode*)state;
 	if (!t) return;
 	cudaFree(t->in_dev.p); cudaFree(t->coef_dev.p); cudaFree(t->ws_dev.p); cudaFree(t->out_dev.p); cudaFree(t->stat_dev.p);
-	cudaFree(t->hcoef_dev.p); cudaFree(t->rs_dev.p);
+	cudaFree(t->hcoef_dev.p); cudaFree(t->rs_dev.p); cudaFree(t->jp_dev.p);
+	if (t->jp_host.p) cudaFreeHost(t->jp_host.p);
 	if (t->in_host.p) cudaFreeHost(t->in_host.p);
 	if (t->out_host.p) cudaFreeHost(t->out_host.p);
 	if (t->stat_host.p) cudaFreeHost(t->stat_host.p);
@@ -182,6 +186,7 @@ struct QsPlan {
 	int go;                                    /* the file takes part in the sub-batches */
 	int host;                                  /* pixels: the host reader decodes it */
 	int smooth, can_up;
+	int out_w, out_h;                          /* pixels: the output picture's size */
 	size_t in_bytes, coef_bytes, up_bytes, cap, pix;
 	size_t ws_dec, ws_run, ws_enc;             /* this file's share of each stage's workspace */
 	size_t fixed, packed;                      /* its share of the buffers outside the workspace; of the packed output */
@@ -262,7 +267,7 @@ static cudaError_t batch_budget(const QsTranscode *t, size_t max_device_bytes, s
 	size_t fr = 0, tot = 0;
 	cudaError_t e = cudaMemGetInfo(&fr, &tot);
 	*budget = (fr + t->in_dev.cap + t->coef_dev.cap + t->ws_dev.cap + t->out_dev.cap + t->stat_dev.cap + t->hcoef_dev.cap +
-			t->rs_dev.cap) / 2;
+			t->rs_dev.cap + t->jp_dev.cap) / 2;
 	return e;
 }
 
@@ -583,10 +588,23 @@ static int host_read(const QsPlan &p, const uint8_t *data, size_t len, uint8_t *
 	return jpegqs_cuda_jpeg_read(data, len, &im);
 }
 
-/* boxes != NULL: each file's picture is cropped and resized (qs_resize.cu) with filter */
+/* the JPEG outputs' device memory per sub-batch of m files (jp_dev): packing descriptors, lengths,
+ * encoder statuses, zero decoder statuses, packing records, then the output slots */
+struct QsJpegLayout {
+	size_t desc, lens, enc, zero, rec, slots;
+	void set(int m) {
+		desc = 0; lens = align256(sizeof(QsPackDesc) * (size_t)m); enc = lens + align256(8 * (size_t)m);
+		zero = enc + align256(4 * (size_t)m); rec = zero + align256(4 * (size_t)m); slots = rec + align256(sizeof(QsPackRec) * (size_t)m);
+	}
+};
+
+/* boxes != NULL: each file's picture is cropped and resized (qs_resize.cu) with filter.  jp != NULL: the
+ * pictures are written as JPEG files with these params (compress_async) into jout / jlen, and on_device
+ * must be 0 (the pictures stay in the context's buffers). */
 static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint8_t *const *data, const size_t *len,
 		int flags, int niter, int layout, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes, int on_device,
-		uint8_t *const *out, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results) {
+		uint8_t *const *out, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results,
+		const jpegqs_cuda_jpeg_params *jp = NULL, uint8_t **jout = NULL, size_t *jlen = NULL) {
 	char msg[512];
 	cudaStream_t st;
 	std::vector<QsPlan> plans((size_t)n);
@@ -613,6 +631,7 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 		const int pw = (int)((p.img.image_width + scale_denom - 1) / scale_denom);
 		const int ph = (int)((p.img.image_height + scale_denom - 1) / scale_denom);
 		p.pix = (size_t)pw * ph * p.img.ncomp;
+		p.out_w = pw; p.out_h = ph;
 		if (boxes) {
 			const char *bad = qs_resize_plan(pw, ph, boxes[i], filter, rsp[i]);
 			if (bad) {
@@ -622,6 +641,7 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 			}
 			pic[i] = p.pix;
 			p.pix = (size_t)boxes[i].width * boxes[i].height * p.img.ncomp;
+			p.out_w = boxes[i].width; p.out_h = boxes[i].height;
 		}
 		p.host = route != JPEGQS_ROUTE_DEVICE;
 		if (p.host) { p.in_bytes = 0; p.ws_dec = 0; results[i].host_decoded = 1; results[i].reason = why; }
@@ -634,6 +654,15 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 			p.fixed += align256(pic[i]) + align256((size_t)rsp[i].mid_h * rsp[i].out_w * p.img.ncomp) +
 					align256(rsp[i].tab.size() * sizeof(int32_t)) + align256(sizeof(QsResizeDesc));
 		p.ws_enc = 0; p.packed = 0;
+		if (jp) {
+			/* JPEG: the compressor's workspace share (coefficients and encoder workspace, with the prefix's
+			 * 256 bytes counted per file), its output slot, the packed copy and the per-file records */
+			const jpegqs_cuda_pixels_in pin = { NULL, p.out_w, p.out_h, p.img.ncomp, (size_t)p.out_w * p.img.ncomp };
+			TQ(jpegqs_cuda_compress_bound(&pin, jp, &p.cap));
+			TQ(jpegqs_cuda_compress_workspace_bytes(1, &pin, jp, &p.ws_enc));
+			p.packed = align16(p.cap);
+			p.fixed += align256(p.cap) + 5 * 256;
+		}
 		p.go = 1;
 	}
 
@@ -659,6 +688,18 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 		}
 		for (int f : files) in_total += plans[f].in_bytes, coef_total += (plans[f].host ? 0 : plans[f].coef_bytes) + plans[f].up_bytes;
 		const int ndec = (int)(g.seq_k.size() + g.scan_k.size());
+		/* JPEG: the compressor and encoder share the workspace once the render is done, then the packed
+		 * files take it; jp_dev holds the slots and the small per-file arrays */
+		QsJpegLayout jl;
+		if (jp) {
+			size_t cws = 256, packed = 0, slots = 0;
+			for (int f : files) { cws += plans[f].ws_enc - 256; packed += plans[f].packed; slots += align256(plans[f].cap); }
+			if (cws > ws) ws = cws;
+			if (packed > ws) ws = packed;
+			jl.set(m);
+			TK(grow_dev(&t->jp_dev, jl.slots + slots));
+			TK(grow_host(&t->jp_host, align256(sizeof(QsPackDesc) * (size_t)m) + sizeof(QsPackRec) * (size_t)m));
+		}
 		TK(grow_dev(&t->in_dev, in_total));
 		TK(grow_dev(&t->coef_dev, coef_total + 256));
 		TK(grow_dev(&t->ws_dev, ws));
@@ -745,8 +786,9 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 		std::vector<size_t> poff(nr);
 		size_t pix_total = st_bytes;
 		for (int j = 0; j < nr; j++) { poff[j] = pix_total; if (!on_device) pix_total += align256(plans[files[rk[j]]].pix); }
+		const size_t down = jp ? st_bytes : pix_total;  /* JPEG: the pictures stay on the device */
 		TK(grow_dev(&t->out_dev, pix_total));
-		TK(grow_host(&t->out_host, pix_total));
+		TK(grow_host(&t->out_host, down));
 		jpegqs_cuda_status *run = (jpegqs_cuda_status*)t->out_dev.p;
 		std::vector<uint8_t*> outs(nr);
 		for (int j = 0; j < nr; j++) outs[j] = on_device ? out[files[rk[j]]] : (uint8_t*)t->out_dev.p + poff[j];
@@ -788,8 +830,41 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 		if (ms < nr) TK(cudaMemsetAsync(run + ms, 0, (size_t)(nr - ms) * sizeof(jpegqs_cuda_status), st));
 		if (nr) TQ(qs_render_images(ctx, nr, rimg.data(), run, boxes ? JPEGQS_RENDER_HWC : layout, 1, scale_denom, outs.data(), st));
 		if (boxes && nr) TK(qs_launch_resize((const QsResizeDesc*)t->rs_dev.p, nr, hblocks, vblocks, st));
+		/* JPEG: compress_async over the pictures into the slots, then the packing kernel into the
+		 * workspace, its records back */
+		uint8_t *jd = (uint8_t*)t->jp_dev.p, *jh = (uint8_t*)t->jp_host.p;
+		const size_t jh_rec = align256(sizeof(QsPackDesc) * (size_t)m);
+		size_t packed = 0;
+		if (jp && nr) {
+			std::vector<jpegqs_cuda_pixels_in> pin(nr);
+			std::vector<uint8_t*> slot(nr);
+			std::vector<size_t> cap(nr);
+			QsPackDesc *pd = (QsPackDesc*)jh;
+			size_t so = 0;
+			for (int j = 0; j < nr; j++) {
+				const QsPlan &p = plans[files[rk[j]]];
+				pin[j].pixels_dev = (const uint8_t*)t->out_dev.p + poff[j];
+				pin[j].width = p.out_w; pin[j].height = p.out_h; pin[j].channels = p.img.ncomp;
+				pin[j].row_bytes = (size_t)p.out_w * p.img.ncomp;
+				slot[j] = jd + jl.slots + so; cap[j] = p.cap;
+				memset(&pd[j], 0, sizeof(pd[j]));
+				pd[j].slot = so; pd[j].cap = p.cap; pd[j].dec_idx = j;
+				so += align256(p.cap); packed += align16(p.cap);
+			}
+			TK(cudaMemcpyAsync(jd + jl.desc, jh, sizeof(QsPackDesc) * (size_t)nr, cudaMemcpyHostToDevice, st));
+			TK(cudaMemsetAsync(jd + jl.zero, 0, 4 * (size_t)nr, st));
+			TQ(jpegqs_cuda_compress_async(ctx, nr, pin.data(), jp, slot.data(), cap.data(), (uint64_t*)(jd + jl.lens),
+					(int32_t*)(jd + jl.enc), t->ws_dev.p, t->ws_dev.cap, st));
+			size_t chunks = (packed + QS_PACK_CHUNK - 1) / QS_PACK_CHUNK, grid = 4 * (size_t)(t->sms > 0 ? t->sms : 1);
+			if (chunks < grid) grid = chunks ? chunks : 1;
+			qs_pack_kernel<<<(unsigned)grid, QS_PACK_THREADS, 0, st>>>(nr, (const QsPackDesc*)(jd + jl.desc), jd + jl.slots,
+					(const int32_t*)(jd + jl.zero), run, (const uint64_t*)(jd + jl.lens), (const int32_t*)(jd + jl.enc),
+					(QsPackRec*)(jd + jl.rec), (uint8_t*)t->ws_dev.p);
+			TK(cudaGetLastError());
+			TK(cudaMemcpyAsync(jh + jh_rec, jd + jl.rec, sizeof(QsPackRec) * (size_t)nr, cudaMemcpyDeviceToHost, st));
+		}
 		/* the run statuses, and the pixels in the same copy when they come back to the host */
-		if (nr) TK(cudaMemcpyAsync(t->out_host.p, t->out_dev.p, pix_total, cudaMemcpyDeviceToHost, st));
+		if (nr) TK(cudaMemcpyAsync(t->out_host.p, t->out_dev.p, down, cudaMemcpyDeviceToHost, st));
 		TK(cudaStreamSynchronize(st));
 		if (ms) {
 			float ms_run = 0;
@@ -800,12 +875,37 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 		for (int j = 0; j < nr; j++) {
 			const int f = files[rk[j]];
 			results[f].smoothed = plans[f].smooth; results[f].stop = rs[j].stop; results[f].upsampled = rs[j].upsampled;
-			if (!on_device) memcpy(out[f], (const uint8_t*)t->out_host.p + poff[j], plans[f].pix);
+			if (!on_device && !jp) memcpy(out[f], (const uint8_t*)t->out_host.p + poff[j], plans[f].pix);
+		}
+		if (jp && nr) {
+			/* every file is clean (8-bit samples cannot make RANGE, the slots hold the bound): exactly the
+			 * packed bytes back */
+			const QsPackRec *rec = (const QsPackRec*)(jh + jh_rec);
+			size_t total = 0;
+			for (int j = 0; j < nr; j++) {
+				if (rec[j].encode || rec[j].len > plans[files[rk[j]]].cap) {
+					snprintf(msg, sizeof(msg), "%s: encoder status %d, length %llu of %zu", who, (int)rec[j].encode,
+							(unsigned long long)rec[j].len, plans[files[rk[j]]].cap);
+					qs_ctx_decode_done(ctx, 0, msg); ret = JPEGQS_ERR_CUDA; goto fail;
+				}
+				if (rec[j].off + rec[j].len > total) total = rec[j].off + rec[j].len;
+			}
+			TK(grow_host(&t->out_host, total));
+			TK(cudaMemcpyAsync(t->out_host.p, t->ws_dev.p, total, cudaMemcpyDeviceToHost, st));
+			TK(cudaStreamSynchronize(st));
+			for (int j = 0; j < nr; j++) {
+				const int f = files[rk[j]];
+				jout[f] = (uint8_t*)malloc(rec[j].len);
+				if (!jout[f]) { snprintf(msg, sizeof(msg), "%s: out of memory", who); qs_ctx_decode_done(ctx, 0, msg); ret = JPEGQS_ERR_ARG; goto fail; }
+				memcpy(jout[f], (const uint8_t*)t->out_host.p + rec[j].off, rec[j].len);
+				jlen[f] = rec[j].len;
+			}
 		}
 	}
 	return 0;
 	}
 fail:
+	if (jout) for (int i = 0; i < n; i++) { free(jout[i]); jout[i] = NULL; jlen[i] = 0; }
 	return ret;
 }
 #undef TK
@@ -852,6 +952,45 @@ extern "C" int jpegqs_cuda_pixels_batch_resized(jpegqs_cuda_ctx *ctx, int n, con
 		uint8_t *const *out, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results) {
 	return pixels_entry(ctx, "jpegqs_cuda_pixels_batch_resized", n, data, len, flags, niter, layout, scale_denom, 1, filter, boxes,
 			out_on_device, out, max_device_bytes, rc, results);
+}
+
+extern "C" int jpegqs_cuda_pixels_batch_jpeg(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
+		const jpegqs_cuda_jpeg_params *params, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results,
+		uint8_t **out, size_t *out_len) {
+	static const char who[] = "jpegqs_cuda_pixels_batch_jpeg";
+	char msg[200];
+	if (!ctx) return JPEGQS_ERR_ARG;
+	if (n < 0) { snprintf(msg, sizeof(msg), "%s: negative file count", who); qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG; }
+	if (!n) return 0;
+	if (!data || !len || !out || !out_len || !rc || !results || !params) {
+		snprintf(msg, sizeof(msg), "%s: NULL argument", who); qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG;
+	}
+	if (params->quality < 1 || params->quality > 100 || params->subsampling < 0 || params->subsampling > 2 ||
+			(params->optimize != 0 && params->optimize != 1)) {
+		snprintf(msg, sizeof(msg), "%s: params: quality outside 1..100, subsampling outside 0..2 or optimize other than 0 / 1", who);
+		qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG;
+	}
+	for (int i = 0; i < n; i++) if (!data[i]) {
+		snprintf(msg, sizeof(msg), "%s: file %d: NULL data", who, i);
+		qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG;
+	}
+	if (scale_denom != 1 && scale_denom != 2 && scale_denom != 4 && scale_denom != 8) {
+		snprintf(msg, sizeof(msg), "%s: scale_denom must be 1, 2, 4 or 8", who); qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG;
+	}
+	if (boxes) {
+		if (!qs_resize_filter_ok(filter)) {
+			snprintf(msg, sizeof(msg), "%s: filter %d: expected LANCZOS (1), BILINEAR (2), BICUBIC (3), BOX (4) or HAMMING (5)", who, filter);
+			qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG;
+		}
+		for (int i = 0; i < n; i++) if (boxes[i].width < 1 || boxes[i].width > 65535 || boxes[i].height < 1 || boxes[i].height > 65535) {
+			snprintf(msg, sizeof(msg), "%s: file %d: output size %d x %d outside 1..65535", who, i, boxes[i].width, boxes[i].height);
+			qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG;
+		}
+	}
+	for (int i = 0; i < n; i++) { memset(&results[i], 0, sizeof(results[i])); results[i].reason = ""; rc[i] = 0; out[i] = NULL; out_len[i] = 0; }
+	return pixels_batch(ctx, who, n, data, len, flags, niter, JPEGQS_RENDER_HWC, scale_denom, filter, boxes, 0, NULL,
+			max_device_bytes, rc, results, params, out, out_len);
 }
 
 extern "C" int jpegqs_cuda_pixels_batch_scaled(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,

@@ -99,6 +99,17 @@ class _ResizeBox(C.Structure):
                 ("width", C.c_int32), ("height", C.c_int32)]
 
 
+class _JpegParams(C.Structure):
+    """jpegqs_cuda_jpeg_params (include/jpegqs_cuda.h)."""
+    _fields_ = [("quality", C.c_int32), ("subsampling", C.c_int32), ("optimize", C.c_int32)]
+
+
+class _PixelsIn(C.Structure):
+    """jpegqs_cuda_pixels_in (include/jpegqs_cuda.h)."""
+    _fields_ = [("pixels_dev", C.c_void_p), ("width", C.c_int32), ("height", C.c_int32), ("channels", C.c_int32),
+                ("row_bytes", C.c_size_t)]
+
+
 class _Job(C.Structure):
     _fields_ = [("coef", C.c_void_p), ("plane", C.c_void_p), ("plane2", C.c_void_p),
                 ("wblk", C.c_uint32), ("hblk", C.c_uint32), ("quant", C.c_uint16 * 64),
@@ -231,6 +242,19 @@ def load():
                                                      C.POINTER(_PixelsResult)]
     lib.jpegqs_cuda_resize_model.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                              C.POINTER(_ResizeBox), C.c_void_p]
+    lib.jpegqs_cuda_compress_bound.argtypes = [C.POINTER(_PixelsIn), C.POINTER(_JpegParams), C.POINTER(C.c_size_t)]
+    lib.jpegqs_cuda_compress_workspace_bytes.argtypes = [C.c_int, C.POINTER(_PixelsIn), C.POINTER(_JpegParams),
+                                                         C.POINTER(C.c_size_t)]
+    lib.jpegqs_cuda_compress_async.argtypes = [C.c_void_p, C.c_int, C.POINTER(_PixelsIn), C.POINTER(_JpegParams),
+                                               C.c_void_p, C.POINTER(C.c_size_t), C.c_void_p, C.c_void_p, C.c_void_p,
+                                               C.c_size_t, C.c_void_p]
+    lib.jpegqs_cuda_compress_model.argtypes = [C.POINTER(_PixelsIn), C.POINTER(_JpegParams), C.c_void_p, C.c_size_t,
+                                               C.POINTER(C.c_uint64), C.POINTER(C.c_int32)]
+    lib.jpegqs_cuda_pixels_batch_jpeg.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_size_t),
+                                                  C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(_ResizeBox),
+                                                  C.POINTER(_JpegParams), C.c_size_t, C.POINTER(C.c_int),
+                                                  C.POINTER(_PixelsResult), C.POINTER(C.c_void_p),
+                                                  C.POINTER(C.c_size_t)]
     lib.jpegqs_cuda_tables.argtypes = [C.c_int, C.c_void_p]
     lib.jpegqs_cuda_orig_coef.argtypes = [C.c_int, C.c_int]
     _lib = lib
@@ -723,6 +747,68 @@ def encode_model(image: CoefImage, arrays, prefix: bytes, comp_ids, quant_tbls, 
                                     C.byref(n), C.byref(st)) < 0:
         raise QsError(lib.jpegqs_cuda_last_error(None).decode())
     return out[:min(n.value, cap)].tobytes(), int(st.value)
+
+
+# ---- pictures to JPEG files (include/jpegqs_cuda.h "8-bit pictures -> JPEG files") ----
+SUBSAMPLINGS = {"4:4:4": 0, "4:2:2": 1, "4:2:0": 2}
+
+
+def _jpeg_params(quality, subsampling, optimize, who: str) -> _JpegParams:
+    """Pillow's save keywords: quality 1..100; subsampling "4:4:4" / "4:2:2" / "4:2:0" or 0 / 1 / 2"""
+    if isinstance(quality, bool) or not isinstance(quality, (int, np.integer)) or not 1 <= int(quality) <= 100:
+        raise ValueError(f"{who}: quality {quality!r}: expected an integer in 1..100")
+    if isinstance(subsampling, str) and subsampling in SUBSAMPLINGS:
+        s = SUBSAMPLINGS[subsampling]
+    elif not isinstance(subsampling, (str, bool)) and isinstance(subsampling, (int, np.integer)) and int(subsampling) in (0, 1, 2):
+        s = int(subsampling)
+    else:
+        raise ValueError(f"{who}: subsampling {subsampling!r}: expected '4:4:4', '4:2:2', '4:2:0' or 0, 1, 2")
+    return _JpegParams(int(quality), s, int(bool(optimize)))
+
+
+def _pixels_in(ptr, shape, row_bytes) -> _PixelsIn:
+    h, w, c = shape
+    return _PixelsIn(ptr, int(w), int(h), int(c), int(row_bytes))
+
+
+def _host_picture(pixels, who: str) -> np.ndarray:
+    a = np.asarray(pixels.cpu() if hasattr(pixels, "cpu") else pixels)
+    if a.dtype != np.uint8:
+        raise ValueError(f"{who}: dtype {a.dtype}, expected uint8")
+    if a.ndim == 2:
+        a = a[:, :, None]
+    if a.ndim != 3 or a.shape[2] not in (1, 3):
+        raise ValueError(f"{who}: shape {a.shape}, expected [H, W, 1] or [H, W, 3]")
+    return np.ascontiguousarray(a)
+
+
+def compress_bound(shape, quality=75, subsampling="4:2:0", optimize=False) -> int:
+    """Output bytes compress_async never exceeds for an [H, W, C] picture (host-only)."""
+    lib = load()
+    pin, out = _pixels_in(None, shape, int(shape[1]) * int(shape[2])), C.c_size_t(0)
+    jp = _jpeg_params(quality, subsampling, optimize, "compress_bound")
+    if lib.jpegqs_cuda_compress_bound(C.byref(pin), C.byref(jp), C.byref(out)) < 0:
+        raise QsError(lib.jpegqs_cuda_last_error(None).decode())
+    return int(out.value)
+
+
+def compress_model(pixels, quality=75, subsampling="4:2:0", optimize=False, capacity=None) -> bytes:
+    """compress_async's algorithm on one CPU thread for one picture (jpegqs_cuda_compress_model): a uint8
+    array [H, W, 3] (RGB), [H, W, 1] or [H, W] (grey) to the bytes of Pillow's
+    Image.fromarray(P).save(f, "JPEG", quality=quality, subsampling=subsampling, optimize=optimize).
+    capacity: output bytes (default compress_bound); a file that does not fit raises QsError."""
+    lib = load()
+    a = _host_picture(pixels, "compress_model")
+    jp = _jpeg_params(quality, subsampling, optimize, "compress_model")
+    cap = int(capacity) if capacity is not None else compress_bound(a.shape, quality, subsampling, optimize)
+    out = np.zeros(max(cap, 1), dtype=np.uint8)
+    pin = _pixels_in(a.ctypes.data, a.shape, a.shape[1] * a.shape[2])
+    n, st = C.c_uint64(0), C.c_int32(0)
+    if lib.jpegqs_cuda_compress_model(C.byref(pin), C.byref(jp), out.ctypes.data, cap, C.byref(n), C.byref(st)) < 0:
+        raise QsError(lib.jpegqs_cuda_last_error(None).decode())
+    if st.value:
+        raise QsError(f"compress_model: encoder status {st.value}, {n.value} bytes needed of {cap}")
+    return out[:n.value].tobytes()
 
 
 def _stream_handle(stream) -> C.c_void_p:
@@ -1437,6 +1523,130 @@ class QsContext:
                 _stream_handle(stream)))
         return out, lengths, st
 
+    def compress_async(self, pixels, quality=75, subsampling="4:2:0", optimize=False, out=None, stream=None):
+        """Write device pictures as the JPEG files Pillow's Image.save(quality=, subsampling=,
+        optimize=) writes for them, without blocking the calling thread (jpegqs_cuda_compress_async).
+
+        pixels: uint8 CUDA tensors [H, W, C], C = 3 (RGB) or 1 (grey), whose last two dimensions are
+        contiguous (a row stride of at least W * C is taken, so crops of a bigger picture work).
+        quality / subsampling / optimize: Pillow's keywords ("4:4:4", "4:2:2", "4:2:0" or 0, 1, 2;
+        grey pictures ignore subsampling).  out[i] (optional): 1-D uint8 CUDA tensors to write, their
+        size the capacity; by default allocated on the stream at compress_bound's size.  stream: a
+        torch.cuda.Stream (default: the current one).  Returns (out, lengths [n] int64, status [n]
+        int32), all on the device; status is 0, or ENCODE_OVERFLOW with lengths[i] the size needed.
+        Capturable with torch.cuda.graph: a replay compresses the current contents of the same tensors."""
+        import torch
+        jp = _jpeg_params(quality, subsampling, optimize, "compress_async")
+        n = len(pixels)
+        if out is not None and len(out) != n:
+            raise ValueError("compress_async: out must have one entry per picture")
+        device = self.device if self.device >= 0 else torch.cuda.current_device()
+        pins = (_PixelsIn * max(n, 1))()
+        for i, t in enumerate(pixels):
+            if not isinstance(t, torch.Tensor):
+                raise TypeError(f"compress_async: pixels[{i}]: expected a torch.Tensor, got {type(t).__name__}")
+            if t.dtype != torch.uint8 or t.dim() != 3 or t.shape[2] not in (1, 3):
+                raise ValueError(f"compress_async: pixels[{i}]: expected a uint8 tensor [H, W, 1|3], got {t.dtype} "
+                                 f"{tuple(t.shape)}")
+            if t.stride(2) != 1 or t.stride(1) != t.shape[2] or t.stride(0) < t.shape[1] * t.shape[2]:
+                raise ValueError(f"compress_async: pixels[{i}]: each row must be contiguous ([H, W, C] with strides "
+                                 "(>= W * C, C, 1))")
+            if not t.is_cuda or t.device.index != device:
+                raise ValueError(f"compress_async: pixels[{i}]: on {t.device}, expected cuda:{device}")
+            pins[i] = _pixels_in(t.data_ptr(), tuple(t.shape), t.stride(0))
+        caps = []
+        if out is not None:
+            for i, t in enumerate(out):
+                if not isinstance(t, torch.Tensor) or t.dtype != torch.uint8 or t.dim() != 1 or not t.is_contiguous():
+                    raise ValueError(f"compress_async: out[{i}]: expected a contiguous 1-D uint8 tensor")
+                if not t.is_cuda or t.device.index != device:
+                    raise ValueError(f"compress_async: out[{i}]: on {t.device}, expected cuda:{device}")
+                caps.append(t.numel())
+        else:
+            for i in range(n):
+                b = C.c_size_t(0)
+                self._check(self.lib.jpegqs_cuda_compress_bound(C.byref(pins[i]), C.byref(jp), C.byref(b)))
+                caps.append(int(b.value))
+        stream = stream if stream is not None else torch.cuda.current_stream(device)
+        with torch.cuda.device(device), torch.cuda.stream(stream):
+            if out is None:
+                out = [torch.empty(c, dtype=torch.uint8, device=device) for c in caps]
+            out = list(out)
+            size = C.c_size_t(0)
+            self._check(self.lib.jpegqs_cuda_compress_workspace_bytes(n, pins, C.byref(jp), C.byref(size)))
+            # allocated on `stream`: reused only by work queued after this call's kernels
+            ws = torch.empty(max(size.value, 1), dtype=torch.uint8, device=device)
+            lengths = torch.empty((n,), dtype=torch.int64, device=device)
+            st = torch.empty((n,), dtype=torch.int32, device=device)
+            outs = (C.c_void_p * max(n, 1))(*[t.data_ptr() for t in out])
+            capa = (C.c_size_t * max(n, 1))(*caps)
+            self._check(self.lib.jpegqs_cuda_compress_async(
+                self.h, n, pins, C.byref(jp), outs, capa, lengths.data_ptr() if n else None, st.data_ptr() if n else None,
+                ws.data_ptr(), size.value, _stream_handle(stream)))
+        return out, lengths, st
+
+    def reencode(self, datas, flags: int, niter: int, quality=75, subsampling="4:2:0", optimize=False, scale_denom=1,
+                 size=None, crop=None, filter="bicubic", max_device_bytes: int = 0):
+        """Many JPEG files to JPEG files of their smoothed pixels (jpegqs_cuda_pixels_batch_jpeg): each
+        file's output is exactly Pillow's Image.fromarray(P).save(f, "JPEG", quality=quality,
+        subsampling=subsampling, optimize=optimize), where P is the picture decode_pixels gives for the
+        same flags, niter, scale_denom, size, crop and filter (a grey file gives a grey JPEG).  Only the
+        files cross the bus.  Returns, in the order of datas, one record per file:
+            (data: bytes, warnings, host_decoded, smoothed, stop, upsampled, reason)
+        with the fields of decode_pixels' records.  ValueError naming the file for a bad quality,
+        subsampling, size, crop or filter, before anything runs; QsError naming a file the reader
+        rejects, the render cannot take, or whose crop falls outside its picture."""
+        if isinstance(datas, (bytes, bytearray, memoryview, str)) or not hasattr(datas, "__len__"):
+            raise TypeError("reencode: datas must be a sequence of bytes-like files")
+        files = [_file_bytes(d, f"reencode: file {i}") for i, d in enumerate(datas)]
+        jp = _jpeg_params(quality, subsampling, optimize, "reencode")
+        if int(max_device_bytes) < 0:
+            raise ValueError("reencode: max_device_bytes must be >= 0")
+        scale = _scale_denom(scale_denom, "reencode")
+        n = len(files)
+        resize = size is not None or crop is not None
+        fcode = _resize_filter(filter, "reencode")
+        if resize:
+            sizes, crops = _resize_boxes(n, size, crop, "reencode")
+        if not n:
+            return []
+        boxes = None
+        if resize:
+            boxes = (_ResizeBox * n)()
+            for i, d in enumerate(files):
+                info = _FileInfo()
+                if self.lib.jpegqs_cuda_transcode_route(d, len(d), None, C.byref(info)) < 0:
+                    raise QsError(f"reencode: file {i}: the reader rejects the file")
+                h, w, _ = _scaled_shape(info.image_width, info.image_height, 1, "hwc", scale)
+                boxes[i] = _resize_box(w, h, sizes[i], crops[i], i, "reencode")
+        ptrs = (C.c_char_p * n)(*files)
+        lens = (C.c_size_t * n)(*[len(d) for d in files])
+        rc = (C.c_int * n)()
+        res = (_PixelsResult * n)()
+        outs = (C.c_void_p * n)()
+        olen = (C.c_size_t * n)()
+        self._check(self.lib.jpegqs_cuda_pixels_batch_jpeg(self.h, n, ptrs, lens, int(flags), int(niter), scale, fcode, boxes,
+                                                           C.byref(jp), int(max_device_bytes), rc, res, outs, olen))
+        try:
+            records, bad = [], None
+            for i in range(n):
+                if rc[i] < 0:
+                    if bad is None:
+                        bad = i
+                    records.append(None)
+                    continue
+                records.append((C.string_at(outs[i], olen[i]), res[i].warnings, res[i].host_decoded, res[i].smoothed,
+                                res[i].stop, res[i].upsampled, (res[i].reason or b"").decode()))
+        finally:
+            for i in range(n):
+                if outs[i]:
+                    self.lib.jpegqs_cuda_transcode_free(outs[i])
+        if bad is not None:
+            if rc[bad] == -2:
+                raise QsError(f"reencode: file {bad}: {self.lib.jpegqs_cuda_last_error(self.h).decode()}")
+            raise QsError(f"reencode: file {bad}: the render takes 1 or 3 components with integral sampling ratios only")
+        return records
+
     # ---- one slab of a sharded image (include/jpegqs_cuda.h "one image sharded by MCU rows") ----
     def run_slab(self, link, slab: CoefImage, rank: int, world: int, row0: Sequence[int],
                  hblk_total: Sequence[int], flags: int, niter: int, coef_ptrs=None, up_ptrs=None, stream: int = 0):
@@ -1707,3 +1917,23 @@ def decode_pixels(datas, flags: int, niter: int, layout: str = "hwc", device: st
     conventions)."""
     return default_context(gpu).decode_pixels(datas, flags, niter, layout, device, max_device_bytes, scale_denom,
                                               size, crop, filter)
+
+
+def compress_async(pixels, quality=75, subsampling="4:2:0", optimize=False, out=None, stream=None):
+    """QsContext.compress_async on the default context of the tensors' device: writes uint8 CUDA pictures
+    [H, W, C] as Pillow's JPEG files in CUDA uint8 tensors, enqueued on `stream` (default: the current
+    one) without waiting.  Returns (out, lengths [n] int64, status [n] int32), all on the device."""
+    import torch
+    first = next(iter(pixels), None)
+    if not isinstance(first, torch.Tensor) or not first.is_cuda:
+        raise ValueError("compress_async: the pixel tensors must be CUDA tensors")
+    return default_context(first.device.index).compress_async(pixels, quality, subsampling, optimize, out, stream)
+
+
+def reencode(datas, flags: int, niter: int, quality=75, subsampling="4:2:0", optimize=False, scale_denom=1, size=None,
+             crop=None, filter="bicubic", max_device_bytes: int = 0, gpu: int = -1):
+    """QsContext.reencode on the default context of CUDA device `gpu`: one record (data, warnings,
+    host_decoded, smoothed, stop, upsampled, reason) per file, data the JPEG file Pillow's save writes for
+    the picture decode_pixels gives with the same arguments."""
+    return default_context(gpu).reencode(datas, flags, niter, quality, subsampling, optimize, scale_denom, size, crop,
+                                         filter, max_device_bytes)
