@@ -241,6 +241,53 @@ int jpegqs_cuda_render_scaled_async(jpegqs_cuda_ctx *ctx, int nimages, const jpe
  * render_async does not render); jpegqs_cuda_last_error(NULL) says why. */
 int jpegqs_cuda_render_model(const jpegqs_cuda_image *img, int upsampled, int layout, int scale_denom, uint8_t *out);
 
+/* ---- EXIF orientation ---------------------------------------------------------------------------
+ * Orientation o (1..8) is the transform Pillow's ImageOps.exif_transpose applies.  The oriented picture
+ * is W' x H' (W' = H, H' = W for o = 5..8), and its pixel (x', y') is pixel (x, y) of the W x H stored one:
+ *     o  Pillow's Image.transpose   (x, y)
+ *     1  (none)                     (x', y')
+ *     2  FLIP_LEFT_RIGHT            (W-1-x', y')
+ *     3  ROTATE_180                 (W-1-x', H-1-y')
+ *     4  FLIP_TOP_BOTTOM            (x', H-1-y')
+ *     5  TRANSPOSE                  (y', x')
+ *     6  ROTATE_270                 (y', H-1-x')
+ *     7  TRANSVERSE                 (W-1-y', H-1-x')
+ *     8  ROTATE_90                  (W-1-y', x')
+ *
+ * jpegqs_cuda_render_scaled_async with a host array of one orientation 1..8 per image (NULL: all 1,
+ * which is render_scaled_async; render_async and render_scaled_async are this call with NULL).
+ * out_dev[i] receives the oriented picture: W' x H' pixels in the layout (CHW planes W' x H'), the
+ * same number of bytes.  The transform happens in the render's store, not as a second pass.  Same
+ * stream rules (no allocation, no synchronisation, graph-capturable; the orientations are fixed at
+ * capture).  A value outside 1..8 returns JPEGQS_ERR_ARG with nothing enqueued. */
+int jpegqs_cuda_render_oriented_async(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image *imgs,
+		const jpegqs_cuda_status *status_dev, int layout, int scale_denom, const int32_t *orientation,
+		uint8_t *const *out_dev, void *stream);
+
+/* Host-only, no device needed.  *orientation = the orientation ImageOps.exif_transpose(Image.open(f))
+ * applies to file f, 1 for none - including every file where Pillow's getexif() raises.  The rules are
+ * those of Pillow 12.2 (JpegImagePlugin, Image.getexif, Image.Exif.load, TiffImagePlugin
+ * ImageFileDirectory_v2), not the EXIF specification's:
+ *   - Segments: only those before the first SOS.  The first APP1 starting "Exif\0\0" is the EXIF
+ *     block and later ones are appended without those 6 bytes; of the APP1s starting
+ *     "http://ns.adobe.com/xap/1.0/\0" (XMP), the last one counts.
+ *   - EXIF: leading "Exif\0\0"s are dropped; an empty block has no tags.  A TIFF header "II*\0",
+ *     "MM\0*" (or the swapped "II\0*", "MM*\0") and IFD0 at its offset; any other header, a BigTIFF
+ *     one or fewer than 8 bytes make getexif raise (1, XMP not read).  Of IFD0's 0x0112 entries the
+ *     last one kept wins.  An entry of an unknown type or with count 0 is skipped; an entry cut short,
+ *     or whose data lies past the block, ends the IFD and keeps the entries before it.
+ *   - Value: the first value, as Pillow decodes the type, looked up in a dict of 2..8: SHORT, LONG,
+ *     the signed integers, FLOAT / DOUBLE and (SIGNED) RATIONAL equal to one of them count (6, 6.0 and
+ *     12/2 all give 6); BYTE, UNDEFINED and ASCII decode to bytes or str and give 1, as does any
+ *     other number.
+ *   - XMP, only when the EXIF has no 0x0112 entry: the first match of tiff:Orientation(="|>)([0-9]);
+ *     its digit if 2..8, else 1.
+ * Only [data, data + len) is read, whatever the offsets and counts say, and nothing past the first SOS
+ * segment.  Returns 0, or JPEGQS_ERR_ARG for a file whose markers up to the first SOS the tool's reader
+ * rejects (jpegqs_cuda_jpeg_parse's header walk; jpegqs_cuda_last_error(NULL) has the message). */
+#define JPEGQS_ORIENT_FILE 0  /* in the batch calls' orientation arrays: the file's own orientation */
+int jpegqs_cuda_jpeg_orientation(const uint8_t *data, size_t len, int32_t *orientation);
+
 /* ---- JPEG files to quantized coefficients -----------------------------------------------------
  * The first stage of a device pipeline: JPEG bytes -> the coefficients jpeg_read_coefficients gives,
  * as [hblk][wblk][64] int16 arrays, exactly what jpegqs_cuda_run_async and jpegqs_cuda_render_async
@@ -699,6 +746,22 @@ int jpegqs_cuda_pixels_batch_resized(jpegqs_cuda_ctx *ctx, int n, const uint8_t 
 int jpegqs_cuda_resize_model(const uint8_t *src, int width, int height, int channels, int layout, int filter,
 		const jpegqs_cuda_resize_box *box, uint8_t *out);
 
+/* jpegqs_cuda_pixels_batch_resized (boxes != NULL) or _scaled (boxes NULL, filter ignored) with one
+ * orientation per file: 1..8 as for jpegqs_cuda_render_oriented_async, or JPEGQS_ORIENT_FILE (0) for
+ * the file's own (jpegqs_cuda_jpeg_orientation's).  orientation NULL is 1 for every file: the call is
+ * then byte for byte the existing one.
+ *   - The render writes the oriented picture; the crop and the resize then take it as it is, so a box
+ *     is in the oriented 1/d picture (Pillow's exif_transpose, then crop, then resize).  A crop valid
+ *     only in the unoriented picture fails that file alone with JPEGQS_ERR_ARG.
+ *   - Unresized, out[i] is the oriented picture: for 5..8, H' x W' x C (or C planes of H' rows of W')
+ *     with W' and H' as in the table above - the same number of bytes.  Budgets do not change.
+ *   - Return.  As the existing calls', and an entry outside 0..8 is a bad argument (JPEGQS_ERR_ARG,
+ *     nothing done). */
+int jpegqs_cuda_pixels_batch_oriented(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int layout, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
+		const int32_t *orientation, int out_on_device, uint8_t *const *out, size_t max_device_bytes, int *rc,
+		jpegqs_cuda_pixels_result *results);
+
 /* ---- 8-bit pictures -> JPEG files: Pillow's Image.save, byte for byte ---------------------------
  * Picture i's file is exactly what Pillow (with its libjpeg-turbo) writes for
  *     Image.fromarray(P).save(f, "JPEG", quality=quality, subsampling=subsampling, optimize=optimize)
@@ -785,6 +848,14 @@ int jpegqs_cuda_pixels_batch_jpeg(jpegqs_cuda_ctx *ctx, int n, const uint8_t *co
 		int flags, int niter, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
 		const jpegqs_cuda_jpeg_params *params, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results,
 		uint8_t **out, size_t *out_len);
+
+/* jpegqs_cuda_pixels_batch_jpeg with orientation as for jpegqs_cuda_pixels_batch_oriented: file i is
+ * Pillow's exif_transpose(P) (or P.transpose for an explicit value), then crop / resize, then save - a
+ * JFIF file with upright pixels and no orientation tag.  NULL: byte for byte pixels_batch_jpeg. */
+int jpegqs_cuda_pixels_batch_jpeg_oriented(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
+		const jpegqs_cuda_jpeg_params *params, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results,
+		uint8_t **out, size_t *out_len, const int32_t *orientation);
 
 /* ---- one image sharded by MCU rows over several GPUs (SURVEY.md 8e) ----------------------
  * Every rank - a device of this process, or another process on the same box - smooths one slab

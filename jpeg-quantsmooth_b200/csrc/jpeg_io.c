@@ -266,3 +266,146 @@ int jpegqs_cuda_jpeg_prefix(const uint8_t *data, size_t len, int copy, uint8_t *
 	if (out && cap < n) { qs_set_host_error("jpegqs_cuda_jpeg_prefix: the prefix does not fit out (*out_len holds its size)"); return JPEGQS_ERR_ARG; }
 	return 0;
 }
+
+/* ------------------------------------------------------------------------------------------
+ * EXIF orientation (include/jpegqs_cuda.h jpegqs_cuda_jpeg_orientation): the transform Pillow's
+ * ImageOps.exif_transpose applies after Image.open, restated from what Pillow does with the bytes,
+ * not from the EXIF specification.  Every read stays inside the segment it belongs to.
+ * ------------------------------------------------------------------------------------------ */
+#define EXIF_RAISES (-1)      /* Pillow's getexif raises: no transform, and no XMP fallback */
+#define EXIF_NO_TAG 0         /* no 0x0112 entry: the XMP packet decides */
+
+static uint32_t exif_u16(const uint8_t *p, int be) { return be ? (uint32_t)p[0] << 8 | p[1] : (uint32_t)p[1] << 8 | p[0]; }
+static uint32_t exif_u32(const uint8_t *p, int be) {
+	return be ? (uint32_t)p[0] << 24 | (uint32_t)p[1] << 16 | (uint32_t)p[2] << 8 | p[3]
+	          : (uint32_t)p[3] << 24 | (uint32_t)p[2] << 16 | (uint32_t)p[1] << 8 | p[0];
+}
+
+/* bytes per value of each TIFF type Pillow loads (TiffImagePlugin's _load_dispatch); 0: skipped */
+static int exif_unit(uint32_t typ) {
+	static const unsigned char unit[17] = {0, 1, 1, 2, 4, 8, 1, 1, 2, 4, 8, 4, 8, 4, 0, 0, 8};
+	return typ < 17 ? unit[typ] : 0;
+}
+
+/* 2..8 when the first value of an entry of type typ, as Pillow decodes it, equals that integer in a
+ * Python dict lookup; 1 otherwise (bytes, str, NaN, other numbers) */
+static int exif_value(uint32_t typ, const uint8_t *v, int be) {
+	int64_t k = 0;
+	switch (typ) {
+	case 3: k = exif_u16(v, be); break;                               /* SHORT */
+	case 4: case 13: k = exif_u32(v, be); break;                      /* LONG, IFD */
+	case 6: k = (int8_t)v[0]; break;                                  /* SIGNED BYTE */
+	case 8: k = (int16_t)exif_u16(v, be); break;                      /* SIGNED SHORT */
+	case 9: k = (int32_t)exif_u32(v, be); break;                      /* SIGNED LONG */
+	case 16: {                                                        /* LONG8 */
+		uint64_t hi = exif_u32(v + (be ? 0 : 4), be), lo = exif_u32(v + (be ? 4 : 0), be);
+		k = hi ? 0 : (int64_t)lo; break;
+	}
+	case 5: case 10: {                                                /* (SIGNED) RATIONAL: a Fraction */
+		uint32_t a = exif_u32(v, be), b = exif_u32(v + 4, be);
+		int64_t num = typ == 5 ? (int64_t)a : (int64_t)(int32_t)a, den = typ == 5 ? (int64_t)b : (int64_t)(int32_t)b;
+		k = den != 0 && num % den == 0 ? num / den : 0; break;
+	}
+	case 11: case 12: {                                               /* FLOAT, DOUBLE */
+		double d;
+		if (typ == 11) { uint32_t u = exif_u32(v, be); float f; memcpy(&f, &u, 4); d = f; }
+		else { uint64_t u = (uint64_t)exif_u32(v + (be ? 0 : 4), be) << 32 | exif_u32(v + (be ? 4 : 0), be); memcpy(&d, &u, 8); }
+		k = d >= 2 && d <= 8 && d == (double)(int)d ? (int)d : 0; break;
+	}
+	default: return 1;                                                /* BYTE, ASCII, UNDEFINED */
+	}
+	return k >= 2 && k <= 8 ? (int)k : 1;
+}
+
+/* Image.Exif.load and ImageFileDirectory_v2.load on the EXIF bytes d[0 .. n) (the first block without,
+ * the later ones with their "Exif\0\0" stripped): EXIF_RAISES, EXIF_NO_TAG, or 1..8 from the last 0x0112
+ * entry of IFD0 that Pillow keeps */
+static int exif_ifd0_orientation(const uint8_t *d, size_t n) {
+	size_t p, i, count; int be, found = EXIF_NO_TAG;
+	while (n >= 6 && !memcmp(d, "Exif\0\0", 6)) { d += 6; n -= 6; }
+	if (!n) return EXIF_NO_TAG;
+	/* the TIFF header: byte order, 42 (or the swapped 42 Pillow also accepts); a BigTIFF header (43)
+	 * raises, as does one shorter than 8 bytes */
+	if (n < 4 || (memcmp(d, "MM\0*", 4) && memcmp(d, "II*\0", 4) && memcmp(d, "MM*\0", 4) && memcmp(d, "II\0*", 4)))
+		return EXIF_RAISES;
+	if (n < 8) return EXIF_RAISES;
+	be = d[0] == 'M';
+	p = exif_u32(d + 4, be);
+	if (p > n || n - p < 2) return EXIF_NO_TAG;       /* the entry count cannot be read: an empty IFD */
+	count = exif_u16(d + p, be);
+	p += 2;
+	for (i = 0; i < count; i++, p += 12) {
+		uint32_t tag, typ; uint64_t size; const uint8_t *v;
+		if (n - p < 12) break;                         /* a cut entry ends the IFD, keeping what was read */
+		tag = exif_u16(d + p, be); typ = exif_u16(d + p + 2, be);
+		if (!exif_unit(typ)) continue;                 /* a type Pillow does not load */
+		size = (uint64_t)exif_u32(d + p + 4, be) * (uint64_t)exif_unit(typ);
+		v = d + p + 8;
+		if (size > 4) {
+			uint32_t off = exif_u32(d + p + 8, be);
+			if (off > n || n - off < size) break;          /* a read past the data ends the IFD */
+			v = d + off;
+		}
+		if (!size) continue;                           /* an entry without data is not kept */
+		if (tag == 0x0112) found = exif_value(typ, v, be);
+	}
+	return found;
+}
+
+/* the first decimal digit of the first "tiff:Orientation=\"" or "tiff:Orientation>" directly followed
+ * by one (Pillow's regular expression), as the orientation; 1 if none */
+static int xmp_orientation(const uint8_t *x, size_t n) {
+	static const char key[] = "tiff:Orientation";
+	const size_t k = sizeof(key) - 1;
+	size_t i;
+	for (i = 0; i + k < n; i++) {
+		size_t j = i + k;
+		if (memcmp(x + i, key, k)) continue;
+		if (x[j] == '=' && j + 2 < n && x[j + 1] == '"' && x[j + 2] >= '0' && x[j + 2] <= '9') j += 2;
+		else if (x[j] == '>' && j + 1 < n && x[j + 1] >= '0' && x[j + 1] <= '9') j += 1;
+		else continue;
+		return x[j] >= '2' && x[j] <= '8' ? x[j] - '0' : 1;
+	}
+	return 1;
+}
+
+int jpegqs_cuda_jpeg_orientation(const uint8_t *data, size_t len, int32_t *orientation) {
+	static const char xmp_id[] = "http://ns.adobe.com/xap/1.0/";     /* with its NUL: 29 bytes */
+	jq_image im; jq_header h; char err[256]; size_t p = 2, xmp_at = 0, xmp_len = 0, nexif = 0; uint8_t *exif = NULL; int o;
+	if (!data || !orientation) { qs_set_host_error("jpegqs_cuda_jpeg_orientation: NULL argument"); return JPEGQS_ERR_ARG; }
+	/* the reader's walk up to the first SOS, where Pillow stops too: no entropy-coded byte is read */
+	if (jq_read_header(data, len, &im, &h, err)) { qs_set_host_error(err); return JPEGQS_ERR_ARG; }
+	jq_free(&im);
+	/* the segments before the first SOS, as Pillow's JpegImageFile._open walks them */
+	while (p < len) {
+		unsigned m; size_t seg;
+		if (data[p] != 0xFF) { p++; continue; }
+		while (p < len && data[p] == 0xFF) p++;
+		if (p >= len) break;
+		m = data[p++];
+		if (m == 0xDA) break;
+		if (m == 0 || m == 0x01 || (m >= 0xD0 && m <= 0xD9)) continue;   /* no length field */
+		if (len - p < 2) break;
+		seg = (size_t)data[p] << 8 | data[p + 1];
+		if (seg < 2 || seg > len - p) break;
+		if (m == 0xE1) {
+			const uint8_t *s = data + p + 2; size_t sn = seg - 2;
+			if (sn >= 6 && !memcmp(s, "Exif\0\0", 6)) {
+				/* the first block whole, the later ones without their prefix */
+				const uint8_t *add = nexif ? s + 6 : s; size_t an = nexif ? sn - 6 : sn;
+				uint8_t *grown = (uint8_t *)realloc(exif, nexif + an + 1);
+				if (!grown) { free(exif); qs_set_host_error("jpegqs_cuda_jpeg_orientation: out of memory"); return JPEGQS_ERR_ARG; }
+				exif = grown; memcpy(exif + nexif, add, an); nexif += an;
+			} else if (sn >= sizeof(xmp_id) && !memcmp(s, xmp_id, sizeof(xmp_id))) {
+				xmp_at = p + 2 + sizeof(xmp_id); xmp_len = sn - sizeof(xmp_id);
+			}
+		}
+		p += seg;
+	}
+	o = exif ? exif_ifd0_orientation(exif, nexif) : EXIF_NO_TAG;
+	free(exif);
+	if (o == EXIF_RAISES) o = 1;
+	else if (o == EXIF_NO_TAG) o = xmp_len ? xmp_orientation(data + xmp_at, xmp_len) : 1;
+	*orientation = o;
+	return 0;
+}

@@ -302,6 +302,7 @@ extern "C" int jpegqs_cuda_create(int device, jpegqs_cuda_ctx **out) {
 			CK(qs_set_chunks(ch, n));
 		}
 		CK(qs_smooth_configure());
+		CK(qs_render_configure());
 		CK(cudaMalloc(&ctx->jobs_dev, 2 * QS_MAX_JOBS * sizeof(QsJob)));
 		CK(cudaMalloc(&ctx->flags_dev, (QS_MAX_JOBS + 1) * sizeof(int)));
 		CK(cudaMallocHost(&ctx->flags_host, QS_MAX_JOBS * sizeof(int)));
@@ -2166,23 +2167,26 @@ static int qs_render_desc(const jpegqs_cuda_image *im, int scale_denom, int stat
 	}
 	r.width = (int32_t)((im->image_width + scale_denom - 1) / scale_denom);
 	r.height = (int32_t)((im->image_height + scale_denom - 1) / scale_denom);
-	r.out = out; r.ncomp = (uint8_t)im->ncomp; r.ycc = im->is_ycbcr ? 1 : 0;
+	r.out = out; r.ncomp = (uint8_t)im->ncomp; r.ycc = im->is_ycbcr ? 1 : 0; r.orient = 1;
 	return 0;
 }
 
-/* jpegqs_cuda_render_scaled_async with the layout and scale checked by the caller; grey_store != 0 writes
+/* jpegqs_cuda_render_oriented_async with the layout and scale checked by the caller; grey_store != 0 writes
  * 1-component images with one byte per pixel (either layout: the single plane).  Consecutive images of
- * one store mode share a launch. */
+ * one store mode share a launch.  orient: NULL (all 1) or 1..8 per image. */
 int qs_render_images(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image *imgs,
-		const jpegqs_cuda_status *status_dev, int layout, int grey_store, int scale_denom, uint8_t *const *out_dev,
-		void *stream) {
+		const jpegqs_cuda_status *status_dev, int layout, int grey_store, int scale_denom, const int32_t *orient,
+		uint8_t *const *out_dev, void *stream) {
 	const char *bad = nimages < 0 || (nimages && (!imgs || !out_dev)) ? "images or outputs missing" : NULL;
+	for (int i = 0; i < nimages && !bad && orient; i++)
+		if (orient[i] < 1 || orient[i] > 8) bad = "orientation outside 1..8";
 	std::vector<QsRenderImg> d(bad ? 0 : nimages);
 	std::vector<int> store(d.size());
 	int unsupported = 0;
 	for (int i = 0; i < nimages && !bad && !unsupported; i++) {
 		const jpegqs_cuda_image *im = &imgs[i];
 		unsupported = qs_render_desc(im, scale_denom, status_dev != NULL, 0, out_dev[i], d[i], bad);
+		if (orient) d[i].orient = (uint8_t)orient[i];
 		store[i] = grey_store && im->ncomp == 1 ? QS_RENDER_GREY : layout;
 	}
 	if (unsupported) {
@@ -2216,8 +2220,9 @@ static int qs_scale_ok(int scale_denom) {
 	return scale_denom == 1 || scale_denom == 2 || scale_denom == 4 || scale_denom == 8;
 }
 
-extern "C" int jpegqs_cuda_render_scaled_async(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image *imgs,
-		const jpegqs_cuda_status *status_dev, int layout, int scale_denom, uint8_t *const *out_dev, void *stream) {
+extern "C" int jpegqs_cuda_render_oriented_async(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image *imgs,
+		const jpegqs_cuda_status *status_dev, int layout, int scale_denom, const int32_t *orientation,
+		uint8_t *const *out_dev, void *stream) {
 	if (!ctx) return JPEGQS_ERR_ARG;
 	if (!(nimages < 0 || (nimages && (!imgs || !out_dev))) && layout != JPEGQS_RENDER_HWC && layout != JPEGQS_RENDER_CHW) {
 		snprintf(ctx->err, sizeof(ctx->err), "render_async: unknown layout");
@@ -2227,7 +2232,12 @@ extern "C" int jpegqs_cuda_render_scaled_async(jpegqs_cuda_ctx *ctx, int nimages
 		snprintf(ctx->err, sizeof(ctx->err), "render_async: scale_denom must be 1, 2, 4 or 8");
 		return JPEGQS_ERR_ARG;
 	}
-	return qs_render_images(ctx, nimages, imgs, status_dev, layout, 0, scale_denom, out_dev, stream);
+	return qs_render_images(ctx, nimages, imgs, status_dev, layout, 0, scale_denom, orientation, out_dev, stream);
+}
+
+extern "C" int jpegqs_cuda_render_scaled_async(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image *imgs,
+		const jpegqs_cuda_status *status_dev, int layout, int scale_denom, uint8_t *const *out_dev, void *stream) {
+	return jpegqs_cuda_render_oriented_async(ctx, nimages, imgs, status_dev, layout, scale_denom, NULL, out_dev, stream);
 }
 
 extern "C" int jpegqs_cuda_render_async(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image *imgs,

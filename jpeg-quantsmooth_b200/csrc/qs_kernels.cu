@@ -23,6 +23,7 @@
 #include <stdint.h>
 #include <limits.h>
 #include <string.h>
+#include <type_traits>
 #include <vector>
 #include "qs_common.h"
 #include "qs_kernels.h"
@@ -1948,6 +1949,7 @@ __host__ __device__ __forceinline__ void qs_idct_scaled(const int *cf, int ss, u
 static_assert(QS_RENDER_TW == 128 && QS_RENDER_TH == 64, "the shared sample window is sized for 128 x 64 tiles");
 
 struct QsRenderPack { QsRenderImg img[QS_RENDER_PACK]; };
+static_assert(sizeof(QsRenderImg) == 496, "orient sits in the padding before q");
 static_assert(sizeof(QsRenderPack) + 2 * sizeof(void *) + 2 * sizeof(int) <= 32764,
 		"QS_RENDER_PACK exceeds the kernel parameter space");
 
@@ -1959,10 +1961,47 @@ struct QsSmemPx {
 
 struct QsRenderComp { const int16_t *coef; int wblk, bx0, by0, nbx, nby, cw, ch, hs, vs; };
 
+/* the oriented store's staging (orientations 5..8): one byte plane per channel of the tile's 64 rows, each
+ * padded to an odd pitch so that the column reads of a half-warp fall in different banks */
+#define QS_RT_TB_PITCH (QS_RENDER_TW + 1)
+#define QS_RT_TB_PLANE (QS_RENDER_TH * QS_RT_TB_PITCH)
+#define QS_RT_TB_BYTES (3 * QS_RT_TB_PLANE)
+
+/* pixels px[0 .. cnt) (cnt >= 4: all four) to the consecutive output pixels pos, pos + 1, ...; plane: the
+ * pixels of one CHW plane.  Aligned groups of four go out as 32-bit words. */
+template <int STORE>
+__device__ __forceinline__ void qs_render_store4(uint8_t *out, size_t plane, size_t pos, const uint32_t px[4], int cnt) {
+	if (STORE == QS_RENDER_HWC) {
+		uint8_t *o = out + pos * 3;
+		if (cnt >= 4 && !((uintptr_t)o & 3)) {
+			uint32_t *o4 = (uint32_t *)o;
+			o4[0] = px[0] | (px[1] << 24);
+			o4[1] = (px[1] >> 8) | (px[2] << 16);
+			o4[2] = (px[2] >> 16) | (px[3] << 8);
+		} else {
+			for (int i = 0; i < 4 && i < cnt; i++) {
+				o[3 * i] = (uint8_t)px[i]; o[3 * i + 1] = (uint8_t)(px[i] >> 8); o[3 * i + 2] = (uint8_t)(px[i] >> 16);
+			}
+		}
+	} else {
+#pragma unroll
+		for (int k = 0; k < (STORE == QS_RENDER_GREY ? 1 : 3); k++) {
+			uint8_t *o = out + (size_t)k * plane + pos;
+			if (cnt >= 4 && !((uintptr_t)o & 3)) {
+				*(uint32_t *)o = __byte_perm(__byte_perm(px[0], px[1], 0x0040 + 0x0011 * k),
+						__byte_perm(px[2], px[3], 0x0040 + 0x0011 * k), 0x5410);
+			} else {
+				for (int i = 0; i < 4 && i < cnt; i++) o[i] = (uint8_t)(px[i] >> (8 * k));
+			}
+		}
+	}
+}
+
 /* STORE: QS_RENDER_HWC / QS_RENDER_CHW (three bytes per pixel), or QS_RENDER_GREY (one byte per pixel,
  * the CHW store of plane 0 only; for 1-component images).  D: the scale denominator (1, 2, 4, 8); the
- * descriptors then hold the scaled geometry (qs_render_images). */
-template <int STORE, int D>
+ * descriptors then hold the scaled geometry (qs_render_images).  ORIENTED: some image of the launch has an
+ * orientation other than 1; without it the kernel holds only the unoriented store. */
+template <int STORE, int D, bool ORIENTED>
 __global__ void __launch_bounds__(QS_RT_THREADS, 2) qs_render_async_kernel(const __grid_constant__ QsRenderPack p,
 		int n, const int2 *__restrict__ status) {
 	__shared__ __align__(16) uint8_t pix[3][QS_RS_H * QS_RS_W];
@@ -2051,56 +2090,112 @@ __global__ void __launch_bounds__(QS_RT_THREADS, 2) qs_render_async_kernel(const
 	const int ls0 = D == 1 ? 3 : glss[0], ls1 = D == 1 ? 3 : glss[1], ls2 = D == 1 ? 3 : glss[2];
 	const QsSmemPx P0{pix[0], g[0].bx0 << ls0, g[0].by0 << ls0}, P1{pix[1], g[1].bx0 << ls1, g[1].by0 << ls1},
 			P2{pix[2], g[2].bx0 << ls2, g[2].by0 << ls2};
-	const int lane = threadIdx.x & 31, ox = x0 + lane * 4;
-	if (ox > x1) return;
+	const int lane = threadIdx.x & 31;
 	const bool ycc = nc >= 3 && im.ycc;
-	for (int oy = y0 + (threadIdx.x >> 5); oy <= y1; oy += QS_RT_THREADS / 32) {
-		uint32_t px[4];
-#pragma unroll
-		for (int i = 0; i < 4; i++) {
-			const int x = min(ox + i, x1);
-			const int y = qs_upsample_at<D != 8>(P0, g[0].hs, g[0].vs, g[0].cw, g[0].ch, x, oy);
-			int c1 = y, c2 = y;
-			if (nc >= 3) {
-				c1 = qs_upsample_at<D != 8>(P1, g[1].hs, g[1].vs, g[1].cw, g[1].ch, x, oy);
-				c2 = qs_upsample_at<D != 8>(P2, g[2].hs, g[2].vs, g[2].cw, g[2].ch, x, oy);
-			}
-			px[i] = qs_rgb_pixel(y, c1, c2, ycc);
+	const size_t plane = (size_t)W * H;
+	auto pixel = [&](int x, int y) -> uint32_t {
+		const int l = qs_upsample_at<D != 8>(P0, g[0].hs, g[0].vs, g[0].cw, g[0].ch, x, y);
+		int c1 = l, c2 = l;
+		if (nc >= 3) {
+			c1 = qs_upsample_at<D != 8>(P1, g[1].hs, g[1].vs, g[1].cw, g[1].ch, x, y);
+			c2 = qs_upsample_at<D != 8>(P2, g[2].hs, g[2].vs, g[2].cw, g[2].ch, x, y);
 		}
-		const bool full = ox + 3 <= x1;
-		if (STORE == QS_RENDER_HWC) {
-			uint8_t *o = im.out + ((size_t)oy * W + ox) * 3;
-			if (full && !((uintptr_t)o & 3)) {
-				uint32_t *o4 = (uint32_t *)o;
-				o4[0] = px[0] | (px[1] << 24);
-				o4[1] = (px[1] >> 8) | (px[2] << 16);
-				o4[2] = (px[2] >> 16) | (px[3] << 8);
-			} else {
-				for (int i = 0; i < 4 && ox + i <= x1; i++) {
-					o[3 * i] = (uint8_t)px[i]; o[3 * i + 1] = (uint8_t)(px[i] >> 8); o[3 * i + 2] = (uint8_t)(px[i] >> 16);
-				}
-			}
-		} else {
+		return qs_rgb_pixel(l, c1, c2, ycc);
+	};
+	const int orient = ORIENTED ? im.orient : 1;         /* CTA-uniform */
+	if (!ORIENTED || orient < 5) {
+		/* 1 and the flips: a lane renders four consecutive pixels of an output row, output columns c0..c1
+		 * holding the tile's source columns x0..x1 (mirrored for 2 and 3), from output row oy or H-1-oy */
+		auto rows = [&](auto flips) {
+			constexpr bool F = decltype(flips)::value;
+			const bool mx = F && (orient == 2 || orient == 3), my = F && (orient == 3 || orient == 4);
+			const int c0 = mx ? W - 1 - x1 : x0, c1 = mx ? W - 1 - x0 : x1, oc = c0 + lane * 4;
+			if (oc > c1) return;
+			for (int oy = y0 + (threadIdx.x >> 5); oy <= y1; oy += QS_RT_THREADS / 32) {
+				uint32_t px[4];
 #pragma unroll
-			for (int k = 0; k < (STORE == QS_RENDER_GREY ? 1 : 3); k++) {
-				uint8_t *o = im.out + (size_t)k * W * H + (size_t)oy * W + ox;
-				if (full && !((uintptr_t)o & 3)) {
-					*(uint32_t *)o = __byte_perm(__byte_perm(px[0], px[1], 0x0040 + 0x0011 * k),
-							__byte_perm(px[2], px[3], 0x0040 + 0x0011 * k), 0x5410);
-				} else {
-					for (int i = 0; i < 4 && ox + i <= x1; i++) o[i] = (uint8_t)(px[i] >> (8 * k));
+				for (int i = 0; i < 4; i++) {
+					const int c = min(oc + i, c1);
+					px[i] = pixel(mx ? W - 1 - c : c, oy);
+				}
+				qs_render_store4<STORE>(im.out, plane, (size_t)(my ? H - 1 - oy : oy) * W + oc, px, c1 - oc + 1);
+			}
+		};
+		if (orient <= 1) rows(std::false_type());       /* unoriented: the flips compile away */
+		else rows(std::true_type());
+		return;
+	}
+	if constexpr (ORIENTED) {
+		/* 5..8 swap the axes: the tile's pixels go to tb (QS_RT_TB_BYTES of dynamic shared memory, one byte
+		 * plane per channel, QS_RT_TB_PITCH bytes per row), then every source column x0..x1 is written as
+		 * part of output row x (5, 6) or W-1-x (7, 8), a half-warp per row and four pixels per lane, so the
+		 * global stores stay row-contiguous.  The output is H pixels wide. */
+		extern __shared__ __align__(16) uint8_t tb[];
+		constexpr int NK = STORE == QS_RENDER_GREY ? 1 : 3;
+		const int ox = x0 + lane * 4;
+		if (ox <= x1)
+			for (int oy = y0 + (threadIdx.x >> 5); oy <= y1; oy += QS_RT_THREADS / 32) {
+				uint8_t *row = tb + (oy - y0) * QS_RT_TB_PITCH + (ox - x0);
+#pragma unroll
+				for (int i = 0; i < 4; i++) {
+					const uint32_t v = pixel(min(ox + i, x1), oy);
+#pragma unroll
+					for (int k = 0; k < NK; k++) row[k * QS_RT_TB_PLANE + i] = (uint8_t)(v >> (8 * k));
 				}
 			}
+		__syncthreads();
+		const bool mc = orient == 6 || orient == 7, mr = orient == 7 || orient == 8;
+		const int c0 = mc ? H - 1 - y1 : y0, c1 = mc ? H - 1 - y0 : y1, oc = c0 + (threadIdx.x & 15) * 4;
+		if (oc > c1) return;
+		for (int r = threadIdx.x >> 4; r <= x1 - x0; r += QS_RT_THREADS / 16) {
+			uint32_t px[4];
+#pragma unroll
+			for (int i = 0; i < 4; i++) {
+				const int c = min(oc + i, c1);
+				const uint8_t *s = tb + ((mc ? H - 1 - c : c) - y0) * QS_RT_TB_PITCH + r;
+				px[i] = s[0];
+				if (NK == 3) px[i] |= (uint32_t)s[QS_RT_TB_PLANE] << 8 | (uint32_t)s[2 * QS_RT_TB_PLANE] << 16;
+			}
+			const int orow = mr ? W - 1 - (x0 + r) : x0 + r;
+			qs_render_store4<STORE>(im.out, plane, (size_t)orow * H + oc, px, c1 - oc + 1);
 		}
 	}
 }
 
+template <int D, bool O>
+static void qs_launch_render_store(const QsRenderPack &pack, int n, int tiles, const int2 *status, int store,
+		size_t smem, cudaStream_t st) {
+	if (store == QS_RENDER_HWC) qs_render_async_kernel<QS_RENDER_HWC, D, O><<<tiles, QS_RT_THREADS, smem, st>>>(pack, n, status);
+	else if (store == QS_RENDER_CHW) qs_render_async_kernel<QS_RENDER_CHW, D, O><<<tiles, QS_RT_THREADS, smem, st>>>(pack, n, status);
+	else qs_render_async_kernel<QS_RENDER_GREY, D, O><<<tiles, QS_RT_THREADS, smem, st>>>(pack, n, status);
+}
+
+/* oriented: some image has an orientation other than 1; smem: the staging of 5..8, or 0 */
 template <int D>
 static void qs_launch_render_scaled(const QsRenderPack &pack, int n, int tiles, const int2 *status, int store,
-		cudaStream_t st) {
-	if (store == QS_RENDER_HWC) qs_render_async_kernel<QS_RENDER_HWC, D><<<tiles, QS_RT_THREADS, 0, st>>>(pack, n, status);
-	else if (store == QS_RENDER_CHW) qs_render_async_kernel<QS_RENDER_CHW, D><<<tiles, QS_RT_THREADS, 0, st>>>(pack, n, status);
-	else qs_render_async_kernel<QS_RENDER_GREY, D><<<tiles, QS_RT_THREADS, 0, st>>>(pack, n, status);
+		bool oriented, size_t smem, cudaStream_t st) {
+	if (oriented) qs_launch_render_store<D, true>(pack, n, tiles, status, store, smem, st);
+	else qs_launch_render_store<D, false>(pack, n, tiles, status, store, 0, st);
+}
+
+template <int D>
+static cudaError_t qs_render_configure_d(void) {
+	const void *k[3] = {(const void *)qs_render_async_kernel<QS_RENDER_HWC, D, true>,
+			(const void *)qs_render_async_kernel<QS_RENDER_CHW, D, true>,
+			(const void *)qs_render_async_kernel<QS_RENDER_GREY, D, true>};
+	for (int i = 0; i < 3; i++) {
+		cudaError_t e = cudaFuncSetAttribute(k[i], cudaFuncAttributeMaxDynamicSharedMemorySize, QS_RT_TB_BYTES);
+		if (e != cudaSuccess) return e;
+	}
+	return cudaSuccess;
+}
+
+cudaError_t qs_render_configure(void) {
+	cudaError_t e = qs_render_configure_d<1>();
+	if (e == cudaSuccess) e = qs_render_configure_d<2>();
+	if (e == cudaSuccess) e = qs_render_configure_d<4>();
+	if (e == cudaSuccess) e = qs_render_configure_d<8>();
+	return e;
 }
 
 cudaError_t qs_launch_render_async(const QsRenderImg *imgs, int n, int tiles, const int2 *status, int store,
@@ -2110,11 +2205,18 @@ cudaError_t qs_launch_render_async(const QsRenderImg *imgs, int n, int tiles, co
 	QsRenderPack pack;
 	memcpy(pack.img, imgs, (size_t)n * sizeof(QsRenderImg));
 	if (n < QS_RENDER_PACK) memset(pack.img + n, 0, (size_t)(QS_RENDER_PACK - n) * sizeof(QsRenderImg));
+	bool oriented = false;
+	size_t smem = 0;                                     /* the staging of the transposing orientations */
+	for (int i = 0; i < n; i++) {
+		if (imgs[i].orient < 1 || imgs[i].orient > 8) return cudaErrorInvalidValue;
+		if (imgs[i].orient > 1) oriented = true;
+		if (imgs[i].orient >= 5) smem = QS_RT_TB_BYTES;
+	}
 	switch (scale_denom) {
-	case 1: qs_launch_render_scaled<1>(pack, n, tiles, status, store, st); break;
-	case 2: qs_launch_render_scaled<2>(pack, n, tiles, status, store, st); break;
-	case 4: qs_launch_render_scaled<4>(pack, n, tiles, status, store, st); break;
-	case 8: qs_launch_render_scaled<8>(pack, n, tiles, status, store, st); break;
+	case 1: qs_launch_render_scaled<1>(pack, n, tiles, status, store, oriented, smem, st); break;
+	case 2: qs_launch_render_scaled<2>(pack, n, tiles, status, store, oriented, smem, st); break;
+	case 4: qs_launch_render_scaled<4>(pack, n, tiles, status, store, oriented, smem, st); break;
+	case 8: qs_launch_render_scaled<8>(pack, n, tiles, status, store, oriented, smem, st); break;
 	default: return cudaErrorInvalidValue;
 	}
 	return cudaGetLastError();

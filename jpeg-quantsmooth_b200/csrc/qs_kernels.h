@@ -57,6 +57,8 @@ typedef struct {
 	uint8_t up_mode;             /* 0: coef, 1: coef_up (host flag), 2: status[i].upsampled decides */
 	uint8_t lss;                 /* scale_denom > 1: bits 2c..2c+1 hold log2 of component c's DCT scaled
 	                                size; width, height, cw, ch, hs and vs are then the scaled ones */
+	uint8_t orient;              /* 1..8: EXIF orientation of the output (include/jpegqs_cuda.h); width and
+	                                height stay the unoriented picture's, out is H x W for 5..8 */
 	uint16_t q[3][64];           /* multipliers: the raw quant table where it de-quantizes, else ones */
 } QsRenderImg;
 #define QS_RENDER_PACK 60
@@ -66,7 +68,9 @@ typedef struct {
 #define QS_RENDER_CHW 1
 #define QS_RENDER_GREY 2
 /* status: the launch's first image's {stop, upsampled}, or NULL when no image has up_mode 2;
- * scale_denom: 1, 2, 4 or 8 */
+ * scale_denom: 1, 2, 4 or 8; an orient outside 1..8 gives cudaErrorInvalidValue */
+/* the render kernels' opt-in to the dynamic shared memory of orientations 5..8 (once per device) */
+cudaError_t qs_render_configure(void);
 cudaError_t qs_launch_render_async(const QsRenderImg *imgs, int n, int tiles, const int2 *status, int store,
 		int scale_denom, cudaStream_t st);
 /* the same render of one image on the calling thread: host coefficient and output pointers, up_mode 0

@@ -32,8 +32,8 @@ extern "C" int qs_route_plan(const uint8_t *data, size_t len, int copy, jpegqs_c
 		uint8_t **prefix, size_t *prefix_len, const char **reason);
 int qs_render_takes(const jpegqs_cuda_image *im);                     /* qs_cuda.cu */
 int qs_render_images(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image *imgs,
-		const jpegqs_cuda_status *status_dev, int layout, int grey_store, int scale_denom, uint8_t *const *out_dev,
-		void *stream);
+		const jpegqs_cuda_status *status_dev, int layout, int grey_store, int scale_denom, const int32_t *orient,
+		uint8_t *const *out_dev, void *stream);
 
 /* ---- the packing kernel -------------------------------------------------------------------------
  * After encode_async, file k of a sub-batch sits at the start of its bound-sized slot.  One launch
@@ -187,6 +187,7 @@ struct QsPlan {
 	int host;                                  /* pixels: the host reader decodes it */
 	int smooth, can_up;
 	int out_w, out_h;                          /* pixels: the output picture's size */
+	int orient, pic_w;                         /* pixels: the render's orientation (1..8), the rendered picture's width */
 	size_t in_bytes, coef_bytes, up_bytes, cap, pix;
 	size_t ws_dec, ws_run, ws_enc;             /* this file's share of each stage's workspace */
 	size_t fixed, packed;                      /* its share of the buffers outside the workspace; of the packed output */
@@ -600,11 +601,14 @@ struct QsJpegLayout {
 
 /* boxes != NULL: each file's picture is cropped and resized (qs_resize.cu) with filter.  jp != NULL: the
  * pictures are written as JPEG files with these params (compress_async) into jout / jlen, and on_device
- * must be 0 (the pictures stay in the context's buffers). */
+ * must be 0 (the pictures stay in the context's buffers).  orientation: NULL (1 for every file) or 0..8
+ * per file, 0 for the file's own; the render writes the oriented picture, which the crop, the resize
+ * and the compressor then take as it is. */
 static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint8_t *const *data, const size_t *len,
-		int flags, int niter, int layout, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes, int on_device,
-		uint8_t *const *out, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results,
-		const jpegqs_cuda_jpeg_params *jp = NULL, uint8_t **jout = NULL, size_t *jlen = NULL) {
+		int flags, int niter, int layout, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
+		const int32_t *orientation, int on_device, uint8_t *const *out, size_t max_device_bytes, int *rc,
+		jpegqs_cuda_pixels_result *results, const jpegqs_cuda_jpeg_params *jp = NULL, uint8_t **jout = NULL,
+		size_t *jlen = NULL) {
 	char msg[512];
 	cudaStream_t st;
 	std::vector<QsPlan> plans((size_t)n);
@@ -627,11 +631,15 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 			rc[i] = JPEGQS_ERR_ARG; continue;
 		}
 		if (!qs_render_takes(&p.img)) { rc[i] = JPEGQS_ERR_UNSUPPORTED; continue; }
-		/* the picture at scale 1 / scale_denom: ceil(width / d) x ceil(height / d) x channels */
-		const int pw = (int)((p.img.image_width + scale_denom - 1) / scale_denom);
-		const int ph = (int)((p.img.image_height + scale_denom - 1) / scale_denom);
+		/* the picture at scale 1 / scale_denom: ceil(width / d) x ceil(height / d) x channels, its axes
+		 * swapped by orientations 5..8 */
+		p.orient = orientation ? orientation[i] : 1;
+		if (!p.orient && jpegqs_cuda_jpeg_orientation(data[i], len[i], &p.orient)) p.orient = 1;
+		const int sw = (int)((p.img.image_width + scale_denom - 1) / scale_denom);
+		const int sh = (int)((p.img.image_height + scale_denom - 1) / scale_denom);
+		const int pw = p.orient >= 5 ? sh : sw, ph = p.orient >= 5 ? sw : sh;
 		p.pix = (size_t)pw * ph * p.img.ncomp;
-		p.out_w = pw; p.out_h = ph;
+		p.out_w = pw; p.out_h = ph; p.pic_w = pw;
 		if (boxes) {
 			const char *bad = qs_resize_plan(pw, ph, boxes[i], filter, rsp[i]);
 			if (bad) {
@@ -812,8 +820,7 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 			for (int j = 0; j < nr; j++) {
 				const int f = files[rk[j]];
 				const QsResizePlan &r = rsp[f];
-				const int pw = (int)((rimg[j].image_width + scale_denom - 1) / scale_denom);
-				qs_resize_desc(r, pw, rimg[j].ncomp, layout == JPEGQS_RENDER_CHW, desc[j]);
+				qs_resize_desc(r, plans[f].pic_w, rimg[j].ncomp, layout == JPEGQS_RENDER_CHW, desc[j]);
 				memcpy(rh + toff[j], r.tab.data(), r.tab.size() * sizeof(int32_t));
 				desc[j].src = rd + qoff[j]; desc[j].mid = rd + moff[j]; desc[j].out = outs[j];
 				desc[j].tab = (const int32_t*)(rd + toff[j]);
@@ -828,7 +835,10 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 			TK(cudaEventRecord(t->ev1, st));
 		}
 		if (ms < nr) TK(cudaMemsetAsync(run + ms, 0, (size_t)(nr - ms) * sizeof(jpegqs_cuda_status), st));
-		if (nr) TQ(qs_render_images(ctx, nr, rimg.data(), run, boxes ? JPEGQS_RENDER_HWC : layout, 1, scale_denom, outs.data(), st));
+		std::vector<int32_t> ro(nr);
+		for (int j = 0; j < nr; j++) ro[j] = plans[files[rk[j]]].orient;
+		if (nr) TQ(qs_render_images(ctx, nr, rimg.data(), run, boxes ? JPEGQS_RENDER_HWC : layout, 1, scale_denom, ro.data(),
+				outs.data(), st));
 		if (boxes && nr) TK(qs_launch_resize((const QsResizeDesc*)t->rs_dev.p, nr, hblocks, vblocks, st));
 		/* JPEG: compress_async over the pictures into the slots, then the packing kernel into the
 		 * workspace, its records back */
@@ -912,9 +922,20 @@ fail:
 #undef TQ
 
 /* resize != 0: jpegqs_cuda_pixels_batch_resized, with filter and boxes */
+/* an orientation array's check: NULL, or 0..8 per file */
+static int orientation_ok(jpegqs_cuda_ctx *ctx, const char *who, int n, const int32_t *orientation) {
+	char msg[200];
+	for (int i = 0; orientation && i < n; i++) if (orientation[i] < 0 || orientation[i] > 8) {
+		snprintf(msg, sizeof(msg), "%s: file %d: orientation %d outside 0..8", who, i, (int)orientation[i]);
+		qs_ctx_decode_done(ctx, 0, msg); return 0;
+	}
+	return 1;
+}
+
 static int pixels_entry(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint8_t *const *data, const size_t *len,
 		int flags, int niter, int layout, int scale_denom, int resize, int filter, const jpegqs_cuda_resize_box *boxes,
-		int out_on_device, uint8_t *const *out, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results) {
+		int out_on_device, uint8_t *const *out, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results,
+		const int32_t *orientation = NULL) {
 	char msg[200];
 	if (!ctx) return JPEGQS_ERR_ARG;
 	if (n < 0) { snprintf(msg, sizeof(msg), "%s: negative file count", who); qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG; }
@@ -942,9 +963,18 @@ static int pixels_entry(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 			qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG;
 		}
 	}
+	if (!orientation_ok(ctx, who, n, orientation)) return JPEGQS_ERR_ARG;
 	for (int i = 0; i < n; i++) { memset(&results[i], 0, sizeof(results[i])); results[i].reason = ""; rc[i] = 0; }
-	return pixels_batch(ctx, who, n, data, len, flags, niter, layout, scale_denom, filter, resize ? boxes : NULL, out_on_device, out,
-			max_device_bytes, rc, results);
+	return pixels_batch(ctx, who, n, data, len, flags, niter, layout, scale_denom, filter, resize ? boxes : NULL, orientation,
+			out_on_device, out, max_device_bytes, rc, results);
+}
+
+extern "C" int jpegqs_cuda_pixels_batch_oriented(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int layout, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
+		const int32_t *orientation, int out_on_device, uint8_t *const *out, size_t max_device_bytes, int *rc,
+		jpegqs_cuda_pixels_result *results) {
+	return pixels_entry(ctx, "jpegqs_cuda_pixels_batch_oriented", n, data, len, flags, niter, layout, scale_denom,
+			boxes != NULL, filter, boxes, out_on_device, out, max_device_bytes, rc, results, orientation);
 }
 
 extern "C" int jpegqs_cuda_pixels_batch_resized(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
@@ -954,11 +984,10 @@ extern "C" int jpegqs_cuda_pixels_batch_resized(jpegqs_cuda_ctx *ctx, int n, con
 			out_on_device, out, max_device_bytes, rc, results);
 }
 
-extern "C" int jpegqs_cuda_pixels_batch_jpeg(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
+static int pixels_jpeg_entry(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint8_t *const *data, const size_t *len,
 		int flags, int niter, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
 		const jpegqs_cuda_jpeg_params *params, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results,
-		uint8_t **out, size_t *out_len) {
-	static const char who[] = "jpegqs_cuda_pixels_batch_jpeg";
+		uint8_t **out, size_t *out_len, const int32_t *orientation) {
 	char msg[200];
 	if (!ctx) return JPEGQS_ERR_ARG;
 	if (n < 0) { snprintf(msg, sizeof(msg), "%s: negative file count", who); qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG; }
@@ -988,9 +1017,26 @@ extern "C" int jpegqs_cuda_pixels_batch_jpeg(jpegqs_cuda_ctx *ctx, int n, const 
 			qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG;
 		}
 	}
+	if (!orientation_ok(ctx, who, n, orientation)) return JPEGQS_ERR_ARG;
 	for (int i = 0; i < n; i++) { memset(&results[i], 0, sizeof(results[i])); results[i].reason = ""; rc[i] = 0; out[i] = NULL; out_len[i] = 0; }
-	return pixels_batch(ctx, who, n, data, len, flags, niter, JPEGQS_RENDER_HWC, scale_denom, filter, boxes, 0, NULL,
+	return pixels_batch(ctx, who, n, data, len, flags, niter, JPEGQS_RENDER_HWC, scale_denom, filter, boxes, orientation, 0, NULL,
 			max_device_bytes, rc, results, params, out, out_len);
+}
+
+extern "C" int jpegqs_cuda_pixels_batch_jpeg(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
+		const jpegqs_cuda_jpeg_params *params, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results,
+		uint8_t **out, size_t *out_len) {
+	return pixels_jpeg_entry(ctx, "jpegqs_cuda_pixels_batch_jpeg", n, data, len, flags, niter, scale_denom, filter, boxes, params,
+			max_device_bytes, rc, results, out, out_len, NULL);
+}
+
+extern "C" int jpegqs_cuda_pixels_batch_jpeg_oriented(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
+		const jpegqs_cuda_jpeg_params *params, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results,
+		uint8_t **out, size_t *out_len, const int32_t *orientation) {
+	return pixels_jpeg_entry(ctx, "jpegqs_cuda_pixels_batch_jpeg_oriented", n, data, len, flags, niter, scale_denom, filter, boxes,
+			params, max_device_bytes, rc, results, out, out_len, orientation);
 }
 
 extern "C" int jpegqs_cuda_pixels_batch_scaled(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,

@@ -255,6 +255,19 @@ def load():
                                                   C.POINTER(_JpegParams), C.c_size_t, C.POINTER(C.c_int),
                                                   C.POINTER(_PixelsResult), C.POINTER(C.c_void_p),
                                                   C.POINTER(C.c_size_t)]
+    lib.jpegqs_cuda_jpeg_orientation.argtypes = [C.c_char_p, C.c_size_t, C.POINTER(C.c_int32)]
+    lib.jpegqs_cuda_render_oriented_async.argtypes = [C.c_void_p, C.c_int, C.POINTER(_Image), C.c_void_p, C.c_int, C.c_int,
+                                                      C.POINTER(C.c_int32), C.POINTER(C.c_void_p), C.c_void_p]
+    lib.jpegqs_cuda_pixels_batch_oriented.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_size_t),
+                                                      C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(_ResizeBox),
+                                                      C.POINTER(C.c_int32), C.c_int, C.POINTER(C.c_void_p), C.c_size_t,
+                                                      C.POINTER(C.c_int), C.POINTER(_PixelsResult)]
+    lib.jpegqs_cuda_pixels_batch_jpeg_oriented.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_char_p),
+                                                           C.POINTER(C.c_size_t), C.c_int, C.c_int, C.c_int, C.c_int,
+                                                           C.POINTER(_ResizeBox), C.POINTER(_JpegParams), C.c_size_t,
+                                                           C.POINTER(C.c_int), C.POINTER(_PixelsResult),
+                                                           C.POINTER(C.c_void_p), C.POINTER(C.c_size_t),
+                                                           C.POINTER(C.c_int32)]
     lib.jpegqs_cuda_tables.argtypes = [C.c_int, C.c_void_p]
     lib.jpegqs_cuda_orig_coef.argtypes = [C.c_int, C.c_int]
     _lib = lib
@@ -595,6 +608,53 @@ def parse_jpeg_scans(data: bytes):
     if rc not in (0, -3):
         raise QsError(f"parse_jpeg_scans: {lib.jpegqs_cuda_last_error(None).decode()}")
     return image, (ScanList(recs[:n.value]) if rc == 0 else None)
+
+
+def exif_orientation(data: bytes) -> int:
+    """The EXIF orientation 1..8 of a JPEG file (jpegqs_cuda_jpeg_orientation): the transform
+    ImageOps.exif_transpose(Image.open(f)) applies, 1 for none.  QsError for a file the reader rejects."""
+    lib = load()
+    d = _file_bytes(data, "exif_orientation")
+    o = C.c_int32()
+    if lib.jpegqs_cuda_jpeg_orientation(d, len(d), C.byref(o)) < 0:
+        raise QsError(f"exif_orientation: {lib.jpegqs_cuda_last_error(None).decode()}")
+    return o.value
+
+
+def _orient_int(v):
+    return None if isinstance(v, bool) or not isinstance(v, (int, np.integer)) else int(v)
+
+
+def _orientations(orientation, n: int, who: str, lo: int = 0):
+    """None, or one value per file: "exif" gives 0 (the file's own) for every file, an int 1..8 that value
+    for every file, a sequence one value lo..8 per file; ValueError otherwise"""
+    if orientation is None:
+        return None
+    if isinstance(orientation, str):
+        if orientation != "exif":
+            raise ValueError(f"{who}: orientation {orientation!r}: expected 'exif', 1..8 or one value per file")
+        return [0] * n
+    v = _orient_int(orientation)
+    if v is not None:
+        if not 1 <= v <= 8:
+            raise ValueError(f"{who}: orientation {v}: expected 1..8")
+        return [v] * n
+    if isinstance(orientation, (bytes, bytearray)) or not hasattr(orientation, "__len__") or len(orientation) != n:
+        raise ValueError(f"{who}: orientation: expected 'exif', 1..8 or a sequence of {n} values")
+    out = []
+    for i, x in enumerate(orientation):
+        v = _orient_int(x)
+        if v is None or not lo <= v <= 8:
+            raise ValueError(f"{who}: orientation[{i}] {x!r}: expected an int {lo}..8")
+        out.append(v)
+    return out
+
+
+def _oriented_shape(shape, o: int, layout: str):
+    """an unoriented picture's shape as orientation o gives it (5..8 swap width and height)"""
+    if o < 5:
+        return shape
+    return (shape[1], shape[0], shape[2]) if layout == "hwc" else (shape[0], shape[2], shape[1])
 
 
 def _file_bytes(data, what: str) -> bytes:
@@ -938,7 +998,8 @@ class QsContext:
         return out
 
     def decode_pixels(self, datas, flags: int, niter: int, layout: str = "hwc", device: str = "cuda",
-                      max_device_bytes: int = 0, scale_denom: int = 1, size=None, crop=None, filter="bicubic"):
+                      max_device_bytes: int = 0, scale_denom: int = 1, size=None, crop=None, filter="bicubic",
+                      orientation=None):
         """Many JPEG files to the smoothed pixels the jpegqs tool's --ppm writes for them (islow, fancy
         up-sampling, after do_quantsmooth(flags, niter)), in shared launches (jpegqs_cuda_pixels_batch).
         Returns, in the order of datas, one record per file:
@@ -961,7 +1022,12 @@ class QsContext:
         is "bicubic" (Image.resize's default), "bilinear", "lanczos", "box" or "hamming", or Pillow's
         Image.Resampling value of one of them; NEAREST is not supported.  A crop without size returns
         the crop as it is.  Pixels are then [height, width, C] or [C, height, width].  ValueError
-        naming the file index for a bad size, crop or filter, before anything runs."""
+        naming the file index for a bad size, crop or filter, before anything runs.
+        orientation: None (the pixels in the order the file stores them), "exif" (each file's own EXIF
+        orientation, as Pillow's ImageOps.exif_transpose applies it), one int 1..8 for every file, or a
+        sequence of ints 0..8, one per file, 0 meaning the file's own (jpegqs_cuda_pixels_batch_oriented).
+        The picture is turned before the crop and the resize, so crop is in the oriented picture, and for
+        5..8 the unresized pixels have width and height swapped.  ValueError for a bad value or length."""
         if isinstance(datas, (bytes, bytearray, memoryview, str)) or not hasattr(datas, "__len__"):
             raise TypeError("decode_pixels: datas must be a sequence of bytes-like files")
         files = [_file_bytes(d, f"decode_pixels: file {i}") for i, d in enumerate(datas)]
@@ -977,6 +1043,7 @@ class QsContext:
         if resize:
             fcode = _resize_filter(filter, "decode_pixels")
             sizes, crops = _resize_boxes(n, size, crop, "decode_pixels")
+        orient = _orientations(orientation, n, "decode_pixels")
         if not n:
             return []
         # the output size rule of jpegqs_cuda_pixels_batch: transcode_route's width, height and ncomp
@@ -989,6 +1056,9 @@ class QsContext:
                 raise QsError(f"decode_pixels: file {i}: {info.ncomp} components; the render takes 1 or 3")
             c, h, w = info.ncomp, info.image_height, info.image_width
             shapes.append(_scaled_shape(w, h, c, layout, scale))
+        if orient is not None:
+            orient = [exif_orientation(d) if o == 0 else o for d, o in zip(files, orient)]
+            shapes = [_oriented_shape(s, o, layout) for s, o in zip(shapes, orient)]
         if resize:
             boxes = (_ResizeBox * n)()
             for i, s in enumerate(shapes):
@@ -1009,7 +1079,13 @@ class QsContext:
         optrs = (C.c_void_p * n)(*[t.data_ptr() for t in outs])
         rc = (C.c_int * n)()
         res = (_PixelsResult * n)()
-        if resize:
+        if orient is not None:
+            self._check(self.lib.jpegqs_cuda_pixels_batch_oriented(self.h, n, ptrs, lens, int(flags), int(niter),
+                                                                   0 if layout == "hwc" else 1, scale,
+                                                                   fcode if resize else 0, boxes if resize else None,
+                                                                   (C.c_int32 * n)(*orient), int(device == "cuda"),
+                                                                   optrs, int(max_device_bytes), rc, res))
+        elif resize:
             self._check(self.lib.jpegqs_cuda_pixels_batch_resized(self.h, n, ptrs, lens, int(flags), int(niter),
                                                                   0 if layout == "hwc" else 1, scale, fcode, boxes,
                                                                   int(device == "cuda"), optrs, int(max_device_bytes), rc,
@@ -1211,7 +1287,7 @@ class QsContext:
 
     # ---- stream-ordered render to RGB (include/jpegqs_cuda.h jpegqs_cuda_render_async) ----
     def render_async(self, images: Sequence[CoefImage], coefs, status=None, up=None, layout: str = "hwc",
-                     out=None, stream=None, scale_denom: int = 1):
+                     out=None, stream=None, scale_denom: int = 1, orientation=None):
         """Decode device-resident coefficients to 8-bit RGB, as libjpeg would, without blocking the
         calling thread.  The coefficient tensors are only read.
 
@@ -1223,13 +1299,18 @@ class QsContext:
         per-image uint8 CUDA tensors of that shape to write (a batched tensor's unbind(0) will do);
         by default they are allocated on the stream.  stream: a torch.cuda.Stream (default: the
         current one).  scale_denom 2, 4 or 8: libjpeg's scaled decode (jpegqs_cuda_render_scaled_async),
-        H and W then being ceil(height / d) and ceil(width / d).  Capturable with torch.cuda.graph.
-        Returns the list of output tensors."""
+        H and W then being ceil(height / d) and ceil(width / d).  orientation: None, or a sequence of
+        one EXIF orientation 1..8 per image (jpegqs_cuda_render_oriented_async); each output is then the
+        picture as Pillow's Image.transpose turns it, with H and W swapped for 5..8.  Capturable with
+        torch.cuda.graph.  Returns the list of output tensors."""
         import torch
         n = len(images)
         if layout not in ("hwc", "chw"):
             raise ValueError(f"layout {layout!r}: expected 'hwc' or 'chw'")
         d = _scale_denom(scale_denom, "render_async")
+        if orientation is not None and (isinstance(orientation, (str, bytes)) or _orient_int(orientation) is not None):
+            raise ValueError("render_async: orientation: expected a sequence of one value 1..8 per image")
+        orient = _orientations(orientation, n, "render_async", lo=1)
         if len(coefs) != n or (up is not None and len(up) != n) or (out is not None and len(out) != n):
             raise ValueError("images, coefs, up and out must have one entry per image")
         host_up = None
@@ -1259,6 +1340,8 @@ class QsContext:
                 raise ValueError(f"status: expected a contiguous int32 tensor [{n}, 2]")
             tensors.append(("status", status))
         shapes = [_scaled_shape(im.width, im.height, 3, layout, d) for im in images]
+        if orient is not None:
+            shapes = [_oriented_shape(s, o, layout) for s, o in zip(shapes, orient)]
         if out is not None:
             for i, t in enumerate(out):
                 if not isinstance(t, torch.Tensor):
@@ -1287,7 +1370,11 @@ class QsContext:
                 arr[i].upsampled = int(bool(host_up and host_up[i]))
             outs = (C.c_void_p * max(n, 1))(*[t.data_ptr() for t in out])
             st = status.data_ptr() if isinstance(status, torch.Tensor) else None
-            if d == 1:
+            if orient is not None:
+                self._check(self.lib.jpegqs_cuda_render_oriented_async(self.h, n, arr, st, 0 if layout == "hwc" else 1, d,
+                                                                       (C.c_int32 * max(n, 1))(*orient), outs,
+                                                                       _stream_handle(stream)))
+            elif d == 1:
                 self._check(self.lib.jpegqs_cuda_render_async(self.h, n, arr, st, 0 if layout == "hwc" else 1, outs,
                                                               _stream_handle(stream)))
             else:
@@ -1586,7 +1673,7 @@ class QsContext:
         return out, lengths, st
 
     def reencode(self, datas, flags: int, niter: int, quality=75, subsampling="4:2:0", optimize=False, scale_denom=1,
-                 size=None, crop=None, filter="bicubic", max_device_bytes: int = 0):
+                 size=None, crop=None, filter="bicubic", max_device_bytes: int = 0, orientation=None):
         """Many JPEG files to JPEG files of their smoothed pixels (jpegqs_cuda_pixels_batch_jpeg): each
         file's output is exactly Pillow's Image.fromarray(P).save(f, "JPEG", quality=quality,
         subsampling=subsampling, optimize=optimize), where P is the picture decode_pixels gives for the
@@ -1595,7 +1682,9 @@ class QsContext:
             (data: bytes, warnings, host_decoded, smoothed, stop, upsampled, reason)
         with the fields of decode_pixels' records.  ValueError naming the file for a bad quality,
         subsampling, size, crop or filter, before anything runs; QsError naming a file the reader
-        rejects, the render cannot take, or whose crop falls outside its picture."""
+        rejects, the render cannot take, or whose crop falls outside its picture.  orientation: as for
+        decode_pixels (jpegqs_cuda_pixels_batch_jpeg_oriented); "exif" gives Pillow's
+        ImageOps.exif_transpose(P).save(...): upright pixels in a JFIF file without the tag."""
         if isinstance(datas, (bytes, bytearray, memoryview, str)) or not hasattr(datas, "__len__"):
             raise TypeError("reencode: datas must be a sequence of bytes-like files")
         files = [_file_bytes(d, f"reencode: file {i}") for i, d in enumerate(datas)]
@@ -1608,16 +1697,20 @@ class QsContext:
         fcode = _resize_filter(filter, "reencode")
         if resize:
             sizes, crops = _resize_boxes(n, size, crop, "reencode")
+        orient = _orientations(orientation, n, "reencode")
         if not n:
             return []
         boxes = None
+        if orient is not None:
+            orient = [exif_orientation(d) if o == 0 else o for d, o in zip(files, orient)]
         if resize:
             boxes = (_ResizeBox * n)()
             for i, d in enumerate(files):
                 info = _FileInfo()
                 if self.lib.jpegqs_cuda_transcode_route(d, len(d), None, C.byref(info)) < 0:
                     raise QsError(f"reencode: file {i}: the reader rejects the file")
-                h, w, _ = _scaled_shape(info.image_width, info.image_height, 1, "hwc", scale)
+                h, w, _ = _oriented_shape(_scaled_shape(info.image_width, info.image_height, 1, "hwc", scale),
+                                          orient[i] if orient is not None else 1, "hwc")
                 boxes[i] = _resize_box(w, h, sizes[i], crops[i], i, "reencode")
         ptrs = (C.c_char_p * n)(*files)
         lens = (C.c_size_t * n)(*[len(d) for d in files])
@@ -1625,8 +1718,13 @@ class QsContext:
         res = (_PixelsResult * n)()
         outs = (C.c_void_p * n)()
         olen = (C.c_size_t * n)()
-        self._check(self.lib.jpegqs_cuda_pixels_batch_jpeg(self.h, n, ptrs, lens, int(flags), int(niter), scale, fcode, boxes,
-                                                           C.byref(jp), int(max_device_bytes), rc, res, outs, olen))
+        if orient is not None:
+            self._check(self.lib.jpegqs_cuda_pixels_batch_jpeg_oriented(self.h, n, ptrs, lens, int(flags), int(niter), scale,
+                                                                        fcode, boxes, C.byref(jp), int(max_device_bytes),
+                                                                        rc, res, outs, olen, (C.c_int32 * n)(*orient)))
+        else:
+            self._check(self.lib.jpegqs_cuda_pixels_batch_jpeg(self.h, n, ptrs, lens, int(flags), int(niter), scale, fcode,
+                                                               boxes, C.byref(jp), int(max_device_bytes), rc, res, outs, olen))
         try:
             records, bad = [], None
             for i in range(n):
@@ -1872,7 +1970,7 @@ def decode_async(images: Sequence[CoefImage], scans, data, out=None, stream=None
 
 
 def render_async(images: Sequence[CoefImage], coefs, status=None, up=None, layout: str = "hwc", out=None,
-                 stream=None, scale_denom: int = 1):
+                 stream=None, scale_denom: int = 1, orientation=None):
     """QsContext.render_async on the default context of the tensors' device: decodes CUDA
     coefficient tensors to uint8 RGB tensors ([H, W, 3] or [3, H, W], at 1/scale_denom size),
     enqueued on `stream` (default: the current one) without waiting."""
@@ -1880,7 +1978,8 @@ def render_async(images: Sequence[CoefImage], coefs, status=None, up=None, layou
     first = next((t for ts in coefs for t in ts), None)
     if not isinstance(first, torch.Tensor) or not first.is_cuda:
         raise ValueError("render_async: the coefficient tensors must be CUDA tensors")
-    return default_context(first.device.index).render_async(images, coefs, status, up, layout, out, stream, scale_denom)
+    return default_context(first.device.index).render_async(images, coefs, status, up, layout, out, stream, scale_denom,
+                                                            orientation)
 
 
 def encode_async(images: Sequence[CoefImage], coefs, heads, optimize: bool = False, status=None, up=None, out=None,
@@ -1910,13 +2009,13 @@ def transcode_batch(datas, flags: int, niter: int, optimize: bool = False, copy:
 
 
 def decode_pixels(datas, flags: int, niter: int, layout: str = "hwc", device: str = "cuda", max_device_bytes: int = 0,
-                  gpu: int = -1, scale_denom: int = 1, size=None, crop=None, filter="bicubic"):
+                  gpu: int = -1, scale_denom: int = 1, size=None, crop=None, filter="bicubic", orientation=None):
     """QsContext.decode_pixels on the default context of CUDA device `gpu`: one record (pixels, warnings,
     host_decoded, smoothed, stop, upsampled, reason) per file, at 1/scale_denom size, cropped and resized
     as Pillow would with size / crop / filter ((width, height) and (left, top, right, bottom), Pillow's
-    conventions)."""
+    conventions), turned by `orientation` ("exif", 1..8, or one value 0..8 per file) first."""
     return default_context(gpu).decode_pixels(datas, flags, niter, layout, device, max_device_bytes, scale_denom,
-                                              size, crop, filter)
+                                              size, crop, filter, orientation)
 
 
 def compress_async(pixels, quality=75, subsampling="4:2:0", optimize=False, out=None, stream=None):
@@ -1931,9 +2030,9 @@ def compress_async(pixels, quality=75, subsampling="4:2:0", optimize=False, out=
 
 
 def reencode(datas, flags: int, niter: int, quality=75, subsampling="4:2:0", optimize=False, scale_denom=1, size=None,
-             crop=None, filter="bicubic", max_device_bytes: int = 0, gpu: int = -1):
+             crop=None, filter="bicubic", max_device_bytes: int = 0, gpu: int = -1, orientation=None):
     """QsContext.reencode on the default context of CUDA device `gpu`: one record (data, warnings,
     host_decoded, smoothed, stop, upsampled, reason) per file, data the JPEG file Pillow's save writes for
     the picture decode_pixels gives with the same arguments."""
     return default_context(gpu).reencode(datas, flags, niter, quality, subsampling, optimize, scale_denom, size, crop,
-                                         filter, max_device_bytes)
+                                         filter, max_device_bytes, orientation)

@@ -125,3 +125,30 @@ for sub_bytes in (32, 512):
     torch.cuda.synchronize()
     print("decode_scans_async key 9 =", sub_bytes, len(pfiles), "images, status", status.cpu().tolist(), flush=True)
 ctx.set_tuning(9, 512)
+
+
+# EXIF orientation: files with spliced EXIF / XMP payloads (a tag of each transposing kind, a truncated IFD,
+# a value offset past the block, an XMP packet) through the host reader, then the oriented render of
+# every orientation in one launch (the flips and the staged transposes side by side), at d = 1 and 2
+import struct  # noqa: E402
+
+
+def app1(payload):
+    return b"\xff\xe1" + struct.pack(">H", len(payload) + 2) + payload
+
+
+def exif_tag(o, cut=None, off=None):
+    e = struct.pack("<HHLHH", 0x0112, 3, 1 if off is None else 3, o, 0) if off is None else \
+        struct.pack("<HHLL", 0x0112, 3, 3, off)
+    p = b"Exif\0\0II*\0" + struct.pack("<LH", 8, 1) + e + b"\0\0\0\0"
+    return p[:cut] if cut else p
+
+
+payloads = [exif_tag(6), exif_tag(8), exif_tag(5, cut=20), exif_tag(7, off=4000),
+            b"http://ns.adobe.com/xap/1.0/\0<x tiff:Orientation=\"7\"/>"]
+ofiles = [f[:2] + app1(p) + f[2:] for f in (good[0], good[3], good[5]) for p in payloads]
+print("exif orientations", [qs.exif_orientation(f) for f in ofiles], flush=True)
+for d in (1, 2):
+    px = ctx.decode_pixels(ofiles, 3, 1, scale_denom=d, orientation=[0, 1, 2, 3, 4] * 2 + [5, 6, 7, 8, 0])
+    torch.cuda.synchronize()
+    print("decode_pixels oriented d", d, [tuple(p[0].shape) for p in px], flush=True)
