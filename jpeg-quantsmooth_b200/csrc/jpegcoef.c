@@ -1306,22 +1306,23 @@ static void seg_finish(jq_seg *sg) {
 /* MCU rows [y0, y1): walk = 1 only tracks the DC predictors (used for the row above a segment) */
 static int enc_rows(jq_enc *e, JDIMENSION y0, JDIMENSION y1, int *pred, jq_seg *sg, long (*fr)[257], int walk) {
 	struct jpeg_decompress_struct *ci = &e->im->cinfo;
-	JDIMENSION x, y; int k;
+	JDIMENSION x, y; int k, single = ci->num_components == 1;  /* one component: one block per MCU */
 	static const JCOEF zero[64] = { 0 };
 	for (y = y0; y < y1; y++) {
 		JBLOCKROW rows[MAX_COMPONENTS][4];
 		for (k = 0; k < ci->num_components; k++) {
-			jpeg_component_info *c = &ci->comp_info[k]; int v;
-			for (v = 0; v < c->v_samp_factor && v < 4; v++) {
-				JDIMENSION by = y * c->v_samp_factor + v;
+			jpeg_component_info *c = &ci->comp_info[k]; int v, vf = single ? 1 : c->v_samp_factor;
+			for (v = 0; v < vf && v < 4; v++) {
+				JDIMENSION by = y * vf + v;
 				rows[k][v] = by < c->height_in_blocks ?
 						(*ci->mem->access_virt_barray)((j_common_ptr)ci, e->arrays[k], by, 1, FALSE)[0] : NULL;
 			}
 		}
 		for (x = 0; x < e->mcux; x++) for (k = 0; k < ci->num_components; k++) {
 			jpeg_component_info *c = &ci->comp_info[k]; int h, v, t = k ? 1 : 0;
-			for (v = 0; v < c->v_samp_factor; v++) for (h = 0; h < c->h_samp_factor; h++) {
-				JDIMENSION bx = x * c->h_samp_factor + h;
+			int hf = single ? 1 : c->h_samp_factor, vf = single ? 1 : c->v_samp_factor;
+			for (v = 0; v < vf; v++) for (h = 0; h < hf; h++) {
+				JDIMENSION bx = x * hf + h;
 				JCOEF dummy[64];
 				const JCOEF *blk;
 				if (bx < c->width_in_blocks && rows[k][v]) blk = rows[k][v][bx];
@@ -1521,6 +1522,9 @@ static int enc_pass(jq_image *im, jvirt_barray_ptr *arrays, jq_out *o, jq_ehuff 
 	memset(&e, 0, sizeof(e));
 	e.im = im; e.arrays = arrays;
 	e.mcux = (ci->image_width + 8 * maxh - 1) / (8 * maxh); e.mcuy = (ci->image_height + 8 * maxv - 1) / (8 * maxv);
+	if (ci->num_components == 1) {                       /* not interleaved: one block per MCU (A.2.2) */
+		e.mcux = ci->comp_info[0].width_in_blocks; e.mcuy = ci->comp_info[0].height_in_blocks;
+	}
 	if (!e.mcuy || !e.mcux) return 0;
 	for (k = 0; k < ci->num_components; k++) if (ci->comp_info[k].v_samp_factor > 4) return -1;
 	pthread_once(&zz_mask_once, zz_mask_init);
@@ -1612,7 +1616,7 @@ int jq_write(jq_image *im, jvirt_barray_ptr *arrays, int optimize, unsigned char
 	dc = (jq_ehuff*)calloc(2, sizeof(*dc)); ac = (jq_ehuff*)calloc(2, sizeof(*ac));
 	if (!dc || !ac) { free(dc); free(ac); snprintf(err, 256, "out of memory"); return -1; }
 	for (k = 0; k < ci->num_components; k++) blocks += ci->comp_info[k].h_samp_factor * ci->comp_info[k].v_samp_factor;
-	if (blocks > 10) { snprintf(err, 256, "more than 10 blocks per MCU: not written as one interleaved scan"); goto fail; }
+	if (ci->num_components > 1 && blocks > 10) { snprintf(err, 256, "more than 10 blocks per MCU: not written as one interleaved scan"); goto fail; }
 	if (optimize) {
 		if (enc_pass(im, arrays, NULL, dc, ac)) { snprintf(err, 256, "coefficient out of range for Huffman coding"); goto fail; }
 		for (i = 0; i < nt; i++) { ehuff_optimal(&dc[i]); ehuff_optimal(&ac[i]); }

@@ -97,7 +97,8 @@ static const uint8_t qe_std_ac_c[162] = {
 struct QeGeo {                         /* one scan geometry of an image */
 	const int16_t *coef[4];
 	uint32_t wblk[4], hblk[4];
-	uint8_t hs[4], vs[4];
+	uint8_t hs[4], vs[4];              /* blocks of the component in one MCU: 1 x 1 in a scan of one component */
+	uint8_t sof_hv[4];                 /* the sampling factors the SOF gives */
 	uint32_t mcux, mcuy, nblk, pad;
 	uint8_t u_comp[QE_MAX_UNITS], u_h[QE_MAX_UNITS], u_v[QE_MAX_UNITS], pad1[2];
 	uint64_t nunits;                   /* mcux * mcuy * nblk */
@@ -392,7 +393,7 @@ HD static inline uint64_t qe_header(const QeImg &im, const QeGeo &g, const QeTab
 	}
 	o.w(0xFF00 | sof); o.w(8 + 3 * nc); o.b(8);
 	o.w(im.height); o.w(im.width); o.b((unsigned)nc);
-	for (int k = 0; k < nc; k++) { o.b((unsigned)im.comp_id[k]); o.b((unsigned)(g.hs[k] << 4 | g.vs[k])); o.b((unsigned)im.qtbl[k]); }
+	for (int k = 0; k < nc; k++) { o.b((unsigned)im.comp_id[k]); o.b((unsigned)g.sof_hv[k]); o.b((unsigned)im.qtbl[k]); }
 	for (int i = 0; i < nt; i++) for (int a = 0; a < 2; a++) {
 		const QeTab &t = tab[2 * i + a];
 		o.w(0xFFC4); o.w(2 + 1 + 16 + t.nval); o.b((unsigned)(a << 4 | i));
@@ -656,21 +657,23 @@ static const char *qe_geometry(const jpegqs_cuda_image *im, QeGeo *g0, QeGeo *g1
 		uint64_t hb = ((uint64_t)im->image_height * cc.v_samp + 8 * maxv - 1) / (8 * maxv);
 		if (cc.wblk != wb || cc.hblk != hb) return "wblk / hblk are not libjpeg's for this image size";
 		g0->coef[c] = cc.coef; g0->wblk[c] = cc.wblk; g0->hblk[c] = cc.hblk;
-		g0->hs[c] = (uint8_t)cc.h_samp; g0->vs[c] = (uint8_t)cc.v_samp;
-		for (int v = 0; v < cc.v_samp; v++) for (int h = 0; h < cc.h_samp; h++) {
+		/* a scan of one component is not interleaved: its MCU is one block, whatever the factors (A.2.2) */
+		g0->hs[c] = nc == 1 ? 1 : (uint8_t)cc.h_samp; g0->vs[c] = nc == 1 ? 1 : (uint8_t)cc.v_samp;
+		g0->sof_hv[c] = (uint8_t)(cc.h_samp << 4 | cc.v_samp);
+		for (int v = 0; v < g0->vs[c]; v++) for (int h = 0; h < g0->hs[c]; h++) {
 			if (nb >= QE_MAX_UNITS) return "more than 10 blocks per MCU";
 			g0->u_comp[nb] = (uint8_t)c; g0->u_h[nb] = (uint8_t)h; g0->u_v[nb] = (uint8_t)v; nb++;
 		}
 	}
 	g0->nblk = nb;
-	g0->mcux = (uint32_t)(((uint64_t)im->image_width + 8 * maxh - 1) / (8 * maxh));
-	g0->mcuy = (uint32_t)(((uint64_t)im->image_height + 8 * maxv - 1) / (8 * maxv));
+	g0->mcux = nc == 1 ? im->comp[0].wblk : (uint32_t)(((uint64_t)im->image_width + 8 * maxh - 1) / (8 * maxh));
+	g0->mcuy = nc == 1 ? im->comp[0].hblk : (uint32_t)(((uint64_t)im->image_height + 8 * maxv - 1) / (8 * maxv));
 	g0->nunits = (uint64_t)g0->mcux * g0->mcuy * nb;
 	*up_ok = qe_can_up(im);
 	if (*up_ok) {
 		for (int c = 0; c < 3; c++) {
 			g1->coef[c] = c ? im->comp[c].coef_up : im->comp[0].coef;
-			g1->wblk[c] = im->comp[0].wblk; g1->hblk[c] = im->comp[0].hblk; g1->hs[c] = g1->vs[c] = 1;
+			g1->wblk[c] = im->comp[0].wblk; g1->hblk[c] = im->comp[0].hblk; g1->hs[c] = g1->vs[c] = 1; g1->sof_hv[c] = 0x11;
 			g1->u_comp[c] = (uint8_t)c;
 		}
 		g1->nblk = 3;

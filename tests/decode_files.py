@@ -77,7 +77,34 @@ def flavours():
     out.append(("keep_rgb", pillow_jpeg(120, 80, quality=90, keep_rgb=True, subsampling=0)))
     for ss in ("411", "440"):
         out.append((f"writer_{ss}", coef_writer_jpeg(make(75, 53, ss, "k50", "synth", 2))))
+    return out + geometry_files()
+
+
+# sizes of 24k +- 1 and 32k +- 1 and below 8, none a multiple of an MCU
+GEOMETRY_SIZES = ((73, 49), (95, 31), (5, 7), (47, 65))
+
+
+def geometry_files():
+    """(name, bytes) of jpeg_write_coefficients files of every geometry of render_images.GEOMETRIES
+    (at most 10 blocks per MCU, one interleaved scan), without restart markers, with one every 7
+    MCUs and with one every MCU row."""
+    import scan_files as sf
+    from render_images import GEOMETRIES
+    out = []
+    for k, ss in enumerate(GEOMETRIES):
+        w, h = GEOMETRY_SIZES[k % len(GEOMETRY_SIZES)]
+        data = coef_writer_jpeg(make(w, h, ss, ("k50", "k90", "rand")[k % 3], ("synth", "saturated")[k % 2], 2 + k))
+        out += [(f"writer_{ss}", data), (f"writer_{ss}_rst7", sf.rescan(data, restart_interval=7)),
+                (f"writer_{ss}_rows1", sf.rescan(data, restart_rows=1))]
     return out
+
+
+def per_component_files():
+    """(name, bytes) of 3x3 and 4x4 luma (11 and 18 blocks per MCU), which libjpeg writes as one scan
+    per component: the device decoders take single interleaved scans only, so these take the host
+    route."""
+    return [(f"writer_{ss}", coef_writer_jpeg(make(w, h, ss, "k50", c, 4))) for ss, w, h, c in
+            (("33", 73, 47, "synth"), ("44", 95, 65, "saturated"))]
 
 
 def hard_sets():

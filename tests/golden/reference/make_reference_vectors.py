@@ -13,6 +13,9 @@ reference built into oracle/_ref by oracle/Makefile:
                       CLI tests generate (tests/test_cli.py, tests/test_real_libjpeg.py) and of
                       the lossless transcodes of tools/codec_difftest.py
   ref_saturated.npz   the reference's results on small saturated-content images
+                      (the sampling geometries of tests/hard_content.py FACTORS: synthetic
+                      content in ref_driver.npz, grey ones in ref_sweep.npz, saturated
+                      content here)
   ref_saturated.json  golden_io.result_digest of its results on wave-scale saturated-content
                       images (tests/hard_content.py; tests/test_oracle_vs_reference.py)
 
@@ -107,6 +110,10 @@ def driver():
     for case in te.ENTRY_CASES:
         flags, niter, ss = case
         gio.put_result(e, tv.case_key("entry", case), *ol.run_reference(qs.synth.make_image(120, 72, ss), flags, niter, scatter_rows=True))
+    for case in tv.GEOMETRY_CASES:               # grey ones in ref_sweep.npz, to keep each under 1 MB
+        if case[4] == "synth":
+            gio.put_result(e if case[2].startswith("g") else d, tv.case_key("geo", case),
+                           *ol.run_reference(*tv.geometry_case(case)))
     _save_npz(os.path.join(HERE, "ref_driver.npz"), d)
     _save_npz(os.path.join(HERE, "ref_sweep.npz"), e)
 
@@ -116,6 +123,9 @@ def saturated():
     d = {}
     for case in tv.SATURATED_SMALL:
         gio.put_result(d, tv.case_key("sat", case), *ol.run_reference(*tv.saturated_case(case)))
+    for case in tv.GEOMETRY_CASES:
+        if case[4] == "saturated":
+            gio.put_result(d, tv.case_key("geo", case), *ol.run_reference(*tv.geometry_case(case)))
     _save_npz(os.path.join(HERE, "ref_saturated.npz"), d)
     digests = {tv.case_key("satw", case): gio.result_digest(*ol.run_reference(*tv.saturated_case(case)))
                for case in tv.SATURATED_WAVE}

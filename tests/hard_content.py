@@ -26,6 +26,31 @@ from jpegqs_b200.image import CoefImage, Component, JCS_GRAYSCALE, JCS_YCbCr, bl
 SAMPLINGS = ("gray", "444", "422", "420", "440")
 _SAMP = {"444": (1, 1), "422": (2, 1), "420": (2, 2), "440": (1, 2)}
 
+# Every other sampling libjpeg codes with integral ratios, as (h, v) factors of Y / Cb / Cr: factors
+# of 3 (box up-sampling by 3, the clipped last cell of the JOINT_YUV down-sample), of 4 on either
+# axis (10 blocks per MCU at 4x2, MCU rows of 4 block rows), more than 10 blocks per MCU (33, 44),
+# a 16x8 MCU whose ratios are all 1, chroma sampled above luma, and two chroma of different factors;
+# and grey files whose SOF gives the one component factors other than 1x1 (a scan of one component
+# has 1-block MCUs, but the picture is still the component's sample grid).
+FACTORS = {"411": ((4, 1), (1, 1), (1, 1)),
+           "31": ((3, 1), (1, 1), (1, 1)), "13": ((1, 3), (1, 1), (1, 1)),
+           "32": ((3, 2), (1, 1), (1, 1)), "23": ((2, 3), (1, 1), (1, 1)),
+           "410": ((4, 2), (1, 1), (1, 1)), "14": ((1, 4), (1, 1), (1, 1)), "24": ((2, 4), (1, 1), (1, 1)),
+           "33": ((3, 3), (1, 1), (1, 1)), "44": ((4, 4), (1, 1), (1, 1)),
+           "21_21_21": ((2, 1), (2, 1), (2, 1)), "11_22_22": ((1, 1), (2, 2), (2, 2)),
+           "22_21_12": ((2, 2), (2, 1), (1, 2)), "41_21_21": ((4, 1), (2, 1), (2, 1)),
+           "g22": ((2, 2),), "g31": ((3, 1),), "g14": ((1, 4),), "g44": ((4, 4),)}
+GEOMETRIES = tuple(k for k in FACTORS if k != "411")
+
+
+def factors(subsampling: str):
+    """(h, v) per component of a sampling name of SAMPLINGS or FACTORS."""
+    if subsampling == "gray":
+        return ((1, 1),)
+    if subsampling in _SAMP:
+        return (_SAMP[subsampling], (1, 1), (1, 1))
+    return FACTORS[subsampling]
+
 
 def saturated_pixels(c: int, y0: int, y1: int, width: int, sx: int, sy: int, seed: int,
                      height: int, full_width: int) -> np.ndarray:
@@ -52,11 +77,10 @@ def saturated_pixels(c: int, y0: int, y1: int, width: int, sx: int, sy: int, see
 def make_image(width: int, height: int, subsampling: str, tables, content: str = "synth",
                seed: int = 12345, chunk_rows: int = 64) -> CoefImage:
     """An image of either content ('synth': synth.pixels; 'saturated': saturated_pixels),
-    quantized with tables = (luma table, chroma table)."""
-    if subsampling == "gray":
-        samp, cs = [(1, 1)], JCS_GRAYSCALE
-    else:
-        samp, cs = [_SAMP[subsampling], (1, 1), (1, 1)], JCS_YCbCr
+    quantized with tables = (luma table, chroma table); subsampling is a name of SAMPLINGS or
+    FACTORS, or a sequence of (h, v) per component."""
+    samp = factors(subsampling) if isinstance(subsampling, str) else tuple(subsampling)
+    cs = JCS_GRAYSCALE if len(samp) == 1 else JCS_YCbCr
     mh, mv = max(s[0] for s in samp), max(s[1] for s in samp)
     comps = []
     for c, (hs, vs) in enumerate(samp):

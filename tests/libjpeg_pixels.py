@@ -113,6 +113,17 @@ static int decode(const char *in, const char *out, const char *jpg) {
 		arr[c] = co.mem->request_virt_barray((j_common_ptr)&co, JPOOL_IMAGE, TRUE,
 				(JDIMENSION)((h[c][2] + h[c][0] - 1) / h[c][0] * h[c][0]), (JDIMENSION)((h[c][3] + h[c][1] - 1) / h[c][1] * h[c][1]), h[c][1]);
 	}
+	{	/* an interleaved scan holds at most 10 blocks per MCU: more (3x3, 4x4 luma) go one scan per component */
+		static jpeg_scan_info one[MAX_COMPS_IN_SCAN]; int n = 0;
+		for (c = 0; c < hdr[0]; c++) n += h[c][0] * h[c][1];
+		if (n > 10 && hdr[0] > 1 && hdr[0] <= MAX_COMPS_IN_SCAN) {
+			for (c = 0; c < hdr[0]; c++) {
+				one[c].comps_in_scan = 1; one[c].component_index[0] = c;
+				one[c].Ss = 0; one[c].Se = 63; one[c].Ah = 0; one[c].Al = 0;
+			}
+			co.scan_info = one; co.num_scans = hdr[0];
+		}
+	}
 	jpeg_write_coefficients(&co, arr);
 	for (c = 0; c < hdr[0]; c++) {
 		if ((int)co.comp_info[c].width_in_blocks != h[c][2] || (int)co.comp_info[c].height_in_blocks != h[c][3])

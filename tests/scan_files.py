@@ -195,3 +195,19 @@ def hard_progressive():
         except lp.LibjpegError:
             continue
     return out
+
+
+def geometry_progressive():
+    """decode_files.geometry_files re-encoded progressive: successive approximation and split bands,
+    with and without restart markers."""
+    out = []
+    for name, data in df.geometry_files():
+        if name.endswith(("_rst7", "_rows1")):
+            continue
+        g = name[len("writer_"):]
+        nc = 1 if g.startswith("g") else 3
+        out.append((f"succ_{g}", rescan(data, successive(nc))))
+        out.append((f"succ_{g}_rst3", rescan(data, successive(nc), restart_interval=3)))
+        out.append((f"split_{g}", rescan(data, split_bands(nc))))
+        out.append((f"split_{g}_rst5", rescan(data, split_bands(nc), restart_interval=5)))
+    return out

@@ -41,6 +41,19 @@ def test_parse_and_read_match_libjpeg(name, data):
     assert _same([c.coef for c in got.comps], ref)
 
 
+@pytest.mark.parametrize("name,data", df.per_component_files(), ids=[n for n, _ in df.per_component_files()])
+def test_per_component_scans_take_the_host_route(name, data):
+    """3x3 and 4x4 luma: more blocks per MCU than one interleaved scan holds, so libjpeg writes one scan
+    per component; the transcode takes the host route and read_jpeg still reads libjpeg's coefficients"""
+    ref = df.libjpeg_coefficients(data)
+    assert [(c.h_samp, c.v_samp) for c in ref.comps][1:] == [(1, 1), (1, 1)] and ref.comps[0].h_samp >= 3
+    assert qs.transcode_route(data) == ("host", "more than 10 blocks per MCU")
+    im, scan = qs.parse_jpeg(data)
+    assert scan is None
+    assert [(a.h_samp, a.v_samp, a.wblk, a.hblk) for a in im.comps] == [(b.h_samp, b.v_samp, b.wblk, b.hblk) for b in ref.comps]
+    assert _same([c.coef for c in qs.read_jpeg(data).comps], ref)
+
+
 def test_parse_rejects():
     data = df.pillow_jpeg(64, 48, quality=75)
     sos = data.index(b"\xff\xda")

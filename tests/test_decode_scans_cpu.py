@@ -17,6 +17,7 @@ pytestmark = pytest.mark.skipif(lp.JPEG_SO is None, reason="no libjpeg inside Pi
 PILLOW = sf.pillow_progressive()
 SCRIPTED = sf.scripted()
 HARD = sf.hard_progressive()
+GEOMETRY = sf.geometry_progressive()
 KNOBS = [cuda.DECODE_SUB_MIN, cuda.DECODE_SUB_DEFAULT]
 
 
@@ -25,7 +26,7 @@ def _same(a, ref):
 
 
 @pytest.mark.parametrize("sub_bytes", KNOBS)
-@pytest.mark.parametrize("name,data", PILLOW + SCRIPTED + HARD, ids=[n for n, _ in PILLOW + SCRIPTED + HARD])
+@pytest.mark.parametrize("name,data", PILLOW + SCRIPTED + HARD + GEOMETRY, ids=[n for n, _ in PILLOW + SCRIPTED + HARD + GEOMETRY])
 def test_model_equals_libjpeg(name, data, sub_bytes):
     ref = df.libjpeg_coefficients(data)
     im, scans = qs.parse_jpeg_scans(data)

@@ -88,6 +88,19 @@ def test_model_equals_the_tool(tmp_path, name, optimize):
     assert model_bytes(data, optimize) == tool_bytes(tmp_path, data, optimize)
 
 
+@pytest.mark.parametrize("name", [n for n, _ in ALL if n.startswith("writer_")])
+def test_written_file_reads_back(name):
+    """jpeg_read_coefficients of the file the encoder writes gives back the coefficients it was given, on
+    every sampling geometry: grey files whose SOF says 2x2, 3x1, 1x4 or 4x4 among them, whose one scan
+    is not interleaved (one block per MCU, in raster order) whatever the factors"""
+    data = dict(ALL)[name]
+    want = df.libjpeg_coefficients(data)
+    for optimize in (False, True):
+        got = df.libjpeg_coefficients(model_bytes(data, optimize))
+        assert [(c.h_samp, c.v_samp) for c in got.comps] == [(c.h_samp, c.v_samp) for c in want.comps]
+        assert all(np.array_equal(a.coef, b.coef) for a, b in zip(got.comps, want.comps)), optimize
+
+
 def test_sixteen_bit_tables_write_sof1(tmp_path):
     names = [n for n, im, _ in df.hard_sets() if any(c.quant is not None and c.quant.max() > 255 for c in im.comps)]
     assert names

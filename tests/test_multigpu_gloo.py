@@ -14,6 +14,8 @@ import torch.multiprocessing as mp
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
+sys.path.insert(0, HERE)
+from hard_content import FACTORS  # noqa: E402
 
 
 def _free_port():
@@ -38,9 +40,13 @@ def _worker(rank, world, port, cfg, outdir):
     if kind:
         full = adversarial_image(kind)
         w, h = full.width, full.height
+    elif ss in FACTORS:
+        full = _geometry_image(w, h, ss)
     total = (h + 15) // 16 if ss != "gray" and (kind or ss in ("420", "440")) else (h + 7) // 8
+    if ss in FACTORS:
+        total = -(-h // (8 * max(c.v_samp for c in full.comps)))
     rng = mg.split_mcu_rows(total, world)[rank]
-    if kind:
+    if kind or ss in FACTORS:
         comps_src = []
         for c in full.comps:
             r0, r1 = mg.comp_block_rows(rng, c.v_samp, c.hblk)
@@ -49,7 +55,7 @@ def _worker(rank, world, port, cfg, outdir):
         slab = qs.synth.make_image(w, h, ss, mcu_rows=rng)
         comps_src = [(c.coef, c) for c in slab.comps]
     comps = []
-    geom_src = full if kind else qs.synth.make_image(w, h, ss, mcu_rows=(0, 0))
+    geom_src = full if kind or ss in FACTORS else qs.synth.make_image(w, h, ss, mcu_rows=(0, 0))
     fullh = [qs.blocks_for(h, c.v_samp, max(cc.v_samp for cc in geom_src.comps)) for c in geom_src.comps]
     for k, (coef, c) in enumerate(comps_src):
         rows = coef.shape[0]
@@ -68,6 +74,11 @@ def _worker(rank, world, port, cfg, outdir):
     dist.destroy_process_group()
 
 
+def _geometry_image(w, h, ss):
+    import hard_content as hc
+    return hc.make_image(w, h, ss, hc.TABLES["k50"], "saturated", seed=w + h)
+
+
 CFGS = [
     (2, (96, 80, "420", 0, 2, None)),
     (3, (64, 112, "420", 1, 2, None)),         # DIAGONALS, uneven split
@@ -79,6 +90,12 @@ CFGS = [
     (2, (48, 64, "444", 7, 2, None)),          # 4:4:4: the luma plane itself is the predictor
     (2, (90, 72, "420", 7, 1, None)),          # ragged size: edge replication inside the last slab
     (2, (0, 0, "420", 7, 2, "badcoef")),       # stop in the chroma phase
+    # hard_content.FACTORS: MCU rows of 3 and 4 block rows, down- / up-sampling by 3 and 4 across slab
+    # boundaries, chroma with more block rows than luma
+    (2, (121, 223, "13", 3, 2, None)), (3, (121, 223, "13", 7, 2, None)),
+    (3, (64, 193, "14", 3, 2, None)), (2, (64, 193, "14", 7, 2, None)),
+    (2, (121, 223, "24", 3, 2, None)), (3, (96, 190, "24", 7, 2, None)),
+    (2, (121, 223, "11_22_22", 3, 2, None)), (3, (121, 223, "11_22_22", 7, 2, None)),
 ]
 
 
@@ -89,7 +106,7 @@ def test_shard_count_invariance(world, cfg):
     import oracle_lib as ol
     from golden_io import adversarial_image
     w, h, ss, flags, niter, kind = cfg
-    full = adversarial_image(kind) if kind else qs.synth.make_image(w, h, ss)
+    full = adversarial_image(kind) if kind else _geometry_image(w, h, ss) if ss in FACTORS else qs.synth.make_image(w, h, ss)
     want_ret, want = ol.run_oracle(full, flags, niter)
     with tempfile.TemporaryDirectory() as d:
         mp.spawn(_worker, args=(world, _free_port(), cfg, d), nprocs=world, join=True)

@@ -10,7 +10,7 @@ import libjpeg_pixels as lp
 import oracle_lib as ol
 import wave_geometry as wg
 from jpegqs_b200 import cuda as qc
-from render_images import SAMPLINGS, make
+from render_images import GEOMETRIES, SAMPLINGS, make
 
 PIL = pytest.importorskip("PIL.Image")
 needs_libjpeg = pytest.mark.skipif(lp.JPEG_SO is None, reason="no libjpeg inside Pillow")
@@ -35,7 +35,7 @@ def test_round_trip_is_pillows_decode(tmp_path, name, w, h, gray, kw):
 
 
 @needs_libjpeg
-@pytest.mark.parametrize("ss", ["440", "411"])
+@pytest.mark.parametrize("ss", ["440", "411"] + list(GEOMETRIES))
 def test_written_file_is_what_pillow_decodes(tmp_path, ss):
     """Samplings Pillow cannot write: the helper's own file, opened by Pillow."""
     path = str(tmp_path / "out.jpg")
@@ -59,7 +59,7 @@ def test_uncodable_coefficients_fail_loudly():
 # coefficients of synthetic and saturated content (letterbox bars, full-contrast strokes, Nyquist
 # checkers, wrapping ramps) under coarse, fine and random quant tables: no pixel differs.
 @needs_libjpeg
-@pytest.mark.parametrize("ss", SAMPLINGS)
+@pytest.mark.parametrize("ss", SAMPLINGS + GEOMETRIES)
 def test_renderer_arithmetic_is_libjpegs(ss):
     for content in ("synth", "saturated"):
         for table in ("k10", "k90", "rand"):

@@ -1,7 +1,7 @@
 """CPU side of the scaled render (include/jpegqs_cuda.h jpegqs_cuda_render_scaled_async): render_model,
 the library's restatement of the render on one CPU thread, is libjpeg's scaled decode (scale_num 1,
 scale_denom d, JDCT_ISLOW, fancy up-sampling) byte for byte, with the SIMD and the C code paths of the
-library, on every sampling the render takes, on sizes where the up-samplers change branch, and on
+library, on every sampling the render takes (render_images.SAMPLINGS and GEOMETRIES), on sizes where the up-samplers change branch, and on
 quantized, oracle-smoothed and saturated coefficient sets.  A numpy restatement of the same rules
 (_restated) is pinned to render_model, and mutants of it - a reduced-IDCT constant, the "no fancy
 up-sampling at scaled size 1" rule, the downsampled-width rounding - each disagree with libjpeg on
@@ -17,7 +17,7 @@ import libjpeg_scaled as ls
 import oracle_lib as ol
 from jpegqs_b200 import cuda as qc
 from jpegqs_b200.image import JCS_YCbCr
-from render_images import SAMPLINGS, make
+from render_images import GEOMETRIES, SAMPLINGS, make
 
 needs_libjpeg = pytest.mark.skipif(lp.JPEG_SO is None, reason="no libjpeg inside Pillow")
 
@@ -126,7 +126,7 @@ def _restated(image, d, mutant=None):
 # ---- render_model against libjpeg ---------------------------------------------------------------
 
 @needs_libjpeg
-@pytest.mark.parametrize("ss", SAMPLINGS)
+@pytest.mark.parametrize("ss", SAMPLINGS + GEOMETRIES)
 def test_model_full_size_is_libjpeg(ss):
     """d = 1 is the unscaled render: libjpeg_pixels' decode and render_async's arithmetic"""
     for name, im in _coefficient_sets(ss, 203, 149):
@@ -138,7 +138,7 @@ def test_model_full_size_is_libjpeg(ss):
 
 @needs_libjpeg
 @pytest.mark.parametrize("d", SCALES)
-@pytest.mark.parametrize("ss", SAMPLINGS)
+@pytest.mark.parametrize("ss", SAMPLINGS + GEOMETRIES)
 def test_model_is_libjpegs_scaled_decode(ss, d):
     for w, h in SIZES:
         for name, im in _coefficient_sets(ss, w, h):
@@ -151,7 +151,7 @@ def test_model_is_libjpegs_scaled_decode(ss, d):
 
 
 @needs_libjpeg
-@pytest.mark.parametrize("ss", ["422", "420", "440", "411"])
+@pytest.mark.parametrize("ss", ["422", "420", "440", "411"] + list(GEOMETRIES))
 def test_scaled_geometry_is_libjpegs(ss):
     """the DCT scaled sizes jpeg_start_decompress chose are the ones the restatement (and the library,
     through the test above) uses: 4:2:0 chroma at 1/2 takes the full 8x8 IDCT, for instance"""
