@@ -264,6 +264,43 @@ int jpegqs_cuda_render_oriented_async(jpegqs_cuda_ctx *ctx, int nimages, const j
 		const jpegqs_cuda_status *status_dev, int layout, int scale_denom, const int32_t *orientation,
 		uint8_t *const *out_dev, void *stream);
 
+/* ---- colour conversion: Pillow's Image.convert("RGB") / convert("L") of the decoded picture ---------
+ * mode JPEGQS_PIXELS_AS_FILE (0) is the file's own colour, the existing calls' behaviour: RGB for 3
+ * components, one grey sample for 1, and 4 components are not rendered (JPEGQS_ERR_UNSUPPORTED).
+ * JPEGQS_PIXELS_RGB (1) gives 3 channels and JPEGQS_PIXELS_L (2) gives 1, whatever the component count:
+ *   - 1 component: RGB replicates the sample; L is the sample.
+ *   - 3 components: RGB is the existing render; L is Pillow's rgb2l of it,
+ *     (R * 19595 + G * 38470 + B * 7471 + 0x8000) >> 16 - not the file's Y plane.
+ *   - 4 components: what Pillow decodes (libjpeg's JCS_CMYK output with raw mode CMYK;I, which inverts
+ *     all four samples), then its cmyk2rgb: with nk = 255 - K, out = nk - MULDIV255(C, nk) per channel,
+ *     MULDIV255(a, b) = (t = a * b + 128, ((t >> 8) + t) >> 8).  A YCCK file goes through libjpeg's
+ *     ycck_cmyk_convert first (the YCbCr -> RGB of the 3-component render, inverted; K passes through).
+ *     L is rgb2l of that RGB.
+ * The conversion is per pixel, so it commutes with the orientation; the crop, the resize and the
+ * compressor take the converted picture.  Colour space: libjpeg's default_decompress_parms rule, which
+ * jpegqs_cuda_scan.jpeg_color_space gives: 4 components are CMYK without an Adobe marker or with transform
+ * 0, and YCCK with any other transform. */
+#define JPEGQS_PIXELS_AS_FILE 0
+#define JPEGQS_PIXELS_RGB 1
+#define JPEGQS_PIXELS_L 2
+
+/* jpegqs_cuda_render_oriented_async with a colour conversion (render_oriented_async is this call with
+ * color_space NULL and mode 0).  color_space: NULL, or one JCS_* value per image (jpeglib.h numbering:
+ * GRAYSCALE 1, RGB 2, YCbCr 3, CMYK 4, YCCK 5) that decides the conversion in place of is_ycbcr; NULL
+ * derives it from ncomp and is_ycbcr, 4 components being CMYK.  A value the image's component count cannot
+ * have, or a mode other than the three above, returns JPEGQS_ERR_ARG with nothing enqueued.  out_dev[i]:
+ * W' * H' * channels bytes (channels as above; mode 0: 3).  4-component images take 624-byte descriptors,
+ * 52 per launch.  Same stream rules; graph-capturable. */
+int jpegqs_cuda_render_mode_async(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image *imgs,
+		const jpegqs_cuda_status *status_dev, int layout, int scale_denom, const int32_t *orientation,
+		const int32_t *color_space, int mode, uint8_t *const *out_dev, void *stream);
+
+/* jpegqs_cuda_render_model with a colour space (a JCS_* value as above, or -1 to derive it as NULL does)
+ * and a mode; out: W * H * channels bytes (mode 0: 3).  jpegqs_cuda_render_model is this call with -1 and
+ * mode 0. */
+int jpegqs_cuda_render_model_mode(const jpegqs_cuda_image *img, int color_space, int upsampled, int layout,
+		int scale_denom, int mode, uint8_t *out);
+
 /* Host-only, no device needed.  *orientation = the orientation ImageOps.exif_transpose(Image.open(f))
  * applies to file f, 1 for none - including every file where Pillow's getexif() raises.  The rules are
  * those of Pillow 12.2 (JpegImagePlugin, Image.getexif, Image.Exif.load, TiffImagePlugin
@@ -762,6 +799,21 @@ int jpegqs_cuda_pixels_batch_oriented(jpegqs_cuda_ctx *ctx, int n, const uint8_t
 		const int32_t *orientation, int out_on_device, uint8_t *const *out, size_t max_device_bytes, int *rc,
 		jpegqs_cuda_pixels_result *results);
 
+/* jpegqs_cuda_pixels_batch_oriented with a colour mode (JPEGQS_PIXELS_*; 0 is byte for byte the oriented
+ * call).  With mode RGB or L:
+ *   - channels, out[i]'s size, results[i].channels, the budgets and the crop and resize are those of a
+ *     3-channel (RGB) or 1-channel (L) picture for every file; CHW and HWC are the same bytes for L.
+ *   - 4-component files (CMYK, YCCK) are rendered - their colour space is the header's - and smoothed as
+ *     the tool smooths them; sampling ratios that are not integral are JPEGQS_ERR_UNSUPPORTED per file.
+ *   - file i gives Pillow's im = Image.open(F) (im.draft(None, (W // d, H // d)) at d > 1), then
+ *     exif_transpose or the explicit transpose, then im.convert(mode), then crop and resize, with F the
+ *     file jpegqs writes for the same flags and niter (the input where do_quantsmooth returns early).
+ *   - A mode other than 0, 1, 2 is a bad argument (JPEGQS_ERR_ARG, nothing done). */
+int jpegqs_cuda_pixels_batch_mode(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int layout, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
+		const int32_t *orientation, int mode, int out_on_device, uint8_t *const *out, size_t max_device_bytes, int *rc,
+		jpegqs_cuda_pixels_result *results);
+
 /* ---- 8-bit pictures -> JPEG files: Pillow's Image.save, byte for byte ---------------------------
  * Picture i's file is exactly what Pillow (with its libjpeg-turbo) writes for
  *     Image.fromarray(P).save(f, "JPEG", quality=quality, subsampling=subsampling, optimize=optimize)
@@ -856,6 +908,13 @@ int jpegqs_cuda_pixels_batch_jpeg_oriented(jpegqs_cuda_ctx *ctx, int n, const ui
 		int flags, int niter, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
 		const jpegqs_cuda_jpeg_params *params, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results,
 		uint8_t **out, size_t *out_len, const int32_t *orientation);
+
+/* jpegqs_cuda_pixels_batch_jpeg_oriented with a colour mode as for jpegqs_cuda_pixels_batch_mode: the
+ * converted picture is saved (an L picture as a grey file).  Mode 0: byte for byte the oriented call. */
+int jpegqs_cuda_pixels_batch_jpeg_mode(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
+		const jpegqs_cuda_jpeg_params *params, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results,
+		uint8_t **out, size_t *out_len, const int32_t *orientation, int mode);
 
 /* ---- one image sharded by MCU rows over several GPUs (SURVEY.md 8e) ----------------------
  * Every rank - a device of this process, or another process on the same box - smooths one slab

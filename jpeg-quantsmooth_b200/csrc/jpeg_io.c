@@ -185,6 +185,8 @@ int qs_route_plan(const uint8_t *data, size_t len, int copy, jpegqs_cuda_file_in
 		if (!why[0]) { route = JPEGQS_ROUTE_DEVICE; why = seq ? "sequential, one scan" : im.progressive ? "progressive" : "several scans"; }
 	}
 	if (img) fill_image(&im, img);
+	/* every route: the header's colour space, which the pixel path's colour modes read */
+	if (scan) scan->jpeg_color_space = (int32_t)im.cinfo.jpeg_color_space;
 	if (route == JPEGQS_ROUTE_DEVICE) {
 		if (nscans) *nscans = seq ? 0 : n;
 		if (scan && seq) {

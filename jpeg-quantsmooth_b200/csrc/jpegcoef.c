@@ -1073,7 +1073,8 @@ static int jq_read_impl(const unsigned char *data, size_t len, int copy, jq_imag
 	if (im->saw_jfif && im->cinfo.num_components == 3) im->cinfo.jpeg_color_space = JCS_YCbCr;
 	if (adobe >= 0 && !(im->saw_jfif && im->cinfo.num_components == 3)) {      /* jdapimin.c default_decompress_parms */
 		if (im->cinfo.num_components == 3) im->cinfo.jpeg_color_space = adobe == 0 ? JCS_RGB : JCS_YCbCr;
-		if (im->cinfo.num_components == 4) im->cinfo.jpeg_color_space = adobe == 2 ? JCS_YCCK : JCS_CMYK;
+		/* 0: CMYK; 2 and every other value YCCK (libjpeg warns JWRN_ADOBE_XFORM for those, this reader does not) */
+		if (im->cinfo.num_components == 4) im->cinfo.jpeg_color_space = adobe == 0 ? JCS_CMYK : JCS_YCCK;
 	}
 	for (i = 0; i < im->cinfo.num_components; i++) {
 		jpeg_component_info *c = &pv->comps[i];

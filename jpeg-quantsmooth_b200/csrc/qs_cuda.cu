@@ -2097,10 +2097,11 @@ extern "C" int jpegqs_cuda_render_rgb(jpegqs_cuda_ctx *ctx, const jpegqs_cuda_im
 }
 
 /* ---- stream-ordered render of device-resident images (see the header) ----------------------- */
-/* what the render kernel takes: 1 or 3 components whose sampling ratios are integral (libjpeg cannot
- * decode others either); sampling factors outside 1..4 are not rendered */
-int qs_render_takes(const jpegqs_cuda_image *im) {
-	if (im->ncomp != 1 && im->ncomp != 3) return 0;
+/* what the render kernel takes: 1 or 3 components - and 4 with a mode (JPEGQS_PIXELS_RGB / _L) - whose
+ * sampling ratios are integral (libjpeg cannot decode others either); sampling factors outside 1..4 are not
+ * rendered */
+int qs_render_takes(const jpegqs_cuda_image *im, int mode) {
+	if (im->ncomp != 1 && im->ncomp != 3 && (im->ncomp != 4 || mode == JPEGQS_PIXELS_AS_FILE)) return 0;
 	int maxh = 1, maxv = 1;
 	for (int c = 0; c < im->ncomp; c++) {
 		const jpegqs_cuda_comp *cc = &im->comp[c];
@@ -2123,10 +2124,12 @@ int qs_render_takes(const jpegqs_cuda_image *im) {
  * (4:2:0 at 1/2: luma 4x4, chroma 8x8 with no up-sampling).  downsampled_width / height are
  * ceil(image_width * samp * size / (max_samp * 8)), and the up-sampler expands by
  * max_samp * m / (samp * size), an integer by construction. */
+template <class Img>
 static int qs_render_desc(const jpegqs_cuda_image *im, int scale_denom, int status_given, int host, uint8_t *out,
-		QsRenderImg &r, const char *&bad) {
+		Img &r, const char *&bad) {
+	constexpr int NC = sizeof(Img::coef) / sizeof(Img::coef[0]);
 	memset(&r, 0, sizeof(r));
-	if (im->ncomp != 1 && im->ncomp != 3) return 1;
+	if (NC == 3 ? im->ncomp != 1 && im->ncomp != 3 : im->ncomp != 4) return 1;
 	int maxh = 1, maxv = 1;
 	for (int c = 0; c < im->ncomp && !bad; c++) {
 		const jpegqs_cuda_comp *cc = &im->comp[c];
@@ -2137,7 +2140,7 @@ static int qs_render_desc(const jpegqs_cuda_image *im, int scale_denom, int stat
 	}
 	if (!out) bad = "output NULL";
 	if (bad) return 0;
-	if (!qs_render_takes(im)) return 1;
+	if (!qs_render_takes(im, NC == 4)) return 1;
 	const int m = 8 / scale_denom;
 	for (int c = 0; c < im->ncomp && !bad; c++) {
 		const jpegqs_cuda_comp *cc = &im->comp[c];
@@ -2157,7 +2160,7 @@ static int qs_render_desc(const jpegqs_cuda_image *im, int scale_denom, int stat
 		for (int k = 0; k < 64; k++) r.q[c][k] = deq ? cc->quant[k] : 1;
 	}
 	if (bad) return 0;
-	if (im->ncomp == 3) {
+	if constexpr (NC == 3) if (im->ncomp == 3) {
 		r.coef_up[0] = im->comp[1].coef_up; r.coef_up[1] = im->comp[2].coef_up;
 		if (status_given) r.up_mode = r.coef_up[0] && r.coef_up[1] ? 2 : 0;
 		else if (im->upsampled) {
@@ -2171,26 +2174,67 @@ static int qs_render_desc(const jpegqs_cuda_image *im, int scale_denom, int stat
 	return 0;
 }
 
-/* jpegqs_cuda_render_oriented_async with the layout and scale checked by the caller; grey_store != 0 writes
- * 1-component images with one byte per pixel (either layout: the single plane).  Consecutive images of
- * one store mode share a launch.  orient: NULL (all 1) or 1..8 per image. */
+/* the render's colour conversion (qs_kernels.h QS_CONV_*) and store mode of an image of ncomp components
+ * under mode; grey_store != 0 writes 1-component images with one byte per pixel in mode 0 */
+static void qs_render_conv(int ncomp, int mode, int layout, int grey_store, int *conv, int *store) {
+	*conv = ncomp == 4 ? (mode == JPEGQS_PIXELS_L ? QS_CONV_CMYK_L : QS_CONV_CMYK_RGB) :
+			mode == JPEGQS_PIXELS_L ? QS_CONV_L : QS_CONV_NONE;
+	*store = mode == JPEGQS_PIXELS_L || (mode == JPEGQS_PIXELS_AS_FILE && grey_store && ncomp == 1) ? QS_RENDER_GREY : layout;
+}
+
+/* JCS_* of jpeglib.h that the render tells apart */
+#define QS_JCS_GRAYSCALE 1
+#define QS_JCS_RGB 2
+#define QS_JCS_YCbCr 3
+#define QS_JCS_CMYK 4
+#define QS_JCS_YCCK 5
+
+/* an image's colour space: color_space[i], or derived from ncomp / is_ycbcr (4: CMYK) when NULL.  Returns
+ * whether it is one that ncomp can have, and sets *ycc (YCbCr, or YCCK for 4 components). */
+static int qs_render_colour(const jpegqs_cuda_image *im, const int32_t *color_space, int i, uint8_t *ycc) {
+	const int cs = color_space ? color_space[i] : im->ncomp == 1 ? QS_JCS_GRAYSCALE : im->ncomp == 4 ? QS_JCS_CMYK :
+			im->is_ycbcr ? QS_JCS_YCbCr : QS_JCS_RGB;
+	*ycc = cs == QS_JCS_YCbCr || cs == QS_JCS_YCCK;
+	switch (im->ncomp) {
+	case 1: return cs == QS_JCS_GRAYSCALE;
+	case 3: return cs == QS_JCS_RGB || cs == QS_JCS_YCbCr;
+	case 4: return cs == QS_JCS_CMYK || cs == QS_JCS_YCCK;
+	default: return 1;                                 /* not rendered: UNSUPPORTED */
+	}
+}
+
+/* jpegqs_cuda_render_mode_async with the layout, scale and mode checked by the caller; grey_store: see
+ * qs_render_conv.  Consecutive images of one store mode and conversion share a launch.  orient: NULL (all 1)
+ * or 1..8 per image; color_space: NULL or one JCS_* value per image. */
 int qs_render_images(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image *imgs,
 		const jpegqs_cuda_status *status_dev, int layout, int grey_store, int scale_denom, const int32_t *orient,
-		uint8_t *const *out_dev, void *stream) {
+		uint8_t *const *out_dev, void *stream, int mode, const int32_t *color_space) {
 	const char *bad = nimages < 0 || (nimages && (!imgs || !out_dev)) ? "images or outputs missing" : NULL;
 	for (int i = 0; i < nimages && !bad && orient; i++)
 		if (orient[i] < 1 || orient[i] > 8) bad = "orientation outside 1..8";
 	std::vector<QsRenderImg> d(bad ? 0 : nimages);
-	std::vector<int> store(d.size());
+	std::vector<QsRenderImg4> d4;
+	std::vector<int> store(d.size()), conv(d.size());
 	int unsupported = 0;
 	for (int i = 0; i < nimages && !bad && !unsupported; i++) {
 		const jpegqs_cuda_image *im = &imgs[i];
-		unsupported = qs_render_desc(im, scale_denom, status_dev != NULL, 0, out_dev[i], d[i], bad);
-		if (orient) d[i].orient = (uint8_t)orient[i];
-		store[i] = grey_store && im->ncomp == 1 ? QS_RENDER_GREY : layout;
+		uint8_t ycc = 0;
+		if (!qs_render_colour(im, color_space, i, &ycc)) { bad = "color_space does not match the component count"; break; }
+		if (im->ncomp == 4 && mode != JPEGQS_PIXELS_AS_FILE) {
+			if (d4.empty()) d4.resize(nimages);
+			unsupported = qs_render_desc(im, scale_denom, status_dev != NULL, 0, out_dev[i], d4[i], bad);
+			d4[i].ycc = ycc;
+			d[i].width = d4[i].width; d[i].height = d4[i].height;     /* the launch grouping reads them from d */
+			if (orient) d4[i].orient = (uint8_t)orient[i];
+		} else {
+			unsupported = qs_render_desc(im, scale_denom, status_dev != NULL, 0, out_dev[i], d[i], bad);
+			if (color_space && im->ncomp == 3) d[i].ycc = ycc;
+			if (orient) d[i].orient = (uint8_t)orient[i];
+		}
+		qs_render_conv(im->ncomp, mode, layout, grey_store, &conv[i], &store[i]);
 	}
 	if (unsupported) {
-		snprintf(ctx->err, sizeof(ctx->err), "render_async: 1 or 3 components with integral sampling ratios only");
+		snprintf(ctx->err, sizeof(ctx->err), "render_async: 1 or 3 components (4 with a mode) with integral sampling ratios only");
 		return JPEGQS_ERR_UNSUPPORTED;
 	}
 	if (bad) {
@@ -2200,16 +2244,20 @@ int qs_render_images(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image 
 	CK(cudaSetDevice(ctx->device));
 	cudaStream_t st = stream ? (cudaStream_t)stream : ctx->stream;
 	ctx->launches = 0;
-	/* the descriptors travel as kernel parameters: QS_RENDER_PACK images of one store mode per launch */
+	/* the descriptors travel as kernel parameters: QS_RENDER_PACK images (QS_RENDER_PACK4 4-component ones) of
+	 * one store mode and conversion per launch */
 	for (int i0 = 0; i0 < nimages;) {
+		const bool four = conv[i0] >= QS_CONV_CMYK_RGB;
 		int n = 0, tiles = 0;
-		for (; n < QS_RENDER_PACK && i0 + n < nimages && store[i0 + n] == store[i0]; n++) {
-			QsRenderImg &r = d[i0 + n];
-			r.tile_begin = tiles;
+		for (; n < (four ? QS_RENDER_PACK4 : QS_RENDER_PACK) && i0 + n < nimages && store[i0 + n] == store[i0] &&
+				conv[i0 + n] == conv[i0]; n++) {
+			const QsRenderImg &r = d[i0 + n];
+			(four ? d4[i0 + n].tile_begin : d[i0 + n].tile_begin) = tiles;
 			tiles += ((r.width + QS_RENDER_TW - 1) / QS_RENDER_TW) * ((r.height + QS_RENDER_TH - 1) / QS_RENDER_TH);
 		}
-		CK(qs_launch_render_async(d.data() + i0, n, tiles, status_dev ? (const int2 *)(status_dev + i0) : NULL, store[i0],
-				scale_denom, st));
+		if (four) CK(qs_launch_render4_async(d4.data() + i0, n, tiles, store[i0], conv[i0], scale_denom, st));
+		else CK(qs_launch_render_async(d.data() + i0, n, tiles, status_dev ? (const int2 *)(status_dev + i0) : NULL, store[i0],
+				scale_denom, st, conv[i0]));
 		if (tiles) ctx->launches++;
 		i0 += n;
 	}
@@ -2220,9 +2268,13 @@ static int qs_scale_ok(int scale_denom) {
 	return scale_denom == 1 || scale_denom == 2 || scale_denom == 4 || scale_denom == 8;
 }
 
-extern "C" int jpegqs_cuda_render_oriented_async(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image *imgs,
+static int qs_mode_ok(int mode) {
+	return mode == JPEGQS_PIXELS_AS_FILE || mode == JPEGQS_PIXELS_RGB || mode == JPEGQS_PIXELS_L;
+}
+
+extern "C" int jpegqs_cuda_render_mode_async(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image *imgs,
 		const jpegqs_cuda_status *status_dev, int layout, int scale_denom, const int32_t *orientation,
-		uint8_t *const *out_dev, void *stream) {
+		const int32_t *color_space, int mode, uint8_t *const *out_dev, void *stream) {
 	if (!ctx) return JPEGQS_ERR_ARG;
 	if (!(nimages < 0 || (nimages && (!imgs || !out_dev))) && layout != JPEGQS_RENDER_HWC && layout != JPEGQS_RENDER_CHW) {
 		snprintf(ctx->err, sizeof(ctx->err), "render_async: unknown layout");
@@ -2232,7 +2284,19 @@ extern "C" int jpegqs_cuda_render_oriented_async(jpegqs_cuda_ctx *ctx, int nimag
 		snprintf(ctx->err, sizeof(ctx->err), "render_async: scale_denom must be 1, 2, 4 or 8");
 		return JPEGQS_ERR_ARG;
 	}
-	return qs_render_images(ctx, nimages, imgs, status_dev, layout, 0, scale_denom, orientation, out_dev, stream);
+	if (!qs_mode_ok(mode)) {
+		snprintf(ctx->err, sizeof(ctx->err), "render_async: mode must be 0 (as the file), 1 (RGB) or 2 (L)");
+		return JPEGQS_ERR_ARG;
+	}
+	return qs_render_images(ctx, nimages, imgs, status_dev, layout, 0, scale_denom, orientation, out_dev, stream, mode,
+			color_space);
+}
+
+extern "C" int jpegqs_cuda_render_oriented_async(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image *imgs,
+		const jpegqs_cuda_status *status_dev, int layout, int scale_denom, const int32_t *orientation,
+		uint8_t *const *out_dev, void *stream) {
+	return jpegqs_cuda_render_mode_async(ctx, nimages, imgs, status_dev, layout, scale_denom, orientation, NULL,
+			JPEGQS_PIXELS_AS_FILE, out_dev, stream);
 }
 
 extern "C" int jpegqs_cuda_render_scaled_async(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image *imgs,
@@ -2245,19 +2309,32 @@ extern "C" int jpegqs_cuda_render_async(jpegqs_cuda_ctx *ctx, int nimages, const
 	return jpegqs_cuda_render_scaled_async(ctx, nimages, imgs, status_dev, layout, 1, out_dev, stream);
 }
 
-extern "C" int jpegqs_cuda_render_model(const jpegqs_cuda_image *img, int upsampled, int layout, int scale_denom,
-		uint8_t *out) {
+extern "C" int jpegqs_cuda_render_model_mode(const jpegqs_cuda_image *img, int color_space, int upsampled, int layout,
+		int scale_denom, int mode, uint8_t *out) {
 	const char *bad = !img || !out ? "NULL argument" : layout != JPEGQS_RENDER_HWC && layout != JPEGQS_RENDER_CHW ?
-			"unknown layout" : !qs_scale_ok(scale_denom) ? "scale_denom must be 1, 2, 4 or 8" : NULL;
+			"unknown layout" : !qs_scale_ok(scale_denom) ? "scale_denom must be 1, 2, 4 or 8" :
+			!qs_mode_ok(mode) ? "mode must be 0 (as the file), 1 (RGB) or 2 (L)" : NULL;
 	QsRenderImg r;
-	int unsupported = 0;
+	QsRenderImg4 r4;
+	int unsupported = 0, conv = 0, store = 0;
+	uint8_t ycc = 0;
+	const int32_t cs = color_space;
+	if (!bad && color_space >= 0 && !qs_render_colour(img, &cs, 0, &ycc)) bad = "color_space does not match the component count";
 	if (!bad) {
 		jpegqs_cuda_image im = *img;
 		im.upsampled = upsampled ? 1 : 0;
-		unsupported = qs_render_desc(&im, scale_denom, 0, 1, out, r, bad);
+		if (im.ncomp == 4 && mode != JPEGQS_PIXELS_AS_FILE) {
+			unsupported = qs_render_desc(&im, scale_denom, 0, 1, out, r4, bad);
+			if (color_space < 0) qs_render_colour(img, NULL, 0, &ycc);
+			r4.ycc = ycc;
+		} else {
+			unsupported = qs_render_desc(&im, scale_denom, 0, 1, out, r, bad);
+			if (color_space >= 0 && im.ncomp == 3) r.ycc = ycc;
+		}
+		qs_render_conv(im.ncomp, mode, layout, 0, &conv, &store);
 	}
 	if (unsupported) {
-		qs_set_host_error("jpegqs_cuda_render_model: 1 or 3 components with integral sampling ratios only");
+		qs_set_host_error("jpegqs_cuda_render_model: 1 or 3 components (4 with a mode) with integral sampling ratios only");
 		return JPEGQS_ERR_UNSUPPORTED;
 	}
 	if (bad) {
@@ -2265,6 +2342,12 @@ extern "C" int jpegqs_cuda_render_model(const jpegqs_cuda_image *img, int upsamp
 		qs_set_host_error(m);
 		return JPEGQS_ERR_ARG;
 	}
-	qs_render_host(&r, layout, scale_denom);
+	if (img->ncomp == 4) qs_render4_host(&r4, store, scale_denom, conv);
+	else qs_render_host(&r, store, scale_denom, conv);
 	return 0;
+}
+
+extern "C" int jpegqs_cuda_render_model(const jpegqs_cuda_image *img, int upsampled, int layout, int scale_denom,
+		uint8_t *out) {
+	return jpegqs_cuda_render_model_mode(img, -1, upsampled, layout, scale_denom, JPEGQS_PIXELS_AS_FILE, out);
 }

@@ -1805,6 +1805,38 @@ __host__ __device__ __forceinline__ uint32_t qs_rgb_pixel(int y, int c1, int c2,
 	return (uint32_t)r | ((uint32_t)g << 8) | ((uint32_t)b << 16);
 }
 
+/* Pillow's rgb2l (Convert.c, L24 >> 16) of r | g << 8 | b << 16 */
+__host__ __device__ __forceinline__ uint32_t qs_luma(uint32_t v) {
+	return ((v & 255) * 19595 + ((v >> 8) & 255) * 38470 + ((v >> 16) & 255) * 7471 + 0x8000) >> 16;
+}
+
+/* Pillow's MULDIV255(a, b) */
+__host__ __device__ __forceinline__ int qs_muldiv255(int a, int b) {
+	const int t = a * b + 128;
+	return ((t >> 8) + t) >> 8;
+}
+
+/* One 4-component pixel, r | g << 8 | b << 16, as Pillow's convert("RGB") gives it.  Pillow decodes these
+ * files with libjpeg's JCS_CMYK output and raw mode CMYK;I, which inverts all four samples.  YCCK: libjpeg's
+ * ycck_cmyk_convert first gives 255 - (R, G, B) of the YCbCr triple and passes K through, so Pillow's C, M, Y
+ * are R, G, B.  Then cmyk2rgb with nk = 255 - Pillow's K = s3: out = nk - MULDIV255(C, nk), never below 0. */
+__host__ __device__ __forceinline__ uint32_t qs_cmyk_pixel(int s0, int s1, int s2, int s3, bool ycck) {
+	const uint32_t cmy = ycck ? qs_rgb_pixel(s0, s1, s2, true) : 0xffffffu ^ ((uint32_t)s0 | (uint32_t)s1 << 8 | (uint32_t)s2 << 16);
+	const int nk = s3;
+	return (uint32_t)(nk - qs_muldiv255(cmy & 255, nk)) | (uint32_t)(nk - qs_muldiv255((cmy >> 8) & 255, nk)) << 8 |
+			(uint32_t)(nk - qs_muldiv255(cmy >> 16, nk)) << 16;
+}
+
+/* the render's pixel from its up-sampled samples (s3: 4-component conversions only) by conversion CONV
+ * (qs_kernels.h QS_CONV_*) */
+template <int CONV>
+__host__ __device__ __forceinline__ uint32_t qs_convert_pixel(int s0, int s1, int s2, int s3, bool ycc) {
+	if constexpr (CONV == QS_CONV_NONE) return qs_rgb_pixel(s0, s1, s2, ycc);
+	else if constexpr (CONV == QS_CONV_L) return qs_luma(qs_rgb_pixel(s0, s1, s2, ycc));
+	else if constexpr (CONV == QS_CONV_CMYK_RGB) return qs_cmyk_pixel(s0, s1, s2, s3, ycc);
+	else return qs_luma(qs_cmyk_pixel(s0, s1, s2, s3, ycc));
+}
+
 __global__ void qs_render_rgb_kernel(QsRenderArgs a, uint8_t *__restrict__ rgb) {
 	int ox = blockIdx.x * blockDim.x + threadIdx.x, oy = blockIdx.y * blockDim.y + threadIdx.y;
 	if (ox >= a.width || oy >= a.height) return;
@@ -1952,6 +1984,13 @@ struct QsRenderPack { QsRenderImg img[QS_RENDER_PACK]; };
 static_assert(sizeof(QsRenderImg) == 496, "orient sits in the padding before q");
 static_assert(sizeof(QsRenderPack) + 2 * sizeof(void *) + 2 * sizeof(int) <= 32764,
 		"QS_RENDER_PACK exceeds the kernel parameter space");
+struct QsRenderPack4 { QsRenderImg4 img[QS_RENDER_PACK4]; };
+static_assert(sizeof(QsRenderImg4) == 624, "QsRenderImg4 has no padding");
+static_assert(sizeof(QsRenderPack4) + 2 * sizeof(void *) + 2 * sizeof(int) <= 32764 &&
+		sizeof(QsRenderPack4) + sizeof(QsRenderImg4) + 2 * sizeof(void *) + 2 * sizeof(int) > 32764,
+		"QS_RENDER_PACK4 is the most 4-component descriptors the kernel parameter space holds");
+/* the kernel's descriptors: 4 components for the CMYK conversions, QsRenderImg otherwise */
+template <int CONV> using QsRenderPackOf = std::conditional_t<(CONV >= QS_CONV_CMYK_RGB), QsRenderPack4, QsRenderPack>;
 
 /* sample (x, y) of a component's shared window whose first sample is (x0, y0) */
 struct QsSmemPx {
@@ -2000,31 +2039,36 @@ __device__ __forceinline__ void qs_render_store4(uint8_t *out, size_t plane, siz
 /* STORE: QS_RENDER_HWC / QS_RENDER_CHW (three bytes per pixel), or QS_RENDER_GREY (one byte per pixel,
  * the CHW store of plane 0 only; for 1-component images).  D: the scale denominator (1, 2, 4, 8); the
  * descriptors then hold the scaled geometry (qs_render_images).  ORIENTED: some image of the launch has an
- * orientation other than 1; without it the kernel holds only the unoriented store. */
-template <int STORE, int D, bool ORIENTED>
-__global__ void __launch_bounds__(QS_RT_THREADS, 2) qs_render_async_kernel(const __grid_constant__ QsRenderPack p,
+ * orientation other than 1; without it the kernel holds only the unoriented store.  CONV: the colour
+ * conversion (qs_kernels.h QS_CONV_*); the CMYK ones read QsRenderImg4 descriptors and a fourth window,
+ * NONE is the file's own colour and compiles to the kernel it was before the conversions existed. */
+template <int STORE, int D, bool ORIENTED, int CONV = QS_CONV_NONE>
+__global__ void __launch_bounds__(QS_RT_THREADS, 2) qs_render_async_kernel(const __grid_constant__ QsRenderPackOf<CONV> p,
 		int n, const int2 *__restrict__ status) {
-	__shared__ __align__(16) uint8_t pix[3][QS_RS_H * QS_RS_W];
-	__shared__ int qmul[3][64];
-	__shared__ QsRenderComp g[3];
-	__shared__ int glss[3];                              /* D > 1: log2 of each window's DCT scaled size */
+	constexpr int NC = CONV >= QS_CONV_CMYK_RGB ? 4 : 3;  /* windows */
+	__shared__ __align__(16) uint8_t pix[NC][QS_RS_H * QS_RS_W];
+	__shared__ int qmul[NC][64];
+	__shared__ QsRenderComp g[NC];
+	__shared__ int glss[NC];                             /* D > 1: log2 of each window's DCT scaled size */
 	const int tile = blockIdx.x;
 	int lo = 0, hi = n - 1;
 	while (lo < hi) {                                    /* last image with tile_begin <= tile */
 		int mid = (lo + hi + 1) >> 1;
 		if (p.img[mid].tile_begin <= tile) lo = mid; else hi = mid - 1;
 	}
-	const QsRenderImg &im = p.img[lo];
+	const auto &im = p.img[lo];
 	const int W = im.width, H = im.height, nc = im.ncomp, ntx = (W + QS_RENDER_TW - 1) / QS_RENDER_TW;
 	const int t = tile - im.tile_begin, x0 = (t % ntx) * QS_RENDER_TW, y0 = (t / ntx) * QS_RENDER_TH;
 	const int x1 = min(x0 + QS_RENDER_TW, W) - 1, y1 = min(y0 + QS_RENDER_TH, H) - 1;   /* last pixel of the tile */
 	if (threadIdx.x < nc) {
 		const int c = threadIdx.x;
 		/* components 1 and 2 of an up-sampled image: coef_up, at component 0's geometry */
-		const bool up = c > 0 && (im.up_mode == 1 || (im.up_mode == 2 && status[lo].y != 0));
+		bool up = false;
+		if constexpr (NC == 3) up = c > 0 && (im.up_mode == 1 || (im.up_mode == 2 && status[lo].y != 0));
 		const int k = up ? 0 : c;
 		QsRenderComp r;
-		r.coef = up ? im.coef_up[c - 1] : im.coef[c];
+		if constexpr (NC == 3) r.coef = up ? im.coef_up[c - 1] : im.coef[c];
+		else r.coef = im.coef[c];
 		r.wblk = im.wblk[k]; r.cw = im.cw[k]; r.ch = im.ch[k]; r.hs = im.hs[k]; r.vs = im.vs[k];
 		const int rx = r.hs == 2 ? 1 : 0, ry = r.vs == 2 ? 1 : 0;     /* the fancy up-sampler's ring */
 		const int lss = D == 1 ? 3 : (im.lss >> (2 * k)) & 3;
@@ -2039,9 +2083,11 @@ __global__ void __launch_bounds__(QS_RT_THREADS, 2) qs_render_async_kernel(const
 	/* islow IDCT (D > 1: each window's scaled IDCT) of every block of the windows, one thread per block
 	 * (as qs_idct_pass_kernel) */
 	const int nb0 = g[0].nbx * g[0].nby, nb1 = nc > 1 ? g[1].nbx * g[1].nby : 0, nb2 = nc > 2 ? g[2].nbx * g[2].nby : 0;
-	for (int k = threadIdx.x; k < nb0 + nb1 + nb2; k += QS_RT_THREADS) {
-		const int c = k < nb0 ? 0 : k < nb0 + nb1 ? 1 : 2;
-		const int j = k - (c == 0 ? 0 : c == 1 ? nb0 : nb0 + nb1);
+	const int nb3 = NC == 4 ? g[NC - 1].nbx * g[NC - 1].nby : 0;
+	for (int k = threadIdx.x; k < nb0 + nb1 + nb2 + nb3; k += QS_RT_THREADS) {
+		int c = k < nb0 ? 0 : k < nb0 + nb1 ? 1 : 2;
+		int j = k - (c == 0 ? 0 : c == 1 ? nb0 : nb0 + nb1);
+		if (NC == 4 && j >= nb2 && c == 2) { c = 3; j -= nb2; }
 		const QsRenderComp &r = g[c];
 		const int lby = j / r.nbx, lbx = j - lby * r.nbx;
 		const int4 *src = (const int4 *)(r.coef + ((size_t)(r.by0 + lby) * r.wblk + r.bx0 + lbx) * 64);
@@ -2100,7 +2146,13 @@ __global__ void __launch_bounds__(QS_RT_THREADS, 2) qs_render_async_kernel(const
 			c1 = qs_upsample_at<D != 8>(P1, g[1].hs, g[1].vs, g[1].cw, g[1].ch, x, y);
 			c2 = qs_upsample_at<D != 8>(P2, g[2].hs, g[2].vs, g[2].cw, g[2].ch, x, y);
 		}
-		return qs_rgb_pixel(l, c1, c2, ycc);
+		int c3 = 0;
+		if constexpr (NC == 4) {
+			const int ls3 = D == 1 ? 3 : glss[3];
+			const QsSmemPx P3{pix[3], g[3].bx0 << ls3, g[3].by0 << ls3};
+			c3 = qs_upsample_at<D != 8>(P3, g[3].hs, g[3].vs, g[3].cw, g[3].ch, x, y);
+		}
+		return qs_convert_pixel<CONV>(l, c1, c2, c3, ycc);
 	};
 	const int orient = ORIENTED ? im.orient : 1;         /* CTA-uniform */
 	if (!ORIENTED || orient < 5) {
@@ -2162,28 +2214,38 @@ __global__ void __launch_bounds__(QS_RT_THREADS, 2) qs_render_async_kernel(const
 	}
 }
 
-template <int D, bool O>
-static void qs_launch_render_store(const QsRenderPack &pack, int n, int tiles, const int2 *status, int store,
+/* the store modes each conversion is instantiated for: the RGB ones HWC and CHW (NONE also GREY for grey
+ * images), the luma ones GREY; the callers pass no other pair */
+template <int D, bool O, int CONV>
+static void qs_launch_render_store(const QsRenderPackOf<CONV> &pack, int n, int tiles, const int2 *status, int store,
 		size_t smem, cudaStream_t st) {
-	if (store == QS_RENDER_HWC) qs_render_async_kernel<QS_RENDER_HWC, D, O><<<tiles, QS_RT_THREADS, smem, st>>>(pack, n, status);
-	else if (store == QS_RENDER_CHW) qs_render_async_kernel<QS_RENDER_CHW, D, O><<<tiles, QS_RT_THREADS, smem, st>>>(pack, n, status);
-	else qs_render_async_kernel<QS_RENDER_GREY, D, O><<<tiles, QS_RT_THREADS, smem, st>>>(pack, n, status);
+	if constexpr (CONV == QS_CONV_NONE || CONV == QS_CONV_CMYK_RGB) {
+		if (store == QS_RENDER_HWC) qs_render_async_kernel<QS_RENDER_HWC, D, O, CONV><<<tiles, QS_RT_THREADS, smem, st>>>(pack, n, status);
+		else if (store == QS_RENDER_CHW) qs_render_async_kernel<QS_RENDER_CHW, D, O, CONV><<<tiles, QS_RT_THREADS, smem, st>>>(pack, n, status);
+		else if constexpr (CONV == QS_CONV_NONE) qs_render_async_kernel<QS_RENDER_GREY, D, O><<<tiles, QS_RT_THREADS, smem, st>>>(pack, n, status);
+	} else {
+		qs_render_async_kernel<QS_RENDER_GREY, D, O, CONV><<<tiles, QS_RT_THREADS, smem, st>>>(pack, n, status);
+	}
 }
 
 /* oriented: some image has an orientation other than 1; smem: the staging of 5..8, or 0 */
-template <int D>
-static void qs_launch_render_scaled(const QsRenderPack &pack, int n, int tiles, const int2 *status, int store,
+template <int D, int CONV>
+static void qs_launch_render_scaled(const QsRenderPackOf<CONV> &pack, int n, int tiles, const int2 *status, int store,
 		bool oriented, size_t smem, cudaStream_t st) {
-	if (oriented) qs_launch_render_store<D, true>(pack, n, tiles, status, store, smem, st);
-	else qs_launch_render_store<D, false>(pack, n, tiles, status, store, 0, st);
+	if (oriented) qs_launch_render_store<D, true, CONV>(pack, n, tiles, status, store, smem, st);
+	else qs_launch_render_store<D, false, CONV>(pack, n, tiles, status, store, 0, st);
 }
 
 template <int D>
 static cudaError_t qs_render_configure_d(void) {
-	const void *k[3] = {(const void *)qs_render_async_kernel<QS_RENDER_HWC, D, true>,
+	const void *k[7] = {(const void *)qs_render_async_kernel<QS_RENDER_HWC, D, true>,
 			(const void *)qs_render_async_kernel<QS_RENDER_CHW, D, true>,
-			(const void *)qs_render_async_kernel<QS_RENDER_GREY, D, true>};
-	for (int i = 0; i < 3; i++) {
+			(const void *)qs_render_async_kernel<QS_RENDER_GREY, D, true>,
+			(const void *)qs_render_async_kernel<QS_RENDER_GREY, D, true, QS_CONV_L>,
+			(const void *)qs_render_async_kernel<QS_RENDER_HWC, D, true, QS_CONV_CMYK_RGB>,
+			(const void *)qs_render_async_kernel<QS_RENDER_CHW, D, true, QS_CONV_CMYK_RGB>,
+			(const void *)qs_render_async_kernel<QS_RENDER_GREY, D, true, QS_CONV_CMYK_L>};
+	for (int i = 0; i < 7; i++) {
 		cudaError_t e = cudaFuncSetAttribute(k[i], cudaFuncAttributeMaxDynamicSharedMemorySize, QS_RT_TB_BYTES);
 		if (e != cudaSuccess) return e;
 	}
@@ -2198,13 +2260,14 @@ cudaError_t qs_render_configure(void) {
 	return e;
 }
 
-cudaError_t qs_launch_render_async(const QsRenderImg *imgs, int n, int tiles, const int2 *status, int store,
+template <int CONV, class Img>
+static cudaError_t qs_launch_render_pack(const Img *imgs, int n, int tiles, const int2 *status, int store,
 		int scale_denom, cudaStream_t st) {
-	if (tiles <= 0) return cudaSuccess;
-	if (store != QS_RENDER_HWC && store != QS_RENDER_CHW && store != QS_RENDER_GREY) return cudaErrorInvalidValue;
-	QsRenderPack pack;
-	memcpy(pack.img, imgs, (size_t)n * sizeof(QsRenderImg));
-	if (n < QS_RENDER_PACK) memset(pack.img + n, 0, (size_t)(QS_RENDER_PACK - n) * sizeof(QsRenderImg));
+	constexpr int CAP = sizeof(QsRenderPackOf<CONV>::img) / sizeof(Img);
+	if (n > CAP) return cudaErrorInvalidValue;
+	QsRenderPackOf<CONV> pack;
+	memcpy(pack.img, imgs, (size_t)n * sizeof(Img));
+	if (n < CAP) memset(pack.img + n, 0, (size_t)(CAP - n) * sizeof(Img));
 	bool oriented = false;
 	size_t smem = 0;                                     /* the staging of the transposing orientations */
 	for (int i = 0; i < n; i++) {
@@ -2213,13 +2276,33 @@ cudaError_t qs_launch_render_async(const QsRenderImg *imgs, int n, int tiles, co
 		if (imgs[i].orient >= 5) smem = QS_RT_TB_BYTES;
 	}
 	switch (scale_denom) {
-	case 1: qs_launch_render_scaled<1>(pack, n, tiles, status, store, oriented, smem, st); break;
-	case 2: qs_launch_render_scaled<2>(pack, n, tiles, status, store, oriented, smem, st); break;
-	case 4: qs_launch_render_scaled<4>(pack, n, tiles, status, store, oriented, smem, st); break;
-	case 8: qs_launch_render_scaled<8>(pack, n, tiles, status, store, oriented, smem, st); break;
+	case 1: qs_launch_render_scaled<1, CONV>(pack, n, tiles, status, store, oriented, smem, st); break;
+	case 2: qs_launch_render_scaled<2, CONV>(pack, n, tiles, status, store, oriented, smem, st); break;
+	case 4: qs_launch_render_scaled<4, CONV>(pack, n, tiles, status, store, oriented, smem, st); break;
+	case 8: qs_launch_render_scaled<8, CONV>(pack, n, tiles, status, store, oriented, smem, st); break;
 	default: return cudaErrorInvalidValue;
 	}
 	return cudaGetLastError();
+}
+
+cudaError_t qs_launch_render_async(const QsRenderImg *imgs, int n, int tiles, const int2 *status, int store,
+		int scale_denom, cudaStream_t st, int conv) {
+	if (tiles <= 0) return cudaSuccess;
+	if (store != QS_RENDER_HWC && store != QS_RENDER_CHW && store != QS_RENDER_GREY) return cudaErrorInvalidValue;
+	if (conv == QS_CONV_NONE) return qs_launch_render_pack<QS_CONV_NONE>(imgs, n, tiles, status, store, scale_denom, st);
+	if (conv == QS_CONV_L && store == QS_RENDER_GREY)
+		return qs_launch_render_pack<QS_CONV_L>(imgs, n, tiles, status, store, scale_denom, st);
+	return cudaErrorInvalidValue;
+}
+
+cudaError_t qs_launch_render4_async(const QsRenderImg4 *imgs, int n, int tiles, int store, int conv, int scale_denom,
+		cudaStream_t st) {
+	if (tiles <= 0) return cudaSuccess;
+	if (conv == QS_CONV_CMYK_RGB && (store == QS_RENDER_HWC || store == QS_RENDER_CHW))
+		return qs_launch_render_pack<QS_CONV_CMYK_RGB>(imgs, n, tiles, NULL, store, scale_denom, st);
+	if (conv == QS_CONV_CMYK_L && store == QS_RENDER_GREY)
+		return qs_launch_render_pack<QS_CONV_CMYK_L>(imgs, n, tiles, NULL, store, scale_denom, st);
+	return cudaErrorInvalidValue;
 }
 
 /* sample (x, y) of a host plane of `stride` samples per row */
@@ -2228,16 +2311,19 @@ struct QsHostPx {
 	__host__ __device__ int operator()(int x, int y) const { return s[(size_t)y * stride + x]; }
 };
 
-template <int D>
-static void qs_render_host_d(const QsRenderImg &im, int store) {
+template <int D, class Img>
+static void qs_render_host_d(const Img &im, int store, int conv) {
+	constexpr int NC = sizeof(Img::coef) / sizeof(Img::coef[0]);
 	const int nc = im.ncomp, W = im.width, H = im.height;
-	std::vector<uint8_t> plane[3];
-	QsHostPx px[3];
-	int hs[3], vs[3], cw[3], ch[3];
+	std::vector<uint8_t> plane[NC];
+	QsHostPx px[NC];
+	int hs[NC], vs[NC], cw[NC], ch[NC];
 	for (int c = 0; c < nc; c++) {
-		const bool up = c > 0 && im.up_mode == 1;
+		bool up = false;
+		if constexpr (NC == 3) up = c > 0 && im.up_mode == 1;
 		const int k = up ? 0 : c, lss = D == 1 ? 3 : (im.lss >> (2 * k)) & 3, ss = 1 << lss;
-		const int16_t *coef = up ? im.coef_up[c - 1] : im.coef[c];
+		const int16_t *coef = im.coef[c];
+		if constexpr (NC == 3) if (up) coef = im.coef_up[c - 1];
 		hs[c] = im.hs[k]; vs[c] = im.vs[k]; cw[c] = im.cw[k]; ch[c] = im.ch[k];
 		/* the blocks that hold the real samples (the render reads no others) */
 		const int nbx = (cw[c] + ss - 1) >> lss, nby = (ch[c] + ss - 1) >> lss, stride = nbx * ss;
@@ -2255,25 +2341,38 @@ static void qs_render_host_d(const QsRenderImg &im, int store) {
 	for (int oy = 0; oy < H; oy++)
 		for (int ox = 0; ox < W; ox++) {
 			const int y = qs_upsample_at<D != 8>(px[0], hs[0], vs[0], cw[0], ch[0], ox, oy);
-			int c1 = y, c2 = y;
+			int c1 = y, c2 = y, c3 = 0;
 			if (nc >= 3) {
 				c1 = qs_upsample_at<D != 8>(px[1], hs[1], vs[1], cw[1], ch[1], ox, oy);
 				c2 = qs_upsample_at<D != 8>(px[2], hs[2], vs[2], cw[2], ch[2], ox, oy);
 			}
-			const uint32_t v = qs_rgb_pixel(y, c1, c2, ycc);
+			if (nc == 4) c3 = qs_upsample_at<D != 8>(px[NC - 1], hs[NC - 1], vs[NC - 1], cw[NC - 1], ch[NC - 1], ox, oy);
+			const uint32_t v = conv == QS_CONV_L ? qs_convert_pixel<QS_CONV_L>(y, c1, c2, c3, ycc) :
+					conv == QS_CONV_CMYK_RGB ? qs_convert_pixel<QS_CONV_CMYK_RGB>(y, c1, c2, c3, ycc) :
+					conv == QS_CONV_CMYK_L ? qs_convert_pixel<QS_CONV_CMYK_L>(y, c1, c2, c3, ycc) :
+					qs_convert_pixel<QS_CONV_NONE>(y, c1, c2, c3, ycc);
 			const size_t i = (size_t)oy * W + ox;
 			if (store == QS_RENDER_HWC) for (int j = 0; j < 3; j++) im.out[3 * i + j] = (uint8_t)(v >> (8 * j));
 			else for (int j = 0; j < (store == QS_RENDER_GREY ? 1 : 3); j++) im.out[(size_t)j * W * H + i] = (uint8_t)(v >> (8 * j));
 		}
 }
 
-void qs_render_host(const QsRenderImg *im, int store, int scale_denom) {
+template <class Img>
+static void qs_render_host_any(const Img &im, int store, int scale_denom, int conv) {
 	switch (scale_denom) {
-	case 1: qs_render_host_d<1>(*im, store); break;
-	case 2: qs_render_host_d<2>(*im, store); break;
-	case 4: qs_render_host_d<4>(*im, store); break;
-	default: qs_render_host_d<8>(*im, store); break;
+	case 1: qs_render_host_d<1>(im, store, conv); break;
+	case 2: qs_render_host_d<2>(im, store, conv); break;
+	case 4: qs_render_host_d<4>(im, store, conv); break;
+	default: qs_render_host_d<8>(im, store, conv); break;
 	}
+}
+
+void qs_render_host(const QsRenderImg *im, int store, int scale_denom, int conv) {
+	qs_render_host_any(*im, store, scale_denom, conv);
+}
+
+void qs_render4_host(const QsRenderImg4 *im, int store, int scale_denom, int conv) {
+	qs_render_host_any(*im, store, scale_denom, conv);
 }
 
 cudaError_t qs_launch_render_rgb(const uint8_t *const *planes, const int *strides, const int *cw, const int *ch,

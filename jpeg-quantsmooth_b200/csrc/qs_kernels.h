@@ -62,19 +62,47 @@ typedef struct {
 	uint16_t q[3][64];           /* multipliers: the raw quant table where it de-quantizes, else ones */
 } QsRenderImg;
 #define QS_RENDER_PACK 60
+/* the descriptor of a 4-component (CMYK or YCCK) image: QsRenderImg's fields for four components, without
+ * coef_up and up_mode (UPSAMPLE_UV never applies to these); lss holds four 2-bit fields */
+typedef struct {
+	const int16_t *coef[4];
+	uint8_t *out;
+	int32_t width, height, tile_begin;
+	int32_t wblk[4], cw[4], ch[4];
+	uint8_t hs[4], vs[4];
+	uint8_t ncomp;               /* 4 */
+	uint8_t ycc;                 /* 1: YCCK (components 0..2 YCbCr, libjpeg's ycck_cmyk_convert), 0: CMYK */
+	uint8_t lss, orient;
+	uint16_t q[4][64];
+} QsRenderImg4;
+#define QS_RENDER_PACK4 52
 /* store modes of the render kernel: the two public layouts, and one byte per pixel for 1-component
  * images (qs_render_images' grey store) */
 #define QS_RENDER_HWC 0
 #define QS_RENDER_CHW 1
 #define QS_RENDER_GREY 2
+/* colour conversions of the render (Pillow's Image.convert of the decoded picture):
+ *   NONE      the file's own colour: RGB for 3 components, the sample for grey (the existing kernels)
+ *   L         Pillow's rgb2l of that RGB pixel; GREY store
+ *   CMYK_RGB  4 components: Pillow's CMYK;I decode then cmyk2rgb (YCCK through ycck_cmyk_convert first)
+ *   CMYK_L    4 components: rgb2l of CMYK_RGB's pixel; GREY store */
+#define QS_CONV_NONE 0
+#define QS_CONV_L 1
+#define QS_CONV_CMYK_RGB 2
+#define QS_CONV_CMYK_L 3
 /* status: the launch's first image's {stop, upsampled}, or NULL when no image has up_mode 2;
  * scale_denom: 1, 2, 4 or 8; an orient outside 1..8 gives cudaErrorInvalidValue */
 /* the render kernels' opt-in to the dynamic shared memory of orientations 5..8 (once per device) */
 cudaError_t qs_render_configure(void);
+/* conv: QS_CONV_NONE (any store) or QS_CONV_L (QS_RENDER_GREY) */
 cudaError_t qs_launch_render_async(const QsRenderImg *imgs, int n, int tiles, const int2 *status, int store,
-		int scale_denom, cudaStream_t st);
+		int scale_denom, cudaStream_t st, int conv = QS_CONV_NONE);
+/* 4-component images, n <= QS_RENDER_PACK4: conv QS_CONV_CMYK_RGB (HWC or CHW) or QS_CONV_CMYK_L (GREY) */
+cudaError_t qs_launch_render4_async(const QsRenderImg4 *imgs, int n, int tiles, int store, int conv, int scale_denom,
+		cudaStream_t st);
 /* the same render of one image on the calling thread: host coefficient and output pointers, up_mode 0
  * or 1 */
-void qs_render_host(const QsRenderImg *im, int store, int scale_denom);
+void qs_render_host(const QsRenderImg *im, int store, int scale_denom, int conv = QS_CONV_NONE);
+void qs_render4_host(const QsRenderImg4 *im, int store, int scale_denom, int conv);
 
 #endif

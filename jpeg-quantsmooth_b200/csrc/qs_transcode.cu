@@ -30,10 +30,10 @@ void qs_ctx_set_last_ms(jpegqs_cuda_ctx *ctx, float ms);
 extern "C" int qs_route_plan(const uint8_t *data, size_t len, int copy, jpegqs_cuda_file_info *info, jpegqs_cuda_image *img,
 		jpegqs_cuda_scan *scan, jpegqs_cuda_scan_rec *recs, int *nscans, jpegqs_cuda_jpeg_head *head,
 		uint8_t **prefix, size_t *prefix_len, const char **reason);
-int qs_render_takes(const jpegqs_cuda_image *im);                     /* qs_cuda.cu */
+int qs_render_takes(const jpegqs_cuda_image *im, int mode);           /* qs_cuda.cu */
 int qs_render_images(jpegqs_cuda_ctx *ctx, int nimages, const jpegqs_cuda_image *imgs,
 		const jpegqs_cuda_status *status_dev, int layout, int grey_store, int scale_denom, const int32_t *orient,
-		uint8_t *const *out_dev, void *stream);
+		uint8_t *const *out_dev, void *stream, int mode, const int32_t *color_space);
 
 /* ---- the packing kernel -------------------------------------------------------------------------
  * After encode_async, file k of a sub-batch sits at the start of its bound-sized slot.  One launch
@@ -188,6 +188,7 @@ struct QsPlan {
 	int smooth, can_up;
 	int out_w, out_h;                          /* pixels: the output picture's size */
 	int orient, pic_w;                         /* pixels: the render's orientation (1..8), the rendered picture's width */
+	int channels;                              /* pixels: 1 or 3, from the mode (the component count for mode 0) */
 	size_t in_bytes, coef_bytes, up_bytes, cap, pix;
 	size_t ws_dec, ws_run, ws_enc;             /* this file's share of each stage's workspace */
 	size_t fixed, packed;                      /* its share of the buffers outside the workspace; of the packed output */
@@ -603,10 +604,11 @@ struct QsJpegLayout {
  * pictures are written as JPEG files with these params (compress_async) into jout / jlen, and on_device
  * must be 0 (the pictures stay in the context's buffers).  orientation: NULL (1 for every file) or 0..8
  * per file, 0 for the file's own; the render writes the oriented picture, which the crop, the resize
- * and the compressor then take as it is. */
+ * and the compressor then take as it is.  mode: JPEGQS_PIXELS_*; the render converts, so every later stage
+ * takes the converted picture's channels. */
 static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint8_t *const *data, const size_t *len,
 		int flags, int niter, int layout, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
-		const int32_t *orientation, int on_device, uint8_t *const *out, size_t max_device_bytes, int *rc,
+		const int32_t *orientation, int mode, int on_device, uint8_t *const *out, size_t max_device_bytes, int *rc,
 		jpegqs_cuda_pixels_result *results, const jpegqs_cuda_jpeg_params *jp = NULL, uint8_t **jout = NULL,
 		size_t *jlen = NULL) {
 	char msg[512];
@@ -630,7 +632,8 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 			qs_ctx_decode_done(ctx, 0, msg);
 			rc[i] = JPEGQS_ERR_ARG; continue;
 		}
-		if (!qs_render_takes(&p.img)) { rc[i] = JPEGQS_ERR_UNSUPPORTED; continue; }
+		if (!qs_render_takes(&p.img, mode)) { rc[i] = JPEGQS_ERR_UNSUPPORTED; continue; }
+		p.channels = mode == JPEGQS_PIXELS_RGB ? 3 : mode == JPEGQS_PIXELS_L ? 1 : p.img.ncomp;
 		/* the picture at scale 1 / scale_denom: ceil(width / d) x ceil(height / d) x channels, its axes
 		 * swapped by orientations 5..8 */
 		p.orient = orientation ? orientation[i] : 1;
@@ -638,7 +641,7 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 		const int sw = (int)((p.img.image_width + scale_denom - 1) / scale_denom);
 		const int sh = (int)((p.img.image_height + scale_denom - 1) / scale_denom);
 		const int pw = p.orient >= 5 ? sh : sw, ph = p.orient >= 5 ? sw : sh;
-		p.pix = (size_t)pw * ph * p.img.ncomp;
+		p.pix = (size_t)pw * ph * p.channels;
 		p.out_w = pw; p.out_h = ph; p.pic_w = pw;
 		if (boxes) {
 			const char *bad = qs_resize_plan(pw, ph, boxes[i], filter, rsp[i]);
@@ -648,24 +651,24 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 				rc[i] = JPEGQS_ERR_ARG; continue;
 			}
 			pic[i] = p.pix;
-			p.pix = (size_t)boxes[i].width * boxes[i].height * p.img.ncomp;
+			p.pix = (size_t)boxes[i].width * boxes[i].height * p.channels;
 			p.out_w = boxes[i].width; p.out_h = boxes[i].height;
 		}
 		p.host = route != JPEGQS_ROUTE_DEVICE;
 		if (p.host) { p.in_bytes = 0; p.ws_dec = 0; results[i].host_decoded = 1; results[i].reason = why; }
-		results[i].channels = p.img.ncomp;
+		results[i].channels = p.channels;
 		TQ(plan_run(p, flags, niter));
 		/* file, coefficients (+ up-sampled chroma), the output pixels when they come back to the host;
 		 * resized: also the rendered picture, the intermediate, the tables and the descriptor */
 		p.fixed = p.in_bytes + p.coef_bytes + p.up_bytes + (on_device ? 0 : align256(p.pix));
 		if (boxes)
-			p.fixed += align256(pic[i]) + align256((size_t)rsp[i].mid_h * rsp[i].out_w * p.img.ncomp) +
+			p.fixed += align256(pic[i]) + align256((size_t)rsp[i].mid_h * rsp[i].out_w * p.channels) +
 					align256(rsp[i].tab.size() * sizeof(int32_t)) + align256(sizeof(QsResizeDesc));
 		p.ws_enc = 0; p.packed = 0;
 		if (jp) {
 			/* JPEG: the compressor's workspace share (coefficients and encoder workspace, with the prefix's
 			 * 256 bytes counted per file), its output slot, the packed copy and the per-file records */
-			const jpegqs_cuda_pixels_in pin = { NULL, p.out_w, p.out_h, p.img.ncomp, (size_t)p.out_w * p.img.ncomp };
+			const jpegqs_cuda_pixels_in pin = { NULL, p.out_w, p.out_h, p.channels, (size_t)p.out_w * p.channels };
 			TQ(jpegqs_cuda_compress_bound(&pin, jp, &p.cap));
 			TQ(jpegqs_cuda_compress_workspace_bytes(1, &pin, jp, &p.ws_enc));
 			p.packed = align16(p.cap);
@@ -776,15 +779,16 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 			TK(cudaMemcpyAsync(t->hcoef_dev.p, t->hcoef_host.p, hb, cudaMemcpyHostToDevice, st));
 		}
 
-		/* 7: run_async over the files that smooth, then one render over all.  Order: the colour files
-		 * that smooth, the grey files that smooth, the grey files that do not, the colour files that do
-		 * not - run_async's images are a prefix, and the grey store's images are consecutive, so the
-		 * render takes at most three launches per 60 images */
+		/* 7: run_async over the files that smooth, then one render over all.  Order by component count
+		 * 3, 1, 4 among the files that smooth, then 4, 1, 3 among those that do not - run_async's images
+		 * are a prefix, and each launch group's images (one store mode and conversion) are consecutive, so
+		 * the render takes at most five launches per 60 images (three without 4-component files) */
 		std::vector<int> rk;                           /* render order -> group position */
-		for (int pass = 0; pass < 4; pass++)
+		static const int kinds[6] = {3, 1, 4, 4, 1, 3};
+		for (int pass = 0; pass < 6; pass++)
 			for (int k = 0; k < m; k++) {
 				const QsPlan &p = plans[files[k]];
-				if (alive[k] && p.smooth == (pass < 2) && (p.img.ncomp == 1) == (pass == 1 || pass == 2)) rk.push_back(k);
+				if (alive[k] && p.smooth == (pass < 3) && p.img.ncomp == kinds[pass]) rk.push_back(k);
 			}
 		const int nr = (int)rk.size();
 		int ms = 0;
@@ -810,7 +814,7 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 			all = up;
 			for (int j = 0; j < nr; j++) {
 				const QsResizePlan &r = rsp[files[rk[j]]];
-				moff[j] = all; all += align256((size_t)r.mid_h * r.out_w * rimg[j].ncomp);
+				moff[j] = all; all += align256((size_t)r.mid_h * r.out_w * plans[files[rk[j]]].channels);
 			}
 			for (int j = 0; j < nr; j++) { qoff[j] = all; all += align256(pic[files[rk[j]]]); }
 			TK(grow_dev(&t->rs_dev, all));
@@ -820,7 +824,7 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 			for (int j = 0; j < nr; j++) {
 				const int f = files[rk[j]];
 				const QsResizePlan &r = rsp[f];
-				qs_resize_desc(r, plans[f].pic_w, rimg[j].ncomp, layout == JPEGQS_RENDER_CHW, desc[j]);
+				qs_resize_desc(r, plans[f].pic_w, plans[f].channels, layout == JPEGQS_RENDER_CHW, desc[j]);
 				memcpy(rh + toff[j], r.tab.data(), r.tab.size() * sizeof(int32_t));
 				desc[j].src = rd + qoff[j]; desc[j].mid = rd + moff[j]; desc[j].out = outs[j];
 				desc[j].tab = (const int32_t*)(rd + toff[j]);
@@ -835,10 +839,10 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 			TK(cudaEventRecord(t->ev1, st));
 		}
 		if (ms < nr) TK(cudaMemsetAsync(run + ms, 0, (size_t)(nr - ms) * sizeof(jpegqs_cuda_status), st));
-		std::vector<int32_t> ro(nr);
-		for (int j = 0; j < nr; j++) ro[j] = plans[files[rk[j]]].orient;
+		std::vector<int32_t> ro(nr), rcs(nr);
+		for (int j = 0; j < nr; j++) { ro[j] = plans[files[rk[j]]].orient; rcs[j] = plans[files[rk[j]]].scan.jpeg_color_space; }
 		if (nr) TQ(qs_render_images(ctx, nr, rimg.data(), run, boxes ? JPEGQS_RENDER_HWC : layout, 1, scale_denom, ro.data(),
-				outs.data(), st));
+				outs.data(), st, mode, mode ? rcs.data() : NULL));
 		if (boxes && nr) TK(qs_launch_resize((const QsResizeDesc*)t->rs_dev.p, nr, hblocks, vblocks, st));
 		/* JPEG: compress_async over the pictures into the slots, then the packing kernel into the
 		 * workspace, its records back */
@@ -854,8 +858,8 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 			for (int j = 0; j < nr; j++) {
 				const QsPlan &p = plans[files[rk[j]]];
 				pin[j].pixels_dev = (const uint8_t*)t->out_dev.p + poff[j];
-				pin[j].width = p.out_w; pin[j].height = p.out_h; pin[j].channels = p.img.ncomp;
-				pin[j].row_bytes = (size_t)p.out_w * p.img.ncomp;
+				pin[j].width = p.out_w; pin[j].height = p.out_h; pin[j].channels = p.channels;
+				pin[j].row_bytes = (size_t)p.out_w * p.channels;
 				slot[j] = jd + jl.slots + so; cap[j] = p.cap;
 				memset(&pd[j], 0, sizeof(pd[j]));
 				pd[j].slot = so; pd[j].cap = p.cap; pd[j].dec_idx = j;
@@ -932,10 +936,19 @@ static int orientation_ok(jpegqs_cuda_ctx *ctx, const char *who, int n, const in
 	return 1;
 }
 
+/* a colour mode's check: JPEGQS_PIXELS_AS_FILE, _RGB or _L */
+static int mode_ok(jpegqs_cuda_ctx *ctx, const char *who, int mode) {
+	if (mode == JPEGQS_PIXELS_AS_FILE || mode == JPEGQS_PIXELS_RGB || mode == JPEGQS_PIXELS_L) return 1;
+	char msg[200];
+	snprintf(msg, sizeof(msg), "%s: mode %d: expected 0 (as the file), 1 (RGB) or 2 (L)", who, mode);
+	qs_ctx_decode_done(ctx, 0, msg);
+	return 0;
+}
+
 static int pixels_entry(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint8_t *const *data, const size_t *len,
 		int flags, int niter, int layout, int scale_denom, int resize, int filter, const jpegqs_cuda_resize_box *boxes,
 		int out_on_device, uint8_t *const *out, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results,
-		const int32_t *orientation = NULL) {
+		const int32_t *orientation = NULL, int mode = JPEGQS_PIXELS_AS_FILE) {
 	char msg[200];
 	if (!ctx) return JPEGQS_ERR_ARG;
 	if (n < 0) { snprintf(msg, sizeof(msg), "%s: negative file count", who); qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG; }
@@ -963,10 +976,18 @@ static int pixels_entry(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 			qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG;
 		}
 	}
-	if (!orientation_ok(ctx, who, n, orientation)) return JPEGQS_ERR_ARG;
+	if (!orientation_ok(ctx, who, n, orientation) || !mode_ok(ctx, who, mode)) return JPEGQS_ERR_ARG;
 	for (int i = 0; i < n; i++) { memset(&results[i], 0, sizeof(results[i])); results[i].reason = ""; rc[i] = 0; }
 	return pixels_batch(ctx, who, n, data, len, flags, niter, layout, scale_denom, filter, resize ? boxes : NULL, orientation,
-			out_on_device, out, max_device_bytes, rc, results);
+			mode, out_on_device, out, max_device_bytes, rc, results);
+}
+
+extern "C" int jpegqs_cuda_pixels_batch_mode(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int layout, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
+		const int32_t *orientation, int mode, int out_on_device, uint8_t *const *out, size_t max_device_bytes, int *rc,
+		jpegqs_cuda_pixels_result *results) {
+	return pixels_entry(ctx, "jpegqs_cuda_pixels_batch_mode", n, data, len, flags, niter, layout, scale_denom,
+			boxes != NULL, filter, boxes, out_on_device, out, max_device_bytes, rc, results, orientation, mode);
 }
 
 extern "C" int jpegqs_cuda_pixels_batch_oriented(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
@@ -987,7 +1008,7 @@ extern "C" int jpegqs_cuda_pixels_batch_resized(jpegqs_cuda_ctx *ctx, int n, con
 static int pixels_jpeg_entry(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint8_t *const *data, const size_t *len,
 		int flags, int niter, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
 		const jpegqs_cuda_jpeg_params *params, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results,
-		uint8_t **out, size_t *out_len, const int32_t *orientation) {
+		uint8_t **out, size_t *out_len, const int32_t *orientation, int mode) {
 	char msg[200];
 	if (!ctx) return JPEGQS_ERR_ARG;
 	if (n < 0) { snprintf(msg, sizeof(msg), "%s: negative file count", who); qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG; }
@@ -1017,9 +1038,9 @@ static int pixels_jpeg_entry(jpegqs_cuda_ctx *ctx, const char *who, int n, const
 			qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG;
 		}
 	}
-	if (!orientation_ok(ctx, who, n, orientation)) return JPEGQS_ERR_ARG;
+	if (!orientation_ok(ctx, who, n, orientation) || !mode_ok(ctx, who, mode)) return JPEGQS_ERR_ARG;
 	for (int i = 0; i < n; i++) { memset(&results[i], 0, sizeof(results[i])); results[i].reason = ""; rc[i] = 0; out[i] = NULL; out_len[i] = 0; }
-	return pixels_batch(ctx, who, n, data, len, flags, niter, JPEGQS_RENDER_HWC, scale_denom, filter, boxes, orientation, 0, NULL,
+	return pixels_batch(ctx, who, n, data, len, flags, niter, JPEGQS_RENDER_HWC, scale_denom, filter, boxes, orientation, mode, 0, NULL,
 			max_device_bytes, rc, results, params, out, out_len);
 }
 
@@ -1028,7 +1049,7 @@ extern "C" int jpegqs_cuda_pixels_batch_jpeg(jpegqs_cuda_ctx *ctx, int n, const 
 		const jpegqs_cuda_jpeg_params *params, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results,
 		uint8_t **out, size_t *out_len) {
 	return pixels_jpeg_entry(ctx, "jpegqs_cuda_pixels_batch_jpeg", n, data, len, flags, niter, scale_denom, filter, boxes, params,
-			max_device_bytes, rc, results, out, out_len, NULL);
+			max_device_bytes, rc, results, out, out_len, NULL, JPEGQS_PIXELS_AS_FILE);
 }
 
 extern "C" int jpegqs_cuda_pixels_batch_jpeg_oriented(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
@@ -1036,7 +1057,15 @@ extern "C" int jpegqs_cuda_pixels_batch_jpeg_oriented(jpegqs_cuda_ctx *ctx, int 
 		const jpegqs_cuda_jpeg_params *params, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results,
 		uint8_t **out, size_t *out_len, const int32_t *orientation) {
 	return pixels_jpeg_entry(ctx, "jpegqs_cuda_pixels_batch_jpeg_oriented", n, data, len, flags, niter, scale_denom, filter, boxes,
-			params, max_device_bytes, rc, results, out, out_len, orientation);
+			params, max_device_bytes, rc, results, out, out_len, orientation, JPEGQS_PIXELS_AS_FILE);
+}
+
+extern "C" int jpegqs_cuda_pixels_batch_jpeg_mode(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
+		const jpegqs_cuda_jpeg_params *params, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results,
+		uint8_t **out, size_t *out_len, const int32_t *orientation, int mode) {
+	return pixels_jpeg_entry(ctx, "jpegqs_cuda_pixels_batch_jpeg_mode", n, data, len, flags, niter, scale_denom, filter, boxes,
+			params, max_device_bytes, rc, results, out, out_len, orientation, mode);
 }
 
 extern "C" int jpegqs_cuda_pixels_batch_scaled(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,

@@ -268,6 +268,21 @@ def load():
                                                            C.POINTER(C.c_int), C.POINTER(_PixelsResult),
                                                            C.POINTER(C.c_void_p), C.POINTER(C.c_size_t),
                                                            C.POINTER(C.c_int32)]
+    lib.jpegqs_cuda_render_mode_async.argtypes = [C.c_void_p, C.c_int, C.POINTER(_Image), C.c_void_p, C.c_int, C.c_int,
+                                                  C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int,
+                                                  C.POINTER(C.c_void_p), C.c_void_p]
+    lib.jpegqs_cuda_render_model_mode.argtypes = [C.POINTER(_Image), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                                  C.c_void_p]
+    lib.jpegqs_cuda_pixels_batch_mode.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_size_t),
+                                                  C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(_ResizeBox),
+                                                  C.POINTER(C.c_int32), C.c_int, C.c_int, C.POINTER(C.c_void_p),
+                                                  C.c_size_t, C.POINTER(C.c_int), C.POINTER(_PixelsResult)]
+    lib.jpegqs_cuda_pixels_batch_jpeg_mode.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_char_p),
+                                                       C.POINTER(C.c_size_t), C.c_int, C.c_int, C.c_int, C.c_int,
+                                                       C.POINTER(_ResizeBox), C.POINTER(_JpegParams), C.c_size_t,
+                                                       C.POINTER(C.c_int), C.POINTER(_PixelsResult),
+                                                       C.POINTER(C.c_void_p), C.POINTER(C.c_size_t),
+                                                       C.POINTER(C.c_int32), C.c_int]
     lib.jpegqs_cuda_tables.argtypes = [C.c_int, C.c_void_p]
     lib.jpegqs_cuda_orig_coef.argtypes = [C.c_int, C.c_int]
     _lib = lib
@@ -514,15 +529,33 @@ def decode_workspace_bytes(images: Sequence[CoefImage], scans, data_len: Sequenc
     return int(out.value)
 
 
-def render_model(image: CoefImage, upsampled=False, layout: str = "hwc", scale_denom: int = 1):
+# Pillow's output modes (include/jpegqs_cuda.h JPEGQS_PIXELS_*): None keeps the file's own colour
+_MODES = {None: 0, "RGB": 1, "L": 2}
+
+
+def _mode(mode, who: str) -> int:
+    if not isinstance(mode, (str, type(None))) or mode not in _MODES:
+        raise ValueError(f"{who}: mode {mode!r}: expected None, 'RGB' or 'L'")
+    return _MODES[mode]
+
+
+def _mode_channels(ncomp: int, mode: int) -> int:
+    """the output channels of an ncomp-component file in mode (0: the file's own, 3 for colour)"""
+    return (1 if ncomp == 1 else 3) if mode == 0 else 3 if mode == 1 else 1
+
+
+def render_model(image: CoefImage, upsampled=False, layout: str = "hwc", scale_denom: int = 1, mode=None):
     """render_async's algorithm on one CPU thread for one image (jpegqs_cuda_render_model): libjpeg's
     islow / reduced IDCTs, up-sampling and colour conversion at scale 1/scale_denom.  upsampled: None /
     False reads the image's own arrays; otherwise a pair of int16 numpy arrays [hblk, wblk, 64] at
     component 0's geometry, read for components 1 and 2.  Returns a uint8 numpy array [H, W, 3] ("hwc")
-    or [3, H, W] ("chw"), H = ceil(height / d) and W = ceil(width / d)."""
+    or [3, H, W] ("chw"), H = ceil(height / d) and W = ceil(width / d).
+    mode: None, or Pillow's "RGB" / "L" of the picture (jpegqs_cuda_render_model_mode), for any component
+    count 1, 3 or 4, with image.colorspace deciding the conversion; the output then has 3 or 1 channels."""
     if layout not in ("hwc", "chw"):
         raise ValueError(f"render_model: layout {layout!r}: expected 'hwc' or 'chw'")
     d = _scale_denom(scale_denom, "render_model")
+    m = _mode(mode, "render_model")
     lib = load()
     arrays = [np.ascontiguousarray(c.coef, dtype=np.int16) for c in image.comps]
     for c, a in zip(image.comps, arrays):
@@ -538,8 +571,12 @@ def render_model(image: CoefImage, upsampled=False, layout: str = "hwc", scale_d
             raise ValueError(f"render_model: up-sampled arrays must have component 0's shape {(y.hblk, y.wblk, 64)}")
     ci = _Image()
     _fill_image(ci, image, [a.ctypes.data for a in arrays], [None] + [u.ctypes.data for u in ups] if ups else [])
-    out = np.zeros(_scaled_shape(image.width, image.height, 3, layout, d), dtype=np.uint8)
-    rc = lib.jpegqs_cuda_render_model(C.byref(ci), int(bool(ups)), 0 if layout == "hwc" else 1, d, out.ctypes.data)
+    out = np.zeros(_scaled_shape(image.width, image.height, 3 if m < 2 else 1, layout, d), dtype=np.uint8)
+    if m:
+        rc = lib.jpegqs_cuda_render_model_mode(C.byref(ci), int(image.colorspace), int(bool(ups)),
+                                               0 if layout == "hwc" else 1, d, m, out.ctypes.data)
+    else:
+        rc = lib.jpegqs_cuda_render_model(C.byref(ci), int(bool(ups)), 0 if layout == "hwc" else 1, d, out.ctypes.data)
     if rc < 0:
         raise QsError(f"render_model: {lib.jpegqs_cuda_last_error(None).decode()} ({rc})")
     return out
@@ -999,7 +1036,7 @@ class QsContext:
 
     def decode_pixels(self, datas, flags: int, niter: int, layout: str = "hwc", device: str = "cuda",
                       max_device_bytes: int = 0, scale_denom: int = 1, size=None, crop=None, filter="bicubic",
-                      orientation=None):
+                      orientation=None, mode=None):
         """Many JPEG files to the smoothed pixels the jpegqs tool's --ppm writes for them (islow, fancy
         up-sampling, after do_quantsmooth(flags, niter)), in shared launches (jpegqs_cuda_pixels_batch).
         Returns, in the order of datas, one record per file:
@@ -1027,7 +1064,10 @@ class QsContext:
         orientation, as Pillow's ImageOps.exif_transpose applies it), one int 1..8 for every file, or a
         sequence of ints 0..8, one per file, 0 meaning the file's own (jpegqs_cuda_pixels_batch_oriented).
         The picture is turned before the crop and the resize, so crop is in the oriented picture, and for
-        5..8 the unresized pixels have width and height swapped.  ValueError for a bad value or length."""
+        5..8 the unresized pixels have width and height swapped.  ValueError for a bad value or length.
+        mode: None (the file's own colour, as above), "RGB" or "L": Pillow's Image.convert(mode) of each
+        file's picture, before the crop and the resize, so C is 3 or 1 for every file, and CMYK and YCCK
+        files are decoded too (jpegqs_cuda_pixels_batch_mode).  ValueError for any other value."""
         if isinstance(datas, (bytes, bytearray, memoryview, str)) or not hasattr(datas, "__len__"):
             raise TypeError("decode_pixels: datas must be a sequence of bytes-like files")
         files = [_file_bytes(d, f"decode_pixels: file {i}") for i, d in enumerate(datas)]
@@ -1044,6 +1084,7 @@ class QsContext:
             fcode = _resize_filter(filter, "decode_pixels")
             sizes, crops = _resize_boxes(n, size, crop, "decode_pixels")
         orient = _orientations(orientation, n, "decode_pixels")
+        m = _mode(mode, "decode_pixels")
         if not n:
             return []
         # the output size rule of jpegqs_cuda_pixels_batch: transcode_route's width, height and ncomp
@@ -1052,9 +1093,10 @@ class QsContext:
             info = _FileInfo()
             if self.lib.jpegqs_cuda_transcode_route(d, len(d), None, C.byref(info)) < 0:
                 raise QsError(f"decode_pixels: file {i}: the reader rejects the file")
-            if info.ncomp not in (1, 3):
-                raise QsError(f"decode_pixels: file {i}: {info.ncomp} components; the render takes 1 or 3")
-            c, h, w = info.ncomp, info.image_height, info.image_width
+            if info.ncomp not in ((1, 3) if not m else (1, 3, 4)):
+                raise QsError(f"decode_pixels: file {i}: {info.ncomp} components; the render takes "
+                              + ("1, 3 or 4" if m else "1 or 3 (4 with a mode)"))
+            c, h, w = _mode_channels(info.ncomp, m), info.image_height, info.image_width
             shapes.append(_scaled_shape(w, h, c, layout, scale))
         if orient is not None:
             orient = [exif_orientation(d) if o == 0 else o for d, o in zip(files, orient)]
@@ -1079,7 +1121,14 @@ class QsContext:
         optrs = (C.c_void_p * n)(*[t.data_ptr() for t in outs])
         rc = (C.c_int * n)()
         res = (_PixelsResult * n)()
-        if orient is not None:
+        if m:
+            self._check(self.lib.jpegqs_cuda_pixels_batch_mode(self.h, n, ptrs, lens, int(flags), int(niter),
+                                                               0 if layout == "hwc" else 1, scale,
+                                                               fcode if resize else 0, boxes if resize else None,
+                                                               None if orient is None else (C.c_int32 * n)(*orient), m,
+                                                               int(device == "cuda"), optrs, int(max_device_bytes), rc,
+                                                               res))
+        elif orient is not None:
             self._check(self.lib.jpegqs_cuda_pixels_batch_oriented(self.h, n, ptrs, lens, int(flags), int(niter),
                                                                    0 if layout == "hwc" else 1, scale,
                                                                    fcode if resize else 0, boxes if resize else None,
@@ -1287,7 +1336,7 @@ class QsContext:
 
     # ---- stream-ordered render to RGB (include/jpegqs_cuda.h jpegqs_cuda_render_async) ----
     def render_async(self, images: Sequence[CoefImage], coefs, status=None, up=None, layout: str = "hwc",
-                     out=None, stream=None, scale_denom: int = 1, orientation=None):
+                     out=None, stream=None, scale_denom: int = 1, orientation=None, mode=None):
         """Decode device-resident coefficients to 8-bit RGB, as libjpeg would, without blocking the
         calling thread.  The coefficient tensors are only read.
 
@@ -1302,12 +1351,16 @@ class QsContext:
         H and W then being ceil(height / d) and ceil(width / d).  orientation: None, or a sequence of
         one EXIF orientation 1..8 per image (jpegqs_cuda_render_oriented_async); each output is then the
         picture as Pillow's Image.transpose turns it, with H and W swapped for 5..8.  Capturable with
-        torch.cuda.graph.  Returns the list of output tensors."""
+        torch.cuda.graph.  Returns the list of output tensors.
+        mode: None, or "RGB" / "L": Pillow's Image.convert(mode) of the picture
+        (jpegqs_cuda_render_mode_async), 3 or 1 channels for images of 1, 3 or 4 components, each
+        image's CoefImage.colorspace deciding the conversion (4 components: JCS_CMYK or JCS_YCCK)."""
         import torch
         n = len(images)
         if layout not in ("hwc", "chw"):
             raise ValueError(f"layout {layout!r}: expected 'hwc' or 'chw'")
         d = _scale_denom(scale_denom, "render_async")
+        m = _mode(mode, "render_async")
         if orientation is not None and (isinstance(orientation, (str, bytes)) or _orient_int(orientation) is not None):
             raise ValueError("render_async: orientation: expected a sequence of one value 1..8 per image")
         orient = _orientations(orientation, n, "render_async", lo=1)
@@ -1339,7 +1392,7 @@ class QsContext:
             if status.dtype != torch.int32 or tuple(status.shape) != (n, 2) or not status.is_contiguous():
                 raise ValueError(f"status: expected a contiguous int32 tensor [{n}, 2]")
             tensors.append(("status", status))
-        shapes = [_scaled_shape(im.width, im.height, 3, layout, d) for im in images]
+        shapes = [_scaled_shape(im.width, im.height, 3 if m < 2 else 1, layout, d) for im in images]
         if orient is not None:
             shapes = [_oriented_shape(s, o, layout) for s, o in zip(shapes, orient)]
         if out is not None:
@@ -1370,7 +1423,12 @@ class QsContext:
                 arr[i].upsampled = int(bool(host_up and host_up[i]))
             outs = (C.c_void_p * max(n, 1))(*[t.data_ptr() for t in out])
             st = status.data_ptr() if isinstance(status, torch.Tensor) else None
-            if orient is not None:
+            if m:
+                self._check(self.lib.jpegqs_cuda_render_mode_async(
+                    self.h, n, arr, st, 0 if layout == "hwc" else 1, d,
+                    None if orient is None else (C.c_int32 * max(n, 1))(*orient),
+                    (C.c_int32 * max(n, 1))(*[int(im.colorspace) for im in images]), m, outs, _stream_handle(stream)))
+            elif orient is not None:
                 self._check(self.lib.jpegqs_cuda_render_oriented_async(self.h, n, arr, st, 0 if layout == "hwc" else 1, d,
                                                                        (C.c_int32 * max(n, 1))(*orient), outs,
                                                                        _stream_handle(stream)))
@@ -1673,7 +1731,7 @@ class QsContext:
         return out, lengths, st
 
     def reencode(self, datas, flags: int, niter: int, quality=75, subsampling="4:2:0", optimize=False, scale_denom=1,
-                 size=None, crop=None, filter="bicubic", max_device_bytes: int = 0, orientation=None):
+                 size=None, crop=None, filter="bicubic", max_device_bytes: int = 0, orientation=None, mode=None):
         """Many JPEG files to JPEG files of their smoothed pixels (jpegqs_cuda_pixels_batch_jpeg): each
         file's output is exactly Pillow's Image.fromarray(P).save(f, "JPEG", quality=quality,
         subsampling=subsampling, optimize=optimize), where P is the picture decode_pixels gives for the
@@ -1684,7 +1742,9 @@ class QsContext:
         subsampling, size, crop or filter, before anything runs; QsError naming a file the reader
         rejects, the render cannot take, or whose crop falls outside its picture.  orientation: as for
         decode_pixels (jpegqs_cuda_pixels_batch_jpeg_oriented); "exif" gives Pillow's
-        ImageOps.exif_transpose(P).save(...): upright pixels in a JFIF file without the tag."""
+        ImageOps.exif_transpose(P).save(...): upright pixels in a JFIF file without the tag.  mode: as for
+        decode_pixels (jpegqs_cuda_pixels_batch_jpeg_mode): Pillow's P.convert(mode).save(...), so CMYK
+        and YCCK files give RGB files and "L" gives grey files."""
         if isinstance(datas, (bytes, bytearray, memoryview, str)) or not hasattr(datas, "__len__"):
             raise TypeError("reencode: datas must be a sequence of bytes-like files")
         files = [_file_bytes(d, f"reencode: file {i}") for i, d in enumerate(datas)]
@@ -1698,6 +1758,7 @@ class QsContext:
         if resize:
             sizes, crops = _resize_boxes(n, size, crop, "reencode")
         orient = _orientations(orientation, n, "reencode")
+        m = _mode(mode, "reencode")
         if not n:
             return []
         boxes = None
@@ -1718,7 +1779,11 @@ class QsContext:
         res = (_PixelsResult * n)()
         outs = (C.c_void_p * n)()
         olen = (C.c_size_t * n)()
-        if orient is not None:
+        if m:
+            self._check(self.lib.jpegqs_cuda_pixels_batch_jpeg_mode(
+                self.h, n, ptrs, lens, int(flags), int(niter), scale, fcode, boxes, C.byref(jp), int(max_device_bytes),
+                rc, res, outs, olen, None if orient is None else (C.c_int32 * n)(*orient), m))
+        elif orient is not None:
             self._check(self.lib.jpegqs_cuda_pixels_batch_jpeg_oriented(self.h, n, ptrs, lens, int(flags), int(niter), scale,
                                                                         fcode, boxes, C.byref(jp), int(max_device_bytes),
                                                                         rc, res, outs, olen, (C.c_int32 * n)(*orient)))
@@ -1970,16 +2035,16 @@ def decode_async(images: Sequence[CoefImage], scans, data, out=None, stream=None
 
 
 def render_async(images: Sequence[CoefImage], coefs, status=None, up=None, layout: str = "hwc", out=None,
-                 stream=None, scale_denom: int = 1, orientation=None):
+                 stream=None, scale_denom: int = 1, orientation=None, mode=None):
     """QsContext.render_async on the default context of the tensors' device: decodes CUDA
-    coefficient tensors to uint8 RGB tensors ([H, W, 3] or [3, H, W], at 1/scale_denom size),
-    enqueued on `stream` (default: the current one) without waiting."""
+    coefficient tensors to uint8 RGB tensors ([H, W, 3] or [3, H, W], at 1/scale_denom size; one
+    channel for mode "L"), enqueued on `stream` (default: the current one) without waiting."""
     import torch
     first = next((t for ts in coefs for t in ts), None)
     if not isinstance(first, torch.Tensor) or not first.is_cuda:
         raise ValueError("render_async: the coefficient tensors must be CUDA tensors")
     return default_context(first.device.index).render_async(images, coefs, status, up, layout, out, stream, scale_denom,
-                                                            orientation)
+                                                            orientation, mode)
 
 
 def encode_async(images: Sequence[CoefImage], coefs, heads, optimize: bool = False, status=None, up=None, out=None,
@@ -2009,13 +2074,15 @@ def transcode_batch(datas, flags: int, niter: int, optimize: bool = False, copy:
 
 
 def decode_pixels(datas, flags: int, niter: int, layout: str = "hwc", device: str = "cuda", max_device_bytes: int = 0,
-                  gpu: int = -1, scale_denom: int = 1, size=None, crop=None, filter="bicubic", orientation=None):
+                  gpu: int = -1, scale_denom: int = 1, size=None, crop=None, filter="bicubic", orientation=None,
+                  mode=None):
     """QsContext.decode_pixels on the default context of CUDA device `gpu`: one record (pixels, warnings,
     host_decoded, smoothed, stop, upsampled, reason) per file, at 1/scale_denom size, cropped and resized
     as Pillow would with size / crop / filter ((width, height) and (left, top, right, bottom), Pillow's
-    conventions), turned by `orientation` ("exif", 1..8, or one value 0..8 per file) first."""
+    conventions), turned by `orientation` ("exif", 1..8, or one value 0..8 per file) first and converted by
+    `mode` (None, "RGB" or "L", Pillow's Image.convert) before the crop."""
     return default_context(gpu).decode_pixels(datas, flags, niter, layout, device, max_device_bytes, scale_denom,
-                                              size, crop, filter, orientation)
+                                              size, crop, filter, orientation, mode)
 
 
 def compress_async(pixels, quality=75, subsampling="4:2:0", optimize=False, out=None, stream=None):
@@ -2030,9 +2097,9 @@ def compress_async(pixels, quality=75, subsampling="4:2:0", optimize=False, out=
 
 
 def reencode(datas, flags: int, niter: int, quality=75, subsampling="4:2:0", optimize=False, scale_denom=1, size=None,
-             crop=None, filter="bicubic", max_device_bytes: int = 0, gpu: int = -1, orientation=None):
+             crop=None, filter="bicubic", max_device_bytes: int = 0, gpu: int = -1, orientation=None, mode=None):
     """QsContext.reencode on the default context of CUDA device `gpu`: one record (data, warnings,
     host_decoded, smoothed, stop, upsampled, reason) per file, data the JPEG file Pillow's save writes for
     the picture decode_pixels gives with the same arguments."""
     return default_context(gpu).reencode(datas, flags, niter, quality, subsampling, optimize, scale_denom, size, crop,
-                                         filter, max_device_bytes, orientation)
+                                         filter, max_device_bytes, orientation, mode)

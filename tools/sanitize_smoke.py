@@ -152,3 +152,13 @@ for d in (1, 2):
     px = ctx.decode_pixels(ofiles, 3, 1, scale_denom=d, orientation=[0, 1, 2, 3, 4] * 2 + [5, 6, 7, 8, 0])
     torch.cuda.synchronize()
     print("decode_pixels oriented d", d, [tuple(p[0].shape) for p in px], flush=True)
+
+# colour modes: a CMYK and a YCCK file (Adobe transform 0 spliced to 1) beside grey and YCbCr ones, in both
+# modes, with every orientation (the 4-component staging of 5..8 included), at d = 1 and 2
+cm = jpeg(75, 41, "CMYK", quality=80)
+yk = cm[:2] + cm[2:].replace(b"Adobe\x00\x64\x00\x00\x00\x00\x00", b"Adobe\x00\x64\x00\x00\x00\x00\x01", 1)
+mfiles = [cm, yk, jpeg(40, 24, "L"), jpeg(70, 30, "RGB")] * 2
+for d in (1, 2):
+    for mode in ("RGB", "L"):
+        px = ctx.decode_pixels(mfiles, 3, 1, scale_denom=d, mode=mode, orientation=[1, 2, 3, 4, 5, 6, 7, 8])
+        print("decode_pixels mode", mode, "d", d, [tuple(p[0].shape) for p in px], flush=True)
