@@ -831,11 +831,22 @@ int jpegqs_cuda_pixels_batch_mode(jpegqs_cuda_ctx *ctx, int n, const uint8_t *co
  *   - jpegqs_cuda_encode_async then writes the coefficients, so the files are its output for them.
  *   - Grey pictures: the samples do not depend on subsampling, but Pillow sets the luma sampling factors
  *     whatever the component count, so the SOF of a grey file saved with 4:2:2 / 4:2:0 says 2x1 / 2x2
- *     (its single-component scan is coded block by block all the same); so does this one. */
+ *     (its single-component scan is coded block by block all the same); so does this one.
+ *   - Progressive files: optimize | JPEGQS_JPEG_PROGRESSIVE gives Pillow's save(..., progressive=True),
+ *     libjpeg's jpeg_simple_progression with optimal tables, which progressive mode forces: bit 0 then
+ *     changes no byte.  SOF2, then per scan the DHT of every table the scan uses (one marker each,
+ *     tables built from that scan's symbol counts; none for the DC refinement), SOS and the scan's data,
+ *     padded with 1-bits and byte-stuffed on its own.  The scans (Ss-Se, Ah, Al):
+ *       YCbCr  DC of all three 0-0 0 1; Y 1-5 0 2; Cr 1-63 0 1; Cb 1-63 0 1; Y 6-63 0 2; Y 1-63 2 1;
+ *              DC 0-0 1 0; Cr 1-63 1 0; Cb 1-63 1 0; Y 1-63 1 0.
+ *       grey   DC 0-0 0 1; 1-5 0 2; 6-63 0 2; 1-63 2 1; DC 0-0 1 0; 1-63 1 0.
+ *     Any other optimize value (2, 4, 0x200, ...) is JPEGQS_ERR_ARG.  Callers that never set the bit
+ *     get the sequential files and sizes described here. */
+#define JPEGQS_JPEG_PROGRESSIVE 0x100
 typedef struct {
 	int32_t quality;       /* 1..100                                                               */
 	int32_t subsampling;   /* 0 = 4:4:4, 1 = 4:2:2, 2 = 4:2:0 (Pillow's numbers); ignored for grey   */
-	int32_t optimize;      /* 0 / 1: optimal Huffman tables                                        */
+	int32_t optimize;      /* 0 / 1: optimal Huffman tables; | JPEGQS_JPEG_PROGRESSIVE: progressive   */
 } jpegqs_cuda_jpeg_params;
 typedef struct {
 	const uint8_t *pixels_dev; /* DEVICE memory (host memory for compress_model), HWC, any alignment  */
@@ -862,6 +873,15 @@ typedef struct {
  *     coefficients) plus encode_workspace_bytes' term for the picture's geometry:
  *       32768 + A(2 * U) + A(8 * T) + A(4 * Wd) + A(4 * ceil(4 * Wd / 4096)),
  *     T = ceil(U / 256), Wd = ceil(U * 1665 / 32) + 2.  The workspace is 256-byte aligned.
+ *   - Progressive bound and workspace (JPEGQS_JPEG_PROGRESSIVE set): 20 + 6000 + 2 * (ceil(U * 3928 / 8)
+ *     + 10), with 3928 a block's bits over all scans at most (DESIGN.md 3.14); U below 2^27 for 65535 x
+ *     65535, so no term overflows 64 bits.  The encoder's term becomes
+ *       73728 + A(V) + A(2 * V) + A(8 * V) + A(2 * V) + A(8 * V / 256) + A(4 * Wd) + A(4 * ceil(4 * Wd / 4096)),
+ *     Wd = ceil(U * 3928 / 32) + 10242, V = the sum over the scans of their units rounded up to a
+ *     multiple of 256: R(U) twice (the DC scans), R(Y) four times and R(C) twice for each chroma
+ *     component, Y and C = wblk * hblk of the component (grey: R(U) six times).
+ *   - Launches: the compressor, then 13 per group of up to 16 pictures in progressive mode (9 / 10 in
+ *     sequential mode), then the grey SOF fix where it applies.
  *   - Argument errors change nothing: every check runs before the first enqueue and a failed one
  *     returns JPEGQS_ERR_ARG with nothing enqueued.  Checked: NULL pointers (pics, params, out_dev and
  *     its entries, out_cap, len_dev, status_dev, workspace, pixels_dev), quality outside 1..100,

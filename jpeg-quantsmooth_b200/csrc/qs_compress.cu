@@ -190,7 +190,7 @@ static const char *qc_check_params(const jpegqs_cuda_jpeg_params *jp) {
 	if (!jp) return "params NULL";
 	if (jp->quality < 1 || jp->quality > 100) return "quality outside 1..100";
 	if (jp->subsampling < 0 || jp->subsampling > 2) return "subsampling outside 0..2";
-	if (jp->optimize != 0 && jp->optimize != 1) return "optimize other than 0 / 1";
+	if ((jp->optimize & ~(JPEGQS_JPEG_PROGRESSIVE | 1)) != 0) return "optimize other than 0 / 1, ORed with JPEGQS_JPEG_PROGRESSIVE";
 	return NULL;
 }
 
@@ -245,6 +245,17 @@ static jpegqs_cuda_jpeg_head qc_head(const uint8_t *prefix, int nc) {
 	return h;
 }
 
+/* the progressive coder of qs_encode.cu */
+size_t qe_progressive_bound(const jpegqs_cuda_image *img, size_t prefix_len);
+size_t qe_progressive_workspace(const jpegqs_cuda_image *img);
+int qe_progressive_async(jpegqs_cuda_ctx *ctx, int n, const jpegqs_cuda_image *imgs, const jpegqs_cuda_jpeg_head *heads,
+		uint8_t *const *out_dev, const size_t *out_cap, uint64_t *len_dev, int32_t *status_dev, void *workspace,
+		size_t workspace_bytes, cudaStream_t st);
+int qe_progressive_model(const jpegqs_cuda_image *img, const jpegqs_cuda_jpeg_head *head, uint8_t *out, size_t cap,
+		uint64_t *len, int32_t *status);
+
+static bool qc_progressive(const jpegqs_cuda_jpeg_params &jp) { return (jp.optimize & JPEGQS_JPEG_PROGRESSIVE) != 0; }
+
 static size_t qc_coef_bytes(const jpegqs_cuda_image &im) {
 	size_t b = 0;
 	for (int c = 0; c < im.ncomp; c++) b += qc_a256((size_t)im.comp[c].wblk * im.comp[c].hblk * 128);
@@ -257,13 +268,16 @@ extern "C" int jpegqs_cuda_compress_bound(const jpegqs_cuda_pixels_in *pic, cons
 	jpegqs_cuda_image im; QcJob jobs[3];
 	if (!e) e = qc_geometry(*pic, *params, &im, jobs);
 	if (e) { snprintf(m, sizeof(m), "jpegqs_cuda_compress_bound: %s", e); qs_set_host_error(m); return JPEGQS_ERR_ARG; }
+	if (qc_progressive(*params)) { *bytes = qe_progressive_bound(&im, QC_PREFIX_LEN); return 0; }
 	return jpegqs_cuda_encode_bound(&im, QC_PREFIX_LEN, bytes);
 }
 
 /* one picture's share of the workspace: its coefficients and its encoder workspace */
 static int qc_share(const jpegqs_cuda_image &im, int optimize, size_t *bytes) {
 	size_t w = 0;
-	int r = jpegqs_cuda_encode_workspace_bytes(1, &im, optimize, &w);
+	int r = 0;
+	if (optimize & JPEGQS_JPEG_PROGRESSIVE) w = qe_progressive_workspace(&im);
+	else r = jpegqs_cuda_encode_workspace_bytes(1, &im, optimize, &w);
 	*bytes = qc_coef_bytes(im) + w;
 	return r;
 }
@@ -359,7 +373,9 @@ extern "C" int jpegqs_cuda_compress_async(jpegqs_cuda_ctx *ctx, int n, const jpe
 	}
 	std::vector<jpegqs_cuda_jpeg_head> heads((size_t)n);
 	for (int i = 0; i < n; i++) heads[i] = qc_head(prefix, imgs[i].ncomp);
-	int r = jpegqs_cuda_encode_async(ctx, n, imgs.data(), heads.data(), params->optimize, NULL, out_dev, out_cap, len_dev,
+	int r = qc_progressive(*params)
+		? qe_progressive_async(ctx, n, imgs.data(), heads.data(), out_dev, out_cap, len_dev, status_dev, w, ws_enc, st)
+		: jpegqs_cuda_encode_async(ctx, n, imgs.data(), heads.data(), params->optimize, NULL, out_dev, out_cap, len_dev,
 			status_dev, w, ws_enc, st);
 	if (r < 0) return r;
 	launches += jpegqs_cuda_last_launches(ctx);
@@ -399,7 +415,8 @@ extern "C" int jpegqs_cuda_compress_model(const jpegqs_cuda_pixels_in *pic, cons
 			for (uint32_t bx = 0; bx < j.wblk; bx++) qc_block(j, bx, by, j.coef + ((size_t)by * j.wblk + bx) * 64);
 	}
 	jpegqs_cuda_jpeg_head h = qc_head(qc_prefix, im.ncomp);
-	int r = jpegqs_cuda_encode_model(&im, &h, params->optimize, out, cap, len, status);
+	int r = qc_progressive(*params) ? qe_progressive_model(&im, &h, out, cap, len, status)
+		: jpegqs_cuda_encode_model(&im, &h, params->optimize, out, cap, len, status);
 	if (!r && im.ncomp == 1 && params->subsampling && cap > QC_GREY_SOF_SAMP) out[QC_GREY_SOF_SAMP] = qc_grey_samp(*params);
 	return r;
 }

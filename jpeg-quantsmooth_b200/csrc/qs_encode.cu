@@ -376,11 +376,9 @@ struct QeOut {
 	HD void w(unsigned v) { b(v >> 8); b(v & 255); }
 };
 
-/* DQT for every table in use, SOF0 / SOF1, DHT, SOS - jq_write's order - written from prefix_len on
- * (nothing at or past cap).  Returns the header length, prefix included. */
-HD static inline uint64_t qe_header(const QeImg &im, const QeGeo &g, const QeTab *tab, uint8_t *out, uint64_t cap) {
-	QeOut o = { out, cap, im.prefix_len };
-	int nc = im.ncomp, nt = nc > 1 ? 2 : 1, sof = 0xC0;
+/* DQT for every table in use, then SOF0 / SOF1 (SOF2 when progressive) */
+HD static inline void qe_frame(const QeImg &im, const QeGeo &g, QeOut &o, bool progressive) {
+	int nc = im.ncomp, sof = 0xC0;
 	unsigned written = 0;
 	for (int k = 0; k < nc; k++) {
 		int tq = im.qtbl[k] & 3, prec = 0;
@@ -391,9 +389,17 @@ HD static inline uint64_t qe_header(const QeImg &im, const QeGeo &g, const QeTab
 		o.w(0xFFDB); o.w(2 + 1 + (prec ? 128 : 64)); o.b((unsigned)(prec << 4 | tq));
 		for (int i = 0; i < 64; i++) { unsigned v = im.quant[k][qe_nat(i)]; if (prec) o.w(v); else o.b(v); }
 	}
-	o.w(0xFF00 | sof); o.w(8 + 3 * nc); o.b(8);
+	o.w(0xFF00 | (progressive ? 0xC2 : sof)); o.w(8 + 3 * nc); o.b(8);
 	o.w(im.height); o.w(im.width); o.b((unsigned)nc);
 	for (int k = 0; k < nc; k++) { o.b((unsigned)im.comp_id[k]); o.b((unsigned)g.sof_hv[k]); o.b((unsigned)im.qtbl[k]); }
+}
+
+/* DQT for every table in use, SOF0 / SOF1, DHT, SOS - jq_write's order - written from prefix_len on
+ * (nothing at or past cap).  Returns the header length, prefix included. */
+HD static inline uint64_t qe_header(const QeImg &im, const QeGeo &g, const QeTab *tab, uint8_t *out, uint64_t cap) {
+	QeOut o = { out, cap, im.prefix_len };
+	int nc = im.ncomp, nt = nc > 1 ? 2 : 1;
+	qe_frame(im, g, o, false);
 	for (int i = 0; i < nt; i++) for (int a = 0; a < 2; a++) {
 		const QeTab &t = tab[2 * i + a];
 		o.w(0xFFC4); o.w(2 + 1 + 16 + t.nval); o.b((unsigned)(a << 4 | i));
@@ -905,6 +911,756 @@ extern "C" int jpegqs_cuda_encode_model(const jpegqs_cuda_image *img, const jpeg
 	}
 	uint64_t L = pos + 2;
 	int32_t flags = (int32_t)st.flags;
+	if (L > cap) flags |= JPEGQS_ENCODE_OVERFLOW;
+	else { out[pos] = 0xFF; out[pos + 1] = 0xD9; }
+	*len = L; *status = flags;
+	return 0;
+}
+
+/* ================================================================ progressive mode (DESIGN.md section 3.14)
+ * The file libjpeg writes for the same coefficients after jpeg_simple_progression with optimal tables
+ * (progressive mode forces them): SOF2, then per scan [DHT ...] SOS data, each scan's data byte-aligned
+ * with 1-bits and stuffed on its own.  Only compress_async reaches it.
+ *
+ *   unit      (scan, block) in scan order: interleaved MCU order for the DC scans, raster order over the
+ *             component's real blocks for the AC scans.  Each scan's units start at a multiple of QE_T,
+ *             so a tile of units belongs to one scan.
+ *   padding   jccoefct.c compress_first_pass gives an MCU padding block the DC of its source (right
+ *             edge: the last real block of its row; bottom rows: block h_samp - 1 of their MCU in the row
+ *             above).  For the factors compress_async writes that is the last real block of its
+ *             component before it in MCU order, qe_locate's predictor: a DC first difference of 0 and,
+ *             in the DC refinement, bit Al of the source's DC.
+ *   runs      an AC unit's symbols are local; the EOBn symbol of a run of blocks is given to the run's
+ *             first block (after its own symbols) and every block of the run emits its own trailing
+ *             correction bits after it - jcphuff.c's order.  Blocks that emit a symbol split a scan into
+ *             segments; inside one, runs end at 0x7FFF blocks or when the correction bits exceed 937
+ *             (MAX_CORR_BITS - DCTSIZE2 + 1).  qp_class scans (segment breaks, correction bits) per unit,
+ *             qp_tscan per scan, and qp_runs walks each segment from its first block run by run,
+ *             finding each run's end by a galloping search over those prefix sums.
+ *   tables    qp_count gathers per-scan histograms, qp_table builds one optimal table per (scan, table
+ *             used) with qe_optimal; then qp_len / qp_tscan / qp_emit / qp_ffcount / qp_fscan / qp_copy
+ *             as the sequential passes, each scan's raw bytes starting on a chunk of their own.  qp_fscan
+ *             places every scan and writes its DHT / SOS between the stuffed segments.
+ */
+#define QP_MAX_SCANS 10
+#define QP_FIXED 73728                 /* descriptor + state + two tables per scan               */
+#define QP_BLOCK_BITS 3928ull          /* a block's bits over all ten scans at most (DESIGN 3.14)  */
+#define QP_HEAD_MAX 6000ull            /* DQT, SOF2, per scan DHT x 2 and SOS, EOI at most        */
+#define QP_RUN_MAX 0x7FFFu             /* EOBRUN at which libjpeg flushes                         */
+#define QP_BE_MAX 937u                 /* correction bits beyond which libjpeg flushes            */
+
+struct QpScan {
+	uint8_t ncomp, comp, ss, se, ah, al, pad[2];   /* comp: the AC scan's component                 */
+	uint64_t n, ubase;                             /* units; the first (a multiple of QE_T)         */
+};
+struct QpScanState {
+	uint64_t total;                    /* tile-scan total: (breaks << 32 | correction bits), then bits */
+	uint64_t nraw, chunk0, data;       /* entropy-coded bytes; first chunk; file offset of the data   */
+	uint32_t head, pad;                /* bytes of the scan's DHT / SOS                               */
+};
+struct QpState {
+	uint64_t head_len, nchunk, len;    /* prefix + DQT + SOF2; chunks; file length                    */
+	QpScanState sc[QP_MAX_SCANS];
+};
+struct QpImg {
+	QeImg e;                           /* geometry 0, header fields, output, tab [2 per scan], ulen, tile, word, ffc */
+	QpScan scan[QP_MAX_SCANS];
+	int32_t nscan, pad;
+	QpState *ps;
+	uint8_t *cls;                      /* per unit: 1 ends in a run, 2 emits a symbol, correction bits << 2 */
+	uint16_t *run;                     /* per unit: the run it starts, 0 for none                     */
+	uint64_t *pre;                     /* per unit: (breaks << 32 | correction bits) before it in its tile */
+};
+static_assert(sizeof(QpImg) <= 2048 && sizeof(QpState) <= 2048 && 4096 + 2 * QP_MAX_SCANS * sizeof(QeTab) <= QP_FIXED, "qp fixed part");
+
+/* jpeg_simple_progression's scripts for YCbCr and for one component */
+static void qp_script(QpImg *p) {
+	static const uint8_t col[QP_MAX_SCANS][5] = {      /* component (3: all), Ss, Se, Ah, Al */
+		{ 3, 0, 0, 0, 1 }, { 0, 1, 5, 0, 2 }, { 2, 1, 63, 0, 1 }, { 1, 1, 63, 0, 1 }, { 0, 6, 63, 0, 2 },
+		{ 0, 1, 63, 2, 1 }, { 3, 0, 0, 1, 0 }, { 2, 1, 63, 1, 0 }, { 1, 1, 63, 1, 0 }, { 0, 1, 63, 1, 0 } };
+	static const uint8_t grey[6][5] = {
+		{ 3, 0, 0, 0, 1 }, { 0, 1, 5, 0, 2 }, { 0, 6, 63, 0, 2 }, { 0, 1, 63, 2, 1 }, { 3, 0, 0, 1, 0 }, { 0, 1, 63, 1, 0 } };
+	const QeGeo &g = p->e.geo[0];
+	const bool colour = p->e.ncomp > 1;
+	p->nscan = colour ? 10 : 6;
+	uint64_t base = 0;
+	for (int s = 0; s < p->nscan; s++) {
+		const uint8_t *r = colour ? col[s] : grey[s];
+		QpScan &sc = p->scan[s];
+		memset(&sc, 0, sizeof(sc));
+		sc.ncomp = r[0] == 3 ? (uint8_t)p->e.ncomp : 1; sc.comp = r[0] == 3 ? 0 : r[0];
+		sc.ss = r[1]; sc.se = r[2]; sc.ah = r[3]; sc.al = r[4];
+		sc.n = sc.ss == 0 ? g.nunits : (uint64_t)g.wblk[sc.comp] * g.hblk[sc.comp];
+		sc.ubase = base;
+		base += (sc.n + QE_T - 1) / QE_T * QE_T;
+	}
+}
+
+/* table slots a scan uses: DC first 1 per DC table, DC refinement none, AC 1 */
+HD static inline int qp_slots(const QpImg &p, const QpScan &sc) {
+	return sc.ss ? 1 : sc.ah ? 0 : p.e.ncomp > 1 ? 2 : 1;
+}
+
+HD static inline int qp_scan_of(const QpImg &p, uint64_t u) {
+	int s = 0;
+	while (s + 1 < p.nscan && u >= p.scan[s + 1].ubase) s++;
+	return s;
+}
+
+struct QpNull { HD void sym(int, int, uint32_t, int) {} HD void bits(uint32_t, int) {} };
+
+/* n <= 63 buffered correction bits, the first the highest */
+template <class S> HD static inline void qp_corr(S &sink, uint64_t b, int n) {
+	if (n > 32) { sink.bits((uint32_t)(b >> 32), n - 32); n = 32; }
+	if (n) sink.bits((uint32_t)b & (0xFFFFFFFFu >> (32 - n)), n);
+}
+
+/* emit_eobrun's symbol for a run of `run` blocks: EOBn, n = floor(log2 run), and the low n bits */
+template <class S> HD static inline void qp_eobrun(S &sink, uint32_t run) {
+	const int nb = qe_size((int)run) - 1;
+	sink.sym(0, nb << 4, run & ((1u << nb) - 1), nb);
+}
+
+/* Unit i of scan sc, to sink.sym(slot, symbol, value bits, size) / sink.bits(bits, count), with `run`
+ * the EOB run the unit starts (0 for none).  Returns its class: 1 it ends in an EOB run (jcphuff.c's
+ * EOBRUN++), 2 it emits a symbol (so the pending run is flushed before it), and its trailing correction
+ * bits << 2. */
+template <class S> HD static inline uint32_t qp_unit(const QpImg &p, const QpScan &sc, uint64_t i, uint32_t run, S &sink) {
+	const QeGeo &g = p.e.geo[0];
+	const int al = sc.al;
+	if (sc.ss == 0) {                                /* encode_mcu_DC_first / _refine */
+		QeUnit un = qe_locate(g, i);
+		const int dc = un.blk ? un.blk[0] : un.pred;
+		if (sc.ah == 0) {
+			const int diff = (dc >> al) - (un.pred >> al), s = qe_size(diff);
+			sink.sym(un.tsel, s, (uint32_t)(diff + (diff >> 31)) & ((1u << s) - 1), s);
+		} else sink.bits((uint32_t)(dc >> al) & 1u, 1);
+		return 0;
+	}
+	const int16_t *blk = g.coef[sc.comp] + i * 64;
+	uint64_t m = qe_zmask(blk) & ((~0ull << sc.ss) & (~0ull >> (63 - sc.se)));
+	int prev = sc.ss - 1;
+	if (sc.ah == 0) {                                /* encode_mcu_AC_first */
+		uint32_t emits = 0;
+		while (m) {
+			const int k = qe_ctz64(m);
+			m &= m - 1;
+			const int v = blk[qe_nat(k)], a = (v < 0 ? -v : v) >> al;
+			if (!a) continue;
+			int r = k - prev - 1;
+			prev = k; emits = 2;
+			for (; r > 15; r -= 16) sink.sym(0, 0xF0, 0, 0);
+			const int nb = qe_size(a);
+			sink.sym(0, r << 4 | nb, (uint32_t)(v < 0 ? ~a : a) & ((1u << nb) - 1), nb);
+		}
+		if (run) qp_eobrun(sink, run);
+		return (prev != sc.se ? 1u : 0u) | emits;
+	}
+	int eob = -1;                                    /* encode_mcu_AC_refine: the last newly-nonzero */
+	for (uint64_t mm = m; mm; mm &= mm - 1) {
+		const int k = qe_ctz64(mm), v = blk[qe_nat(k)];
+		if (((v < 0 ? -v : v) >> al) == 1) eob = k;
+	}
+	int r = 0, nbr = 0;
+	uint64_t br = 0;
+	while (m) {
+		const int k = qe_ctz64(m);
+		m &= m - 1;
+		const int v = blk[qe_nat(k)], a = (v < 0 ? -v : v) >> al;
+		if (!a) continue;
+		r += k - prev - 1;
+		prev = k;
+		while (r > 15 && k <= eob) { sink.sym(0, 0xF0, 0, 0); r -= 16; qp_corr(sink, br, nbr); br = 0; nbr = 0; }
+		if (a > 1) { br = br << 1 | (uint64_t)(a & 1); nbr++; continue; }
+		sink.sym(0, r << 4 | 1, v < 0 ? 0u : 1u, 1);
+		qp_corr(sink, br, nbr); br = 0; nbr = 0; r = 0;
+	}
+	r += sc.se - prev;
+	if (run) qp_eobrun(sink, run);
+	qp_corr(sink, br, nbr);
+	return (r > 0 || nbr > 0 ? 1u : 0u) | (eob >= 0 ? 2u : 0u) | (uint32_t)nbr << 2;
+}
+
+/* a unit that breaks its scan's runs: not in a run, the scan's first, one that emits a symbol, or one
+ * after a unit not in a run.  Such a unit in a run starts a segment. */
+HD static inline bool qp_break(uint32_t c, uint32_t cprev, uint64_t i) {
+	return !(c & 1) || i == 0 || (c & 2) || !(cprev & 1);
+}
+
+/* (breaks << 32 | correction bits) of units [0, m) of scan s */
+HD static inline uint64_t qp_pre(const QpImg &p, int s, uint64_t m) {
+	const QpScan &sc = p.scan[s];
+	if (m >= sc.n) return p.ps->sc[s].total;
+	const uint64_t u = sc.ubase + m;
+	return p.pre[u] + p.e.tile[u / QE_T];
+}
+
+/* the smallest m in [lo, hi] with field(P(m)) - base > lim (monotone in m), hi + 1 if none: a gallop
+ * from lo, then bisection */
+HD static inline uint64_t qp_first(const QpImg &p, int s, bool high, uint64_t base, uint64_t lim, uint64_t lo, uint64_t hi) {
+	uint64_t a = lo, b = lo, step = 1;
+	for (;;) {
+		if (b > hi) return hi + 1;
+		const uint64_t v = qp_pre(p, s, b), x = high ? v >> 32 : v & 0xFFFFFFFFull;
+		if (x - base > lim) break;
+		a = b + 1;
+		if (b == hi) return hi + 1;
+		b = b + step > hi ? hi : b + step;
+		step <<= 1;
+	}
+	while (a < b) {
+		const uint64_t mid = a + (b - a) / 2, v = qp_pre(p, s, mid), x = high ? v >> 32 : v & 0xFFFFFFFFull;
+		if (x - base > lim) b = mid; else a = mid + 1;
+	}
+	return a;
+}
+
+/* the runs of the segment starting at unit j of scan s: each starts with EOBRUN 0 and BE 0 and ends
+ * after QP_RUN_MAX blocks, after the block that takes BE past QP_BE_MAX, or at the segment's end */
+HD static inline void qp_walk(const QpImg &p, int s, uint64_t j) {
+	const QpScan &sc = p.scan[s];
+	const uint64_t pj = qp_pre(p, s, j);
+	const uint64_t end = qp_first(p, s, true, pj >> 32, 1, j + 2, sc.n) - 1;   /* the next break, or n */
+	for (uint64_t r = j; r < end;) {
+		const uint64_t pr = r == j ? pj : qp_pre(p, s, r);
+		const uint64_t lim = r + QP_RUN_MAX < end ? r + QP_RUN_MAX : end;
+		uint64_t e = qp_first(p, s, false, pr & 0xFFFFFFFFull, QP_BE_MAX, r + 1, lim);
+		if (e > lim) e = lim;
+		p.run[sc.ubase + r] = (uint16_t)(e - r);
+		r = e;
+	}
+}
+
+/* the scan's DHT for every table it uses, then its SOS (jcmarker.c write_scan_header) */
+HD static inline void qp_scan_head(const QpImg &p, int s, const QeTab *tab, QeOut &o) {
+	const QpScan &sc = p.scan[s];
+	for (int t = 0; t < qp_slots(p, sc); t++) {
+		const QeTab &h = tab[2 * s + t];
+		const int id = sc.ss ? (sc.comp ? 1 : 0) : t;
+		o.w(0xFFC4); o.w(2 + 1 + 16 + h.nval); o.b((unsigned)((sc.ss ? 0x10 : 0) | id));
+		for (int l = 1; l <= 16; l++) o.b(h.bits[l]);
+		for (int l = 0; l < h.nval; l++) o.b(h.val[l]);
+	}
+	o.w(0xFFDA); o.w(6 + 2 * sc.ncomp); o.b(sc.ncomp);
+	for (int k = 0; k < sc.ncomp; k++) {
+		const int c = sc.ncomp > 1 ? k : sc.comp;
+		const unsigned td = sc.ss == 0 && sc.ah == 0 && c ? 1 : 0, ta = sc.se && c ? 1 : 0;
+		o.b((unsigned)p.e.comp_id[c]); o.b(td << 4 | ta);
+	}
+	o.b(sc.ss); o.b(sc.se); o.b((unsigned)(sc.ah << 4 | sc.al));
+}
+
+struct QpLenSink {
+	const uint32_t *cs[2]; uint32_t n;
+	HD void sym(int t, int s, uint32_t, int nv) { n += (cs[t][s] & 255) + (uint32_t)nv; }
+	HD void bits(uint32_t, int nv) { n += (uint32_t)nv; }
+};
+struct QpEmitSink {
+	const uint32_t *cs[2]; QeEmitSink e;
+	HD void sym(int t, int s, uint32_t vb, int nv) { const uint32_t c = cs[t][s]; e.put((c >> 8) << nv | vb, (int)(c & 255) + nv); }
+	HD void bits(uint32_t v, int nv) { e.put(v, nv); }
+};
+
+/* unit i of scan s written from bit offset o on; the scan's last unit pads its byte with 1-bits */
+HD static inline void qp_emit_unit(const QpImg &p, int s, uint64_t i, uint32_t run, uint64_t o, const uint32_t *cs0,
+		const uint32_t *cs1, uint64_t total) {
+	QpEmitSink k;
+	k.cs[0] = cs0; k.cs[1] = cs1;
+	k.e.w = p.e.word; k.e.base = o & ~31ull; k.e.acc = 0; k.e.nacc = (int)(o & 31); k.e.shared = (o & 31) != 0;
+	qp_unit(p, p.scan[s], i, run, k);
+	if (i + 1 == p.scan[s].n) {
+		const int pad = (int)((8 - (total & 7)) & 7);
+		if (pad) k.e.put((1u << pad) - 1, pad);
+	}
+	k.e.finish();
+}
+
+/* the scan a chunk of raw bytes belongs to, -1 for none */
+HD static inline int qp_chunk_scan(const QpImg &p, uint64_t c) {
+	for (int s = 0; s < p.nscan; s++) {
+		const QpScanState &t = p.ps->sc[s];
+		if (c >= t.chunk0 && c < t.chunk0 + (t.nraw + QE_CHUNK - 1) / QE_CHUNK) return s;
+	}
+	return -1;
+}
+
+/* ---------------------------------------------------------------- progressive kernels */
+struct QpSetupPack { QpImg img[QE_PACK]; int n; };
+static_assert(sizeof(QpSetupPack) <= 32000, "QpSetupPack exceeds the kernel parameter space");
+struct QpPtrs { const QpImg *img[QE_PACK]; int n; };
+
+__global__ void __launch_bounds__(256) qp_setup_kernel(const __grid_constant__ QpSetupPack P) {
+	const int i = blockIdx.x;
+	if (i >= P.n) return;
+	const QpImg &p = P.img[i];
+	if (threadIdx.x == 0) {
+		*reinterpret_cast<QpImg *>(reinterpret_cast<char *>(p.ps) - 2048) = p;
+		memset(p.ps, 0, sizeof(QpState));
+	}
+	for (int j = threadIdx.x; j < 2 * p.nscan * 257; j += blockDim.x) p.e.tab[j / 257].freq[j % 257] = 0;
+}
+
+/* per tile: every unit's class and run slot; the in-tile exclusive scan of (break << 32 | correction
+ * bits); the tile's sum */
+__global__ void __launch_bounds__(QE_T) qp_class_kernel(const __grid_constant__ QpPtrs P) {
+	if ((int)blockIdx.y >= P.n) return;
+	const QpImg &p = *P.img[blockIdx.y];
+	const uint64_t u0 = (uint64_t)blockIdx.x * QE_T;
+	if (u0 >= p.scan[p.nscan - 1].ubase + p.scan[p.nscan - 1].n) return;
+	const int s = qp_scan_of(p, u0);
+	const QpScan &sc = p.scan[s];
+	const uint64_t u = u0 + threadIdx.x, i = u - sc.ubase;
+	__shared__ uint8_t s_cls[QE_T];
+	QpNull z;
+	uint32_t c = 0;
+	if (i < sc.n) {
+		if (sc.ss) c = qp_unit(p, sc, i, 0, z);
+		p.cls[u] = (uint8_t)c; p.run[u] = 0;
+	}
+	s_cls[threadIdx.x] = (uint8_t)c;
+	__syncthreads();
+	uint64_t v = 0;
+	if (i < sc.n && sc.ss) {
+		uint32_t cp = 0;
+		if (i > 0) cp = threadIdx.x ? s_cls[threadIdx.x - 1] : qp_unit(p, sc, i - 1, 0, z);
+		v = (qp_break(c, cp, i) ? 1ull << 32 : 0) | (c >> 2);
+	}
+	typedef cub::BlockScan<uint64_t, QE_T> S;
+	__shared__ typename S::TempStorage tmp;
+	uint64_t ex, agg;
+	S(tmp).ExclusiveSum(v, ex, agg);
+	if (i < sc.n) p.pre[u] = ex;
+	if (threadIdx.x == 0) p.e.tile[blockIdx.x] = agg;
+}
+
+/* per image: the tile sums scanned per scan (exclusive, restarting at every scan) and each scan's total;
+ * with `bits`, also each scan's raw bytes and first chunk */
+__global__ void __launch_bounds__(QE_SCAN_T) qp_tscan_kernel(const __grid_constant__ QpPtrs P, int bits) {
+	if ((int)blockIdx.x >= P.n) return;
+	const QpImg &p = *P.img[blockIdx.x];
+	typedef cub::BlockScan<uint64_t, QE_SCAN_T> S;
+	__shared__ typename S::TempStorage tmp;
+	for (int s = 0; s < p.nscan; s++) {
+		const QpScan &sc = p.scan[s];
+		const uint64_t t0 = sc.ubase / QE_T, nt = (sc.n + QE_T - 1) / QE_T;
+		uint64_t carry = 0;
+		for (uint64_t base = 0; base < nt; base += QE_SCAN_T) {
+			const uint64_t t = base + threadIdx.x;
+			uint64_t v = t < nt ? p.e.tile[t0 + t] : 0, ex, agg;
+			S(tmp).ExclusiveSum(v, ex, agg);
+			if (t < nt) p.e.tile[t0 + t] = carry + ex;
+			carry += agg;
+			__syncthreads();
+		}
+		if (threadIdx.x == 0) p.ps->sc[s].total = carry;
+	}
+	if (bits && threadIdx.x == 0) {
+		uint64_t c = 0;
+		for (int s = 0; s < p.nscan; s++) {
+			QpScanState &t = p.ps->sc[s];
+			t.nraw = (t.total + 7) >> 3; t.chunk0 = c;
+			c += (t.nraw + QE_CHUNK - 1) / QE_CHUNK;
+		}
+		p.ps->nchunk = c;
+	}
+}
+
+/* per unit: the segments of the AC scans walked from their first units */
+__global__ void __launch_bounds__(QE_T) qp_runs_kernel(const __grid_constant__ QpPtrs P) {
+	if ((int)blockIdx.y >= P.n) return;
+	const QpImg &p = *P.img[blockIdx.y];
+	const uint64_t u0 = (uint64_t)blockIdx.x * QE_T;
+	if (u0 >= p.scan[p.nscan - 1].ubase + p.scan[p.nscan - 1].n) return;
+	const int s = qp_scan_of(p, u0);
+	const QpScan &sc = p.scan[s];
+	const uint64_t u = u0 + threadIdx.x, i = u - sc.ubase;
+	if (!sc.ss || i >= sc.n) return;
+	const uint32_t c = p.cls[u];
+	if ((c & 1) && qp_break(c, i ? p.cls[u - 1] : 0, i)) qp_walk(p, s, i);
+}
+
+struct QpCountSink {
+	uint32_t (*h)[257];
+	__device__ void sym(int t, int s, uint32_t, int) { atomicAdd(&h[t][s], 1u); }
+	__device__ void bits(uint32_t, int) {}
+};
+
+/* per tile: its units' symbols into shared histograms, then into the scan's tables */
+__global__ void __launch_bounds__(QE_T) qp_count_kernel(const __grid_constant__ QpPtrs P) {
+	if ((int)blockIdx.y >= P.n) return;
+	const QpImg &p = *P.img[blockIdx.y];
+	const uint64_t u0 = (uint64_t)blockIdx.x * QE_T;
+	if (u0 >= p.scan[p.nscan - 1].ubase + p.scan[p.nscan - 1].n) return;
+	const int s = qp_scan_of(p, u0);
+	const QpScan &sc = p.scan[s];
+	if (sc.ss == 0 && sc.ah) return;                 /* the DC refinement codes no symbol */
+	__shared__ uint32_t h[2][257];
+	for (int j = threadIdx.x; j < 2 * 257; j += QE_T) h[j / 257][j % 257] = 0;
+	__syncthreads();
+	const uint64_t u = u0 + threadIdx.x, i = u - sc.ubase;
+	if (i < sc.n) { QpCountSink k = { h }; qp_unit(p, sc, i, p.run[u], k); }
+	__syncthreads();
+	for (int j = threadIdx.x; j < 2 * 257; j += QE_T) {
+		const uint32_t v = h[j / 257][j % 257];
+		if (v) atomicAdd(reinterpret_cast<unsigned long long *>(&p.e.tab[2 * s + j / 257].freq[j % 257]), (unsigned long long)v);
+	}
+}
+
+/* blockIdx = (scan, image), warp w = the scan's table w: the optimal table and its codes; the scan's
+ * DHT / SOS length; scan 0 also copies the prefix and writes DQT and SOF2 */
+__global__ void __launch_bounds__(64) qp_table_kernel(const __grid_constant__ QpPtrs P) {
+	if ((int)blockIdx.y >= P.n) return;
+	const QpImg &p = *P.img[blockIdx.y];
+	const int s = blockIdx.x;
+	if (s >= p.nscan) return;
+	__shared__ uint64_t s_freq[2][257];
+	__shared__ int s_size[2][257], s_oth[2][257];
+	const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+	if (w < qp_slots(p, p.scan[s])) {
+		QeTab *t = p.e.tab + 2 * s + w;
+		qe_optimal(t, s_freq[w], s_size[w], s_oth[w], lane, 32);
+		if (lane == 0) qe_codes(t);
+	}
+	if (s == 0) for (uint64_t j = threadIdx.x; j < p.e.prefix_len && j < p.e.cap; j += blockDim.x) p.e.out[j] = p.e.prefix[j];
+	__syncthreads();
+	if (threadIdx.x == 0) {
+		QeOut o = { NULL, 0, 0 };
+		qp_scan_head(p, s, p.e.tab, o);
+		p.ps->sc[s].head = (uint32_t)o.n;
+		if (s == 0) {
+			QeOut f = { p.e.out, p.e.cap, p.e.prefix_len };
+			qe_frame(p.e, p.e.geo[0], f, true);
+			p.ps->head_len = f.n;
+		}
+	}
+}
+
+/* per tile: every unit's bit length with its scan's tables, the tile's sum */
+__global__ void __launch_bounds__(QE_T) qp_len_kernel(const __grid_constant__ QpPtrs P) {
+	if ((int)blockIdx.y >= P.n) return;
+	const QpImg &p = *P.img[blockIdx.y];
+	const uint64_t u0 = (uint64_t)blockIdx.x * QE_T;
+	if (u0 >= p.scan[p.nscan - 1].ubase + p.scan[p.nscan - 1].n) return;
+	const int s = qp_scan_of(p, u0);
+	const QpScan &sc = p.scan[s];
+	__shared__ uint32_t s_cs[2][256];
+	for (int j = threadIdx.x; j < 2 * 256; j += QE_T) s_cs[j >> 8][j & 255] = p.e.tab[2 * s + (j >> 8)].cs[j & 255];
+	__syncthreads();
+	const uint64_t u = u0 + threadIdx.x, i = u - sc.ubase;
+	uint32_t n = 0;
+	if (i < sc.n) {
+		QpLenSink k = { { s_cs[0], s_cs[1] }, 0 };
+		qp_unit(p, sc, i, p.run[u], k);
+		n = k.n;
+		p.e.ulen[u] = (uint16_t)n;
+	}
+	typedef cub::BlockReduce<uint32_t, QE_T> R;
+	__shared__ typename R::TempStorage tmp;
+	const uint32_t sum = R(tmp).Sum(n);
+	if (threadIdx.x == 0) p.e.tile[blockIdx.x] = sum;
+}
+
+/* the words every scan's bits will occupy, and one more, set to zero */
+__global__ void __launch_bounds__(256) qp_zero_kernel(const __grid_constant__ QpPtrs P) {
+	if ((int)blockIdx.y >= P.n) return;
+	const QpImg &p = *P.img[blockIdx.y];
+	const uint64_t nw = p.ps->nchunk * (QE_CHUNK / 4) + 1;
+	for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < nw; j += (uint64_t)gridDim.x * blockDim.x) p.e.word[j] = 0;
+}
+
+/* per tile: the units' bit offsets (scan's first chunk + tile offset + scan inside the tile), their bits */
+__global__ void __launch_bounds__(QE_T) qp_emit_kernel(const __grid_constant__ QpPtrs P) {
+	if ((int)blockIdx.y >= P.n) return;
+	const QpImg &p = *P.img[blockIdx.y];
+	const uint64_t u0 = (uint64_t)blockIdx.x * QE_T;
+	if (u0 >= p.scan[p.nscan - 1].ubase + p.scan[p.nscan - 1].n) return;
+	const int s = qp_scan_of(p, u0);
+	const QpScan &sc = p.scan[s];
+	__shared__ uint32_t s_cs[2][256];
+	for (int j = threadIdx.x; j < 2 * 256; j += QE_T) s_cs[j >> 8][j & 255] = p.e.tab[2 * s + (j >> 8)].cs[j & 255];
+	const uint64_t u = u0 + threadIdx.x, i = u - sc.ubase;
+	const uint32_t n = i < sc.n ? p.e.ulen[u] : 0;
+	uint32_t ex;
+	typedef cub::BlockScan<uint32_t, QE_T> S;
+	__shared__ typename S::TempStorage tmp;
+	S(tmp).ExclusiveSum(n, ex);
+	__syncthreads();
+	if (i < sc.n) {
+		const QpScanState &t = p.ps->sc[s];
+		qp_emit_unit(p, s, i, p.run[u], t.chunk0 * QE_CHUNK * 8 + p.e.tile[blockIdx.x] + ex, s_cs[0], s_cs[1], t.total);
+	}
+}
+
+/* per chunk of a scan's raw bytes: its 0xFF bytes */
+__global__ void __launch_bounds__(QE_BT) qp_ffcount_kernel(const __grid_constant__ QpPtrs P) {
+	if ((int)blockIdx.y >= P.n) return;
+	const QpImg &p = *P.img[blockIdx.y];
+	const uint64_t c = blockIdx.x;
+	if (c >= p.ps->nchunk) return;
+	const int s = qp_chunk_scan(p, c);
+	const uint64_t end = s < 0 ? 0 : p.ps->sc[s].chunk0 * QE_CHUNK + p.ps->sc[s].nraw;
+	const uint64_t j0 = c * QE_CHUNK + threadIdx.x * 16, j1 = j0 + 16 < end ? j0 + 16 : end;
+	const uint32_t n = j0 < end ? qe_ffs(p.e.word, j0, j1) : 0;
+	typedef cub::BlockReduce<uint32_t, QE_BT> R;
+	__shared__ typename R::TempStorage tmp;
+	const uint32_t sum = R(tmp).Sum(n);
+	if (threadIdx.x == 0) p.e.ffc[c] = sum;
+}
+
+/* per image: exclusive scan of the chunk counts; every scan's place in the file and its DHT / SOS; file
+ * length, status, EOI */
+__global__ void __launch_bounds__(QE_SCAN_T) qp_fscan_kernel(const __grid_constant__ QpPtrs P) {
+	if ((int)blockIdx.x >= P.n) return;
+	const QpImg &p = *P.img[blockIdx.x];
+	QpState *ps = p.ps;
+	const uint64_t nchunk = ps->nchunk;
+	uint64_t carry = 0;
+	typedef cub::BlockScan<uint64_t, QE_SCAN_T> S;
+	__shared__ typename S::TempStorage tmp;
+	for (uint64_t base = 0; base < nchunk; base += QE_SCAN_T) {
+		const uint64_t c = base + threadIdx.x;
+		uint64_t v = c < nchunk ? p.e.ffc[c] : 0, ex, agg;
+		S(tmp).ExclusiveSum(v, ex, agg);
+		if (c < nchunk) p.e.ffc[c] = (uint32_t)(carry + ex);
+		carry += agg;
+		__syncthreads();
+	}
+	if (threadIdx.x == 0) {
+		uint64_t pos = ps->head_len;
+		for (int s = 0; s < p.nscan; s++) {
+			QpScanState &t = ps->sc[s];
+			const uint64_t c1 = t.chunk0 + (t.nraw + QE_CHUNK - 1) / QE_CHUNK;
+			const uint64_t ff = (c1 < nchunk ? p.e.ffc[c1] : carry) - (t.chunk0 < nchunk ? p.e.ffc[t.chunk0] : carry);
+			t.data = pos + t.head;
+			pos = t.data + t.nraw + ff;
+		}
+		const uint64_t L = pos + 2;
+		int32_t flags = 0;
+		if (L > p.e.cap) flags |= JPEGQS_ENCODE_OVERFLOW;
+		else { p.e.out[pos] = 0xFF; p.e.out[pos + 1] = 0xD9; }
+		ps->len = L;
+		*p.e.len = L;
+		*p.e.status = flags;
+	}
+	__syncthreads();
+	const int w = threadIdx.x >> 5;
+	if (w < p.nscan && (threadIdx.x & 31) == 0) {
+		QeOut o = { p.e.out, p.e.cap, ps->sc[w].data - ps->sc[w].head };
+		qp_scan_head(p, w, p.e.tab, o);
+	}
+}
+
+/* per chunk: its bytes stuffed to the output */
+__global__ void __launch_bounds__(QE_BT) qp_copy_kernel(const __grid_constant__ QpPtrs P) {
+	if ((int)blockIdx.y >= P.n) return;
+	const QpImg &p = *P.img[blockIdx.y];
+	const uint64_t c = blockIdx.x;
+	if (c >= p.ps->nchunk) return;
+	const int s = qp_chunk_scan(p, c);
+	if (s < 0) return;
+	const QpScanState &t = p.ps->sc[s];
+	const uint64_t b0 = t.chunk0 * QE_CHUNK, end = b0 + t.nraw;
+	const uint64_t j0 = c * QE_CHUNK + threadIdx.x * 16, j1 = j0 + 16 < end ? j0 + 16 : end;
+	uint32_t n = j0 < end ? qe_ffs(p.e.word, j0, j1) : 0, ex;
+	typedef cub::BlockScan<uint32_t, QE_BT> S;
+	__shared__ typename S::TempStorage tmp;
+	S(tmp).ExclusiveSum(n, ex);
+	if (j0 < end) qe_stuff(p.e.word, j0, j1, p.e.out, p.e.cap, t.data + (j0 - b0) + (p.e.ffc[c] - p.e.ffc[t.chunk0]) + ex);
+}
+
+/* ---------------------------------------------------------------- progressive host side */
+struct QpSizes { uint64_t units, tiles, words, chunks; size_t bytes; };
+
+/* the workspace of an image: units of the ten (six) scans, each rounded up to QE_T; raw words for
+ * U * QP_BLOCK_BITS bits plus a chunk of alignment per scan */
+static QpSizes qp_sizes(const QpImg &p) {
+	QpSizes z;
+	const QpScan &last = p.scan[p.nscan - 1];
+	z.units = last.ubase + (last.n + QE_T - 1) / QE_T * QE_T;
+	z.tiles = z.units / QE_T;
+	z.words = (p.e.geo[0].nunits * QP_BLOCK_BITS + 31) / 32 + QP_MAX_SCANS * (QE_CHUNK / 4) + 2;
+	z.chunks = (4 * z.words + QE_CHUNK - 1) / QE_CHUNK;
+	z.bytes = QP_FIXED + qe_a256(z.units) + qe_a256(2 * z.units) + qe_a256(8 * z.units) + qe_a256(2 * z.units) +
+		qe_a256(8 * z.tiles) + qe_a256(4 * z.words) + qe_a256(4 * z.chunks);
+	return z;
+}
+
+static void qp_carve(QpImg *p, const QpSizes &z, char *w) {
+	p->ps = reinterpret_cast<QpState *>(w + 2048);
+	p->e.tab = reinterpret_cast<QeTab *>(w + 4096);
+	w += QP_FIXED;
+	p->cls = reinterpret_cast<uint8_t *>(w); w += qe_a256(z.units);
+	p->run = reinterpret_cast<uint16_t *>(w); w += qe_a256(2 * z.units);
+	p->pre = reinterpret_cast<uint64_t *>(w); w += qe_a256(8 * z.units);
+	p->e.ulen = reinterpret_cast<uint16_t *>(w); w += qe_a256(2 * z.units);
+	p->e.tile = reinterpret_cast<uint64_t *>(w); w += qe_a256(8 * z.tiles);
+	p->e.word = reinterpret_cast<uint32_t *>(w); w += qe_a256(4 * z.words);
+	p->e.ffc = reinterpret_cast<uint32_t *>(w);
+}
+
+/* checks image i with its head and fills its descriptor (no workspace yet) */
+static const char *qp_check(const jpegqs_cuda_image *im, const jpegqs_cuda_jpeg_head *hd, QpImg *p, QpSizes *z) {
+	memset(p, 0, sizeof(*p));
+	QeSizes unused;
+	const char *e = qe_check(im, hd, false, 1, &p->e, &unused);
+	if (e) return e;
+	if (p->e.upmode) return "progressive mode codes the sampled geometry only";
+	if (im->ncomp != 1 && im->ncomp != 3) return "progressive mode takes 1 or 3 components";
+	qp_script(p);
+	*z = qp_sizes(*p);
+	return NULL;
+}
+
+/* the progressive file's bound and workspace for an image compress_async makes */
+size_t qe_progressive_bound(const jpegqs_cuda_image *img, size_t prefix_len) {
+	QeGeo g0, g1; bool up;
+	if (qe_geometry(img, &g0, &g1, &up)) return 0;
+	return prefix_len + QP_HEAD_MAX + 2 * ((g0.nunits * QP_BLOCK_BITS + 7) / 8 + QP_MAX_SCANS);
+}
+size_t qe_progressive_workspace(const jpegqs_cuda_image *img) {
+	QpImg p;
+	memset(&p, 0, sizeof(p));
+	QeGeo g1; bool up;
+	if (qe_geometry(img, &p.e.geo[0], &g1, &up)) return 0;
+	p.e.ncomp = img->ncomp;
+	qp_script(&p);
+	return qp_sizes(p).bytes;
+}
+
+/* the progressive encoder over device coefficients, as encode_async's stream rules; launches as
+ * qs_ctx_decode_done records them */
+int qe_progressive_async(jpegqs_cuda_ctx *ctx, int n, const jpegqs_cuda_image *imgs, const jpegqs_cuda_jpeg_head *heads,
+		uint8_t *const *out_dev, const size_t *out_cap, uint64_t *len_dev, int32_t *status_dev, void *workspace,
+		size_t workspace_bytes, cudaStream_t st) {
+	char msg[512] = "";
+	int launches = 0;
+	std::vector<QpImg> desc((size_t)n);
+	std::vector<QpSizes> sizes((size_t)n);
+	size_t need = 0;
+	for (int i = 0; i < n; i++) {
+		const char *e = qp_check(&imgs[i], &heads[i], &desc[i], &sizes[i]);
+		if (e) { snprintf(msg, sizeof(msg), "progressive encoder: image %d: %s", i, e); qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG; }
+		need += sizes[i].bytes;
+	}
+	if (workspace_bytes < need || ((uintptr_t)workspace & 255)) {
+		snprintf(msg, sizeof(msg), "progressive encoder: workspace of %zu bytes, %zu needed", workspace_bytes, need);
+		qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG;
+	}
+	char *w = (char *)workspace;
+	for (int i = 0; i < n; i++) {
+		QpImg &d = desc[i];
+		qp_carve(&d, sizes[i], w); w += sizes[i].bytes;
+		d.e.index = i; d.e.out = out_dev[i]; d.e.cap = out_cap[i]; d.e.len = len_dev + i; d.e.status = status_dev + i;
+	}
+	for (int g0 = 0; g0 < n; g0 += QE_PACK) {
+		const int g = n - g0 < QE_PACK ? n - g0 : QE_PACK;
+		std::unique_ptr<QpSetupPack> hold(new QpSetupPack());
+		QpSetupPack &pack = *hold;
+		QpPtrs P;
+		memset(&pack, 0, sizeof(pack)); memset(&P, 0, sizeof(P));
+		pack.n = g; P.n = g;
+		uint64_t maxtile = 1, maxchunk = 1;
+		for (int j = 0; j < g; j++) {
+			pack.img[j] = desc[g0 + j];
+			P.img[j] = reinterpret_cast<const QpImg *>(reinterpret_cast<const char *>(desc[g0 + j].ps) - 2048);
+			if (sizes[g0 + j].tiles > maxtile) maxtile = sizes[g0 + j].tiles;
+			if (sizes[g0 + j].chunks > maxchunk) maxchunk = sizes[g0 + j].chunks;
+		}
+		if (maxtile > 0x7FFFFFFFull || maxchunk > 0x7FFFFFFFull) { qs_ctx_decode_done(ctx, launches, "progressive encoder: image too large"); return JPEGQS_ERR_ARG; }
+		const dim3 tiles((unsigned)maxtile, g), chunks((unsigned)maxchunk, g);
+		const unsigned zero_blocks = (unsigned)(maxchunk < 4096 ? maxchunk : 4096);
+		qp_setup_kernel<<<g, 256, 0, st>>>(pack); launches++;
+		qp_class_kernel<<<tiles, QE_T, 0, st>>>(P); launches++;
+		qp_tscan_kernel<<<g, QE_SCAN_T, 0, st>>>(P, 0); launches++;
+		qp_runs_kernel<<<tiles, QE_T, 0, st>>>(P); launches++;
+		qp_count_kernel<<<tiles, QE_T, 0, st>>>(P); launches++;
+		qp_table_kernel<<<dim3(QP_MAX_SCANS, g), 64, 0, st>>>(P); launches++;
+		qp_len_kernel<<<tiles, QE_T, 0, st>>>(P); launches++;
+		qp_tscan_kernel<<<g, QE_SCAN_T, 0, st>>>(P, 1); launches++;
+		qp_zero_kernel<<<dim3(zero_blocks, g), 256, 0, st>>>(P); launches++;
+		qp_emit_kernel<<<tiles, QE_T, 0, st>>>(P); launches++;
+		qp_ffcount_kernel<<<chunks, QE_BT, 0, st>>>(P); launches++;
+		qp_fscan_kernel<<<g, QE_SCAN_T, 0, st>>>(P); launches++;
+		qp_copy_kernel<<<chunks, QE_BT, 0, st>>>(P); launches++;
+		QE_CK(cudaGetLastError());
+	}
+	qs_ctx_decode_done(ctx, launches, "");
+	return 0;
+}
+
+/* the same steps on the calling thread: every per-unit function in the kernels' order, each scan's
+ * prefix sums taken over the whole scan (tile offsets 0) */
+int qe_progressive_model(const jpegqs_cuda_image *img, const jpegqs_cuda_jpeg_head *head, uint8_t *out, size_t cap,
+		uint64_t *len, int32_t *status) {
+	QpImg p; QpSizes z;
+	const char *e = qp_check(img, head, &p, &z);
+	if (!e && cap < head->prefix_len) e = "cap smaller than prefix_len";
+	if (e) { char m[256]; snprintf(m, sizeof(m), "progressive model: %s", e); qs_set_host_error(m); return JPEGQS_ERR_ARG; }
+	QpState ps;
+	memset(&ps, 0, sizeof(ps));
+	std::vector<QeTab> tab(2 * QP_MAX_SCANS);
+	memset(tab.data(), 0, tab.size() * sizeof(QeTab));
+	std::vector<uint8_t> cls(z.units, 0);
+	std::vector<uint16_t> run(z.units, 0);
+	std::vector<uint64_t> pre(z.units, 0), tile(z.tiles, 0);
+	p.ps = &ps; p.e.tab = tab.data(); p.cls = cls.data(); p.run = run.data(); p.pre = pre.data(); p.e.tile = tile.data();
+	p.e.out = out; p.e.cap = cap;
+	QpNull zs;
+	/* qp_class, qp_tscan, qp_runs */
+	for (int s = 0; s < p.nscan; s++) {
+		const QpScan &sc = p.scan[s];
+		if (!sc.ss) continue;
+		uint64_t acc = 0; uint32_t cp = 0;
+		for (uint64_t i = 0; i < sc.n; i++) {
+			const uint32_t c = qp_unit(p, sc, i, 0, zs);
+			cls[sc.ubase + i] = (uint8_t)c;
+			pre[sc.ubase + i] = acc;
+			acc += (qp_break(c, cp, i) ? 1ull << 32 : 0) | (c >> 2);
+			cp = c;
+		}
+		ps.sc[s].total = acc;
+		for (uint64_t i = 0; i < sc.n; i++) {
+			const uint32_t c = cls[sc.ubase + i];
+			if ((c & 1) && qp_break(c, i ? cls[sc.ubase + i - 1] : 0, i)) qp_walk(p, s, i);
+		}
+	}
+	/* qp_count, qp_table */
+	for (int s = 0; s < p.nscan; s++) {
+		const QpScan &sc = p.scan[s];
+		struct { QeTab *t; void sym(int k, int v, uint32_t, int) { t[k].freq[v]++; } void bits(uint32_t, int) {} } cnt = { tab.data() + 2 * s };
+		if (qp_slots(p, sc)) for (uint64_t i = 0; i < sc.n; i++) qp_unit(p, sc, i, run[sc.ubase + i], cnt);
+		for (int t = 0; t < qp_slots(p, sc); t++) {
+			std::vector<uint64_t> f(257); std::vector<int> cs(257), oth(257);
+			qe_optimal(&tab[2 * s + t], f.data(), cs.data(), oth.data(), 0, 1);
+			qe_codes(&tab[2 * s + t]);
+		}
+	}
+	memcpy(out, head->prefix_dev, head->prefix_len);
+	QeOut f = { out, cap, head->prefix_len };
+	qe_frame(p.e, p.e.geo[0], f, true);
+	/* qp_len, qp_emit per scan, then the stuffed copy between the scan headers */
+	uint64_t pos = f.n;
+	for (int s = 0; s < p.nscan; s++) {
+		const QpScan &sc = p.scan[s];
+		const uint32_t *cs0 = tab[2 * s].cs, *cs1 = tab[2 * s + 1].cs;
+		std::vector<uint64_t> off(sc.n + 1, 0);
+		for (uint64_t i = 0; i < sc.n; i++) {
+			QpLenSink k = { { cs0, cs1 }, 0 };
+			qp_unit(p, sc, i, run[sc.ubase + i], k);
+			off[i + 1] = off[i] + k.n;
+		}
+		const uint64_t total = off[sc.n], nraw = (total + 7) >> 3;
+		std::vector<uint32_t> word((size_t)((total + 31) / 32 + 1), 0);
+		p.e.word = word.data();
+		for (uint64_t i = 0; i < sc.n; i++) qp_emit_unit(p, s, i, run[sc.ubase + i], off[i], cs0, cs1, total);
+		QeOut o = { out, cap, pos };
+		qp_scan_head(p, s, tab.data(), o);
+		pos = o.n;
+		qe_stuff(word.data(), 0, nraw, out, cap, pos);
+		pos += nraw + qe_ffs(word.data(), 0, nraw);
+	}
+	const uint64_t L = pos + 2;
+	int32_t flags = 0;
 	if (L > cap) flags |= JPEGQS_ENCODE_OVERFLOW;
 	else { out[pos] = 0xFF; out[pos + 1] = 0xD9; }
 	*len = L; *status = flags;

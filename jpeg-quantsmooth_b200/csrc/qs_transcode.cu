@@ -1017,8 +1017,8 @@ static int pixels_jpeg_entry(jpegqs_cuda_ctx *ctx, const char *who, int n, const
 		snprintf(msg, sizeof(msg), "%s: NULL argument", who); qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG;
 	}
 	if (params->quality < 1 || params->quality > 100 || params->subsampling < 0 || params->subsampling > 2 ||
-			(params->optimize != 0 && params->optimize != 1)) {
-		snprintf(msg, sizeof(msg), "%s: params: quality outside 1..100, subsampling outside 0..2 or optimize other than 0 / 1", who);
+			(params->optimize & ~(JPEGQS_JPEG_PROGRESSIVE | 1)) != 0) {
+		snprintf(msg, sizeof(msg), "%s: params: quality outside 1..100, subsampling outside 0..2 or optimize other than 0 / 1 (| JPEGQS_JPEG_PROGRESSIVE)", who);
 		qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG;
 	}
 	for (int i = 0; i < n; i++) if (!data[i]) {

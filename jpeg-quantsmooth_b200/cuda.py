@@ -848,10 +848,12 @@ def encode_model(image: CoefImage, arrays, prefix: bytes, comp_ids, quant_tbls, 
 
 # ---- pictures to JPEG files (include/jpegqs_cuda.h "8-bit pictures -> JPEG files") ----
 SUBSAMPLINGS = {"4:4:4": 0, "4:2:2": 1, "4:2:0": 2}
+JPEG_PROGRESSIVE = 0x100       # JPEGQS_JPEG_PROGRESSIVE: ORed into jpegqs_cuda_jpeg_params.optimize
 
 
-def _jpeg_params(quality, subsampling, optimize, who: str) -> _JpegParams:
-    """Pillow's save keywords: quality 1..100; subsampling "4:4:4" / "4:2:2" / "4:2:0" or 0 / 1 / 2"""
+def _jpeg_params(quality, subsampling, optimize, who: str, progressive=False) -> _JpegParams:
+    """Pillow's save keywords: quality 1..100; subsampling "4:4:4" / "4:2:2" / "4:2:0" or 0 / 1 / 2;
+    progressive a bool (JPEGQS_JPEG_PROGRESSIVE ORed into optimize)"""
     if isinstance(quality, bool) or not isinstance(quality, (int, np.integer)) or not 1 <= int(quality) <= 100:
         raise ValueError(f"{who}: quality {quality!r}: expected an integer in 1..100")
     if isinstance(subsampling, str) and subsampling in SUBSAMPLINGS:
@@ -860,7 +862,9 @@ def _jpeg_params(quality, subsampling, optimize, who: str) -> _JpegParams:
         s = int(subsampling)
     else:
         raise ValueError(f"{who}: subsampling {subsampling!r}: expected '4:4:4', '4:2:2', '4:2:0' or 0, 1, 2")
-    return _JpegParams(int(quality), s, int(bool(optimize)))
+    if not isinstance(progressive, (bool, np.bool_)):
+        raise ValueError(f"{who}: progressive {progressive!r}: expected True or False")
+    return _JpegParams(int(quality), s, int(bool(optimize)) | (JPEG_PROGRESSIVE if progressive else 0))
 
 
 def _pixels_in(ptr, shape, row_bytes) -> _PixelsIn:
@@ -879,25 +883,26 @@ def _host_picture(pixels, who: str) -> np.ndarray:
     return np.ascontiguousarray(a)
 
 
-def compress_bound(shape, quality=75, subsampling="4:2:0", optimize=False) -> int:
+def compress_bound(shape, quality=75, subsampling="4:2:0", optimize=False, progressive=False) -> int:
     """Output bytes compress_async never exceeds for an [H, W, C] picture (host-only)."""
     lib = load()
     pin, out = _pixels_in(None, shape, int(shape[1]) * int(shape[2])), C.c_size_t(0)
-    jp = _jpeg_params(quality, subsampling, optimize, "compress_bound")
+    jp = _jpeg_params(quality, subsampling, optimize, "compress_bound", progressive)
     if lib.jpegqs_cuda_compress_bound(C.byref(pin), C.byref(jp), C.byref(out)) < 0:
         raise QsError(lib.jpegqs_cuda_last_error(None).decode())
     return int(out.value)
 
 
-def compress_model(pixels, quality=75, subsampling="4:2:0", optimize=False, capacity=None) -> bytes:
+def compress_model(pixels, quality=75, subsampling="4:2:0", optimize=False, capacity=None, progressive=False) -> bytes:
     """compress_async's algorithm on one CPU thread for one picture (jpegqs_cuda_compress_model): a uint8
     array [H, W, 3] (RGB), [H, W, 1] or [H, W] (grey) to the bytes of Pillow's
-    Image.fromarray(P).save(f, "JPEG", quality=quality, subsampling=subsampling, optimize=optimize).
-    capacity: output bytes (default compress_bound); a file that does not fit raises QsError."""
+    Image.fromarray(P).save(f, "JPEG", quality=quality, subsampling=subsampling, optimize=optimize,
+    progressive=progressive).  capacity: output bytes (default compress_bound); a file that does not fit
+    raises QsError."""
     lib = load()
     a = _host_picture(pixels, "compress_model")
-    jp = _jpeg_params(quality, subsampling, optimize, "compress_model")
-    cap = int(capacity) if capacity is not None else compress_bound(a.shape, quality, subsampling, optimize)
+    jp = _jpeg_params(quality, subsampling, optimize, "compress_model", progressive)
+    cap = int(capacity) if capacity is not None else compress_bound(a.shape, quality, subsampling, optimize, progressive)
     out = np.zeros(max(cap, 1), dtype=np.uint8)
     pin = _pixels_in(a.ctypes.data, a.shape, a.shape[1] * a.shape[2])
     n, st = C.c_uint64(0), C.c_int32(0)
@@ -1668,20 +1673,22 @@ class QsContext:
                 _stream_handle(stream)))
         return out, lengths, st
 
-    def compress_async(self, pixels, quality=75, subsampling="4:2:0", optimize=False, out=None, stream=None):
+    def compress_async(self, pixels, quality=75, subsampling="4:2:0", optimize=False, out=None, stream=None,
+                       progressive=False):
         """Write device pictures as the JPEG files Pillow's Image.save(quality=, subsampling=,
         optimize=) writes for them, without blocking the calling thread (jpegqs_cuda_compress_async).
 
         pixels: uint8 CUDA tensors [H, W, C], C = 3 (RGB) or 1 (grey), whose last two dimensions are
         contiguous (a row stride of at least W * C is taken, so crops of a bigger picture work).
         quality / subsampling / optimize: Pillow's keywords ("4:4:4", "4:2:2", "4:2:0" or 0, 1, 2;
-        grey pictures ignore subsampling).  out[i] (optional): 1-D uint8 CUDA tensors to write, their
+        grey pictures ignore subsampling); progressive=True writes Pillow's progressive=True files
+        (jpegqs_cuda_compress_async with JPEGQS_JPEG_PROGRESSIVE).  out[i] (optional): 1-D uint8 CUDA tensors to write, their
         size the capacity; by default allocated on the stream at compress_bound's size.  stream: a
         torch.cuda.Stream (default: the current one).  Returns (out, lengths [n] int64, status [n]
         int32), all on the device; status is 0, or ENCODE_OVERFLOW with lengths[i] the size needed.
         Capturable with torch.cuda.graph: a replay compresses the current contents of the same tensors."""
         import torch
-        jp = _jpeg_params(quality, subsampling, optimize, "compress_async")
+        jp = _jpeg_params(quality, subsampling, optimize, "compress_async", progressive)
         n = len(pixels)
         if out is not None and len(out) != n:
             raise ValueError("compress_async: out must have one entry per picture")
@@ -1731,7 +1738,8 @@ class QsContext:
         return out, lengths, st
 
     def reencode(self, datas, flags: int, niter: int, quality=75, subsampling="4:2:0", optimize=False, scale_denom=1,
-                 size=None, crop=None, filter="bicubic", max_device_bytes: int = 0, orientation=None, mode=None):
+                 size=None, crop=None, filter="bicubic", max_device_bytes: int = 0, orientation=None, mode=None,
+                 progressive=False):
         """Many JPEG files to JPEG files of their smoothed pixels (jpegqs_cuda_pixels_batch_jpeg): each
         file's output is exactly Pillow's Image.fromarray(P).save(f, "JPEG", quality=quality,
         subsampling=subsampling, optimize=optimize), where P is the picture decode_pixels gives for the
@@ -1744,11 +1752,12 @@ class QsContext:
         decode_pixels (jpegqs_cuda_pixels_batch_jpeg_oriented); "exif" gives Pillow's
         ImageOps.exif_transpose(P).save(...): upright pixels in a JFIF file without the tag.  mode: as for
         decode_pixels (jpegqs_cuda_pixels_batch_jpeg_mode): Pillow's P.convert(mode).save(...), so CMYK
-        and YCCK files give RGB files and "L" gives grey files."""
+        and YCCK files give RGB files and "L" gives grey files.  progressive=True: Pillow's
+        save(..., progressive=True) instead."""
         if isinstance(datas, (bytes, bytearray, memoryview, str)) or not hasattr(datas, "__len__"):
             raise TypeError("reencode: datas must be a sequence of bytes-like files")
         files = [_file_bytes(d, f"reencode: file {i}") for i, d in enumerate(datas)]
-        jp = _jpeg_params(quality, subsampling, optimize, "reencode")
+        jp = _jpeg_params(quality, subsampling, optimize, "reencode", progressive)
         if int(max_device_bytes) < 0:
             raise ValueError("reencode: max_device_bytes must be >= 0")
         scale = _scale_denom(scale_denom, "reencode")
@@ -2085,7 +2094,7 @@ def decode_pixels(datas, flags: int, niter: int, layout: str = "hwc", device: st
                                               size, crop, filter, orientation, mode)
 
 
-def compress_async(pixels, quality=75, subsampling="4:2:0", optimize=False, out=None, stream=None):
+def compress_async(pixels, quality=75, subsampling="4:2:0", optimize=False, out=None, stream=None, progressive=False):
     """QsContext.compress_async on the default context of the tensors' device: writes uint8 CUDA pictures
     [H, W, C] as Pillow's JPEG files in CUDA uint8 tensors, enqueued on `stream` (default: the current
     one) without waiting.  Returns (out, lengths [n] int64, status [n] int32), all on the device."""
@@ -2093,13 +2102,15 @@ def compress_async(pixels, quality=75, subsampling="4:2:0", optimize=False, out=
     first = next(iter(pixels), None)
     if not isinstance(first, torch.Tensor) or not first.is_cuda:
         raise ValueError("compress_async: the pixel tensors must be CUDA tensors")
-    return default_context(first.device.index).compress_async(pixels, quality, subsampling, optimize, out, stream)
+    return default_context(first.device.index).compress_async(pixels, quality, subsampling, optimize, out, stream,
+                                                               progressive)
 
 
 def reencode(datas, flags: int, niter: int, quality=75, subsampling="4:2:0", optimize=False, scale_denom=1, size=None,
-             crop=None, filter="bicubic", max_device_bytes: int = 0, gpu: int = -1, orientation=None, mode=None):
+             crop=None, filter="bicubic", max_device_bytes: int = 0, gpu: int = -1, orientation=None, mode=None,
+             progressive=False):
     """QsContext.reencode on the default context of CUDA device `gpu`: one record (data, warnings,
     host_decoded, smoothed, stop, upsampled, reason) per file, data the JPEG file Pillow's save writes for
     the picture decode_pixels gives with the same arguments."""
     return default_context(gpu).reencode(datas, flags, niter, quality, subsampling, optimize, scale_denom, size, crop,
-                                         filter, max_device_bytes, orientation, mode)
+                                         filter, max_device_bytes, orientation, mode, progressive)

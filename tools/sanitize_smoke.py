@@ -162,3 +162,13 @@ for d in (1, 2):
     for mode in ("RGB", "L"):
         px = ctx.decode_pixels(mfiles, 3, 1, scale_denom=d, mode=mode, orientation=[1, 2, 3, 4, 5, 6, 7, 8])
         print("decode_pixels mode", mode, "d", d, [tuple(p[0].shape) for p in px], flush=True)
+
+# progressive files: grey and RGB pictures of every sampling, sizes with odd block counts, one flat
+# picture whose AC scans are one long run segment
+rng = np.random.RandomState(12)
+pics = [torch.from_numpy(rng.randint(0, 256, (h, w, c)).astype(np.uint8)).cuda()
+        for h, w, c in ((23, 39, 3), (40, 24, 1), (9, 130, 3))] + [torch.full((200, 296, 3), 90, dtype=torch.uint8).cuda()]
+for sub in ("4:4:4", "4:2:2", "4:2:0"):
+    out, lens, st = ctx.compress_async(pics, 90, sub, progressive=True)
+    torch.cuda.synchronize()
+    print("compress_async progressive", sub, lens.tolist(), st.tolist(), flush=True)
