@@ -936,6 +936,80 @@ int jpegqs_cuda_pixels_batch_jpeg_mode(jpegqs_cuda_ctx *ctx, int n, const uint8_
 		const jpegqs_cuda_jpeg_params *params, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results,
 		uint8_t **out, size_t *out_len, const int32_t *orientation, int mode);
 
+/* ---- thumbnails and reducing_gap: Pillow's Image.thumbnail and Image.resize(reducing_gap=) --------
+ * Pillow's thumbnail((bw, bh), filter, reducing_gap) of a W x H JPEG file:
+ *   1. the size: preserve_aspect_ratio (round_aspect of the bound's aspect), or nothing at all when the
+ *      bound covers the picture on both axes;
+ *   2. the draft scale s: the first of 8, 4, 2, 1 at most min(W // int(bw * gap), H // int(bh * gap)),
+ *      and the picture at 1/s (libjpeg's scaled decode); no draft for gap None, or when the picture was
+ *      loaded first (exif_transpose, transpose and convert load it, and draft then does nothing);
+ *   3. no resize when the drafted picture already has the thumbnail's size; otherwise
+ *      Image.resize(size, filter, box = (0, 0, W / s, H / s), reducing_gap):
+ *   4. factor = int(box_w / out_w / gap) or 1 per axis; when one is above 1, Image.reduce by the factors
+ *      over _get_safe_box (the box widened by the filter's support less 0.5 in source samples, then
+ *      rounded outwards), and the box shifted and divided by the factors;
+ *   5. the convolution resize of the (reduced) picture from that box, which Pillow's C layer takes as
+ *      float: scale = (double)(float)(in1 - in0) / out, centres in0 + (xx + 0.5) * scale in double.
+ * Reduce arithmetic (Reduce.c): each output sample covers the n = fx * fy samples of its cell, fewer in
+ * the partial cells at the right and bottom edges of the box, and is ((sum + n / 2) * m) >> 24 with
+ * m = (uint32)((float)2^32 / (float)(256 * n)), in 32-bit unsigned arithmetic - not the rounded mean.
+ * A cell of 2^23 samples or more (256 * n would overflow Pillow's int) is refused; so is a picture more
+ * than 100 times taller than wide after the reduce, which Pillow resizes vertically first.  Both fail the
+ * file alone with JPEGQS_ERR_ARG.
+ *
+ * jpegqs_cuda_thumbnail_geometry: steps 1 and 2 (host-only), so callers can size out[i].  width and
+ * height are the picture thumbnail sees (oriented for 5..8); loaded = 1 when an orientation or a mode is
+ * given (then *scale_denom is 1).  reducing_gap 0.0 means None, otherwise finite and at least 1.0; bounds
+ * and sizes 1..65535.  Returns 0 or JPEGQS_ERR_ARG; jpegqs_cuda_last_error(NULL) says why. */
+int jpegqs_cuda_thumbnail_geometry(int width, int height, int bound_w, int bound_h, double reducing_gap, int loaded,
+		int *scale_denom, int *out_w, int *out_h);
+
+/* jpegqs_cuda_pixels_batch_mode with thumbnails and reducing_gap.  reducing_gap 0.0 means None; any
+ * other value must be finite and at least 1.0.
+ *   - thumbnail 0: boxes mean what they mean for the mode call, and file i is Pillow's
+ *     Image.fromarray(P).crop(box).resize(size, filter, reducing_gap=reducing_gap); reducing_gap 0.0 is
+ *     byte for byte the mode call.
+ *   - thumbnail 1: file i is Pillow's Image.open(F) [exif_transpose / transpose] [convert(mode)] then
+ *     thumbnail((boxes[i].width, boxes[i].height), filter, reducing_gap) (steps 1-5 above): out[i] is
+ *     jpegqs_cuda_thumbnail_geometry's out_w x out_h.  Every box has left..bottom 0, scale_denom must
+ *     be 1 (the scale is thumbnail's own), and filter is one of the five convolution filters.
+ *   - Per sub-batch: every distinct draft scale is rendered by its own render call (at most four, more
+ *     when smoothed and unsmoothed files, or CHW outputs that need neither stage, interleave); one reduce
+ *     launch over the files with a factor above 1; the two resize launches over the files whose size
+ *     changes.  A file that needs neither is stored by the render in the caller's layout.  The budget
+ *     also counts each reduced picture.
+ *   - Return.  As the mode call's; also JPEGQS_ERR_ARG with nothing done for a bad reducing_gap or
+ *     thumbnail, a thumbnail box with an offset, or scale_denom other than 1 with thumbnail 1. */
+int jpegqs_cuda_pixels_batch_reduced(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int layout, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
+		const int32_t *orientation, int mode, int out_on_device, uint8_t *const *out, size_t max_device_bytes, int *rc,
+		jpegqs_cuda_pixels_result *results, int thumbnail, double reducing_gap);
+
+/* jpegqs_cuda_pixels_batch_jpeg_mode with thumbnail and reducing_gap as for pixels_batch_reduced: the
+ * thumbnail (or reduced resize) is saved, progressive output included.  thumbnail 0 with reducing_gap
+ * 0.0: byte for byte the mode call. */
+int jpegqs_cuda_pixels_batch_jpeg_reduced(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
+		const jpegqs_cuda_jpeg_params *params, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results,
+		uint8_t **out, size_t *out_len, const int32_t *orientation, int mode, int thumbnail, double reducing_gap);
+
+/* The reduce of pixels_batch_reduced on the calling thread (host-only): Pillow's Image.reduce((factor_x,
+ * factor_y), box) of a width x height x channels HWC picture (channels 1 or 3).  box: (left, top, right,
+ * bottom) integers, or NULL for the whole picture.  out: ceil(box_w / factor_x) x ceil(box_h / factor_y)
+ * x channels bytes, HWC.  Returns 0 or JPEGQS_ERR_ARG (NULL pointer, a factor below 1 or a cell of 2^23
+ * samples or more, a box outside the picture or empty). */
+int jpegqs_cuda_reduce_model(const uint8_t *src, int width, int height, int channels, int factor_x, int factor_y,
+		const int32_t *box, uint8_t *out);
+
+/* Steps 4 and 5 above on the calling thread (host-only), with the planning the batch uses: Pillow's
+ * Image.resize((out_w, out_h), filter, box, reducing_gap) of a width x height x channels HWC picture.
+ * box: (left, top, right, bottom) as doubles, as Pillow's Python layer holds it, or NULL for the whole
+ * picture; reducing_gap 0.0 means None.  out: out_w x out_h x channels in layout HWC or CHW.  Returns 0
+ * or JPEGQS_ERR_ARG (the checks of jpegqs_cuda_resize_model, a box outside the picture or empty, and the
+ * refusals above). */
+int jpegqs_cuda_resize_model_box(const uint8_t *src, int width, int height, int channels, int layout, int filter,
+		const double *box, int out_w, int out_h, double reducing_gap, uint8_t *out);
+
 /* ---- one image sharded by MCU rows over several GPUs (SURVEY.md 8e) ----------------------
  * Every rank - a device of this process, or another process on the same box - smooths one slab
  * of contiguous MCU rows and exchanges ONE pixel row per plane with each neighbour after every

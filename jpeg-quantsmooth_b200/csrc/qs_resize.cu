@@ -60,24 +60,25 @@ static double qs_rs_filter(int filter, double x) {
 	}
 }
 
-static double qs_rs_support(int filter) {
+double qs_resize_support(int filter) {
 	return filter == JPEGQS_RESIZE_BOX ? 0.5 : filter == JPEGQS_RESIZE_BICUBIC ? 2.0 : filter == JPEGQS_RESIZE_LANCZOS ? 3.0 : 1.0;
 }
 
 int qs_resize_filter_ok(int filter) { return filter >= JPEGQS_RESIZE_LANCZOS && filter <= JPEGQS_RESIZE_HAMMING; }
 
-/* precompute_coeffs + normalize_coeffs_8bpc for in_size -> out_size: appends the bounds (first sample,
- * count) and the rounded weights (row stride ksize, unused entries 0) to tab; returns ksize */
-static int qs_rs_axis(int in_size, int out_size, int filter, std::vector<int32_t> &bounds, std::vector<int32_t> &kk) {
-	const double scale = (double)in_size / out_size;
+/* precompute_coeffs + normalize_coeffs_8bpc for out_size samples centred at in0 + (xx + 0.5) * scale of
+ * in_size: the bounds (first sample, count) and the rounded weights (row stride ksize, unused entries 0);
+ * returns ksize */
+static int qs_rs_axis_at(int in_size, double in0, double scale, int out_size, int filter, std::vector<int32_t> &bounds,
+		std::vector<int32_t> &kk) {
 	const double filterscale = scale < 1.0 ? 1.0 : scale;
-	const double support = qs_rs_support(filter) * filterscale;
+	const double support = qs_resize_support(filter) * filterscale;
 	const int ksize = (int)ceil(support) * 2 + 1;
 	std::vector<double> w((size_t)ksize);
 	bounds.assign((size_t)out_size * 2, 0);
 	kk.assign((size_t)out_size * ksize, 0);
 	for (int xx = 0; xx < out_size; xx++) {
-		const double center = (xx + 0.5) * scale, ss = 1.0 / filterscale;
+		const double center = in0 + (xx + 0.5) * scale, ss = 1.0 / filterscale;
 		double ww = 0.0;
 		int xmin = (int)(center - support + 0.5);
 		if (xmin < 0) xmin = 0;
@@ -94,6 +95,23 @@ static int qs_rs_axis(int in_size, int out_size, int filter, std::vector<int32_t
 	return ksize;
 }
 
+/* the whole of in_size -> out_size */
+static int qs_rs_axis(int in_size, int out_size, int filter, std::vector<int32_t> &bounds, std::vector<int32_t> &kk) {
+	return qs_rs_axis_at(in_size, 0.0, (double)in_size / out_size, out_size, filter, bounds, kk);
+}
+
+/* the plan from both axes' tables: the rows the vertical pass reads (bounds are monotonic) are the only
+ * ones the horizontal pass makes */
+static void qs_rs_finish(int l, int t, int out_w, int out_h, std::vector<int32_t> &hb, std::vector<int32_t> &hk,
+		std::vector<int32_t> &vb, std::vector<int32_t> &vk, QsResizePlan &rp) {
+	const int first = vb[0], last = vb[2 * (out_h - 1)] + vb[2 * (out_h - 1) + 1];
+	for (int y = 0; y < out_h; y++) vb[2 * y] -= first;
+	rp.left = l; rp.top = t + first; rp.out_w = out_w; rp.out_h = out_h; rp.mid_h = last - first;
+	rp.tab.clear();
+	rp.tab.reserve(hb.size() + hk.size() + vb.size() + vk.size());
+	for (const std::vector<int32_t> *v : {&hb, &hk, &vb, &vk}) rp.tab.insert(rp.tab.end(), v->begin(), v->end());
+}
+
 const char *qs_resize_plan(int pic_w, int pic_h, const jpegqs_cuda_resize_box &box, int filter, QsResizePlan &rp) {
 	if (box.width < 1 || box.width > 65535 || box.height < 1 || box.height > 65535) return "output size outside 1..65535";
 	int l = box.left, t = box.top, r = box.right, b = box.bottom;
@@ -103,13 +121,20 @@ const char *qs_resize_plan(int pic_w, int pic_h, const jpegqs_cuda_resize_box &b
 	std::vector<int32_t> hb, hk, vb, vk;
 	rp.ksh = qs_rs_axis(r - l, box.width, filter, hb, hk);
 	rp.ksv = qs_rs_axis(b - t, box.height, filter, vb, vk);
-	/* the rows the vertical pass reads (bounds are monotonic): the horizontal pass makes only those */
-	const int first = vb[0], last = vb[2 * (box.height - 1)] + vb[2 * (box.height - 1) + 1];
-	for (int y = 0; y < box.height; y++) vb[2 * y] -= first;
-	rp.left = l; rp.top = t + first; rp.out_w = box.width; rp.out_h = box.height; rp.mid_h = last - first;
-	rp.tab.clear();
-	rp.tab.reserve(hb.size() + hk.size() + vb.size() + vk.size());
-	for (const std::vector<int32_t> *v : {&hb, &hk, &vb, &vk}) rp.tab.insert(rp.tab.end(), v->begin(), v->end());
+	qs_rs_finish(l, t, box.width, box.height, hb, hk, vb, vk, rp);
+	return NULL;
+}
+
+/* Pillow's C layer takes the box as float: scale = (double)(float)(in1 - in0) / out, and each centre is
+ * in0 + (xx + 0.5) * scale in double, over the whole picture (samples outside the box are read) */
+const char *qs_resize_plan_box(int pic_w, int pic_h, const float box[4], int out_w, int out_h, int filter, QsResizePlan &rp) {
+	if (out_w < 1 || out_w > 65535 || out_h < 1 || out_h > 65535) return "output size outside 1..65535";
+	if (!(box[0] >= 0.0f && box[1] >= 0.0f && box[2] <= (float)pic_w && box[3] <= (float)pic_h)) return "box outside the picture";
+	if (!(box[2] > box[0] && box[3] > box[1])) return "empty box";
+	std::vector<int32_t> hb, hk, vb, vk;
+	rp.ksh = qs_rs_axis_at(pic_w, box[0], (double)(float)(box[2] - box[0]) / out_w, out_w, filter, hb, hk);
+	rp.ksv = qs_rs_axis_at(pic_h, box[1], (double)(float)(box[3] - box[1]) / out_h, out_h, filter, vb, vk);
+	qs_rs_finish(0, 0, out_w, out_h, hb, hk, vb, vk, rp);
 	return NULL;
 }
 
@@ -217,13 +242,17 @@ extern "C" int jpegqs_cuda_resize_model(const uint8_t *src, int width, int heigh
 		qs_set_host_error(m);
 		return JPEGQS_ERR_ARG;
 	}
+	qs_resize_run_model(rp, src, width, channels, layout == JPEGQS_RENDER_CHW, out);
+	return 0;
+}
+
+void qs_resize_run_model(const QsResizePlan &rp, const uint8_t *src, int src_w, int ch, int chw, uint8_t *out) {
 	QsResizeDesc d;
-	qs_resize_desc(rp, width, channels, layout == JPEGQS_RENDER_CHW, d);
+	qs_resize_desc(rp, src_w, ch, chw, d);
 	std::vector<uint8_t> mid((size_t)d.mid_h * qs_rs_hlen(d));
 	d.src = src; d.mid = mid.data(); d.out = out; d.tab = rp.tab.data();
 	for (uint32_t y = 0; y < (uint32_t)d.mid_h; y++)
 		for (uint32_t j = 0; j < qs_rs_hlen(d); j++) mid[(size_t)y * qs_rs_hlen(d) + j] = qs_rs_h(d, y, j);
 	for (uint32_t r = 0; r < qs_rs_vrows(d); r++)
 		for (uint32_t j = 0; j < qs_rs_vlen(d); j++) out[(size_t)r * qs_rs_vlen(d) + j] = qs_rs_v(d, r, j);
-	return 0;
 }

@@ -33,9 +33,17 @@ struct QsResizeDesc {
 
 /* the filter is one of JPEGQS_RESIZE_LANCZOS .. JPEGQS_RESIZE_HAMMING */
 int qs_resize_filter_ok(int filter);
+/* the filter's support (Pillow's _filters_support) */
+double qs_resize_support(int filter);
 /* Plans the crop box of a pic_w x pic_h picture resized to box.width x box.height.  Returns NULL, or
  * why the box does not fit (the crop outside the picture or empty; the output size outside 1..65535). */
 const char *qs_resize_plan(int pic_w, int pic_h, const jpegqs_cuda_resize_box &box, int filter, QsResizePlan &rp);
+/* Plans Pillow's Image.resize((out_w, out_h), filter, box) of the whole pic_w x pic_h picture from a float
+ * box (left, top, right, bottom), as Pillow's C layer takes it.  For an integer box equal to the picture
+ * the tables are qs_resize_plan's.  Returns NULL, or why the box does not fit. */
+const char *qs_resize_plan_box(int pic_w, int pic_h, const float box[4], int out_w, int out_h, int filter, QsResizePlan &rp);
+/* the host model of the two passes over src (src_w pixels of ch bytes a row) into out */
+void qs_resize_run_model(const QsResizePlan &rp, const uint8_t *src, int src_w, int ch, int chw, uint8_t *out);
 /* fills d's geometry from rp (the pointers are the caller's) */
 void qs_resize_desc(const QsResizePlan &rp, int src_w, int ch, int chw, QsResizeDesc &d);
 /* numbers the blocks of both launches over the descriptors: sets each hblk / vblk, returns the totals */

@@ -7,9 +7,11 @@
  * files into one buffer so that a sub-batch comes back in one copy.
  * jpegqs_cuda_pixels_batch: the same files to the smoothed pixels the tool's --ppm writes, through
  * the same plans, sub-batches and decoder launches, the host reader, run_async and the fused render;
- * jpegqs_cuda_pixels_batch_resized adds qs_resize.cu's crop and resize after the render.
+ * jpegqs_cuda_pixels_batch_resized adds qs_resize.cu's crop and resize after the render, and
+ * jpegqs_cuda_pixels_batch_reduced qs_reduce.cu's reduce before the resize, and thumbnail's own scales.
  */
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -17,6 +19,7 @@
 #include "jpegqs_cuda.h"
 #include "qs_common.h"
 #include "qs_resize.h"
+#include "qs_reduce.h"
 
 /* include/libjpegqs.h's JPEGQS_FLAGS_MASK and JPEGQS_ITER_MAX (that header needs <jpeglib.h>) */
 #define QS_FLAGS_MASK 0x7f
@@ -188,6 +191,8 @@ struct QsPlan {
 	int smooth, can_up;
 	int out_w, out_h;                          /* pixels: the output picture's size */
 	int orient, pic_w;                         /* pixels: the render's orientation (1..8), the rendered picture's width */
+	int scale;                                 /* pixels: the render's scale denominator */
+	int resized, reduced;                      /* pixels: the file goes through the resize; through the reduce first */
 	int channels;                              /* pixels: 1 or 3, from the mode (the component count for mode 0) */
 	size_t in_bytes, coef_bytes, up_bytes, cap, pix;
 	size_t ws_dec, ws_run, ws_enc;             /* this file's share of each stage's workspace */
@@ -600,22 +605,35 @@ struct QsJpegLayout {
 	}
 };
 
+/* the crop of a resize box in a pw x ph picture (all 0: the whole picture), or why it does not fit */
+static const char *crop_of(const jpegqs_cuda_resize_box &b, int pw, int ph, int c[4]) {
+	c[0] = b.left; c[1] = b.top; c[2] = b.right; c[3] = b.bottom;
+	if (!c[0] && !c[1] && !c[2] && !c[3]) { c[2] = pw; c[3] = ph; }
+	if (c[0] < 0 || c[1] < 0 || c[2] > pw || c[3] > ph) return "crop outside the picture";
+	if (c[0] >= c[2] || c[1] >= c[3]) return "empty crop";
+	return NULL;
+}
+
 /* boxes != NULL: each file's picture is cropped and resized (qs_resize.cu) with filter.  jp != NULL: the
  * pictures are written as JPEG files with these params (compress_async) into jout / jlen, and on_device
  * must be 0 (the pictures stay in the context's buffers).  orientation: NULL (1 for every file) or 0..8
  * per file, 0 for the file's own; the render writes the oriented picture, which the crop, the resize
  * and the compressor then take as it is.  mode: JPEGQS_PIXELS_*; the render converts, so every later stage
- * takes the converted picture's channels. */
+ * takes the converted picture's channels.  gap > 0: Pillow's reducing_gap, a reduce (qs_reduce.cu) before
+ * the resize where its factor is above 1.  thumbnail: boxes hold bounds, each file is rendered at its
+ * own draft scale and goes through the reduce and the resize only where Pillow's thumbnail does. */
 static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint8_t *const *data, const size_t *len,
 		int flags, int niter, int layout, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
 		const int32_t *orientation, int mode, int on_device, uint8_t *const *out, size_t max_device_bytes, int *rc,
 		jpegqs_cuda_pixels_result *results, const jpegqs_cuda_jpeg_params *jp = NULL, uint8_t **jout = NULL,
-		size_t *jlen = NULL) {
+		size_t *jlen = NULL, int thumbnail = 0, double gap = 0.0) {
 	char msg[512];
 	cudaStream_t st;
 	std::vector<QsPlan> plans((size_t)n);
 	std::vector<QsResizePlan> rsp(boxes ? (size_t)n : 0);
+	std::vector<QsReducePlan> rdp(boxes ? (size_t)n : 0);
 	std::vector<size_t> pic(boxes ? (size_t)n : 0);  /* resized files: the rendered picture's bytes */
+	const int loaded = orientation != NULL || mode != JPEGQS_PIXELS_AS_FILE;   /* thumbnail's draft does nothing */
 	int ret = 0;
 	{
 	QsTranscode *t = NULL;
@@ -638,32 +656,61 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 		 * swapped by orientations 5..8 */
 		p.orient = orientation ? orientation[i] : 1;
 		if (!p.orient && jpegqs_cuda_jpeg_orientation(data[i], len[i], &p.orient)) p.orient = 1;
-		const int sw = (int)((p.img.image_width + scale_denom - 1) / scale_denom);
-		const int sh = (int)((p.img.image_height + scale_denom - 1) / scale_denom);
+		const int fw = (int)(p.orient >= 5 ? p.img.image_height : p.img.image_width);
+		const int fh = (int)(p.orient >= 5 ? p.img.image_width : p.img.image_height);
+		int tw = 0, th = 0;                         /* thumbnail: its size */
+		p.scale = scale_denom;
+		if (thumbnail) qs_thumbnail_geometry(fw, fh, boxes[i].width, boxes[i].height, gap, loaded, &p.scale, &tw, &th);
+		const int sw = (int)((p.img.image_width + p.scale - 1) / p.scale);
+		const int sh = (int)((p.img.image_height + p.scale - 1) / p.scale);
 		const int pw = p.orient >= 5 ? sh : sw, ph = p.orient >= 5 ? sw : sh;
 		p.pix = (size_t)pw * ph * p.channels;
 		p.out_w = pw; p.out_h = ph; p.pic_w = pw;
-		if (boxes) {
-			const char *bad = qs_resize_plan(pw, ph, boxes[i], filter, rsp[i]);
+		p.resized = boxes && (!thumbnail || pw != tw || ph != th);
+		p.reduced = 0;
+		if (p.resized) {
+			const char *bad = NULL;
+			if (thumbnail) {
+				/* Image.resize(size, filter, box = draft's (0, 0, W / s, H / s), reducing_gap) */
+				const double box[4] = {0.0, 0.0, gap > 0.0 && !loaded ? (double)fw / p.scale : (double)pw,
+						gap > 0.0 && !loaded ? (double)fh / p.scale : (double)ph};
+				bad = qs_reduced_plan(pw, ph, box, tw, th, filter, gap, rdp[i], rsp[i]);
+			} else if (gap > 0.0) {
+				/* crop, then Image.resize(size, filter, reducing_gap) of the crop */
+				int c[4];
+				bad = crop_of(boxes[i], pw, ph, c);
+				if (!bad) {
+					const double box[4] = {0.0, 0.0, (double)(c[2] - c[0]), (double)(c[3] - c[1])};
+					bad = qs_reduced_plan(c[2] - c[0], c[3] - c[1], box, boxes[i].width, boxes[i].height, filter, gap, rdp[i], rsp[i]);
+				}
+				if (!bad && (rdp[i].fx > 1 || rdp[i].fy > 1)) { rdp[i].left += c[0]; rdp[i].top += c[1]; }
+				else if (!bad) { rsp[i].left += c[0]; rsp[i].top += c[1]; }
+			} else {
+				bad = qs_resize_plan(pw, ph, boxes[i], filter, rsp[i]);
+			}
 			if (bad) {
 				snprintf(msg, sizeof(msg), "%s: file %d: %s (picture %d x %d)", who, i, bad, pw, ph);
 				qs_ctx_decode_done(ctx, 0, msg);
 				rc[i] = JPEGQS_ERR_ARG; continue;
 			}
+			p.reduced = (thumbnail || gap > 0.0) && (rdp[i].fx > 1 || rdp[i].fy > 1);
 			pic[i] = p.pix;
-			p.pix = (size_t)boxes[i].width * boxes[i].height * p.channels;
-			p.out_w = boxes[i].width; p.out_h = boxes[i].height;
+			p.out_w = rsp[i].out_w; p.out_h = rsp[i].out_h;
+			p.pix = (size_t)p.out_w * p.out_h * p.channels;
 		}
 		p.host = route != JPEGQS_ROUTE_DEVICE;
 		if (p.host) { p.in_bytes = 0; p.ws_dec = 0; results[i].host_decoded = 1; results[i].reason = why; }
 		results[i].channels = p.channels;
 		TQ(plan_run(p, flags, niter));
 		/* file, coefficients (+ up-sampled chroma), the output pixels when they come back to the host;
-		 * resized: also the rendered picture, the intermediate, the tables and the descriptor */
+		 * resized: also the rendered picture, the intermediate, the tables and the descriptor; reduced: the
+		 * reduced picture and its descriptor */
 		p.fixed = p.in_bytes + p.coef_bytes + p.up_bytes + (on_device ? 0 : align256(p.pix));
-		if (boxes)
+		if (p.resized)
 			p.fixed += align256(pic[i]) + align256((size_t)rsp[i].mid_h * rsp[i].out_w * p.channels) +
 					align256(rsp[i].tab.size() * sizeof(int32_t)) + align256(sizeof(QsResizeDesc));
+		if (p.reduced)
+			p.fixed += align256((size_t)rdp[i].out_w * rdp[i].out_h * p.channels) + align256(sizeof(QsReduceDesc));
 		p.ws_enc = 0; p.packed = 0;
 		if (jp) {
 			/* JPEG: the compressor's workspace share (coefficients and encoder workspace, with the prefix's
@@ -779,17 +826,22 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 			TK(cudaMemcpyAsync(t->hcoef_dev.p, t->hcoef_host.p, hb, cudaMemcpyHostToDevice, st));
 		}
 
-		/* 7: run_async over the files that smooth, then one render over all.  Order by component count
-		 * 3, 1, 4 among the files that smooth, then 4, 1, 3 among those that do not - run_async's images
-		 * are a prefix, and each launch group's images (one store mode and conversion) are consecutive, so
-		 * the render takes at most five launches per 60 images (three without 4-component files) */
+		/* 7: run_async over the files that smooth, then one render per render key (scale and layout; one
+		 * key unless thumbnail).  Order the files that smooth by key, then by component count 3, 1, 4, and
+		 * those that do not by key, then 4, 1, 3 - run_async's images are a prefix, each key's images are
+		 * consecutive within each part, and each launch group's images (one store mode and conversion) are
+		 * consecutive, so with one key the render takes at most five launches per 60 images (three without
+		 * 4-component files) */
 		std::vector<int> rk;                           /* render order -> group position */
 		static const int kinds[6] = {3, 1, 4, 4, 1, 3};
-		for (int pass = 0; pass < 6; pass++)
-			for (int k = 0; k < m; k++) {
-				const QsPlan &p = plans[files[k]];
-				if (alive[k] && p.smooth == (pass < 3) && p.img.ncomp == kinds[pass]) rk.push_back(k);
-			}
+		auto rkey = [&](const QsPlan &p) { return p.scale * 2 + (p.resized ? JPEGQS_RENDER_HWC : layout); };
+		for (int pass = 0; pass < 6; pass += 3)
+			for (int key = 2; key <= 17; key++)
+				for (int q = pass; q < pass + 3; q++)
+					for (int k = 0; k < m; k++) {
+						const QsPlan &p = plans[files[k]];
+						if (alive[k] && p.smooth == (pass < 3) && p.img.ncomp == kinds[q] && rkey(p) == key) rk.push_back(k);
+					}
 		const int nr = (int)rk.size();
 		int ms = 0;
 		std::vector<jpegqs_cuda_image> rimg(nr);
@@ -804,33 +856,55 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 		jpegqs_cuda_status *run = (jpegqs_cuda_status*)t->out_dev.p;
 		std::vector<uint8_t*> outs(nr);
 		for (int j = 0; j < nr; j++) outs[j] = on_device ? out[files[rk[j]]] : (uint8_t*)t->out_dev.p + poff[j];
-		/* resized: the render writes each picture into rs_dev, which holds the descriptors and tables (one
-		 * upload from rs_host), then the intermediates, then the pictures; the resize writes outs */
-		uint32_t hblocks = 0, vblocks = 0;
-		if (boxes && nr) {
-			size_t up = align256(sizeof(QsResizeDesc) * (size_t)nr), all;
-			std::vector<size_t> toff(nr), moff(nr), qoff(nr);
-			for (int j = 0; j < nr; j++) { toff[j] = up; up += align256(rsp[files[rk[j]]].tab.size() * sizeof(int32_t)); }
+		/* resized: the render writes each picture into rs_dev, which holds the resize descriptors, the
+		 * reduce descriptors and the tables (one upload from rs_host), then the intermediates, then the
+		 * pictures, then the reduced pictures; the reduce writes those, the resize writes outs */
+		std::vector<int> rsj, rdj;                     /* render positions of the resized and the reduced files */
+		for (int j = 0; j < nr; j++) {
+			if (plans[files[rk[j]]].resized) rsj.push_back(j);
+			if (plans[files[rk[j]]].reduced) rdj.push_back(j);
+		}
+		const int nrs = (int)rsj.size(), nrd = (int)rdj.size();
+		uint32_t hblocks = 0, vblocks = 0, rblocks = 0;
+		const size_t rdo = align256(sizeof(QsResizeDesc) * (size_t)nrs);
+		if (nrs) {
+			size_t up = rdo + align256(sizeof(QsReduceDesc) * (size_t)nrd), all;
+			std::vector<size_t> toff(nrs), moff(nrs), qoff(nrs), roff(nrs);
+			for (int q = 0; q < nrs; q++) { toff[q] = up; up += align256(rsp[files[rk[rsj[q]]]].tab.size() * sizeof(int32_t)); }
 			all = up;
-			for (int j = 0; j < nr; j++) {
-				const QsResizePlan &r = rsp[files[rk[j]]];
-				moff[j] = all; all += align256((size_t)r.mid_h * r.out_w * plans[files[rk[j]]].channels);
+			for (int q = 0; q < nrs; q++) {
+				const QsResizePlan &r = rsp[files[rk[rsj[q]]]];
+				moff[q] = all; all += align256((size_t)r.mid_h * r.out_w * plans[files[rk[rsj[q]]]].channels);
 			}
-			for (int j = 0; j < nr; j++) { qoff[j] = all; all += align256(pic[files[rk[j]]]); }
+			for (int q = 0; q < nrs; q++) { qoff[q] = all; all += align256(pic[files[rk[rsj[q]]]]); }
+			for (int q = 0; q < nrs; q++) {
+				const int f = files[rk[rsj[q]]];
+				roff[q] = all;
+				if (plans[f].reduced) all += align256((size_t)rdp[f].out_w * rdp[f].out_h * plans[f].channels);
+			}
 			TK(grow_dev(&t->rs_dev, all));
 			TK(grow_host(&t->rs_host, up));
 			uint8_t *rd = (uint8_t*)t->rs_dev.p, *rh = (uint8_t*)t->rs_host.p;
 			QsResizeDesc *desc = (QsResizeDesc*)rh;
-			for (int j = 0; j < nr; j++) {
-				const int f = files[rk[j]];
+			QsReduceDesc *rdesc = (QsReduceDesc*)(rh + rdo);
+			int nq = 0;
+			for (int q = 0; q < nrs; q++) {
+				const int j = rsj[q], f = files[rk[j]];
 				const QsResizePlan &r = rsp[f];
-				qs_resize_desc(r, plans[f].pic_w, plans[f].channels, layout == JPEGQS_RENDER_CHW, desc[j]);
-				memcpy(rh + toff[j], r.tab.data(), r.tab.size() * sizeof(int32_t));
-				desc[j].src = rd + qoff[j]; desc[j].mid = rd + moff[j]; desc[j].out = outs[j];
-				desc[j].tab = (const int32_t*)(rd + toff[j]);
-				outs[j] = rd + qoff[j];
+				const QsPlan &p = plans[f];
+				qs_resize_desc(r, p.reduced ? rdp[f].out_w : p.pic_w, p.channels, layout == JPEGQS_RENDER_CHW, desc[q]);
+				memcpy(rh + toff[q], r.tab.data(), r.tab.size() * sizeof(int32_t));
+				desc[q].src = rd + (p.reduced ? roff[q] : qoff[q]); desc[q].mid = rd + moff[q]; desc[q].out = outs[j];
+				desc[q].tab = (const int32_t*)(rd + toff[q]);
+				if (p.reduced) {
+					qs_reduce_desc(rdp[f], p.pic_w, p.channels, rdesc[nq]);
+					rdesc[nq].src = rd + qoff[q]; rdesc[nq].out = rd + roff[q];
+					nq++;
+				}
+				outs[j] = rd + qoff[q];
 			}
-			qs_resize_number(desc, nr, &hblocks, &vblocks);
+			qs_resize_number(desc, nrs, &hblocks, &vblocks);
+			rblocks = qs_reduce_number(rdesc, nrd);
 			TK(cudaMemcpyAsync(rd, rh, up, cudaMemcpyHostToDevice, st));
 		}
 		if (ms) {
@@ -841,9 +915,14 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 		if (ms < nr) TK(cudaMemsetAsync(run + ms, 0, (size_t)(nr - ms) * sizeof(jpegqs_cuda_status), st));
 		std::vector<int32_t> ro(nr), rcs(nr);
 		for (int j = 0; j < nr; j++) { ro[j] = plans[files[rk[j]]].orient; rcs[j] = plans[files[rk[j]]].scan.jpeg_color_space; }
-		if (nr) TQ(qs_render_images(ctx, nr, rimg.data(), run, boxes ? JPEGQS_RENDER_HWC : layout, 1, scale_denom, ro.data(),
-				outs.data(), st, mode, mode ? rcs.data() : NULL));
-		if (boxes && nr) TK(qs_launch_resize((const QsResizeDesc*)t->rs_dev.p, nr, hblocks, vblocks, st));
+		for (int j0 = 0, j1; j0 < nr; j0 = j1) {
+			const QsPlan &p0 = plans[files[rk[j0]]];
+			for (j1 = j0 + 1; j1 < nr && rkey(plans[files[rk[j1]]]) == rkey(p0); j1++) {}
+			TQ(qs_render_images(ctx, j1 - j0, rimg.data() + j0, run + j0, p0.resized ? JPEGQS_RENDER_HWC : layout, 1, p0.scale,
+					ro.data() + j0, outs.data() + j0, st, mode, mode ? rcs.data() + j0 : NULL));
+		}
+		if (nrd) TK(qs_launch_reduce((const QsReduceDesc*)((uint8_t*)t->rs_dev.p + rdo), nrd, rblocks, st));
+		if (nrs) TK(qs_launch_resize((const QsResizeDesc*)t->rs_dev.p, nrs, hblocks, vblocks, st));
 		/* JPEG: compress_async over the pictures into the slots, then the packing kernel into the
 		 * workspace, its records back */
 		uint8_t *jd = (uint8_t*)t->jp_dev.p, *jh = (uint8_t*)t->jp_host.p;
@@ -945,10 +1024,29 @@ static int mode_ok(jpegqs_cuda_ctx *ctx, const char *who, int mode) {
 	return 0;
 }
 
+/* reducing_gap and thumbnail's checks: gap 0 (None) or finite and at least 1; with thumbnail, boxes that
+ * hold only bounds and scale_denom 1 */
+static int reduced_ok(jpegqs_cuda_ctx *ctx, const char *who, int n, const jpegqs_cuda_resize_box *boxes, int scale_denom,
+		int thumbnail, double gap) {
+	char msg[200];
+	const char *bad = !(gap == 0.0 || (isfinite(gap) && gap >= 1.0)) ? "reducing_gap must be 0 (None) or a finite value of at least 1.0" :
+			thumbnail != 0 && thumbnail != 1 ? "thumbnail must be 0 or 1" :
+			thumbnail && !boxes ? "boxes NULL" : thumbnail && scale_denom != 1 ? "scale_denom must be 1 with thumbnail" : NULL;
+	for (int i = 0; i < n && !bad && thumbnail; i++)
+		if (boxes[i].left || boxes[i].top || boxes[i].right || boxes[i].bottom) {
+			snprintf(msg, sizeof(msg), "%s: file %d: a thumbnail box has no crop (left..bottom must be 0)", who, i);
+			qs_ctx_decode_done(ctx, 0, msg); return 0;
+		}
+	if (!bad) return 1;
+	snprintf(msg, sizeof(msg), "%s: %s", who, bad);
+	qs_ctx_decode_done(ctx, 0, msg);
+	return 0;
+}
+
 static int pixels_entry(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint8_t *const *data, const size_t *len,
 		int flags, int niter, int layout, int scale_denom, int resize, int filter, const jpegqs_cuda_resize_box *boxes,
 		int out_on_device, uint8_t *const *out, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results,
-		const int32_t *orientation = NULL, int mode = JPEGQS_PIXELS_AS_FILE) {
+		const int32_t *orientation = NULL, int mode = JPEGQS_PIXELS_AS_FILE, int thumbnail = 0, double gap = 0.0) {
 	char msg[200];
 	if (!ctx) return JPEGQS_ERR_ARG;
 	if (n < 0) { snprintf(msg, sizeof(msg), "%s: negative file count", who); qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG; }
@@ -976,10 +1074,20 @@ static int pixels_entry(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 			qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG;
 		}
 	}
-	if (!orientation_ok(ctx, who, n, orientation) || !mode_ok(ctx, who, mode)) return JPEGQS_ERR_ARG;
+	if (!orientation_ok(ctx, who, n, orientation) || !mode_ok(ctx, who, mode) ||
+			!reduced_ok(ctx, who, n, boxes, scale_denom, thumbnail, gap)) return JPEGQS_ERR_ARG;
 	for (int i = 0; i < n; i++) { memset(&results[i], 0, sizeof(results[i])); results[i].reason = ""; rc[i] = 0; }
 	return pixels_batch(ctx, who, n, data, len, flags, niter, layout, scale_denom, filter, resize ? boxes : NULL, orientation,
-			mode, out_on_device, out, max_device_bytes, rc, results);
+			mode, out_on_device, out, max_device_bytes, rc, results, NULL, NULL, NULL, thumbnail, gap);
+}
+
+extern "C" int jpegqs_cuda_pixels_batch_reduced(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int layout, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
+		const int32_t *orientation, int mode, int out_on_device, uint8_t *const *out, size_t max_device_bytes, int *rc,
+		jpegqs_cuda_pixels_result *results, int thumbnail, double reducing_gap) {
+	return pixels_entry(ctx, "jpegqs_cuda_pixels_batch_reduced", n, data, len, flags, niter, layout, scale_denom,
+			boxes != NULL, filter, boxes, out_on_device, out, max_device_bytes, rc, results, orientation, mode, thumbnail,
+			reducing_gap);
 }
 
 extern "C" int jpegqs_cuda_pixels_batch_mode(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
@@ -1008,7 +1116,7 @@ extern "C" int jpegqs_cuda_pixels_batch_resized(jpegqs_cuda_ctx *ctx, int n, con
 static int pixels_jpeg_entry(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint8_t *const *data, const size_t *len,
 		int flags, int niter, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
 		const jpegqs_cuda_jpeg_params *params, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results,
-		uint8_t **out, size_t *out_len, const int32_t *orientation, int mode) {
+		uint8_t **out, size_t *out_len, const int32_t *orientation, int mode, int thumbnail = 0, double gap = 0.0) {
 	char msg[200];
 	if (!ctx) return JPEGQS_ERR_ARG;
 	if (n < 0) { snprintf(msg, sizeof(msg), "%s: negative file count", who); qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG; }
@@ -1038,10 +1146,19 @@ static int pixels_jpeg_entry(jpegqs_cuda_ctx *ctx, const char *who, int n, const
 			qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG;
 		}
 	}
-	if (!orientation_ok(ctx, who, n, orientation) || !mode_ok(ctx, who, mode)) return JPEGQS_ERR_ARG;
+	if (!orientation_ok(ctx, who, n, orientation) || !mode_ok(ctx, who, mode) ||
+			!reduced_ok(ctx, who, n, boxes, scale_denom, thumbnail, gap)) return JPEGQS_ERR_ARG;
 	for (int i = 0; i < n; i++) { memset(&results[i], 0, sizeof(results[i])); results[i].reason = ""; rc[i] = 0; out[i] = NULL; out_len[i] = 0; }
 	return pixels_batch(ctx, who, n, data, len, flags, niter, JPEGQS_RENDER_HWC, scale_denom, filter, boxes, orientation, mode, 0, NULL,
-			max_device_bytes, rc, results, params, out, out_len);
+			max_device_bytes, rc, results, params, out, out_len, thumbnail, gap);
+}
+
+extern "C" int jpegqs_cuda_pixels_batch_jpeg_reduced(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
+		const jpegqs_cuda_jpeg_params *params, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results,
+		uint8_t **out, size_t *out_len, const int32_t *orientation, int mode, int thumbnail, double reducing_gap) {
+	return pixels_jpeg_entry(ctx, "jpegqs_cuda_pixels_batch_jpeg_reduced", n, data, len, flags, niter, scale_denom, filter, boxes,
+			params, max_device_bytes, rc, results, out, out_len, orientation, mode, thumbnail, reducing_gap);
 }
 
 extern "C" int jpegqs_cuda_pixels_batch_jpeg(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,

@@ -9,6 +9,7 @@ There is no CPU fallback: a missing library or device raises QsError.
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 from typing import List, Optional, Sequence
 
@@ -283,6 +284,23 @@ def load():
                                                        C.POINTER(C.c_int), C.POINTER(_PixelsResult),
                                                        C.POINTER(C.c_void_p), C.POINTER(C.c_size_t),
                                                        C.POINTER(C.c_int32), C.c_int]
+    lib.jpegqs_cuda_thumbnail_geometry.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_int,
+                                                   C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]
+    lib.jpegqs_cuda_pixels_batch_reduced.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_size_t),
+                                                     C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(_ResizeBox),
+                                                     C.POINTER(C.c_int32), C.c_int, C.c_int, C.POINTER(C.c_void_p),
+                                                     C.c_size_t, C.POINTER(C.c_int), C.POINTER(_PixelsResult), C.c_int,
+                                                     C.c_double]
+    lib.jpegqs_cuda_pixels_batch_jpeg_reduced.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_char_p),
+                                                          C.POINTER(C.c_size_t), C.c_int, C.c_int, C.c_int, C.c_int,
+                                                          C.POINTER(_ResizeBox), C.POINTER(_JpegParams), C.c_size_t,
+                                                          C.POINTER(C.c_int), C.POINTER(_PixelsResult),
+                                                          C.POINTER(C.c_void_p), C.POINTER(C.c_size_t),
+                                                          C.POINTER(C.c_int32), C.c_int, C.c_int, C.c_double]
+    lib.jpegqs_cuda_reduce_model.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                             C.POINTER(C.c_int32), C.c_void_p]
+    lib.jpegqs_cuda_resize_model_box.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                                 C.POINTER(C.c_double), C.c_int, C.c_int, C.c_double, C.c_void_p]
     lib.jpegqs_cuda_tables.argtypes = [C.c_int, C.c_void_p]
     lib.jpegqs_cuda_orig_coef.argtypes = [C.c_int, C.c_int]
     _lib = lib
@@ -418,6 +436,132 @@ def _resize_box(pw: int, ph: int, size, crop, i: int, who: str) -> _ResizeBox:
         raise ValueError(f"{who}: file {i}: crop {crop!r} outside the {pw} x {ph} picture")
     w, h = size if size is not None else (right - left, bottom - top)
     return _ResizeBox(left, top, right, bottom, w, h)
+
+
+class _GapDefault:
+    """reducing_gap's default: Pillow's, 2.0 for thumbnail and None for size"""
+
+    def __repr__(self):
+        return "<Pillow's default>"
+
+
+_GAP_DEFAULT = _GapDefault()
+
+
+def _reducing_gap(gap, thumbnail: bool, who: str) -> float:
+    """the C value of reducing_gap: 0.0 for None, else a finite value >= 1.0; the default is Pillow's"""
+    if gap is _GAP_DEFAULT:
+        return 2.0 if thumbnail else 0.0
+    if gap is None:
+        return 0.0
+    if isinstance(gap, bool) or not isinstance(gap, (int, float, np.integer, np.floating)) or \
+            not math.isfinite(float(gap)) or float(gap) < 1.0:
+        raise ValueError(f"{who}: reducing_gap {gap!r}: expected None or a finite number of at least 1.0")
+    return float(gap)
+
+
+def _thumbnail_bounds(n: int, bound, who: str):
+    """per file, a thumbnail bound (width, height), each 1..65535; ValueError names the file index"""
+    def one(v, i):
+        t = _int_tuple(v, 2)
+        if t is None or not (1 <= t[0] <= 65535 and 1 <= t[1] <= 65535):
+            raise ValueError(f"{who}: file {i}: thumbnail {v!r}: expected (width, height), each in 1..65535")
+        return t
+    if _int_tuple(bound, 2) is not None:
+        return [one(bound, i) for i in range(n)]
+    if isinstance(bound, (list, tuple)) and len(bound) == n:
+        return [one(v, i) for i, v in enumerate(bound)]
+    raise ValueError(f"{who}: thumbnail must be (width, height) or a list of {n} of them")
+
+
+def thumbnail_geometry(width: int, height: int, bound, reducing_gap=2.0, loaded: bool = False):
+    """Pillow's Image.thumbnail(bound, reducing_gap=reducing_gap) of a width x height JPEG file, host-only
+    (jpegqs_cuda_thumbnail_geometry): (scale_denom, (out_width, out_height)).  scale_denom is the draft's
+    libjpeg scale (1 when the bound covers the picture, for reducing_gap None, or loaded: the picture was
+    decoded before, as exif_transpose and convert do); the size is the thumbnail's.  ValueError for a bad
+    argument."""
+    (bw, bh), = _thumbnail_bounds(1, bound, "thumbnail_geometry")
+    gap = _reducing_gap(reducing_gap, True, "thumbnail_geometry")
+    lib = load()
+    s, w, h = C.c_int(), C.c_int(), C.c_int()
+    if lib.jpegqs_cuda_thumbnail_geometry(int(width), int(height), bw, bh, gap, int(bool(loaded)), C.byref(s), C.byref(w),
+                                          C.byref(h)) < 0:
+        raise ValueError(f"thumbnail_geometry: {lib.jpegqs_cuda_last_error(None).decode()}")
+    return s.value, (w.value, h.value)
+
+
+def _host_pixels(pixels, who: str):
+    a = np.asarray(pixels)
+    if a.dtype != np.uint8 or a.ndim not in (2, 3) or (a.ndim == 3 and a.shape[2] not in (1, 3)) or 0 in a.shape:
+        raise ValueError(f"{who}: pixels must be uint8 [H, W] or [H, W, 1|3], not {a.dtype} {a.shape}")
+    return np.ascontiguousarray(a), (1 if a.ndim == 2 else a.shape[2])
+
+
+def reduce_model(pixels, factor, box=None):
+    """The device reduce on one CPU thread (jpegqs_cuda_reduce_model): byte for byte Pillow's
+    Image.fromarray(pixels).reduce(factor, box).  pixels: uint8 [H, W] or [H, W, 1|3]; factor an int or
+    (fx, fy); box (left, top, right, bottom) ints or None.  Returns [ceil(bh / fy), ceil(bw / fx)(, C)]."""
+    a, c = _host_pixels(pixels, "reduce_model")
+    f = _int_tuple((factor, factor) if _orient_int(factor) is not None else factor, 2)
+    if f is None:
+        raise ValueError(f"reduce_model: factor {factor!r}: expected an int or (fx, fy)")
+    h, w = a.shape[:2]
+    b = (0, 0, w, h) if box is None else _int_tuple(box, 4)
+    if b is None:
+        raise ValueError(f"reduce_model: box {box!r}: expected (left, top, right, bottom) ints")
+    ow, oh = -(-(b[2] - b[0]) // max(f[0], 1)), -(-(b[3] - b[1]) // max(f[1], 1))
+    out = np.zeros((max(oh, 0), max(ow, 0), c), dtype=np.uint8)
+    lib = load()
+    rc = lib.jpegqs_cuda_reduce_model(a.ctypes.data, w, h, c, f[0], f[1], (C.c_int32 * 4)(*b), out.ctypes.data)
+    if rc < 0:
+        raise ValueError(f"reduce_model: {lib.jpegqs_cuda_last_error(None).decode()} ({rc})")
+    return out.reshape(oh, ow) if a.ndim == 2 else out
+
+
+def resize_model_box(pixels, size, box=None, filter="bicubic", reducing_gap=None, layout: str = "hwc"):
+    """The device reduce and resize on one CPU thread, planned as the batch plans them
+    (jpegqs_cuda_resize_model_box): byte for byte Pillow's Image.fromarray(pixels).resize(size, filter,
+    box=box, reducing_gap=reducing_gap), box (left, top, right, bottom) floats or None.  Returns
+    [height, width] for a 2-D input, else [height, width, C] ("hwc") or [C, height, width] ("chw")."""
+    if layout not in ("hwc", "chw"):
+        raise ValueError(f"resize_model_box: layout {layout!r}: expected 'hwc' or 'chw'")
+    a, c = _host_pixels(pixels, "resize_model_box")
+    fcode = _resize_filter(filter, "resize_model_box")
+    sz = _int_tuple(size, 2)
+    if sz is None:
+        raise ValueError(f"resize_model_box: size {size!r}: expected (width, height)")
+    gap = _reducing_gap(reducing_gap, False, "resize_model_box")
+    h, w = a.shape[:2]
+    cbox = None
+    if box is not None:
+        if isinstance(box, (str, bytes)) or not hasattr(box, "__len__") or len(box) != 4:
+            raise ValueError(f"resize_model_box: box {box!r}: expected (left, top, right, bottom)")
+        cbox = (C.c_double * 4)(*[float(v) for v in box])
+    shape = (max(sz[1], 0), max(sz[0], 0), c) if layout == "hwc" else (c, max(sz[1], 0), max(sz[0], 0))
+    out = np.zeros(shape, dtype=np.uint8)
+    lib = load()
+    rc = lib.jpegqs_cuda_resize_model_box(a.ctypes.data, w, h, c, 0 if layout == "hwc" else 1, fcode, cbox, sz[0], sz[1],
+                                          gap, out.ctypes.data)
+    if rc < 0:
+        raise ValueError(f"resize_model_box: {lib.jpegqs_cuda_last_error(None).decode()} ({rc})")
+    return out.reshape(sz[1], sz[0]) if a.ndim == 2 else out
+
+
+def thumbnail_model(pixels, full_size, bound, filter="bicubic", reducing_gap=2.0, loaded: bool = False):
+    """Pillow's Image.thumbnail(bound, filter, reducing_gap) on one CPU thread, with the batch's planning:
+    pixels is the picture thumbnail_geometry(W, H, bound, reducing_gap, loaded)'s draft gives, the
+    W x H = full_size file at 1/scale_denom ([ceil(H / s), ceil(W / s)(, C)], as render_model gives it).
+    Returns the thumbnail's pixels."""
+    a, _ = _host_pixels(pixels, "thumbnail_model")
+    W, H = (int(v) for v in full_size)
+    s, (tw, th) = thumbnail_geometry(W, H, bound, reducing_gap, loaded)
+    if a.shape[:2] != (-(-H // s), -(-W // s)):
+        raise ValueError(f"thumbnail_model: pixels {a.shape[:2]}: expected the 1/{s} picture of {W} x {H}")
+    if a.shape[:2] == (th, tw):
+        return a.copy()
+    gap = _reducing_gap(reducing_gap, True, "thumbnail_model")
+    box = (0.0, 0.0, W / s, H / s) if gap and not loaded else None
+    return resize_model_box(a, (tw, th), box, filter, gap or None)
 
 
 def _fill_image(ci: _Image, image: CoefImage, coef_ptrs: Sequence[int], up_ptrs: Sequence[Optional[int]]):
@@ -1041,7 +1185,7 @@ class QsContext:
 
     def decode_pixels(self, datas, flags: int, niter: int, layout: str = "hwc", device: str = "cuda",
                       max_device_bytes: int = 0, scale_denom: int = 1, size=None, crop=None, filter="bicubic",
-                      orientation=None, mode=None):
+                      orientation=None, mode=None, thumbnail=None, reducing_gap=_GAP_DEFAULT):
         """Many JPEG files to the smoothed pixels the jpegqs tool's --ppm writes for them (islow, fancy
         up-sampling, after do_quantsmooth(flags, niter)), in shared launches (jpegqs_cuda_pixels_batch).
         Returns, in the order of datas, one record per file:
@@ -1072,7 +1216,15 @@ class QsContext:
         5..8 the unresized pixels have width and height swapped.  ValueError for a bad value or length.
         mode: None (the file's own colour, as above), "RGB" or "L": Pillow's Image.convert(mode) of each
         file's picture, before the crop and the resize, so C is 3 or 1 for every file, and CMYK and YCCK
-        files are decoded too (jpegqs_cuda_pixels_batch_mode).  ValueError for any other value."""
+        files are decoded too (jpegqs_cuda_pixels_batch_mode).  ValueError for any other value.
+        thumbnail: (width, height), or one per file: Pillow's Image.open(F) [exif_transpose] [convert(mode)]
+        .thumbnail(bound, filter, reducing_gap) of the file F jpegqs writes (jpegqs_cuda_pixels_batch_reduced):
+        each file is decoded at its own draft scale, reduced and resized as Pillow does; pixels are
+        thumbnail_geometry's size.  An orientation (any value, 1 included) or a mode loads the picture
+        first, as exif_transpose and convert do, so there is no draft.  reducing_gap: Pillow's, default 2.0 with thumbnail and None with size
+        (an explicit None is None in both); with size, Image.resize(size, filter, reducing_gap=) of the
+        crop.  ValueError naming the file for a bad bound, for thumbnail with size, crop or scale_denom
+        other than 1, or for a reducing_gap below 1.0, before anything runs."""
         if isinstance(datas, (bytes, bytearray, memoryview, str)) or not hasattr(datas, "__len__"):
             raise TypeError("decode_pixels: datas must be a sequence of bytes-like files")
         files = [_file_bytes(d, f"decode_pixels: file {i}") for i, d in enumerate(datas)]
@@ -1090,6 +1242,11 @@ class QsContext:
             sizes, crops = _resize_boxes(n, size, crop, "decode_pixels")
         orient = _orientations(orientation, n, "decode_pixels")
         m = _mode(mode, "decode_pixels")
+        bounds = self._thumbnail_args(n, thumbnail, resize, scale, "decode_pixels")
+        # reducing_gap acts only in a resize
+        gap = _reducing_gap(reducing_gap, bounds is not None, "decode_pixels") if resize or bounds is not None else 0.0
+        if bounds is not None:
+            fcode = _resize_filter(filter, "decode_pixels")
         if not n:
             return []
         # the output size rule of jpegqs_cuda_pixels_batch: transcode_route's width, height and ncomp
@@ -1106,7 +1263,11 @@ class QsContext:
         if orient is not None:
             orient = [exif_orientation(d) if o == 0 else o for d, o in zip(files, orient)]
             shapes = [_oriented_shape(s, o, layout) for s, o in zip(shapes, orient)]
-        if resize:
+        if bounds is not None:
+            boxes = self._thumbnail_boxes(shapes, bounds, layout, gap, orient is not None or m != 0)
+            shapes = [s for s, _ in boxes]
+            boxes = (_ResizeBox * n)(*[b for _, b in boxes])
+        elif resize:
             boxes = (_ResizeBox * n)()
             for i, s in enumerate(shapes):
                 ph, pw = (s[0], s[1]) if layout == "hwc" else (s[1], s[2])
@@ -1126,7 +1287,13 @@ class QsContext:
         optrs = (C.c_void_p * n)(*[t.data_ptr() for t in outs])
         rc = (C.c_int * n)()
         res = (_PixelsResult * n)()
-        if m:
+        if bounds is not None or gap:
+            self._check(self.lib.jpegqs_cuda_pixels_batch_reduced(self.h, n, ptrs, lens, int(flags), int(niter),
+                                                                  0 if layout == "hwc" else 1, scale, fcode, boxes,
+                                                                  None if orient is None else (C.c_int32 * n)(*orient),
+                                                                  m, int(device == "cuda"), optrs, int(max_device_bytes),
+                                                                  rc, res, int(bounds is not None), gap))
+        elif m:
             self._check(self.lib.jpegqs_cuda_pixels_batch_mode(self.h, n, ptrs, lens, int(flags), int(niter),
                                                                0 if layout == "hwc" else 1, scale,
                                                                fcode if resize else 0, boxes if resize else None,
@@ -1160,6 +1327,29 @@ class QsContext:
                               "sampling ratios only")
         return [(outs[i], res[i].warnings, res[i].host_decoded, res[i].smoothed, res[i].stop, res[i].upsampled,
                  (res[i].reason or b"").decode()) for i in range(n)]
+
+    @staticmethod
+    def _thumbnail_args(n: int, thumbnail, resize: bool, scale: int, who: str):
+        """thumbnail's bounds per file, or None; ValueError with size, crop or scale_denom other than 1"""
+        if thumbnail is None:
+            return None
+        if resize or scale != 1:
+            raise ValueError(f"{who}: thumbnail takes no size, crop or scale_denom (thumbnail scales each file itself)")
+        return _thumbnail_bounds(n, thumbnail, who)
+
+    @staticmethod
+    def _thumbnail_boxes(shapes, bounds, layout: str, gap: float, loaded: bool):
+        """per file, the thumbnail's output shape and its C box (the bound): shapes are the full-size
+        (oriented) pictures', read as thumbnail sees them"""
+        lib = load()
+        out = []
+        for i, (sh, (bw, bh)) in enumerate(zip(shapes, bounds)):
+            h, w, c = sh if layout == "hwc" else (sh[1], sh[2], sh[0])
+            s, tw, th = C.c_int(), C.c_int(), C.c_int()
+            if lib.jpegqs_cuda_thumbnail_geometry(w, h, bw, bh, gap, int(loaded), C.byref(s), C.byref(tw), C.byref(th)) < 0:
+                raise ValueError(f"thumbnail: file {i}: {lib.jpegqs_cuda_last_error(None).decode()}")
+            out.append(((th.value, tw.value, c) if layout == "hwc" else (c, th.value, tw.value), _ResizeBox(0, 0, 0, 0, bw, bh)))
+        return out
 
     # ---- whole image, host buffers (the call a user of the reference makes) ----
     def do_quantsmooth(self, image: CoefImage, flags: int, niter: int, progprec: int = 0,
@@ -1739,7 +1929,7 @@ class QsContext:
 
     def reencode(self, datas, flags: int, niter: int, quality=75, subsampling="4:2:0", optimize=False, scale_denom=1,
                  size=None, crop=None, filter="bicubic", max_device_bytes: int = 0, orientation=None, mode=None,
-                 progressive=False):
+                 progressive=False, thumbnail=None, reducing_gap=_GAP_DEFAULT):
         """Many JPEG files to JPEG files of their smoothed pixels (jpegqs_cuda_pixels_batch_jpeg): each
         file's output is exactly Pillow's Image.fromarray(P).save(f, "JPEG", quality=quality,
         subsampling=subsampling, optimize=optimize), where P is the picture decode_pixels gives for the
@@ -1753,7 +1943,9 @@ class QsContext:
         ImageOps.exif_transpose(P).save(...): upright pixels in a JFIF file without the tag.  mode: as for
         decode_pixels (jpegqs_cuda_pixels_batch_jpeg_mode): Pillow's P.convert(mode).save(...), so CMYK
         and YCCK files give RGB files and "L" gives grey files.  progressive=True: Pillow's
-        save(..., progressive=True) instead."""
+        save(..., progressive=True) instead.  thumbnail / reducing_gap: as for decode_pixels
+        (jpegqs_cuda_pixels_batch_jpeg_reduced): Pillow's thumbnail (or resize with reducing_gap), then
+        save."""
         if isinstance(datas, (bytes, bytearray, memoryview, str)) or not hasattr(datas, "__len__"):
             raise TypeError("reencode: datas must be a sequence of bytes-like files")
         files = [_file_bytes(d, f"reencode: file {i}") for i, d in enumerate(datas)]
@@ -1768,12 +1960,16 @@ class QsContext:
             sizes, crops = _resize_boxes(n, size, crop, "reencode")
         orient = _orientations(orientation, n, "reencode")
         m = _mode(mode, "reencode")
+        bounds = self._thumbnail_args(n, thumbnail, resize, scale, "reencode")
+        gap = _reducing_gap(reducing_gap, bounds is not None, "reencode") if resize or bounds is not None else 0.0
         if not n:
             return []
         boxes = None
         if orient is not None:
             orient = [exif_orientation(d) if o == 0 else o for d, o in zip(files, orient)]
-        if resize:
+        if bounds is not None:
+            boxes = (_ResizeBox * n)(*[_ResizeBox(0, 0, 0, 0, bw, bh) for bw, bh in bounds])
+        elif resize:
             boxes = (_ResizeBox * n)()
             for i, d in enumerate(files):
                 info = _FileInfo()
@@ -1788,7 +1984,11 @@ class QsContext:
         res = (_PixelsResult * n)()
         outs = (C.c_void_p * n)()
         olen = (C.c_size_t * n)()
-        if m:
+        if bounds is not None or gap:
+            self._check(self.lib.jpegqs_cuda_pixels_batch_jpeg_reduced(
+                self.h, n, ptrs, lens, int(flags), int(niter), scale, fcode, boxes, C.byref(jp), int(max_device_bytes),
+                rc, res, outs, olen, None if orient is None else (C.c_int32 * n)(*orient), m, int(bounds is not None), gap))
+        elif m:
             self._check(self.lib.jpegqs_cuda_pixels_batch_jpeg_mode(
                 self.h, n, ptrs, lens, int(flags), int(niter), scale, fcode, boxes, C.byref(jp), int(max_device_bytes),
                 rc, res, outs, olen, None if orient is None else (C.c_int32 * n)(*orient), m))
@@ -2084,14 +2284,15 @@ def transcode_batch(datas, flags: int, niter: int, optimize: bool = False, copy:
 
 def decode_pixels(datas, flags: int, niter: int, layout: str = "hwc", device: str = "cuda", max_device_bytes: int = 0,
                   gpu: int = -1, scale_denom: int = 1, size=None, crop=None, filter="bicubic", orientation=None,
-                  mode=None):
+                  mode=None, thumbnail=None, reducing_gap=_GAP_DEFAULT):
     """QsContext.decode_pixels on the default context of CUDA device `gpu`: one record (pixels, warnings,
     host_decoded, smoothed, stop, upsampled, reason) per file, at 1/scale_denom size, cropped and resized
     as Pillow would with size / crop / filter ((width, height) and (left, top, right, bottom), Pillow's
     conventions), turned by `orientation` ("exif", 1..8, or one value 0..8 per file) first and converted by
-    `mode` (None, "RGB" or "L", Pillow's Image.convert) before the crop."""
+    `mode` (None, "RGB" or "L", Pillow's Image.convert) before the crop; or Pillow's thumbnail(bound, filter,
+    reducing_gap) with `thumbnail`."""
     return default_context(gpu).decode_pixels(datas, flags, niter, layout, device, max_device_bytes, scale_denom,
-                                              size, crop, filter, orientation, mode)
+                                              size, crop, filter, orientation, mode, thumbnail, reducing_gap)
 
 
 def compress_async(pixels, quality=75, subsampling="4:2:0", optimize=False, out=None, stream=None, progressive=False):
@@ -2108,9 +2309,10 @@ def compress_async(pixels, quality=75, subsampling="4:2:0", optimize=False, out=
 
 def reencode(datas, flags: int, niter: int, quality=75, subsampling="4:2:0", optimize=False, scale_denom=1, size=None,
              crop=None, filter="bicubic", max_device_bytes: int = 0, gpu: int = -1, orientation=None, mode=None,
-             progressive=False):
+             progressive=False, thumbnail=None, reducing_gap=_GAP_DEFAULT):
     """QsContext.reencode on the default context of CUDA device `gpu`: one record (data, warnings,
     host_decoded, smoothed, stop, upsampled, reason) per file, data the JPEG file Pillow's save writes for
     the picture decode_pixels gives with the same arguments."""
     return default_context(gpu).reencode(datas, flags, niter, quality, subsampling, optimize, scale_denom, size, crop,
-                                         filter, max_device_bytes, orientation, mode, progressive)
+                                         filter, max_device_bytes, orientation, mode, progressive, thumbnail,
+                                         reducing_gap)

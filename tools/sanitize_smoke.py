@@ -172,3 +172,12 @@ for sub in ("4:4:4", "4:2:2", "4:2:0"):
     out, lens, st = ctx.compress_async(pics, 90, sub, progressive=True)
     torch.cuda.synchronize()
     print("compress_async progressive", sub, lens.tolist(), st.tolist(), flush=True)
+
+# thumbnails: files drafted to 1, 2 and 4 in one call, reduce cells with partial right and bottom edges
+# (a loaded picture: orientation given, no draft), and reducing_gap on the crop path
+tfiles = [jpeg(90, 50, quality=75), jpeg(333, 211, quality=85), jpeg(33, 17, "L", quality=100), jpeg(161, 97, quality=90)]
+for o in (None, 6):
+    px = ctx.decode_pixels(tfiles, 3, 1, thumbnail=[(40, 40), (30, 30), (8, 8), (13, 7)], orientation=o)
+    print("decode_pixels thumbnail orientation", o, [tuple(p[0].shape) for p in px], flush=True)
+px = ctx.decode_pixels(tfiles, 3, 1, size=(9, 5), crop=[None, (3, 5, 300, 200), None, (1, 1, 160, 96)], reducing_gap=1.0)
+print("decode_pixels reducing_gap", [tuple(p[0].shape) for p in px], flush=True)
