@@ -1010,6 +1010,67 @@ int jpegqs_cuda_reduce_model(const uint8_t *src, int width, int height, int chan
 int jpegqs_cuda_resize_model_box(const uint8_t *src, int width, int height, int channels, int layout, int filter,
 		const double *box, int out_w, int out_h, double reducing_gap, uint8_t *out);
 
+/* ---- blur and sharpen: Pillow's ImageFilter.BoxBlur, GaussianBlur and UnsharpMask ----------------
+ * Each channel byte is filtered on its own, in 32-bit unsigned integer arithmetic (libImaging BoxBlur.c
+ * and UnsharpMask.c):
+ *   - one box pass of radius R >= 0 along a line of n samples p, with r = (int)R,
+ *     ww = (uint32)(2^24 / (float)(2R + 1)) in float, fw = (2^24 - (2r + 1) ww) / 2 and c(i) the index
+ *     clamped to 0..n-1, gives (sum_{k=-r..r} p[c(x+k)] ww + (p[c(x-r-1)] + p[c(x+r+1)]) fw + 2^23) >> 24;
+ *     every pass stores 8-bit samples;
+ *   - BOX_BLUR (radius_x, radius_y): one pass along every row with radius_x, then one along every column
+ *     with radius_y; an axis of radius 0 is skipped.  A negative radius is refused.
+ *   - GAUSSIAN_BLUR (radius_x, radius_y): three row passes, then three column passes, with the box radius
+ *     g(s) Pillow derives from the standard deviation s in float (sigma2 = s s / 3,
+ *     L = sqrt(12 sigma2 + 1), l = floor((L - 1) / 2), g = l + (2l + 1)(l (l + 1) - 3 sigma2) /
+ *     (6 (sigma2 - (l + 1)^2))); g(0) = 0 skips the axis, and a negative s acts as |s|.
+ *   - UNSHARP_MASK (radius_x = radius_y = radius, percent, threshold): b = GAUSSIAN_BLUR(radius) of the
+ *     input; per byte d = in - b, and the output is clamp(in + d * percent / 100, 0, 255) (C's truncating
+ *     division) where |d| > threshold, else in.
+ * Refused, because Pillow's 32-bit arithmetic would overflow: a radius (either axis, any kind) that is
+ * not finite or whose magnitude is above JPEGQS_FILTER_MAX_RADIUS, and |percent| above
+ * JPEGQS_FILTER_MAX_PERCENT (|d * percent| reaches 2^31).  percent and threshold are ignored by the
+ * blurs. */
+#define JPEGQS_FILTER_BOX_BLUR       1
+#define JPEGQS_FILTER_GAUSSIAN_BLUR  2
+#define JPEGQS_FILTER_UNSHARP_MASK   3
+#define JPEGQS_FILTER_MAX_RADIUS     65535.0f
+#define JPEGQS_FILTER_MAX_PERCENT    8421504
+typedef struct jpegqs_cuda_image_filter {
+	int32_t kind;                      /* JPEGQS_FILTER_* */
+	float radius_x, radius_y;
+	int32_t percent, threshold;        /* UNSHARP_MASK */
+} jpegqs_cuda_image_filter;
+
+/* jpegqs_cuda_pixels_batch_reduced, then filters[0..nfilters) applied in order to every file's picture:
+ * file i is Pillow's [crop().resize() | thumbnail()].filter(F1).filter(F2)... of the picture the reduced
+ * call gives.  The filter is the last stage: the earlier ones write HWC into the context's buffers and the
+ * last filter pass writes out[i] in the caller's layout.  Per sub-batch and filter: one row launch over
+ * the files whose rows (width x channels bytes) are at most 16384 bytes (every row pass fused in
+ * shared memory), one launch per row pass over the wider ones, one launch per column pass over all.  The
+ * budget counts three pictures of scratch per file.  nfilters 0 is byte for byte the reduced call.
+ *   - Return.  As the reduced call's; also JPEGQS_ERR_ARG with nothing done for filters NULL with
+ *     nfilters > 0, nfilters outside 0..64, or a filter refused above. */
+int jpegqs_cuda_pixels_batch_filtered(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int layout, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
+		const int32_t *orientation, int mode, int out_on_device, uint8_t *const *out, size_t max_device_bytes, int *rc,
+		jpegqs_cuda_pixels_result *results, int thumbnail, double reducing_gap, const jpegqs_cuda_image_filter *filters,
+		int nfilters);
+
+/* jpegqs_cuda_pixels_batch_jpeg_reduced with filters as for pixels_batch_filtered: the filtered picture is
+ * saved.  nfilters 0 is byte for byte the reduced call. */
+int jpegqs_cuda_pixels_batch_jpeg_filtered(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
+		const jpegqs_cuda_jpeg_params *params, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results,
+		uint8_t **out, size_t *out_len, const int32_t *orientation, int mode, int thumbnail, double reducing_gap,
+		const jpegqs_cuda_image_filter *filters, int nfilters);
+
+/* The filters of pixels_batch_filtered on the calling thread (host-only), through the same per-sample
+ * functions and pass plan: filters[0..nfilters) applied in order to a width x height x channels HWC
+ * picture (channels 1 or 3) into out (the same size, HWC; it may not overlap src).  Returns 0 or
+ * JPEGQS_ERR_ARG (NULL pointer, bad size or channels, the refusals above). */
+int jpegqs_cuda_image_filter_model(const uint8_t *src, int width, int height, int channels,
+		const jpegqs_cuda_image_filter *filters, int nfilters, uint8_t *out);
+
 /* ---- one image sharded by MCU rows over several GPUs (SURVEY.md 8e) ----------------------
  * Every rank - a device of this process, or another process on the same box - smooths one slab
  * of contiguous MCU rows and exchanges ONE pixel row per plane with each neighbour after every

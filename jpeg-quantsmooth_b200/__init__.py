@@ -45,7 +45,7 @@ def __getattr__(name):
                 "parse_jpeg_scans", "decode_scans_async", "decode_scans_workspace_bytes", "decode_scans_model",
                 "transcode_route", "transcode", "transcode_batch", "decode_pixels", "render_model", "resize_model",
                 "compress_model", "compress_bound", "compress_async", "reencode", "exif_orientation",
-                "thumbnail_geometry", "thumbnail_model", "reduce_model", "resize_model_box"):
+                "thumbnail_geometry", "thumbnail_model", "reduce_model", "resize_model_box", "image_filter_model"):
         import importlib
         _cuda = importlib.import_module(__name__ + ".cuda")
         if name == "cuda":

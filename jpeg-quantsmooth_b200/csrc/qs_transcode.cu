@@ -8,7 +8,8 @@
  * jpegqs_cuda_pixels_batch: the same files to the smoothed pixels the tool's --ppm writes, through
  * the same plans, sub-batches and decoder launches, the host reader, run_async and the fused render;
  * jpegqs_cuda_pixels_batch_resized adds qs_resize.cu's crop and resize after the render, and
- * jpegqs_cuda_pixels_batch_reduced qs_reduce.cu's reduce before the resize, and thumbnail's own scales.
+ * jpegqs_cuda_pixels_batch_reduced qs_reduce.cu's reduce before the resize, and thumbnail's own scales;
+ * jpegqs_cuda_pixels_batch_filtered qs_filter.cu's blurs after every other stage.
  */
 #include <cuda_runtime.h>
 #include <math.h>
@@ -20,6 +21,7 @@
 #include "qs_common.h"
 #include "qs_resize.h"
 #include "qs_reduce.h"
+#include "qs_filter.h"
 
 /* include/libjpegqs.h's JPEGQS_FLAGS_MASK and JPEGQS_ITER_MAX (that header needs <jpeglib.h>) */
 #define QS_FLAGS_MASK 0x7f
@@ -132,6 +134,8 @@ struct QsTranscode {
 	QsBuf jp_dev, jp_host;                     /* JPEG outputs: packing descriptors, lengths, statuses, records
 	                                              and the encoder's output slots; the staging of descriptors
 	                                              and records */
+	QsBuf ft_dev, ft_host;                     /* filtered pixels: descriptors, then each file's picture before
+	                                              the filter and two scratch pictures; the descriptors' staging */
 	cudaEvent_t ev0, ev1;                      /* around run_async: jpegqs_cuda_last_device_ms */
 	int sms;
 	jpegqs_cuda_scan_rec recs[JPEGQS_MAX_SCANS];
@@ -144,7 +148,8 @@ void qs_transcode_release(void *state) {
 	QsTranscode *t = (QsTranscode*)state;
 	if (!t) return;
 	cudaFree(t->in_dev.p); cudaFree(t->coef_dev.p); cudaFree(t->ws_dev.p); cudaFree(t->out_dev.p); cudaFree(t->stat_dev.p);
-	cudaFree(t->hcoef_dev.p); cudaFree(t->rs_dev.p); cudaFree(t->jp_dev.p);
+	cudaFree(t->hcoef_dev.p); cudaFree(t->rs_dev.p); cudaFree(t->jp_dev.p); cudaFree(t->ft_dev.p);
+	if (t->ft_host.p) cudaFreeHost(t->ft_host.p);
 	if (t->jp_host.p) cudaFreeHost(t->jp_host.p);
 	if (t->in_host.p) cudaFreeHost(t->in_host.p);
 	if (t->out_host.p) cudaFreeHost(t->out_host.p);
@@ -274,7 +279,7 @@ static cudaError_t batch_budget(const QsTranscode *t, size_t max_device_bytes, s
 	size_t fr = 0, tot = 0;
 	cudaError_t e = cudaMemGetInfo(&fr, &tot);
 	*budget = (fr + t->in_dev.cap + t->coef_dev.cap + t->ws_dev.cap + t->out_dev.cap + t->stat_dev.cap + t->hcoef_dev.cap +
-			t->rs_dev.cap + t->jp_dev.cap) / 2;
+			t->rs_dev.cap + t->jp_dev.cap + t->ft_dev.cap) / 2;
 	return e;
 }
 
@@ -621,12 +626,15 @@ static const char *crop_of(const jpegqs_cuda_resize_box &b, int pw, int ph, int 
  * and the compressor then take as it is.  mode: JPEGQS_PIXELS_*; the render converts, so every later stage
  * takes the converted picture's channels.  gap > 0: Pillow's reducing_gap, a reduce (qs_reduce.cu) before
  * the resize where its factor is above 1.  thumbnail: boxes hold bounds, each file is rendered at its
- * own draft scale and goes through the reduce and the resize only where Pillow's thumbnail does. */
+ * own draft scale and goes through the reduce and the resize only where Pillow's thumbnail does.
+ * nfilters > 0: the earlier stages write each picture HWC into ft_dev, and filters (qs_filter.cu) take it
+ * from there to the destination. */
 static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint8_t *const *data, const size_t *len,
 		int flags, int niter, int layout, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
 		const int32_t *orientation, int mode, int on_device, uint8_t *const *out, size_t max_device_bytes, int *rc,
 		jpegqs_cuda_pixels_result *results, const jpegqs_cuda_jpeg_params *jp = NULL, uint8_t **jout = NULL,
-		size_t *jlen = NULL, int thumbnail = 0, double gap = 0.0) {
+		size_t *jlen = NULL, int thumbnail = 0, double gap = 0.0, const jpegqs_cuda_image_filter *filters = NULL,
+		int nfilters = 0) {
 	char msg[512];
 	cudaStream_t st;
 	std::vector<QsPlan> plans((size_t)n);
@@ -711,6 +719,8 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 					align256(rsp[i].tab.size() * sizeof(int32_t)) + align256(sizeof(QsResizeDesc));
 		if (p.reduced)
 			p.fixed += align256((size_t)rdp[i].out_w * rdp[i].out_h * p.channels) + align256(sizeof(QsReduceDesc));
+		/* filtered: the picture before the filter, two scratch pictures and the pass descriptors */
+		if (nfilters) p.fixed += 3 * align256(p.pix) + sizeof(QsFilterDesc) * QS_FILTER_MAX_STEPS * (size_t)nfilters;
 		p.ws_enc = 0; p.packed = 0;
 		if (jp) {
 			/* JPEG: the compressor's workspace share (coefficients and encoder workspace, with the prefix's
@@ -834,7 +844,7 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 		 * 4-component files) */
 		std::vector<int> rk;                           /* render order -> group position */
 		static const int kinds[6] = {3, 1, 4, 4, 1, 3};
-		auto rkey = [&](const QsPlan &p) { return p.scale * 2 + (p.resized ? JPEGQS_RENDER_HWC : layout); };
+		auto rkey = [&](const QsPlan &p) { return p.scale * 2 + (p.resized || nfilters ? JPEGQS_RENDER_HWC : layout); };
 		for (int pass = 0; pass < 6; pass += 3)
 			for (int key = 2; key <= 17; key++)
 				for (int q = pass; q < pass + 3; q++)
@@ -856,6 +866,29 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 		jpegqs_cuda_status *run = (jpegqs_cuda_status*)t->out_dev.p;
 		std::vector<uint8_t*> outs(nr);
 		for (int j = 0; j < nr; j++) outs[j] = on_device ? out[files[rk[j]]] : (uint8_t*)t->out_dev.p + poff[j];
+		/* filtered: the passes' descriptors (one upload from ft_host), then per file the picture the earlier
+		 * stages write (outs from here on) and two scratch pictures; the last pass writes the destination */
+		std::vector<QsFilterLaunch> flaunch;
+		if (nfilters && nr) {
+			std::vector<QsFilterPic> fp(nr);
+			std::vector<QsFilterDesc> fdesc;
+			size_t fo = align256(sizeof(QsFilterDesc) * QS_FILTER_MAX_STEPS * (size_t)nfilters * nr), all = fo;
+			for (int j = 0; j < nr; j++) all += 3 * align256(plans[files[rk[j]]].pix);
+			TK(grow_dev(&t->ft_dev, all));
+			uint8_t *fd = (uint8_t*)t->ft_dev.p;
+			for (int j = 0; j < nr; j++) {
+				const QsPlan &p = plans[files[rk[j]]];
+				const size_t a = align256(p.pix);
+				fp[j].in = fd + fo; fp[j].a = fd + fo + a; fp[j].b = fd + fo + 2 * a; fp[j].out = outs[j];
+				fp[j].w = p.out_w; fp[j].h = p.out_h; fp[j].ch = p.channels; fp[j].chw = layout == JPEGQS_RENDER_CHW;
+				outs[j] = fp[j].in;
+				fo += 3 * a;
+			}
+			qs_filter_plan(filters, nfilters, fp.data(), nr, fdesc, flaunch);
+			TK(grow_host(&t->ft_host, sizeof(QsFilterDesc) * fdesc.size()));
+			memcpy(t->ft_host.p, fdesc.data(), sizeof(QsFilterDesc) * fdesc.size());
+			TK(cudaMemcpyAsync(fd, t->ft_host.p, sizeof(QsFilterDesc) * fdesc.size(), cudaMemcpyHostToDevice, st));
+		}
 		/* resized: the render writes each picture into rs_dev, which holds the resize descriptors, the
 		 * reduce descriptors and the tables (one upload from rs_host), then the intermediates, then the
 		 * pictures, then the reduced pictures; the reduce writes those, the resize writes outs */
@@ -892,7 +925,7 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 				const int j = rsj[q], f = files[rk[j]];
 				const QsResizePlan &r = rsp[f];
 				const QsPlan &p = plans[f];
-				qs_resize_desc(r, p.reduced ? rdp[f].out_w : p.pic_w, p.channels, layout == JPEGQS_RENDER_CHW, desc[q]);
+				qs_resize_desc(r, p.reduced ? rdp[f].out_w : p.pic_w, p.channels, layout == JPEGQS_RENDER_CHW && !nfilters, desc[q]);
 				memcpy(rh + toff[q], r.tab.data(), r.tab.size() * sizeof(int32_t));
 				desc[q].src = rd + (p.reduced ? roff[q] : qoff[q]); desc[q].mid = rd + moff[q]; desc[q].out = outs[j];
 				desc[q].tab = (const int32_t*)(rd + toff[q]);
@@ -918,11 +951,12 @@ static int pixels_batch(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 		for (int j0 = 0, j1; j0 < nr; j0 = j1) {
 			const QsPlan &p0 = plans[files[rk[j0]]];
 			for (j1 = j0 + 1; j1 < nr && rkey(plans[files[rk[j1]]]) == rkey(p0); j1++) {}
-			TQ(qs_render_images(ctx, j1 - j0, rimg.data() + j0, run + j0, p0.resized ? JPEGQS_RENDER_HWC : layout, 1, p0.scale,
+			TQ(qs_render_images(ctx, j1 - j0, rimg.data() + j0, run + j0, p0.resized || nfilters ? JPEGQS_RENDER_HWC : layout, 1, p0.scale,
 					ro.data() + j0, outs.data() + j0, st, mode, mode ? rcs.data() + j0 : NULL));
 		}
 		if (nrd) TK(qs_launch_reduce((const QsReduceDesc*)((uint8_t*)t->rs_dev.p + rdo), nrd, rblocks, st));
 		if (nrs) TK(qs_launch_resize((const QsResizeDesc*)t->rs_dev.p, nrs, hblocks, vblocks, st));
+		if (!flaunch.empty()) TK(qs_filter_enqueue(flaunch, (const QsFilterDesc*)t->ft_dev.p, st));
 		/* JPEG: compress_async over the pictures into the slots, then the packing kernel into the
 		 * workspace, its records back */
 		uint8_t *jd = (uint8_t*)t->jp_dev.p, *jh = (uint8_t*)t->jp_host.p;
@@ -1043,10 +1077,24 @@ static int reduced_ok(jpegqs_cuda_ctx *ctx, const char *who, int n, const jpegqs
 	return 0;
 }
 
+/* the filters' check: nfilters 0..64, each one qs_filter_check takes */
+static int filters_ok(jpegqs_cuda_ctx *ctx, const char *who, const jpegqs_cuda_image_filter *filters, int nfilters) {
+	char msg[240];
+	const char *bad = nfilters < 0 || nfilters > 64 ? "nfilters outside 0..64" : nfilters && !filters ? "filters NULL" : NULL;
+	int k = 0;
+	for (; k < nfilters && !bad; k++) bad = qs_filter_check(filters[k]);
+	if (!bad) return 1;
+	if (k) snprintf(msg, sizeof(msg), "%s: filter %d: %s", who, k - 1, bad);
+	else snprintf(msg, sizeof(msg), "%s: %s", who, bad);
+	qs_ctx_decode_done(ctx, 0, msg);
+	return 0;
+}
+
 static int pixels_entry(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint8_t *const *data, const size_t *len,
 		int flags, int niter, int layout, int scale_denom, int resize, int filter, const jpegqs_cuda_resize_box *boxes,
 		int out_on_device, uint8_t *const *out, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results,
-		const int32_t *orientation = NULL, int mode = JPEGQS_PIXELS_AS_FILE, int thumbnail = 0, double gap = 0.0) {
+		const int32_t *orientation = NULL, int mode = JPEGQS_PIXELS_AS_FILE, int thumbnail = 0, double gap = 0.0,
+		const jpegqs_cuda_image_filter *filters = NULL, int nfilters = 0) {
 	char msg[200];
 	if (!ctx) return JPEGQS_ERR_ARG;
 	if (n < 0) { snprintf(msg, sizeof(msg), "%s: negative file count", who); qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG; }
@@ -1075,10 +1123,21 @@ static int pixels_entry(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint
 		}
 	}
 	if (!orientation_ok(ctx, who, n, orientation) || !mode_ok(ctx, who, mode) ||
-			!reduced_ok(ctx, who, n, boxes, scale_denom, thumbnail, gap)) return JPEGQS_ERR_ARG;
+			!reduced_ok(ctx, who, n, boxes, scale_denom, thumbnail, gap) || !filters_ok(ctx, who, filters, nfilters))
+		return JPEGQS_ERR_ARG;
 	for (int i = 0; i < n; i++) { memset(&results[i], 0, sizeof(results[i])); results[i].reason = ""; rc[i] = 0; }
 	return pixels_batch(ctx, who, n, data, len, flags, niter, layout, scale_denom, filter, resize ? boxes : NULL, orientation,
-			mode, out_on_device, out, max_device_bytes, rc, results, NULL, NULL, NULL, thumbnail, gap);
+			mode, out_on_device, out, max_device_bytes, rc, results, NULL, NULL, NULL, thumbnail, gap, filters, nfilters);
+}
+
+extern "C" int jpegqs_cuda_pixels_batch_filtered(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int layout, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
+		const int32_t *orientation, int mode, int out_on_device, uint8_t *const *out, size_t max_device_bytes, int *rc,
+		jpegqs_cuda_pixels_result *results, int thumbnail, double reducing_gap, const jpegqs_cuda_image_filter *filters,
+		int nfilters) {
+	return pixels_entry(ctx, "jpegqs_cuda_pixels_batch_filtered", n, data, len, flags, niter, layout, scale_denom,
+			boxes != NULL, filter, boxes, out_on_device, out, max_device_bytes, rc, results, orientation, mode, thumbnail,
+			reducing_gap, filters, nfilters);
 }
 
 extern "C" int jpegqs_cuda_pixels_batch_reduced(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
@@ -1116,7 +1175,8 @@ extern "C" int jpegqs_cuda_pixels_batch_resized(jpegqs_cuda_ctx *ctx, int n, con
 static int pixels_jpeg_entry(jpegqs_cuda_ctx *ctx, const char *who, int n, const uint8_t *const *data, const size_t *len,
 		int flags, int niter, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
 		const jpegqs_cuda_jpeg_params *params, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results,
-		uint8_t **out, size_t *out_len, const int32_t *orientation, int mode, int thumbnail = 0, double gap = 0.0) {
+		uint8_t **out, size_t *out_len, const int32_t *orientation, int mode, int thumbnail = 0, double gap = 0.0,
+		const jpegqs_cuda_image_filter *filters = NULL, int nfilters = 0) {
 	char msg[200];
 	if (!ctx) return JPEGQS_ERR_ARG;
 	if (n < 0) { snprintf(msg, sizeof(msg), "%s: negative file count", who); qs_ctx_decode_done(ctx, 0, msg); return JPEGQS_ERR_ARG; }
@@ -1147,10 +1207,20 @@ static int pixels_jpeg_entry(jpegqs_cuda_ctx *ctx, const char *who, int n, const
 		}
 	}
 	if (!orientation_ok(ctx, who, n, orientation) || !mode_ok(ctx, who, mode) ||
-			!reduced_ok(ctx, who, n, boxes, scale_denom, thumbnail, gap)) return JPEGQS_ERR_ARG;
+			!reduced_ok(ctx, who, n, boxes, scale_denom, thumbnail, gap) || !filters_ok(ctx, who, filters, nfilters))
+		return JPEGQS_ERR_ARG;
 	for (int i = 0; i < n; i++) { memset(&results[i], 0, sizeof(results[i])); results[i].reason = ""; rc[i] = 0; out[i] = NULL; out_len[i] = 0; }
 	return pixels_batch(ctx, who, n, data, len, flags, niter, JPEGQS_RENDER_HWC, scale_denom, filter, boxes, orientation, mode, 0, NULL,
-			max_device_bytes, rc, results, params, out, out_len, thumbnail, gap);
+			max_device_bytes, rc, results, params, out, out_len, thumbnail, gap, filters, nfilters);
+}
+
+extern "C" int jpegqs_cuda_pixels_batch_jpeg_filtered(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,
+		int flags, int niter, int scale_denom, int filter, const jpegqs_cuda_resize_box *boxes,
+		const jpegqs_cuda_jpeg_params *params, size_t max_device_bytes, int *rc, jpegqs_cuda_pixels_result *results,
+		uint8_t **out, size_t *out_len, const int32_t *orientation, int mode, int thumbnail, double reducing_gap,
+		const jpegqs_cuda_image_filter *filters, int nfilters) {
+	return pixels_jpeg_entry(ctx, "jpegqs_cuda_pixels_batch_jpeg_filtered", n, data, len, flags, niter, scale_denom, filter, boxes,
+			params, max_device_bytes, rc, results, out, out_len, orientation, mode, thumbnail, reducing_gap, filters, nfilters);
 }
 
 extern "C" int jpegqs_cuda_pixels_batch_jpeg_reduced(jpegqs_cuda_ctx *ctx, int n, const uint8_t *const *data, const size_t *len,

@@ -100,6 +100,12 @@ class _ResizeBox(C.Structure):
                 ("width", C.c_int32), ("height", C.c_int32)]
 
 
+class _ImageFilter(C.Structure):
+    """jpegqs_cuda_image_filter (include/jpegqs_cuda.h)."""
+    _fields_ = [("kind", C.c_int32), ("radius_x", C.c_float), ("radius_y", C.c_float), ("percent", C.c_int32),
+                ("threshold", C.c_int32)]
+
+
 class _JpegParams(C.Structure):
     """jpegqs_cuda_jpeg_params (include/jpegqs_cuda.h)."""
     _fields_ = [("quality", C.c_int32), ("subsampling", C.c_int32), ("optimize", C.c_int32)]
@@ -301,6 +307,20 @@ def load():
                                              C.POINTER(C.c_int32), C.c_void_p]
     lib.jpegqs_cuda_resize_model_box.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                                  C.POINTER(C.c_double), C.c_int, C.c_int, C.c_double, C.c_void_p]
+    lib.jpegqs_cuda_pixels_batch_filtered.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_size_t),
+                                                      C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(_ResizeBox),
+                                                      C.POINTER(C.c_int32), C.c_int, C.c_int, C.POINTER(C.c_void_p),
+                                                      C.c_size_t, C.POINTER(C.c_int), C.POINTER(_PixelsResult), C.c_int,
+                                                      C.c_double, C.POINTER(_ImageFilter), C.c_int]
+    lib.jpegqs_cuda_pixels_batch_jpeg_filtered.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_char_p),
+                                                           C.POINTER(C.c_size_t), C.c_int, C.c_int, C.c_int, C.c_int,
+                                                           C.POINTER(_ResizeBox), C.POINTER(_JpegParams), C.c_size_t,
+                                                           C.POINTER(C.c_int), C.POINTER(_PixelsResult),
+                                                           C.POINTER(C.c_void_p), C.POINTER(C.c_size_t),
+                                                           C.POINTER(C.c_int32), C.c_int, C.c_int, C.c_double,
+                                                           C.POINTER(_ImageFilter), C.c_int]
+    lib.jpegqs_cuda_image_filter_model.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(_ImageFilter), C.c_int,
+                                                   C.c_void_p]
     lib.jpegqs_cuda_tables.argtypes = [C.c_int, C.c_void_p]
     lib.jpegqs_cuda_orig_coef.argtypes = [C.c_int, C.c_int]
     _lib = lib
@@ -562,6 +582,81 @@ def thumbnail_model(pixels, full_size, bound, filter="bicubic", reducing_gap=2.0
     gap = _reducing_gap(reducing_gap, True, "thumbnail_model")
     box = (0.0, 0.0, W / s, H / s) if gap and not loaded else None
     return resize_model_box(a, (tw, th), box, filter, gap or None)
+
+
+# include/jpegqs_cuda.h: the largest radius magnitude (any axis, any filter) and UnsharpMask percent taken;
+# beyond them Pillow's 32-bit sums would overflow
+FILTER_MAX_RADIUS = 65535.0
+FILTER_MAX_PERCENT = 8421504
+
+
+def _filter_radius(v, who: str):
+    import numbers
+    if not isinstance(v, numbers.Real):
+        raise ValueError(f"{who}: radius {v!r}: expected a number")
+    r = float(v)
+    if not abs(r) <= FILTER_MAX_RADIUS:
+        raise ValueError(f"{who}: radius {v!r}: expected a finite value of magnitude at most {FILTER_MAX_RADIUS:g}")
+    return r
+
+
+def _filter_int(v, what: str, lim: int, who: str):
+    import numbers
+    if not isinstance(v, numbers.Integral) or not -lim <= int(v) <= lim:
+        raise ValueError(f"{who}: {what} {v!r}: expected an int in -{lim}..{lim}")
+    return int(v)
+
+
+def _image_filters(image_filter, who: str):
+    """image_filter (None, one filter or a sequence of them: Pillow's ImageFilter.GaussianBlur, BoxBlur or
+    UnsharpMask, instances or classes) as a C array of jpegqs_cuda_image_filter, or None for no filter.
+    ValueError names any other filter and a value Pillow's arithmetic cannot take."""
+    if image_filter is None:
+        return None
+    seq = list(image_filter) if isinstance(image_filter, (list, tuple)) else [image_filter]
+    if not seq:
+        return None
+    from PIL import ImageFilter
+    kinds = {ImageFilter.BoxBlur: 1, ImageFilter.GaussianBlur: 2, ImageFilter.UnsharpMask: 3}
+    out = (_ImageFilter * len(seq))()
+    for k, f in enumerate(seq):
+        w = f"{who}: image_filter {k}"
+        if isinstance(f, type):
+            if f not in kinds:
+                raise ValueError(f"{w}: {f.__name__}: expected ImageFilter.GaussianBlur, BoxBlur or UnsharpMask")
+            f = f()                                       # Image.filter's instance of a class: Pillow's defaults
+        kind = kinds.get(type(f))
+        if kind is None:
+            raise ValueError(f"{w}: {type(f).__name__}: expected ImageFilter.GaussianBlur, BoxBlur or UnsharpMask")
+        if kind == 3:
+            r = _filter_radius(f.radius, w)
+            out[k] = _ImageFilter(3, r, r, _filter_int(f.percent, "percent", FILTER_MAX_PERCENT, w),
+                                  _filter_int(f.threshold, "threshold", 2 ** 31 - 1, w))
+            continue
+        xy = f.radius if isinstance(f.radius, (tuple, list)) else (f.radius, f.radius)
+        if len(xy) != 2:
+            raise ValueError(f"{w}: radius {f.radius!r}: expected a number or (x, y)")
+        rx, ry = _filter_radius(xy[0], w), _filter_radius(xy[1], w)
+        if kind == 1 and (rx < 0 or ry < 0):
+            raise ValueError(f"{w}: radius {f.radius!r}: radius must be >= 0")
+        out[k] = _ImageFilter(kind, rx, ry, 0, 0)
+    return out
+
+
+def image_filter_model(pixels, image_filter):
+    """The device filters on one CPU thread, through the same pass plan (jpegqs_cuda_image_filter_model):
+    byte for byte Pillow's Image.fromarray(pixels).filter(F1).filter(F2)... for image_filter F1 or
+    [F1, F2, ...] (ImageFilter.GaussianBlur, BoxBlur or UnsharpMask).  pixels: uint8 [H, W] or
+    [H, W, 1|3]; returns the same shape."""
+    a, c = _host_pixels(pixels, "image_filter_model")
+    filt = _image_filters(image_filter, "image_filter_model")
+    h, w = a.shape[:2]
+    out = np.empty_like(a)
+    lib = load()
+    rc = lib.jpegqs_cuda_image_filter_model(a.ctypes.data, w, h, c, filt, len(filt) if filt else 0, out.ctypes.data)
+    if rc < 0:
+        raise ValueError(f"image_filter_model: {lib.jpegqs_cuda_last_error(None).decode()} ({rc})")
+    return out
 
 
 def _fill_image(ci: _Image, image: CoefImage, coef_ptrs: Sequence[int], up_ptrs: Sequence[Optional[int]]):
@@ -1185,7 +1280,7 @@ class QsContext:
 
     def decode_pixels(self, datas, flags: int, niter: int, layout: str = "hwc", device: str = "cuda",
                       max_device_bytes: int = 0, scale_denom: int = 1, size=None, crop=None, filter="bicubic",
-                      orientation=None, mode=None, thumbnail=None, reducing_gap=_GAP_DEFAULT):
+                      orientation=None, mode=None, thumbnail=None, reducing_gap=_GAP_DEFAULT, image_filter=None):
         """Many JPEG files to the smoothed pixels the jpegqs tool's --ppm writes for them (islow, fancy
         up-sampling, after do_quantsmooth(flags, niter)), in shared launches (jpegqs_cuda_pixels_batch).
         Returns, in the order of datas, one record per file:
@@ -1224,7 +1319,13 @@ class QsContext:
         first, as exif_transpose and convert do, so there is no draft.  reducing_gap: Pillow's, default 2.0 with thumbnail and None with size
         (an explicit None is None in both); with size, Image.resize(size, filter, reducing_gap=) of the
         crop.  ValueError naming the file for a bad bound, for thumbnail with size, crop or scale_denom
-        other than 1, or for a reducing_gap below 1.0, before anything runs."""
+        other than 1, or for a reducing_gap below 1.0, before anything runs.
+        image_filter: None, one of Pillow's ImageFilter.GaussianBlur, BoxBlur or UnsharpMask (an instance, or
+        the class for Pillow's defaults), or a sequence of them: each file's picture as above, then
+        .filter(F1).filter(F2)... on the device (jpegqs_cuda_pixels_batch_filtered), the last stage.  None
+        and [] are the call without it.  ValueError naming any other filter, a negative BoxBlur radius, a
+        radius above FILTER_MAX_RADIUS or a percent above FILTER_MAX_PERCENT in magnitude, or a non-int
+        percent or threshold, before anything runs."""
         if isinstance(datas, (bytes, bytearray, memoryview, str)) or not hasattr(datas, "__len__"):
             raise TypeError("decode_pixels: datas must be a sequence of bytes-like files")
         files = [_file_bytes(d, f"decode_pixels: file {i}") for i, d in enumerate(datas)]
@@ -1247,6 +1348,7 @@ class QsContext:
         gap = _reducing_gap(reducing_gap, bounds is not None, "decode_pixels") if resize or bounds is not None else 0.0
         if bounds is not None:
             fcode = _resize_filter(filter, "decode_pixels")
+        filt = _image_filters(image_filter, "decode_pixels")
         if not n:
             return []
         # the output size rule of jpegqs_cuda_pixels_batch: transcode_route's width, height and ncomp
@@ -1287,7 +1389,15 @@ class QsContext:
         optrs = (C.c_void_p * n)(*[t.data_ptr() for t in outs])
         rc = (C.c_int * n)()
         res = (_PixelsResult * n)()
-        if bounds is not None or gap:
+        if filt is not None:
+            sized = bounds is not None or resize
+            self._check(self.lib.jpegqs_cuda_pixels_batch_filtered(self.h, n, ptrs, lens, int(flags), int(niter),
+                                                                  0 if layout == "hwc" else 1, scale,
+                                                                  fcode if sized else 0, boxes if sized else None,
+                                                                  None if orient is None else (C.c_int32 * n)(*orient),
+                                                                  m, int(device == "cuda"), optrs, int(max_device_bytes),
+                                                                  rc, res, int(bounds is not None), gap, filt, len(filt)))
+        elif bounds is not None or gap:
             self._check(self.lib.jpegqs_cuda_pixels_batch_reduced(self.h, n, ptrs, lens, int(flags), int(niter),
                                                                   0 if layout == "hwc" else 1, scale, fcode, boxes,
                                                                   None if orient is None else (C.c_int32 * n)(*orient),
@@ -1929,7 +2039,7 @@ class QsContext:
 
     def reencode(self, datas, flags: int, niter: int, quality=75, subsampling="4:2:0", optimize=False, scale_denom=1,
                  size=None, crop=None, filter="bicubic", max_device_bytes: int = 0, orientation=None, mode=None,
-                 progressive=False, thumbnail=None, reducing_gap=_GAP_DEFAULT):
+                 progressive=False, thumbnail=None, reducing_gap=_GAP_DEFAULT, image_filter=None):
         """Many JPEG files to JPEG files of their smoothed pixels (jpegqs_cuda_pixels_batch_jpeg): each
         file's output is exactly Pillow's Image.fromarray(P).save(f, "JPEG", quality=quality,
         subsampling=subsampling, optimize=optimize), where P is the picture decode_pixels gives for the
@@ -1945,7 +2055,8 @@ class QsContext:
         and YCCK files give RGB files and "L" gives grey files.  progressive=True: Pillow's
         save(..., progressive=True) instead.  thumbnail / reducing_gap: as for decode_pixels
         (jpegqs_cuda_pixels_batch_jpeg_reduced): Pillow's thumbnail (or resize with reducing_gap), then
-        save."""
+        save.  image_filter: as for decode_pixels (jpegqs_cuda_pixels_batch_jpeg_filtered): the picture is
+        filtered on the device, then saved."""
         if isinstance(datas, (bytes, bytearray, memoryview, str)) or not hasattr(datas, "__len__"):
             raise TypeError("reencode: datas must be a sequence of bytes-like files")
         files = [_file_bytes(d, f"reencode: file {i}") for i, d in enumerate(datas)]
@@ -1962,6 +2073,7 @@ class QsContext:
         m = _mode(mode, "reencode")
         bounds = self._thumbnail_args(n, thumbnail, resize, scale, "reencode")
         gap = _reducing_gap(reducing_gap, bounds is not None, "reencode") if resize or bounds is not None else 0.0
+        filt = _image_filters(image_filter, "reencode")
         if not n:
             return []
         boxes = None
@@ -1984,7 +2096,12 @@ class QsContext:
         res = (_PixelsResult * n)()
         outs = (C.c_void_p * n)()
         olen = (C.c_size_t * n)()
-        if bounds is not None or gap:
+        if filt is not None:
+            self._check(self.lib.jpegqs_cuda_pixels_batch_jpeg_filtered(
+                self.h, n, ptrs, lens, int(flags), int(niter), scale, fcode, boxes, C.byref(jp), int(max_device_bytes),
+                rc, res, outs, olen, None if orient is None else (C.c_int32 * n)(*orient), m, int(bounds is not None), gap,
+                filt, len(filt)))
+        elif bounds is not None or gap:
             self._check(self.lib.jpegqs_cuda_pixels_batch_jpeg_reduced(
                 self.h, n, ptrs, lens, int(flags), int(niter), scale, fcode, boxes, C.byref(jp), int(max_device_bytes),
                 rc, res, outs, olen, None if orient is None else (C.c_int32 * n)(*orient), m, int(bounds is not None), gap))
@@ -2284,15 +2401,17 @@ def transcode_batch(datas, flags: int, niter: int, optimize: bool = False, copy:
 
 def decode_pixels(datas, flags: int, niter: int, layout: str = "hwc", device: str = "cuda", max_device_bytes: int = 0,
                   gpu: int = -1, scale_denom: int = 1, size=None, crop=None, filter="bicubic", orientation=None,
-                  mode=None, thumbnail=None, reducing_gap=_GAP_DEFAULT):
+                  mode=None, thumbnail=None, reducing_gap=_GAP_DEFAULT, image_filter=None):
     """QsContext.decode_pixels on the default context of CUDA device `gpu`: one record (pixels, warnings,
     host_decoded, smoothed, stop, upsampled, reason) per file, at 1/scale_denom size, cropped and resized
     as Pillow would with size / crop / filter ((width, height) and (left, top, right, bottom), Pillow's
     conventions), turned by `orientation` ("exif", 1..8, or one value 0..8 per file) first and converted by
     `mode` (None, "RGB" or "L", Pillow's Image.convert) before the crop; or Pillow's thumbnail(bound, filter,
-    reducing_gap) with `thumbnail`."""
+    reducing_gap) with `thumbnail`; then Pillow's Image.filter of each of `image_filter` (GaussianBlur, BoxBlur
+    or UnsharpMask) in turn."""
     return default_context(gpu).decode_pixels(datas, flags, niter, layout, device, max_device_bytes, scale_denom,
-                                              size, crop, filter, orientation, mode, thumbnail, reducing_gap)
+                                              size, crop, filter, orientation, mode, thumbnail, reducing_gap,
+                                              image_filter)
 
 
 def compress_async(pixels, quality=75, subsampling="4:2:0", optimize=False, out=None, stream=None, progressive=False):
@@ -2309,10 +2428,10 @@ def compress_async(pixels, quality=75, subsampling="4:2:0", optimize=False, out=
 
 def reencode(datas, flags: int, niter: int, quality=75, subsampling="4:2:0", optimize=False, scale_denom=1, size=None,
              crop=None, filter="bicubic", max_device_bytes: int = 0, gpu: int = -1, orientation=None, mode=None,
-             progressive=False, thumbnail=None, reducing_gap=_GAP_DEFAULT):
+             progressive=False, thumbnail=None, reducing_gap=_GAP_DEFAULT, image_filter=None):
     """QsContext.reencode on the default context of CUDA device `gpu`: one record (data, warnings,
     host_decoded, smoothed, stop, upsampled, reason) per file, data the JPEG file Pillow's save writes for
     the picture decode_pixels gives with the same arguments."""
     return default_context(gpu).reencode(datas, flags, niter, quality, subsampling, optimize, scale_denom, size, crop,
                                          filter, max_device_bytes, orientation, mode, progressive, thumbnail,
-                                         reducing_gap)
+                                         reducing_gap, image_filter)

@@ -181,3 +181,12 @@ for o in (None, 6):
     print("decode_pixels thumbnail orientation", o, [tuple(p[0].shape) for p in px], flush=True)
 px = ctx.decode_pixels(tfiles, 3, 1, size=(9, 5), crop=[None, (3, 5, 300, 200), None, (1, 1, 160, 96)], reducing_gap=1.0)
 print("decode_pixels reducing_gap", [tuple(p[0].shape) for p in px], flush=True)
+
+# blur and sharpen: fused rows and a row wider than the fused kernel holds (7000 x 3 bytes), a chain ending
+# in UnsharpMask, CHW output, and a filtered reencode
+from PIL import ImageFilter  # noqa: E402
+ffiles = [jpeg(90, 50, quality=75), jpeg(7000, 9, quality=85), jpeg(33, 17, "L", quality=100)]
+px = ctx.decode_pixels(ffiles, 3, 1, "chw", image_filter=[ImageFilter.GaussianBlur(5), ImageFilter.UnsharpMask(2, 150, 3)])
+print("decode_pixels image_filter", [tuple(p[0].shape) for p in px], flush=True)
+enc = ctx.reencode(ffiles, 3, 1, thumbnail=(40, 40), image_filter=ImageFilter.BoxBlur((3, 0)))
+print("reencode image_filter", [len(r[0]) for r in enc], flush=True)
