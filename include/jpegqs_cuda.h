@@ -376,6 +376,12 @@ int jpegqs_cuda_jpeg_read(const uint8_t *data, size_t len, const jpegqs_cuda_ima
  *     the JPEGQS_DECODE_* bits below.  status 0 => the coefficients equal jpeg_read_coefficients'.  A
  *     flagged image's coefficients are unspecified, but every write stays inside that image's arrays
  *     and every loop is bounded by the data length; the other images are not affected.
+ *   - Stream features.  Accepted (status 0): FF fill bytes before the marker that ends the segment,
+ *     restart intervals of any length up to 65535 (also the MCU count and more), any component
+ *     identifiers and table slots, Huffman codes up to 16 bits.  Flagged (the host reader, which
+ *     accepts them as libjpeg does, decodes these): FF fill bytes before an RSTn (the segment ends at
+ *     the first FF, so RESTART | UNITS), and an interval's padding with 0-bits instead of 1-bits
+ *     (UNITS, with TRUNCATED for a sequential scan).  tests/stream_files.py holds a file of each.
  *   - Argument errors change nothing: every check runs before the first enqueue and a failed one
  *     returns JPEGQS_ERR_ARG with nothing enqueued.  Checked: NULL pointers (imgs, scans, data_dev and
  *     its entries, data_len, status_dev, coef), a coef not 16-byte aligned, rows / rows_up set, a

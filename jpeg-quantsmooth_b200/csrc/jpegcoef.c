@@ -214,8 +214,13 @@ static void bits_fill(jq_bits *b) {
 		if (!b->hit_marker && b->p < b->end) {
 			c = *b->p;
 			if (c == 0xFF) {
-				if (b->p + 1 < b->end && b->p[1] == 0) b->p += 2;
-				else { b->hit_marker = 1; c = 0; }
+				/* any number of FF fill bytes may precede a marker (B.1.1.2); like libjpeg's
+				 * jpeg_fill_bit_buffer, FF..FF 00 reads as one stuffed FF.  A marker leaves p on the
+				 * FF right before its code, where the restart and end-of-scan logic look for it. */
+				const unsigned char *q = b->p + 1;
+				while (q < b->end && *q == 0xFF) q++;
+				if (q < b->end && *q == 0) b->p = q + 1;
+				else { b->p = q - 1; b->hit_marker = 1; c = 0; }
 			} else b->p++;
 		}
 		b->buf = (b->buf << 8) | c; b->nbits += 8;
@@ -636,16 +641,18 @@ static int dec_scan_parallel(jq_dec *d, const jq_scan *s, const unsigned char *p
 		if (!q->range) goto out;
 		q->range[0].p = p;
 		for (t = p; (t = (const unsigned char*)memchr(t, 0xFF, (size_t)(end - t))) != NULL; ) {
-			if (t + 1 >= end) { segend = t; break; }
-			if (t[1] == 0) { t += 2; continue; }
-			if ((t[1] & 0xF8) == 0xD0) {
-				if (j + 1 >= nint || (unsigned)(t[1] & 7) != (unsigned)(j & 7)) goto out;
-				q->range[j].end = t; j++; q->range[j].p = t + 2;
-				t += 2; continue;
+			const unsigned char *u = t + 1;
+			while (u < end && *u == 0xFF) u++;          /* fill bytes before a marker: the range ends at the first */
+			if (u >= end) { segend = t; break; }
+			if (*u == 0) { if (u > t + 1) goto out; t += 2; continue; }    /* FF..FF 00: left to the plain decoder */
+			if ((*u & 0xF8) == 0xD0) {
+				if (j + 1 >= nint || (unsigned)(*u & 7) != (unsigned)(j & 7)) goto out;
+				q->range[j].end = t; j++; q->range[j].p = u + 1;
+				t = u + 1; continue;
 			}
 			segend = t; break;
 		}
-		if (!segend || j + 1 != nint || segend[0] != 0xFF || (segend + 1 < end && segend[1] == 0xFF)) goto out;
+		if (!segend || j + 1 != nint) goto out;
 		q->range[j].end = segend;
 		for (j = 0; j < nint; j++) {
 			q->range[j].m0 = j * (unsigned)ri;
@@ -661,12 +668,15 @@ static int dec_scan_parallel(jq_dec *d, const jq_scan *s, const unsigned char *p
 		goto out;
 	}
 
-	/* the segment ends at the first FF that is not followed by 00; it must be a real marker */
+	/* the segment ends at the first FF that is not followed by 00; it and any fill bytes after it must
+	 * lead to a real marker */
 	for (t = p; (t = (const unsigned char*)memchr(t, 0xFF, (size_t)(end - t))) != NULL; ) {
 		if (t + 1 < end && t[1] == 0) { t += 2; continue; }
 		segend = t; break;
 	}
-	if (!segend || segend + 1 >= end || segend[1] == 0xFF || (segend[1] & 0xF8) == 0xD0) goto out;
+	if (!segend) goto out;
+	for (t = segend + 1; t < end && *t == 0xFF; t++);
+	if (t >= end || *t == 0 || (*t & 0xF8) == 0xD0) goto out;
 	len = (size_t)(segend - p);
 	if (len < min_bytes) goto out;
 	q->segend = segend;
